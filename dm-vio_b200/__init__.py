@@ -1,1 +1,1 @@
-"""B200-native DM-VIO photometric hot path (package root; see DESIGN.md)."""
+"""H100-native DM-VIO photometric hot path (package root; see DESIGN.md)."""

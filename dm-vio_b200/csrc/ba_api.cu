@@ -84,8 +84,7 @@ int dmv_ba_create(const dmv_ba_config* cfg, dmv_ba** out) {
   if (cfg->device < 0 || cfg->device >= ndev) return set_error(DMV_ERR_INVALID, "device %d out of range (%d devices)", cfg->device, ndev);
   CK(cudaSetDevice(cfg->device));
   {  // L2 -> DRAM fetch granularity: 32 B instead of the driver default 64 B.  The hot path gathers 16-byte texels at data-dependent addresses;
-     // with 64-byte fetches every missed 32-byte sector drags its neighbour along: measured 7.58 -> 5.69 MB DRAM reads per launch at C3 (1.38x ->
-     // 1.04x the algorithmic bytes, profiles/r02_a_l2fetch_*), no change in kernel time.  A device-wide hint; DMV_L2_FETCH=64|128 restores / widens it.
+     // with 64-byte fetches every missed 32-byte sector drags its neighbour along.  A device-wide hint; DMV_L2_FETCH=64|128 restores / widens it.
     int g = 32;
     if (const char* e = getenv("DMV_L2_FETCH")) g = atoi(e);
     if (g == 32 || g == 64 || g == 128) { cudaDeviceSetLimit(cudaLimitMaxL2FetchGranularity, (size_t)g); cudaGetLastError(); }
@@ -110,7 +109,7 @@ static int ba_allocate(dmv_ba* b, const dmv_ba_config* cfg) {
   b->P = b->P_auto ? 16 : cfg->chunk_points;
   {
     int sms = 0;
-    if (cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, cfg->device) != cudaSuccess || sms < 1) sms = 148;
+    if (cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, cfg->device) != cudaSuccess || sms < 1) sms = 132;
     b->sms = sms;
   }
   b->mp = (cfg->max_points + 31) & ~31;

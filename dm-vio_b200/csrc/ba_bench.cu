@@ -17,7 +17,7 @@ int dmv_ba_bench_device(dmv_ba* b, const double* x, int iters, int flush_l2, flo
   if (x && !b->have_committed) return set_error(DMV_ERR_STATE, "no committed linearisation to resubstitute");
   CK(cudaSetDevice(b->device));
   if (flush_l2 && !b->d_flush) {
-    b->flush_n = (size_t)256 * 1024 * 1024 / sizeof(float4);  // 256 MiB > 126 MB L2
+    b->flush_n = (size_t)256 * 1024 * 1024 / sizeof(float4);  // 256 MiB > 50 MB L2
     CK(cudaMalloc(&b->d_flush, b->flush_n * sizeof(float4)));
     CK(cudaMemset(b->d_flush, 0, b->flush_n * sizeof(float4)));
   }

@@ -3,7 +3,7 @@
 //   AccumulatedSCHessianSSE::addPoint + both stitchDouble passes (AccumulatedTopHessian.cpp:L241-303, AccumulatedSCHessian.cpp:L78-157)
 //   + the point half of resubstituteF_MT / doStepFromBackup of the PREVIOUS iteration (EnergyFunctional.cpp:L295-321).
 //
-// B200 design: ONE THREAD PER POINT-RESIDUAL.  A residual is a ~1000-instruction chain whose reductions over the 8 pattern pixels
+// Design: ONE THREAD PER POINT-RESIDUAL.  A residual is a ~1000-instruction chain whose reductions over the 8 pattern pixels
 // stay in registers (no shuffles, nothing per-residual is computed twice), and the 16 / 32 residuals of one (host, target) pair sit in
 // adjacent lanes, so the pair's 13x13 block is reduced with a transposing butterfly (96 exchanges per pair instead of 96 x log2 P).
 //

@@ -30,7 +30,7 @@ struct dmv_ba {
   cudaEvent_t ev[4] = {nullptr, nullptr, nullptr, nullptr};
   int P = 16;            // points per chunk of the CURRENT window (16 or 32)
   bool P_auto = true;    // dmv_ba_config::chunk_points == 0: chosen per window in dmv_ba_set_points
-  int sms = 148;
+  int sms = 132;
   int mp = 0;  // point capacity (slot pitch)
   int nf = 0, npts = 0, nres = 0, nchunks = 0, max_chunks = 0;
   int N = 0, NW = 0, T = 0, ntiles = 0;

@@ -1,4 +1,4 @@
-// Small sm_100a kernels of the bundle-adjustment path next to ba_fused_kernel (ba_fused.cu):
+// Small sm_90a kernels of the bundle-adjustment path next to ba_fused_kernel (ba_fused.cu):
 //   ba_resub_kernel     stand-alone EnergyFunctional::resubstituteFPt + point part of doStepFromBackup (the hot loop uses the fused prologue)
 //   repack_aos3_kernel / make_dI_kernel   image ingestion (float4 texels)
 //   l2_flush_kernel     larger-than-L2 scrub used by the bench between timed iterations
@@ -77,6 +77,6 @@ void launch_resub_kernel(const BAWinDev& W, const BAIter& it, int apply, double*
 }
 void launch_repack(const float* src, float4* dst, int n, cudaStream_t s) { repack_aos3_kernel<<<(n + 255) / 256, 256, 0, s>>>(src, dst, n); }
 void launch_make_dI(const float* img, float4* dst, int w, int h, cudaStream_t s) { make_dI_kernel<<<(w * h + 255) / 256, 256, 0, s>>>(img, dst, w, h); }
-void launch_l2_flush(float4* buf, size_t n, cudaStream_t s) { l2_flush_kernel<<<148 * 8, 256, 0, s>>>(buf, n); }
+void launch_l2_flush(float4* buf, size_t n, cudaStream_t s) { l2_flush_kernel<<<132 * 8, 256, 0, s>>>(buf, n); }
 
 }  // namespace dmv

@@ -1,4 +1,4 @@
-// sm_100a kernel + C-ABI of CoarseInitializer::calcResAndGS (FullSystem/CoarseInitializer.cpp:L333-625): the two-frame direct initialiser's
+// sm_90a kernel + C-ABI of CoarseInitializer::calcResAndGS (FullSystem/CoarseInitializer.cpp:L333-625): the two-frame direct initialiser's
 // linearisation — 8-pixel pattern per point, one inverse depth per point eliminated by a Schur complement (DESIGN.md §5c).
 //
 //   ci_res_gs_kernel   8 lanes per point (one per pattern pixel), 4 points per warp: project, 4-tap float4 gather from the new frame's level

@@ -68,7 +68,7 @@ void nccl_destroy(void* comm) { if (comm && p_destroy) p_destroy(comm); }
 
 extern "C" {
 const char* dmv_last_error(void) { return dmv::g_err; }
-const char* dmv_version(void) { return "dmvio_b200 0.1 (sm_100a)"; }
+const char* dmv_version(void) { return "dmvio_b200 0.1 (sm_90a)"; }
 int dmv_device_count(void) {
   int n = 0;
   if (cudaGetDeviceCount(&n) != cudaSuccess) { cudaGetLastError(); return 0; }

@@ -1,4 +1,4 @@
-// sm_100a kernels + C-ABI of the coarse direct-image-alignment path (DESIGN.md §5).
+// sm_90a kernels + C-ABI of the coarse direct-image-alignment path (DESIGN.md §5).
 //
 //   ct_res_gs_kernel   CoarseTracker::calcRes (CoarseTracker.cpp:L361-517) fused with calcGSSSE (L299-356): one thread per
 //                      reference point: project, 4-tap float4 gather from the new frame's level plane, Huber residual,

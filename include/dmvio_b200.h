@@ -1,4 +1,4 @@
-/* dmvio_b200.h — C ABI of the B200-native DM-VIO photometric hot path.
+/* dmvio_b200.h — C ABI of the H100-native DM-VIO photometric hot path.
  *
  * Drop-in boundary (SURVEY.md §8b).  Plain C, opaque handles, int status codes, caller-owned host
  * buffers, one CUDA stream per handle, no global mutable state: a BA handle (mapper thread) and a
@@ -122,7 +122,8 @@ typedef struct dmv_ba_lin_result {
 int dmv_ba_linearize(dmv_ba* ba, dmv_ba_lin_result* out);
 
 /* Per-residual outputs of the last linearize, in the order given to dmv_ba_set_residuals
- * (state_NewState, state_NewEnergy, state_NewEnergyWithOutlier, centerProjectedTo; Residuals.h:L64-84). Any pointer may be NULL. */
+ * (state_NewState, state_NewEnergy, state_NewEnergyWithOutlier, centerProjectedTo; Residuals.h:L64-84) and JpJdF, which is defined for
+ * residuals with state_NewState == IN only (EFResidual::takeDataF runs on active residuals). Any pointer may be NULL. */
 int dmv_ba_get_residual_outputs(dmv_ba* ba, int32_t* newState, float* newEnergy, float* newEnergyWithOutlier, float* centerProjectedTo3,
                                 float* JpJdF8);
 
@@ -300,7 +301,7 @@ int dmv_ct_calc_res_gs(dmv_ct* ct, int level, const float RKi[9], const float t[
  * doubling, level repeat) runs on the device; the host gets the tracked pose back.  Same semantics as driving dmv_ct_calc_res_gs from the
  * host loop: R,t = lastToNew_out (refToNew, row-major), a,b = aff_g2l_out; on an aborted track (NaN residual or > 1.5*minResForAbort)
  * trackingGood = 0, status = 2 and R,t,a,b are returned unchanged, like the reference's early `return false`.
- * Needs all ceil(n/256) CTAs co-resident (n <= 148*256 reference points per level); otherwise DMV_ERR_INVALID. */
+ * Needs all ceil(n/256) CTAs co-resident (n <= #SMs*256 reference points per level: 132*256 on an H100); otherwise DMV_ERR_INVALID. */
 typedef struct dmv_ct_track_args {
   double R[9], t[3];          /* in: initial refToNew */
   double a, b;                /* in: initial aff_g2l of the new frame */

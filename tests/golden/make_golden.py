@@ -4,7 +4,7 @@
 The reference has no golden vectors or known-answer tests for this path (SURVEY.md §4, §8c).  These vectors come from the CPU
 oracle in its fp64-accumulating mode (precision=1) AFTER the oracle has been pinned bit-exact against the reference's own
 compiled code (oracle/_ref, tests/test_ref_pin.py — run that first): they freeze its outputs (a) to detect drift of the oracle
-or of the synthetic generator and (b) as a file-based checker for the CUDA path on the GPU box, where /root/reference does not exist.
+or of the synthetic generator and (b) as a file-based checker for the CUDA path on a GPU machine without the reference sources.
 
   golden_small_ba.npz    complete inputs (96x64 images) + every intermediate of one GN iteration  -> self-contained
   golden_c1_ba.npz       BASELINE config 1 (2 KF / 200 pts / 640x480): seed + input checksum + outputs

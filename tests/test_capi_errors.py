@@ -51,7 +51,7 @@ def test_no_device_means_error_not_cpu_fallback(capi):
 
 
 def test_version_string(capi):
-    assert b"sm_100a" in capi.lib().dmv_version()
+    assert b"sm_90a" in capi.lib().dmv_version()
 
 
 def test_keyframe_entry_points_validate_arguments(capi):

@@ -12,7 +12,7 @@ pytestmark = pytest.mark.gpu
 def hostapi():
     import dmvio_b200.capi as c
     if c.lib().dmv_device_count() < 1:
-        pytest.fail("no CUDA device visible: GPU tests must run on the B200 box")
+        pytest.fail("no CUDA device visible: GPU tests must run on the H100")
     import dmvio_b200.hostapi as h
     return h
 
