@@ -131,7 +131,7 @@ SYMBOLS = [
     "dmv_ba_set_window", "dmv_ba_set_points", "dmv_ba_set_residuals", "dmv_ba_set_adjoints", "dmv_ba_set_state", "dmv_ba_linearize",
     "dmv_ba_get_residual_outputs", "dmv_ba_get_target_energies", "dmv_ba_apply_res", "dmv_ba_accumulate", "dmv_ba_get_point_outputs", "dmv_ba_get_solve_HdiF",
     "dmv_ba_resubstitute", "dmv_ba_backup_points", "dmv_ba_restore_points", "dmv_ba_get_idepth", "dmv_ba_gn_step", "dmv_nccl_unique_id",
-    "dmv_ba_comm_init", "dmv_ba_activate_points", "dmv_ba_marginalize_points", "dmv_ba_drop_residuals", "dmv_ba_reset_oob", "dmv_ba_p2p_export", "dmv_ba_p2p_import", "dmv_ba_last_timing", "dmv_ba_bench_device", "dmv_ba_kernel_launch_count", "dmv_ba_io_bytes", "dmv_ba_set_timing", "dmv_ba_bench_e2e",
+    "dmv_ba_comm_init", "dmv_ba_activate_points", "dmv_ba_marginalize_points", "dmv_ba_drop_residuals", "dmv_ba_reset_oob", "dmv_ba_p2p_export", "dmv_ba_p2p_import", "dmv_ba_last_timing", "dmv_ba_bench_device", "dmv_ba_bench_phases", "dmv_ba_kernel_launch_count", "dmv_ba_io_bytes", "dmv_ba_set_timing", "dmv_ba_bench_e2e",
     "dmv_ba_batch_create", "dmv_ba_batch_destroy", "dmv_ba_batch_gn_step", "dmv_ba_batch_set_timing", "dmv_ba_batch_last_kernel_ms", "dmv_ba_batch_bench",
     "dmv_ct_create", "dmv_ct_destroy", "dmv_ct_set_K", "dmv_ct_set_ref", "dmv_ct_make_coarse_depth", "dmv_ct_get_ref", "dmv_ct_upload_new", "dmv_ct_upload_new_image", "dmv_ct_set_huber",
     "dmv_ci_create", "dmv_ci_destroy", "dmv_ci_set_K", "dmv_ci_upload_first", "dmv_ci_upload_new", "dmv_ci_set_points", "dmv_ci_calc_res_and_gs", "dmv_ci_kernel_launch_count",
@@ -179,6 +179,7 @@ def lib():
         L.dmv_ba_p2p_import.argtypes = [vp, C.c_int, C.c_int, vp]
         L.dmv_ba_last_timing.argtypes = [vp, f32p]
         L.dmv_ba_bench_device.argtypes = [vp, vp, C.c_int, C.c_int, C.POINTER(C.c_float), C.POINTER(C.c_float)]
+        L.dmv_ba_bench_phases.argtypes = [vp, vp, C.c_int, C.c_int, C.c_int, vp, C.POINTER(C.c_int), f32p]
         L.dmv_ba_kernel_launch_count.argtypes = [vp, C.POINTER(C.c_longlong)]
         L.dmv_ba_set_timing.argtypes = [vp, C.c_int]
         L.dmv_ba_bench_e2e.argtypes = [vp, vp, C.POINTER(BAState), C.c_int, C.POINTER(C.c_double)]
@@ -376,6 +377,15 @@ class BA:
         xx = _c(x, np.float64)
         check(self.L.dmv_ba_bench_device(self.h, _p(xx), iters, int(flush_l2), C.byref(a), C.byref(b)))
         return a.value, b.value
+
+    def bench_phases(self, x=None, iters=100, flush_l2=True, max_ctas=1024):
+        """phase clock of `iters` launches: (stamps [iters, n_ctas, 9] uint64 ns, CUDA-event ms per launch [iters])"""
+        st = np.zeros((iters, max_ctas, 9), np.uint64)
+        ms = np.zeros(iters, np.float32)
+        n = C.c_int(0)
+        xx = _c(x, np.float64)
+        check(self.L.dmv_ba_bench_phases(self.h, _p(xx), iters, int(flush_l2), max_ctas, st.ctypes.data, C.byref(n), ms))
+        return st[:, :n.value], ms
 
     def launch_count(self):
         n = C.c_longlong(0)

@@ -9,8 +9,11 @@ using namespace dmv;
 extern "C" {
 
 // iters x { [L2 scrub] ; ba_fused_kernel ; [NCCL all-reduce] } with everything resident in HBM; CUDA events on the handle's stream
-// bracket every launch: ms_per_iter = kernel + exchange, ms_kernel = ba_fused_kernel alone
-int dmv_ba_bench_device(dmv_ba* b, const double* x, int iters, int flush_l2, float* ms_per_iter, float* ms_kernel) {
+// bracket every launch: ms[i] = kernel + exchange, ms_k[i] = ba_fused_kernel alone.  clk != nullptr: the clocked instantiation of the
+// kernel writes its phase stamps to clk + i * clk_rows * FUSED_NCLK (the caller checked clk_rows >= the window's chunks >= the grid),
+// the grid goes to *grid.
+static int bench_loop(dmv_ba* b, const double* x, int iters, int flush_l2, std::vector<float>& ms, std::vector<float>& ms_k,
+                      unsigned long long* clk, int clk_rows, int* grid) {
   int rc = dmv_ba_check_ready(b);
   if (rc != DMV_OK) return rc;
   if (iters < 1 || iters > 4096) return set_error(DMV_ERR_INVALID, "iters out of range");
@@ -30,7 +33,8 @@ int dmv_ba_bench_device(dmv_ba* b, const double* x, int iters, int flush_l2, flo
     dmv_ba_next_exchange(b);
     HostUpload& U = *b->h_up;
     CK(cudaEventRecord(e[3 * i], b->stream));
-    CK(launch_fused_kernel(U.win, U.it, false, b->stream, &b->bar_count));
+    if (clk) CK(launch_fused_kernel_clocked(U.win, U.it, b->stream, &b->bar_count, clk + (size_t)i * clk_rows * FUSED_NCLK, grid));
+    else CK(launch_fused_kernel(U.win, U.it, false, b->stream, &b->bar_count));
     CK(cudaEventRecord(e[3 * i + 1], b->stream));
     if (b->nccl_comm && !b->xchg_on) {  // a separate all-reduce follows the kernel: the step ends behind it
       rc = dmv_ba_enqueue_exchange(b);
@@ -41,19 +45,53 @@ int dmv_ba_bench_device(dmv_ba* b, const double* x, int iters, int flush_l2, flo
   }
   CK(cudaGetLastError());
   CK(cudaStreamSynchronize(b->stream));
-  double tot = 0, pk = 0;
+  ms.assign(iters, 0.f);
+  ms_k.assign(iters, 0.f);
   for (int i = 0; i < iters; i++) {
-    float a = 0, c = 0;
-    cudaEventElapsedTime(&c, e[3 * i], e[3 * i + 1]);
-    if (b->nccl_comm && !b->xchg_on) cudaEventElapsedTime(&a, e[3 * i], e[3 * i + 2]);
-    else a = c;  // the step IS the kernel (the peer exchange, if any, happens inside it)
-    tot += a; pk += c;
+    cudaEventElapsedTime(&ms_k[i], e[3 * i], e[3 * i + 1]);
+    if (b->nccl_comm && !b->xchg_on) cudaEventElapsedTime(&ms[i], e[3 * i], e[3 * i + 2]);
+    else ms[i] = ms_k[i];  // the step IS the kernel (the peer exchange, if any, happens inside it)
   }
   for (auto& ev : e) cudaEventDestroy(ev);
-  if (ms_per_iter) *ms_per_iter = (float)(tot / iters);
-  if (ms_kernel) *ms_kernel = (float)(pk / iters);
   b->h_up->it.have_x = 0;
   b->have_tentative = true;
+  return DMV_OK;
+}
+
+int dmv_ba_bench_device(dmv_ba* b, const double* x, int iters, int flush_l2, float* ms_per_iter, float* ms_kernel) {
+  std::vector<float> ms, ms_k;
+  const int rc = bench_loop(b, x, iters, flush_l2, ms, ms_k, nullptr, 0, nullptr);
+  if (rc != DMV_OK) return rc;
+  double tot = 0, pk = 0;
+  for (int i = 0; i < iters; i++) { tot += ms[i]; pk += ms_k[i]; }
+  if (ms_per_iter) *ms_per_iter = (float)(tot / iters);
+  if (ms_kernel) *ms_kernel = (float)(pk / iters);
+  return DMV_OK;
+}
+
+int dmv_ba_bench_phases(dmv_ba* b, const double* x, int iters, int flush_l2, int max_ctas, unsigned long long* stamps, int* n_ctas, float* ms_kernel) {
+  if (!b || !stamps || !n_ctas || !ms_kernel || max_ctas < 1) return set_error(DMV_ERR_INVALID, "bad argument");
+  if (iters < 1 || iters > 4096) return set_error(DMV_ERR_INVALID, "iters out of range");
+  int rc = dmv_ba_check_ready(b);
+  if (rc != DMV_OK) return rc;
+  if (b->nccl_comm) return set_error(DMV_ERR_STATE, "the phase clock times the launch alone: no NCCL communicator");
+  rc = dmv_ba_fill_descriptor(b);
+  if (rc != DMV_OK) return rc;
+  if (b->h_up->win.nchunks > max_ctas) return set_error(DMV_ERR_INVALID, "max_ctas below the window's chunk count");
+  const size_t n = (size_t)iters * max_ctas * FUSED_NCLK;
+  CK(cudaSetDevice(b->device));
+  unsigned long long* d_clk = nullptr;
+  CK(cudaMalloc(&d_clk, n * sizeof(unsigned long long)));
+  if (cudaMemset(d_clk, 0, n * sizeof(unsigned long long)) != cudaSuccess) rc = set_error(DMV_ERR_CUDA, "cudaMemset failed");
+  std::vector<float> ms, ms_k;
+  int grid = 0;
+  if (rc == DMV_OK) rc = bench_loop(b, x, iters, flush_l2, ms, ms_k, d_clk, max_ctas, &grid);
+  if (rc == DMV_OK && cudaMemcpy(stamps, d_clk, n * sizeof(unsigned long long), cudaMemcpyDeviceToHost) != cudaSuccess)
+    rc = set_error(DMV_ERR_CUDA, "cudaMemcpy failed");
+  cudaFree(d_clk);
+  if (rc != DMV_OK) return rc;
+  *n_ctas = grid;
+  for (int i = 0; i < iters; i++) ms_kernel[i] = ms_k[i];
   return DMV_OK;
 }
 

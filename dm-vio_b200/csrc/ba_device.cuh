@@ -17,6 +17,7 @@ constexpr int TOP_USED = TOP_TRI + 6;              // 91
 constexpr int TOP_PART = 92;
 __host__ __device__ constexpr int top_off(int r) { return r * TOP_COLS - (r * (r - 1)) / 2; }  // offset of entry (r, r); entry (r, c>=r) = top_off(r) + c - r
 constexpr int RES_NONE = 255, RES_IN = 0, RES_OOB = 1, RES_OUTLIER = 2;
+constexpr int FUSED_NCLK = 9;      // phase-clock stamps per CTA of the measurement-only clocked launch (ba_fused.cu: clk_stamp)
 constexpr int ACC_MISC = 8;         // energy, n_in, n_oob, n_outlier, sum step^2, sum |idepth_backup|, npts, error flag (barrier / peer timeout)
 // Partial blob of one chunk (P points of host frame h), fp64, written by phase C of ba_fused_kernel with plain stores and summed in a
 // fixed order by phase D.  Per frame slot t: [O 64 | D 64 | C 32 | b 8]: t != h: O = contribution to H[h,t], D to H[t,t], C to H[t,C],

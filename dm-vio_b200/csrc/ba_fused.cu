@@ -107,6 +107,7 @@ struct FusedSmem {
   float rec[MAXF][16][P];      // per target: adHost*JpJdF [8], Hdd, bd, Hcd[4], active, pad   (lane = point: conflict-free)
   float Wv[P][8 * MAXF + 8];   // Schur vectors
   float hdi[P];
+  float prior[P];              // priorF of the chunk's points (staged with the adjoints: phase B has no load round trip of its own)
   float id[P], idz[P];
   float misc[16][8];           // per warp: energy, n_in, n_oob, n_outlier, step^2, |idepth_backup|, count
   double red[16][32];          // phase E: per-warp partials of up to two 4x4 tiles
@@ -135,23 +136,38 @@ __device__ __forceinline__ unsigned ld_acquire_u32(const unsigned* p) {
   return v;
 }
 // all CTAs of the (cooperative) grid; monotonic arrival counter, target = arrivals expected so far.  Bounded: a lost CTA can delay the
-// launch by ~0.1 s but never hang the GPU (the result then carries the error flag).
+// launch by ~0.1 s but never hang the GPU (the result then carries the error flag).  Visibility of the other CTAs' part / wg / hdig stores
+// rests on the release add and the acquire poll of thread 0, extended to the whole CTA by the block barriers on both sides (release and
+// acquire are cumulative over what the barrier ordered): no sequentially consistent fence is needed.
 __device__ __forceinline__ bool grid_barrier(unsigned* bar, unsigned target) {
   __shared__ int ok_s;
   __syncthreads();
   if (threadIdx.x == 0) {
-    __threadfence();
-    atomicAdd(bar, 1u);
+    asm volatile("red.release.gpu.global.add.u32 [%0], 1;" ::"l"(bar) : "memory");
     int ok = 1;
     const long long t0 = clock64();
     while ((int)(ld_acquire_u32(bar) - target) < 0) {
       if (clock64() - t0 > 200000000ll) { ok = 0; break; }
     }
-    __threadfence();
     ok_s = ok;
   }
   __syncthreads();
   return ok_s != 0;
+}
+
+// phase clock of the measurement-only instantiation (CLK = true, dmv_ba_bench_phases): thread 0 of the CTA writes %globaltimer to slot k of
+// its row of clk once `dep`, a value the timed phase produced, is available (the predicate on it orders the read after the producing
+// load).  Compiles to nothing in the product kernels.
+constexpr int NCLK = FUSED_NCLK;  // entry, chunk decoded, first loads, taps, end A, end C, barrier released, end D, end E
+template <bool CLK>
+__device__ __forceinline__ void clk_stamp(unsigned long long* clk, int k, unsigned dep = 0u) {
+  if constexpr (CLK) {
+    if (threadIdx.x == 0) {
+      unsigned long long t = 0;
+      asm volatile("{\n\t.reg .pred p;\n\tsetp.ne.u32 p, %1, 0x7fbadbad;\n\t@p mov.u64 %0, %%globaltimer;\n\t}" : "+l"(t) : "r"(dep) : "memory");
+      clk[(size_t)blockIdx.x * NCLK + k] = t;
+    }
+  }
 }
 
 // ---- exchange of result entries between ranks (sharded BA, SURVEY.md §8e): "LL" packets over NVLink peer memory.  Every result
@@ -232,8 +248,8 @@ __device__ __forceinline__ double xchg_pull_sum_group(const BAXchg& X, int idx, 
 // (EnergyFunctionalStructs.cpp:L88-114) turns resF into res_toZeroF, and the accumulation is AccumulatedTopHessian::addPoint<2> +
 // AccumulatedSCHessian::addPoint(p, shiftPriorToZero = false) with priorF * idepthFixPriorMargFac (EnergyFunctional.cpp:L678-742).
 // phases A-C for one chunk of one window (W / it may live in kernel-parameter space or in global memory)
-template <int P, int LPR, bool MARG>
-__device__ __forceinline__ void fused_chunk(const BAWinDev& W, const BAIter& it, FusedSmem<P, LPR>& S, const int chunk) {
+template <int P, int LPR, bool MARG, bool CLK = false>
+__device__ __forceinline__ void fused_chunk(const BAWinDev& W, const BAIter& it, FusedSmem<P, LPR>& S, const int chunk, unsigned long long* clk = nullptr) {
   constexpr int LOGP = (P == 32) ? 5 : 4;
   constexpr int NH = FusedSmem<P, LPR>::NH;
   const int nf = W.nf, N = W.N, mp = W.mp;
@@ -246,11 +262,13 @@ __device__ __forceinline__ void fused_chunk(const BAWinDev& W, const BAIter& it,
   h = min(h, nf - 1);
   const int ch_start = W.host_start[h] + (chunk - W.chunk_beg[h]) * P;
   const int ch_count = min(P, W.host_start[h + 1] - ch_start);
+  clk_stamp<CLK>(clk, 1, (unsigned)ch_count);
 
   // ---- stage the host's adjoint blocks (fp64 for phase C, fp32 for the Schur vectors); waited for at the first block barrier,
   // except the fp32 block of a warp's own pair(s), which the warp fetches itself below
   for (int i = tid; i < nf * 32; i += nthreads) cp_async16(&S.AhD[i >> 5][(i & 31) * 2], &A->adHost[h * nf + (i >> 5)][(i & 31) * 2]);
   for (int i = tid; i < nf * 4; i += nthreads) cp_async16(&S.dT[i >> 2][(i & 3) * 2], &A->adTdiag[h * nf + (i >> 2)][(i & 3) * 2]);
+  if (tid < ch_count) cp_async4(&S.prior[tid], W.priorF + ch_start + tid);
   asm volatile("cp.async.commit_group;" ::: "memory");
 
   float e_sum = 0.f, rs_step2 = 0.f, rs_nid = 0.f, rs_cnt = 0.f;
@@ -338,6 +356,7 @@ __device__ __forceinline__ void fused_chunk(const BAWinDev& W, const BAIter& it,
       idz = __ldg(W.idepth_zero + p);
     }
     if (r == 0 && valid) { S.id[pl] = idepth; S.idz[pl] = idz; }
+    clk_stamp<CLK>(clk, 2, __float_as_uint(idepth) ^ __float_as_uint(uv.x) ^ (unsigned)st);
     bool live = (st != RES_NONE) && (st != RES_OOB);
 
     // ---- centre pixel at the FEJ point (ResidualProjections.h:L62-87, Residuals.cpp:L108-157)
@@ -424,6 +443,7 @@ __device__ __forceinline__ void fused_chunk(const BAWinDev& W, const BAIter& it,
       }
       }
     }
+    clk_stamp<CLK>(clk, 3, __float_as_uint(s.JI00));
 
     // ---- classification (Residuals.cpp:L260-273) and per-residual outputs
     int newState;
@@ -555,33 +575,38 @@ __device__ __forceinline__ void fused_chunk(const BAWinDev& W, const BAIter& it,
     for (int u = 0; u < 4; u++) ah[u] = __ldg(reinterpret_cast<const float4*>(&A->adHostF[h * nf + t][q * 16]) + u);
     const float2 at2 = __ldg(reinterpret_cast<const float2*>(&A->adTdiagF[h * nf + t][q * 2]));
     float idepth, idz;
-    if (it.have_x) {  // fused resubstituteFPt + point step, as in the LPR = 1 path (every lane of the point recomputes the same step)
+    if (it.have_x) {  // fused resubstituteFPt + point step: lane q of the residual takes targets 2q, 2q+1, two butterfly steps add the 4 lanes'
+      // partial sums (commutative pairs: the sum, hence the step, is bit-identical in the 4 lanes and in every pair-warp of the point; it
+      // differs in the last bits from the sequential sum of the LPR = 1 path and of resub_point)
+      static_assert(MAXF == 8, "4 lanes x 2 targets cover the MAXF frame slots");
       const float4 po0 = __ldg(reinterpret_cast<const float4*>(W.c_pout + (size_t)p * 8));
       const float4 po1 = __ldg(reinterpret_cast<const float4*>(W.c_pout + (size_t)p * 8) + 1);
       const float idb = __ldg(W.idepth_backup + p);
-      float b = po1.w - (it.xc[0] * po0.z + it.xc[1] * po0.w + it.xc[2] * po1.x + it.xc[3] * po1.y);
+      int stc[2];
+      float4 a0[2], a1[2];
+#pragma unroll
+      for (int u = 0; u < 2; u++) {
+        const int cs = min(2 * q + u, nf - 1) * mp + p;
+        stc[u] = __ldg(W.c_st + cs);
+        a0[u] = __ldg(reinterpret_cast<const float4*>(W.c_jpjd + (size_t)cs * 8));
+        a1[u] = __ldg(reinterpret_cast<const float4*>(W.c_jpjd + (size_t)cs * 8) + 1);
+      }
+      float bt = 0.f;
       int ngood = 0;
 #pragma unroll
-      for (int t4 = 0; t4 < MAXF; t4 += 4) {
-        int stc[4];
-        float4 a0[4], a1[4];
-#pragma unroll
-        for (int u = 0; u < 4; u++) {
-          const int cs = min(t4 + u, nf - 1) * mp + p;
-          stc[u] = __ldg(W.c_st + cs);
-          a0[u] = __ldg(reinterpret_cast<const float4*>(W.c_jpjd + (size_t)cs * 8));
-          a1[u] = __ldg(reinterpret_cast<const float4*>(W.c_jpjd + (size_t)cs * 8) + 1);
-        }
-#pragma unroll
-        for (int u = 0; u < 4; u++) {
-          const int tt = t4 + u;
-          const bool good = tt < nf && tt != h && stc[u] == RES_IN;
-          const float* xa = it.xAd[h * nf + min(tt, nf - 1)];
-          const float dot = xa[0] * a0[u].x + xa[1] * a0[u].y + xa[2] * a0[u].z + xa[3] * a0[u].w + xa[4] * a1[u].x + xa[5] * a1[u].y + xa[6] * a1[u].z + xa[7] * a1[u].w;
-          b -= good ? dot : 0.f;
-          ngood += good;
-        }
+      for (int u = 0; u < 2; u++) {
+        const int tt = 2 * q + u;
+        const bool good = tt < nf && tt != h && stc[u] == RES_IN;
+        const float* xa = it.xAd[h * nf + min(tt, nf - 1)];
+        const float dot = xa[0] * a0[u].x + xa[1] * a0[u].y + xa[2] * a0[u].z + xa[3] * a0[u].w + xa[4] * a1[u].x + xa[5] * a1[u].y + xa[6] * a1[u].z + xa[7] * a1[u].w;
+        bt += good ? dot : 0.f;
+        ngood += good;
       }
+      bt += __shfl_xor_sync(0xffffffffu, bt, 1);
+      bt += __shfl_xor_sync(0xffffffffu, bt, 2);
+      ngood += __shfl_xor_sync(0xffffffffu, ngood, 1);
+      ngood += __shfl_xor_sync(0xffffffffu, ngood, 2);
+      const float b = (po1.w - (it.xc[0] * po0.z + it.xc[1] * po0.w + it.xc[2] * po1.x + it.xc[3] * po1.y)) - bt;
       const float step = ngood > 0 ? -b * po1.z : 0.f;
       idepth = idb + step;
       idz = idepth;
@@ -595,6 +620,7 @@ __device__ __forceinline__ void fused_chunk(const BAWinDev& W, const BAIter& it,
       idz = __ldg(W.idepth_zero + p);
     }
     if (r == 0 && q == 0 && valid) { S.id[pl] = idepth; S.idz[pl] = idz; }
+    clk_stamp<CLK>(clk, 2, __float_as_uint(idepth) ^ __float_as_uint(uv.x) ^ (unsigned)st);
     bool live = (st != RES_NONE) && (st != RES_OOB);
 
     // ---- centre pixel at the FEJ point (every lane)
@@ -683,6 +709,7 @@ __device__ __forceinline__ void fused_chunk(const BAWinDev& W, const BAIter& it,
         sv[16] += hw * hw * (gx * gx + gy * gy);
       }
     }
+    clk_stamp<CLK>(clk, 3, __float_as_uint(sv[0]));
     {  // every sample finite, and the sums of the residual's 8 pixels in all 4 lanes (butterfly over the lane bits 0, 1)
       const unsigned bal = __ballot_sync(0xffffffffu, fin);
       live = live && (((bal >> (lane & ~3)) & 0xfu) == 0xfu);
@@ -832,6 +859,7 @@ __device__ __forceinline__ void fused_chunk(const BAWinDev& W, const BAIter& it,
   }
   cp_async_wait_all();
   __syncthreads();
+  clk_stamp<CLK>(clk, 4);
 
   // ---------------------------------------------------------------- phase B: per point (AccumulatedSCHessian.cpp:L36-58)
   for (int e = tid; e < ch_count * 9; e += nthreads) {
@@ -849,7 +877,7 @@ __device__ __forceinline__ void fused_chunk(const BAWinDev& W, const BAIter& it,
         Hdd += S.rec[tt][8][pl2]; bd += S.rec[tt][9][pl2]; c0 += S.rec[tt][10][pl2]; c1 += S.rec[tt][11][pl2];
         c2 += S.rec[tt][12][pl2]; c3 += S.rec[tt][13][pl2]; ngood += S.rec[tt][14][pl2];
       }
-      float prior = __ldg(W.priorF + p);
+      float prior = S.prior[pl2];
       bool masked = true;
       if constexpr (MARG) { masked = __ldg(W.marg_mask + p) != 0; prior *= __ldg(&W.marg->priorFac); }
       float HdiF = 0.f, bdSum = 0.f, w0 = 0.f, w1 = 0.f, w2 = 0.f, w3 = 0.f;
@@ -937,11 +965,13 @@ __device__ __forceinline__ void fused_chunk(const BAWinDev& W, const BAIter& it,
     }
   }
   __syncthreads();  // shared memory is reused by the next chunk (persistent case)
+  clk_stamp<CLK>(clk, 5);
 }
 
 // phases D / E for one window: the work is split over `ncta` CTAs, this one acting as CTA `vcta`
-template <int P, int LPR>
-__device__ __forceinline__ void fused_reduce(const BAWinDev& W, FusedSmem<P, LPR>& S, bool ok, const int vcta, const int ncta) {
+template <int P, int LPR, bool CLK = false>
+__device__ __forceinline__ void fused_reduce(const BAWinDev& W, FusedSmem<P, LPR>& S, bool ok, const int vcta, const int ncta,
+                                             unsigned long long* clk = nullptr) {
   const int nf = W.nf, N = W.N, mp = W.mp;
   const int tid = threadIdx.x, nthreads = blockDim.x;
   const int warp = tid >> 5, lane = tid & 31, nwarps = nthreads >> 5;
@@ -963,8 +993,11 @@ __device__ __forceinline__ void fused_reduce(const BAWinDev& W, FusedSmem<P, LPR
   const int nch = W.nchunks;
   // with the peer exchange on: pass 0 (sum + push) -> phase E (Gram tiles + push) -> pass 1 (pull) -> phase E pull: the NVLink round trip of
   // the H_top entries overlaps the Gram computation
+  // items are dealt from the LAST CTA down: the first CTAs carry the second Schur tile of phase E (tile vcta + ncta), so the two tails
+  // land on different CTAs
+  const int dcta = ncta - 1 - vcta;
   auto phase_d = [&](const int pass) {
-    for (int base = vcta * groups_per_cta; base < nitems; base += ncta * groups_per_cta) {  // CTA-uniform trip count (shuffles below)
+    for (int base = dcta * groups_per_cta; base < nitems; base += ncta * groups_per_cta) {  // CTA-uniform trip count (shuffles below)
       const int item = base + grp;
       const bool act = item < nitems;
       // decode: up to two (offset, chunk range) segments and up to two destinations
@@ -999,16 +1032,27 @@ __device__ __forceinline__ void fused_reduce(const BAWinDev& W, FusedSmem<P, LPR
       }
       if (pass == 0) {
         double sum = 0.0;
+        if (hi0 - lo0 <= 96 && hi1 - lo1 <= 96) {  // both segments in one round trip: <= 6 partials per lane each, summed in the same order
+          double v[12];
+#pragma unroll
+          for (int u = 0; u < 12; u++) {
+            const int c = (u < 6 ? lo0 : lo1) + gl + 16 * (u % 6);
+            v[u] = (c < (u < 6 ? hi0 : hi1)) ? __ldcg(part + (u < 6 ? off0 : off1) + (size_t)c * PART_STRIDE) : 0.0;
+          }
+#pragma unroll
+          for (int u = 0; u < 12; u++) sum += v[u];
+        } else {
 #pragma unroll 1
-        for (int seg = 0; seg < 2; seg++) {
-          const int lo = seg ? lo1 : lo0, hi = seg ? hi1 : hi0;
-          const double* __restrict__ src = part + (seg ? off1 : off0);
-          for (int c0 = lo + gl; c0 < hi; c0 += 192) {
-            double v[12];
+          for (int seg = 0; seg < 2; seg++) {
+            const int lo = seg ? lo1 : lo0, hi = seg ? hi1 : hi0;
+            const double* __restrict__ src = part + (seg ? off1 : off0);
+            for (int c0 = lo + gl; c0 < hi; c0 += 192) {
+              double v[12];
 #pragma unroll
-            for (int u = 0; u < 12; u++) v[u] = (c0 + 16 * u < hi) ? __ldcg(src + (size_t)(c0 + 16 * u) * PART_STRIDE) : 0.0;
+              for (int u = 0; u < 12; u++) v[u] = (c0 + 16 * u < hi) ? __ldcg(src + (size_t)(c0 + 16 * u) * PART_STRIDE) : 0.0;
 #pragma unroll
-            for (int u = 0; u < 12; u++) sum += v[u];
+              for (int u = 0; u < 12; u++) sum += v[u];
+            }
           }
         }
         sum += __shfl_xor_sync(0xffffffffu, sum, 8);
@@ -1029,6 +1073,7 @@ __device__ __forceinline__ void fused_reduce(const BAWinDev& W, FusedSmem<P, LPR
     }
     };
   phase_d(0);
+  clk_stamp<CLK>(clk, 7);
 
   // ---------------------------------------------------------------- phase E: [H_sc | b_sc] = sum_p HdiF w_p w_p^T as 4x4 tiles over ALL points
   // of the window: a CTA takes tiles vcta, vcta + ncta (both in ONE pass over the points when the grid has fewer CTAs than tiles)
@@ -1109,6 +1154,7 @@ __device__ __forceinline__ void fused_reduce(const BAWinDev& W, FusedSmem<P, LPR
       __syncthreads();
     }
   }
+  clk_stamp<CLK>(clk, 8);
   if (xch) {
     phase_d(1);
     if (tid < 32) {  // pull of the Gram tiles: same (tile, lane) ownership as above, so R[idx] is this lane's own earlier store
@@ -1138,16 +1184,19 @@ __device__ __forceinline__ void fused_reduce(const BAWinDev& W, FusedSmem<P, LPR
 //                     chunk_points = 32 -> (P = 32, LPR = 1): 224 threads, one thread per residual (fewest instructions: batches / large windows)
 template <int P> struct FusedCfgOf { static constexpr int LPR = (P == 16) ? 4 : 1, TPB = (P == 16) ? 448 : 224; };
 
-template <int P, bool MARG>
+// CLK = true: the phase clock (clk_stamp) into clk[gridDim.x][NCLK]; measurement only, launched by launch_fused_kernel_clocked alone
+template <int P, bool MARG, bool CLK = false>
 __global__ void __launch_bounds__(FusedCfgOf<P>::TPB, 1)
-    ba_fused_kernel(const __grid_constant__ BAWinDev W, const __grid_constant__ BAIter it) {
+    ba_fused_kernel(const __grid_constant__ BAWinDev W, const __grid_constant__ BAIter it, unsigned long long* clk) {
   constexpr int LPR = FusedCfgOf<P>::LPR;
   extern __shared__ __align__(16) unsigned char smem_raw[];
   FusedSmem<P, LPR>& S = *reinterpret_cast<FusedSmem<P, LPR>*>(smem_raw);
+  clk_stamp<CLK>(clk, 0);
 #pragma unroll 1
-  for (int chunk = blockIdx.x; chunk < W.nchunks; chunk += gridDim.x) fused_chunk<P, LPR, MARG>(W, it, S, chunk);
+  for (int chunk = blockIdx.x; chunk < W.nchunks; chunk += gridDim.x) fused_chunk<P, LPR, MARG, CLK>(W, it, S, chunk, clk);
   const bool ok = grid_barrier(W.bar, W.bar_target);  // every chunk of the window is done
-  fused_reduce<P, LPR>(W, S, ok, blockIdx.x, gridDim.x);
+  clk_stamp<CLK>(clk, 6);
+  fused_reduce<P, LPR, CLK>(W, S, ok, blockIdx.x, gridDim.x, clk);
 }
 
 // Batched variant (SURVEY.md §8d): B independent windows in ONE launch.  Descriptors and per-iteration tables come from global memory;
@@ -1177,8 +1226,8 @@ __global__ void __launch_bounds__(FusedCfgOf<P>::TPB, P == 32 ? 2 : 1)
 struct FusedCfg { bool done = false; int max_ctas = 0; };
 static std::mutex g_cfg_mutex;
 
-template <int P, bool MARG>
-static cudaError_t launch_cfg(BAWinDev& W, const BAIter& it, cudaStream_t s, unsigned* bar_count) {
+template <int P, bool MARG, bool CLK = false>
+static cudaError_t launch_cfg(BAWinDev& W, const BAIter& it, cudaStream_t s, unsigned* bar_count, unsigned long long* clk = nullptr) {
   static FusedCfg cfg[64];
   constexpr int TPB = FusedCfgOf<P>::TPB;
   int dev = 0;
@@ -1191,10 +1240,10 @@ static cudaError_t launch_cfg(BAWinDev& W, const BAIter& it, cudaStream_t s, uns
     std::lock_guard<std::mutex> lk(g_cfg_mutex);
     FusedCfg& c = cfg[dev & 63];
     if (!c.done) {
-      e = cudaFuncSetAttribute(ba_fused_kernel<P, MARG>, cudaFuncAttributeMaxDynamicSharedMemorySize, smem);
+      e = cudaFuncSetAttribute(ba_fused_kernel<P, MARG, CLK>, cudaFuncAttributeMaxDynamicSharedMemorySize, smem);
       if (e != cudaSuccess) return e;
       int per_sm = 0, sms = 0;
-      e = cudaOccupancyMaxActiveBlocksPerMultiprocessor(&per_sm, ba_fused_kernel<P, MARG>, TPB, smem);
+      e = cudaOccupancyMaxActiveBlocksPerMultiprocessor(&per_sm, ba_fused_kernel<P, MARG, CLK>, TPB, smem);
       if (e != cudaSuccess) return e;
       e = cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, dev);
       if (e != cudaSuccess) return e;
@@ -1206,8 +1255,8 @@ static cudaError_t launch_cfg(BAWinDev& W, const BAIter& it, cudaStream_t s, uns
   const int grid = min(W.nchunks, max_ctas);
   *bar_count += (unsigned)grid;   // monotonic arrival counter: every CTA of this launch adds one
   W.bar_target = *bar_count;
-  void* args[2] = {(void*)&W, (void*)&it};
-  return cudaLaunchCooperativeKernel((const void*)ba_fused_kernel<P, MARG>, dim3(grid), dim3(threads), args, (size_t)smem, s);
+  void* args[3] = {(void*)&W, (void*)&it, (void*)&clk};
+  return cudaLaunchCooperativeKernel((const void*)ba_fused_kernel<P, MARG, CLK>, dim3(grid), dim3(threads), args, (size_t)smem, s);
 }
 
 template <int P>
@@ -1252,6 +1301,14 @@ cudaError_t launch_fused_batch_kernel(int P, const BAWinDev* gW, const BAIter* g
 cudaError_t launch_fused_kernel(BAWinDev& W, const BAIter& it, bool marg, cudaStream_t s, unsigned* bar_count) {
   if (W.P == 32) return marg ? launch_cfg<32, true>(W, it, s, bar_count) : launch_cfg<32, false>(W, it, s, bar_count);
   return marg ? launch_cfg<16, true>(W, it, s, bar_count) : launch_cfg<16, false>(W, it, s, bar_count);
+}
+
+// the linearisation launch with the phase clock (measurement only): clk holds >= grid x NCLK stamps, *grid receives the CTA count
+cudaError_t launch_fused_kernel_clocked(BAWinDev& W, const BAIter& it, cudaStream_t s, unsigned* bar_count, unsigned long long* clk, int* grid) {
+  const unsigned before = *bar_count;
+  const cudaError_t e = (W.P == 32) ? launch_cfg<32, false, true>(W, it, s, bar_count, clk) : launch_cfg<16, false, true>(W, it, s, bar_count, clk);
+  *grid = (int)(*bar_count - before);
+  return e;
 }
 
 }  // namespace dmv
