@@ -68,13 +68,12 @@ __device__ __forceinline__ float top_entry(const float (&x)[10], const float (&y
   else return 0.f;
 }
 
-// (r, c) of the symmetric 13x13 block from the packed float layout; NH partial blocks (one per warp of the pair) are added
+// (r, c) of the symmetric 13x13 block from the packed float layout; NH partial blocks (one per warp of the pair) are added.  The
+// (a, b, r) entries follow row 9 exactly as rows 10..12 of a full upper-triangular packing would, so one formula indexes every entry.
+static_assert(top_off(10) == TOP_TRI && top_off(11) == TOP_TRI + 3 && top_off(12) == TOP_TRI + 5, "bottom block = rows 10..12 of the packing");
 template <int NH>
-__device__ __forceinline__ float h13f(const float (*S)[96], int r, int c) {
-  if (r > c) { const int t = r; r = c; c = t; }
-  int idx;
-  if (r < TOP_ROWS) idx = top_off(r) + c - r;
-  else { const int rr = r - 10, cc = c - 10; idx = TOP_TRI + (rr == 0 ? cc : (rr == 1 ? 2 + cc : 5)); }
+__device__ __forceinline__ float pair_entry(const float (*S)[96], int r, int c) {
+  const int a = min(r, c), idx = top_off(a) + max(r, c) - a;
   if constexpr (NH == 2) return S[0][idx] + S[1][idx];
   else return S[0][idx];
 }
@@ -100,7 +99,7 @@ struct FusedSmem {
   static constexpr int NH = (LPR == 4) ? 2 : 1;   // warps per (host, target) pair: each leaves its own partial pair block
   double AhD[MAXF][64];        // adHost(h, t) fp64, row-major, slot = target frame
   double dT[MAXF][8];          // diag adTarget(h, t)
-  double G[MAXF][104];         // adHost * [P | Q | p]
+  double G[MAXF][8][16];       // adHost * [P | Q | p]: row i = columns 0..7 P, 8..11 Q, 12 p (16-byte aligned rows)
   float adH[MAXF][64];         // fp32 copies used for the Schur vector (the reference's adHostF / adTargetF); LPR = 1 only
   float adT[MAXF][8];
   float pair[MAXF][NH][96];    // the chunk's pair blocks (91 used), slot = target frame
@@ -861,107 +860,152 @@ __device__ __forceinline__ void fused_chunk(const BAWinDev& W, const BAIter& it,
   __syncthreads();
   clk_stamp<CLK>(clk, 4);
 
-  // ---------------------------------------------------------------- phase B: per point (AccumulatedSCHessian.cpp:L36-58)
-  for (int e = tid; e < ch_count * 9; e += nthreads) {
-    const int k = e / ch_count, pl2 = e - k * ch_count;  // lanes = points: conflict-free reads of rec[t][k][.]
-    if (k < 8) {  // host block of the Schur vector
-      float sum = 0.f;
-      for (int tt = 0; tt < nf; tt++)
-        if (tt != h) sum += S.rec[tt][k][pl2];
-      S.Wv[pl2][4 + 8 * h + k] = sum;
-    } else {
-      const int p = ch_start + pl2;
-      float Hdd = 0.f, bd = 0.f, c0 = 0.f, c1 = 0.f, c2 = 0.f, c3 = 0.f, ngood = 0.f;
-      for (int tt = 0; tt < nf; tt++) {
-        if (tt == h) continue;
-        Hdd += S.rec[tt][8][pl2]; bd += S.rec[tt][9][pl2]; c0 += S.rec[tt][10][pl2]; c1 += S.rec[tt][11][pl2];
-        c2 += S.rec[tt][12][pl2]; c3 += S.rec[tt][13][pl2]; ngood += S.rec[tt][14][pl2];
-      }
-      float prior = S.prior[pl2];
-      bool masked = true;
-      if constexpr (MARG) { masked = __ldg(W.marg_mask + p) != 0; prior *= __ldg(&W.marg->priorFac); }
-      float HdiF = 0.f, bdSum = 0.f, w0 = 0.f, w1 = 0.f, w2 = 0.f, w3 = 0.f;
-      if (ngood > 0.f) {
-        float H = Hdd + prior;
-        if (H < 1e-10f) H = 1e-10f;
-        HdiF = 1.0f / H;
-        bdSum = MARG ? bd : bd + prior * (S.id[pl2] - S.idz[pl2]);  // shiftPriorToZero (AccumulatedSCHessian.cpp:L47-50)
-        w0 = c0; w1 = c1; w2 = c2; w3 = c3;
-      }
-      S.Wv[pl2][0] = w0; S.Wv[pl2][1] = w1; S.Wv[pl2][2] = w2; S.Wv[pl2][3] = w3;
-      S.Wv[pl2][N] = bdSum;
-      for (int c = N + 1; c < W.NW; c++) S.Wv[pl2][c] = 0.f;  // padding columns of the last 4x4 tiles
-      S.hdi[pl2] = HdiF;
-      if (masked) {
-        float4* po = reinterpret_cast<float4*>(W.pout + (size_t)p * 8);
-        po[0] = make_float4(Hdd, bd, c0, c1);
-        po[1] = make_float4(c2, c3, HdiF, bdSum);
+  // ---------------------------------------------------------------- phases B and C: two block-wide passes over regular items, long items
+  // first (at P = 16 and up to 7 frames every item of a pass has its own thread).  Every entry keeps the summation order of the formulas quoted below, so the
+  // partial blob, the Schur vectors and pout are the same bit for bit however the items are dealt.  Loops over the targets are rolled
+  // where unrolling would only add code: this code runs once per chunk and is fetched cold.
+  const int nt = nf - 1;  // target slot r <-> frame r + (r >= h)
+  double* __restrict__ out = W.part + (size_t)chunk * PART_STRIDE;
+  {  // pass 1: G and the target blocks, phase B, H[C,C] / b[C] and the counters: everything that reads only phase A's results
+    const int nG = nt * 26;
+#pragma unroll 1
+    for (int e = tid; e < nG + 9 * P + 28; e += nthreads) {
+      if (e < nG) {
+        // target t, column c of [P | Q | p](h,t), rows i0..i0+3: [P|Q|p][k][c] = H13[4+k][col], col = 4..11 (P), 0..3 (Q), 12 (p).
+        // G(t)[i][c] = sum_k adHost[i][k] [P|Q|p][k][c] (k ascending), and the target's own blocks, which need no adHost:
+        // H[t,t] = At P At^T, H[t,C] = At Q, b[t] = At p (AccumulatedTopHessian.cpp:L270-286)
+        const int rh = e / 13, c = e - rh * 13, i0 = (rh & 1) * 4;
+        const int t = (rh >> 1) + ((rh >> 1) >= h ? 1 : 0);
+        const int col = (c < 8) ? 4 + c : (c < 12 ? c - 8 : 12);
+        double m[8];
+#pragma unroll
+        for (int k = 0; k < 8; k++) m[k] = (double)pair_entry<NH>(S.pair[t], 4 + k, col);
+        const double dTc = S.dT[t][c & 7];
+        // partial-blob slot of target row i in column c: [D 64 | C 32 | b 8] -> first row i0, stride per row
+        const int os = (c < 8) ? 8 : (c < 12 ? 4 : 1);
+        double* o = out + t * PART_SLOT + ((c < 8) ? 64 + c : (c < 12 ? 120 + c : 160)) + i0 * os;
+#pragma unroll
+        for (int ii = 0; ii < 4; ii++) {
+          const int i = i0 + ii;
+          double g = 0.0;
+#pragma unroll
+          for (int k = 0; k < 8; k++) g += S.AhD[t][i * 8 + k] * m[k];
+          S.G[t][i][c] = g;
+          double v = S.dT[t][i] * (i0 ? m[4 + ii] : m[ii]);
+          if (c < 8) v = v * dTc;
+          o[ii * os] = v;
+        }
+      } else if (e < nG + 9 * P) {  // phase B: per point (AccumulatedSCHessian.cpp:L36-58); lanes = points: conflict-free reads of rec[t][k][.]
+        const int k = (e - nG) / P, pl2 = (e - nG) & (P - 1);
+        if (pl2 >= ch_count) continue;
+        if (k < 8) {  // host block of the Schur vector: sum over the targets, ascending
+          float sum = 0.f;
+#pragma unroll
+          for (int tt = 0; tt < MAXF; tt++) {
+            const float v = S.rec[tt][k][pl2];
+            if (tt < nf && tt != h) sum += v;
+          }
+          S.Wv[pl2][4 + 8 * h + k] = sum;
+        } else {
+          const int p = ch_start + pl2;
+          float Hdd = 0.f, bd = 0.f, c0 = 0.f, c1 = 0.f, c2 = 0.f, c3 = 0.f, ngood = 0.f;
+#pragma unroll 1
+          for (int r = 0; r < nt; r++) {
+            const int tt = r + (r >= h ? 1 : 0);
+            Hdd += S.rec[tt][8][pl2]; bd += S.rec[tt][9][pl2]; c0 += S.rec[tt][10][pl2]; c1 += S.rec[tt][11][pl2];
+            c2 += S.rec[tt][12][pl2]; c3 += S.rec[tt][13][pl2]; ngood += S.rec[tt][14][pl2];
+          }
+          float prior = S.prior[pl2];
+          bool masked = true;
+          if constexpr (MARG) { masked = __ldg(W.marg_mask + p) != 0; prior *= __ldg(&W.marg->priorFac); }
+          float HdiF = 0.f, bdSum = 0.f, w0 = 0.f, w1 = 0.f, w2 = 0.f, w3 = 0.f;
+          if (ngood > 0.f) {
+            float H = Hdd + prior;
+            if (H < 1e-10f) H = 1e-10f;
+            HdiF = 1.0f / H;
+            bdSum = MARG ? bd : bd + prior * (S.id[pl2] - S.idz[pl2]);  // shiftPriorToZero (AccumulatedSCHessian.cpp:L47-50)
+            w0 = c0; w1 = c1; w2 = c2; w3 = c3;
+          }
+          S.Wv[pl2][0] = w0; S.Wv[pl2][1] = w1; S.Wv[pl2][2] = w2; S.Wv[pl2][3] = w3;
+          S.Wv[pl2][N] = bdSum;
+#pragma unroll 1
+          for (int c = N + 1; c < W.NW; c++) S.Wv[pl2][c] = 0.f;  // padding columns of the last 4x4 tiles
+          S.hdi[pl2] = HdiF;
+          if (masked) {
+            float4* po = reinterpret_cast<float4*>(W.pout + (size_t)p * 8);
+            po[0] = make_float4(Hdd, bd, c0, c1);
+            po[1] = make_float4(c2, c3, HdiF, bdSum);
+          }
+        }
+      } else if (e < nG + 9 * P + 20) {  // H[C,C] (4x4) and b[C] = sum_t Q-block / p of the pair blocks, t ascending
+        const int i = (e - nG - 9 * P) / 5, j = (e - nG - 9 * P) - i * 5;
+        double val = 0.0;
+#pragma unroll 1
+        for (int r = 0; r < nt; r++) val += (double)pair_entry<NH>(S.pair[r + (r >= h ? 1 : 0)], i, j < 4 ? j : 12);
+        out[PART_CC + (j < 4 ? i * 4 + j : 16 + i)] = val;
+      } else {  // the counters: warp sums in warp order, 4 loads in flight
+        const int k = e - nG - 9 * P - 20;
+        double val = 0.0;
+#pragma unroll 1
+        for (int wv = 0; wv < nwarps; wv += 4) {
+          float v[4];
+#pragma unroll
+          for (int u = 0; u < 4; u++) v[u] = S.misc[min(wv + u, 15)][k];
+#pragma unroll
+          for (int u = 0; u < 4; u++)
+            if (wv + u < nwarps) val += (double)v[u];
+        }
+        out[PART_MISC + k] = val;
       }
     }
-  }
-  // ---- phase C, first half: G(t) = adHost(h,t) * [P | Q | p](h,t) in fp64, [P|Q|p][k][c] = H13[4+k][col(c)], col = 4..11, 0..3, 12
-  for (int e = tid; e < nf * 104; e += nthreads) {
-    const int tt = e / 104, rr = e - tt * 104, i = rr / 13, c = rr - i * 13;
-    if (tt == h) continue;
-    const int colc = (c < 8) ? 4 + c : (c < 12 ? c - 8 : 12);
-    double m = 0.0;
-#pragma unroll
-    for (int k = 0; k < 8; k++) m += S.AhD[tt][i * 8 + k] * (double)h13f<NH>(S.pair[tt], 4 + k, colc);
-    S.G[tt][rr] = m;
   }
   __syncthreads();
-
-  // ---- Schur vectors -> global, transposed ([4-column group][point] float4) so that phase E reads them coalesced
-  {
-    const int T = W.T;
-    for (int e = tid; e < ch_count * T; e += nthreads) {
-      const int g4 = e / ch_count, pl2 = e - g4 * ch_count;
-      W.wg[(size_t)g4 * mp + ch_start + pl2] = *reinterpret_cast<const float4*>(&S.Wv[pl2][4 * g4]);
-    }
-    if (tid < ch_count) W.hdig[ch_start + tid] = S.hdi[tid];
-  }
-  // ---- phase C, second half: the chunk's contributions in absolute coordinates -> partial blob (AccumulatedTopHessian.cpp:L270-286)
-  {
-    double* __restrict__ out = W.part + (size_t)chunk * PART_STRIDE;
-    for (int e = tid; e < nf * PART_SLOT; e += nthreads) {
-      const int tt = e / PART_SLOT, q = e - tt * PART_SLOT;
-      double val;
-      if (tt != h) {
-        const float (*B)[96] = S.pair[tt];
-        if (q < 64) { const int i = q >> 3, j = q & 7; val = S.G[tt][i * 13 + j] * S.dT[tt][j]; }                               // H[h,t] = (Ah P) At^T
-        else if (q < 128) { const int i = (q - 64) >> 3, j = q & 7; val = S.dT[tt][i] * (double)h13f<NH>(B, 4 + i, 4 + j) * S.dT[tt][j]; }  // H[t,t] = At P At^T
-        else if (q < 160) { const int i = (q - 128) >> 2, c = q & 3; val = S.dT[tt][i] * (double)h13f<NH>(B, 4 + i, c); }           // H[t,C] = At Q
-        else { const int i = q - 160; val = S.dT[tt][i] * (double)h13f<NH>(B, 4 + i, 12); }                                          // b[t] = At p
-      } else {
-        if (q < 64) continue;  // H[h,h] goes to the diagonal slot below
-        val = 0.0;
-        if (q < 128) {  // H[h,h] = sum_t (Ah P) Ah^T
-          const int i = (q - 64) >> 3, j = q & 7;
-          for (int t2 = 0; t2 < nf; t2++) {
-            if (t2 == h) continue;
+  {  // pass 2: what needs G, and the Schur vectors -> global.  The 64 H[h,h] items (48-term chains) come first.
+    const int nO = nt * 16;
+#pragma unroll 1
+    for (int e = tid; e < 64 + nO + 8 + P * W.T; e += nthreads) {
+      if (e < 64) {  // H[h,h] = sum_t (Ah P) Ah^T: t ascending, then k; the next target's operands load under the current 8-term chain
+        const int i = e >> 3, j = e & 7;
+        double val = 0.0;
+        double2 g[4], a[4];
+        const int t0 = (h == 0) ? 1 : 0;
 #pragma unroll
-            for (int k = 0; k < 8; k++) val += S.G[t2][i * 13 + k] * S.AhD[t2][j * 8 + k];
-          }
-        } else if (q < 160) {  // H[h,C] = sum_t Ah Q
-          const int i = (q - 128) >> 2, c = q & 3;
-          for (int t2 = 0; t2 < nf; t2++) if (t2 != h) val += S.G[t2][i * 13 + 8 + c];
-        } else {  // b[h] = sum_t Ah p
-          const int i = q - 160;
-          for (int t2 = 0; t2 < nf; t2++) if (t2 != h) val += S.G[t2][i * 13 + 12];
+        for (int u = 0; u < 4; u++) { g[u] = reinterpret_cast<const double2*>(&S.G[t0][i][0])[u]; a[u] = reinterpret_cast<const double2*>(&S.AhD[t0][j * 8])[u]; }
+#pragma unroll 1
+        for (int r = 0; r < nt; r++) {
+          const int tn = min(r + 1 + (r + 1 >= h ? 1 : 0), MAXF - 1);  // next target (in bounds on the last trip; not used there)
+          double2 gn[4], an[4];
+#pragma unroll
+          for (int u = 0; u < 4; u++) { gn[u] = reinterpret_cast<const double2*>(&S.G[tn][i][0])[u]; an[u] = reinterpret_cast<const double2*>(&S.AhD[tn][j * 8])[u]; }
+#pragma unroll
+          for (int u = 0; u < 4; u++) { val += g[u].x * a[u].x; val += g[u].y * a[u].y; }
+#pragma unroll
+          for (int u = 0; u < 4; u++) { g[u] = gn[u]; a[u] = an[u]; }
         }
+        out[h * PART_SLOT + 64 + e] = val;
+      } else if (e < 64 + nO) {  // H[h,t] = (Ah P) At^T: 4 entries of row i
+        const int eo = e - 64, r = eo >> 4, i = (eo >> 1) & 7, j0 = (eo & 1) * 4;
+        const int t = r + (r >= h ? 1 : 0);
+#pragma unroll
+        for (int v = 0; v < 4; v++) out[t * PART_SLOT + i * 8 + j0 + v] = S.G[t][i][j0 + v] * S.dT[t][j0 + v];
+      } else if (e < 64 + nO + 8) {  // row i of H[h,C] = sum_t Ah Q and b[h] = sum_t Ah p, t ascending
+        const int i = e - 64 - nO;
+        double c0 = 0.0, c1 = 0.0, c2 = 0.0, c3 = 0.0, bh = 0.0;
+#pragma unroll 1
+        for (int r = 0; r < nt; r++) {
+          const int t2 = r + (r >= h ? 1 : 0);
+          const double2 q01 = *reinterpret_cast<const double2*>(&S.G[t2][i][8]), q23 = *reinterpret_cast<const double2*>(&S.G[t2][i][10]);
+          c0 += q01.x; c1 += q01.y; c2 += q23.x; c3 += q23.y; bh += S.G[t2][i][12];
+        }
+        double* o = out + h * PART_SLOT;
+        o[128 + i * 4] = c0; o[128 + i * 4 + 1] = c1; o[128 + i * 4 + 2] = c2; o[128 + i * 4 + 3] = c3;
+        o[160 + i] = bh;
+      } else {  // Schur vectors -> global, transposed ([4-column group][point] float4) so that phase E reads them coalesced
+        const int ew = e - 64 - nO - 8, g4 = ew / P, pl2 = ew & (P - 1);
+        if (pl2 >= ch_count) continue;
+        W.wg[(size_t)g4 * mp + ch_start + pl2] = *reinterpret_cast<const float4*>(&S.Wv[pl2][4 * g4]);
+        if (g4 == 0) W.hdig[ch_start + pl2] = S.hdi[pl2];
       }
-      out[e] = val;
-    }
-    if (tid < 20) {  // H[C,C] (4x4) and b[C]
-      const int i = tid / 5, j = tid - i * 5;
-      double val = 0.0;
-      for (int t2 = 0; t2 < nf; t2++) if (t2 != h) val += (double)h13f<NH>(S.pair[t2], i, j < 4 ? j : 12);
-      out[PART_CC + (j < 4 ? i * 4 + j : 16 + i)] = val;
-    } else if (tid >= 32 && tid < 40) {
-      const int k = tid - 32;
-      double val = 0.0;
-      for (int wv = 0; wv < nwarps; wv++) val += (double)S.misc[wv][k];
-      out[PART_MISC + k] = val;
     }
   }
   __syncthreads();  // shared memory is reused by the next chunk (persistent case)

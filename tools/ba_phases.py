@@ -6,6 +6,8 @@ Builds bench.py's headline window (7 KF / 2000 points / 640x480, seed 1234) with
 thread 0 of every CTA record %globaltimer at 9 points.  Prints, per segment, the mean over launches of the mean and of the max over the
 CTAs, next to the CUDA-event time of the same launches.  The per-chunk stamps are exact when every CTA runs one chunk, as in the
 headline window (129 chunks of 16 points).  The clock itself is a few global stores per CTA; the product kernels have none.
+--no-flush skips the L2 scrub, so code and data stay warm in L2 between launches: the difference to the scrubbed run is what cold
+fetches cost each phase.
 """
 import argparse
 import json
@@ -29,13 +31,15 @@ def main():
     ap.add_argument("--warmup", type=int, default=20)
     ap.add_argument("--chunk", type=int, default=0, help="points per thread block (16/32, 0 = library default)")
     ap.add_argument("--json", default=None, help="also write the table as JSON to this file")
+    ap.add_argument("--no-flush", action="store_true", help="no L2 scrub between launches (warm L2)")
     args = ap.parse_args()
     C = bench.Case(bench.Dist(1, 0), 0, 1, 0, bench.NPTS, args.chunk, "none")
     for _ in range(max(3, args.warmup)):
         C.ba.gn_step(C.x, C.k8, C.precalc, C.TH)
         C.ba.apply_res()
-    C.ba.bench_phases(C.x, iters=max(3, args.warmup))
-    st, ms = C.ba.bench_phases(C.x, iters=args.iters)
+    flush = not args.no_flush
+    C.ba.bench_phases(C.x, iters=max(3, args.warmup), flush_l2=flush)
+    st, ms = C.ba.bench_phases(C.x, iters=args.iters, flush_l2=flush)
     C.close()
     t = np.where(st == 0, np.nan, st.astype(np.float64))          # [launch, cta, stamp] ns; 0 = not reached
     t0 = np.nanmin(t[:, :, 0], axis=1)[:, None]                  # first CTA entry of each launch
@@ -44,10 +48,10 @@ def main():
     seg["entry -> end E"] = t[:, :, 8] - t[:, :, 0]
     rows = {k: {"mean_us": float(np.nanmean(np.nanmean(v, axis=1)) / 1e3), "max_us": float(np.nanmean(np.nanmax(v, axis=1)) / 1e3)} for k, v in seg.items()}
     first_to_last = np.nanmax(t[:, :, 8], axis=1) - t0[:, 0]
-    out = {"ctas": int(st.shape[1]), "launches": int(st.shape[0]), "segments": rows,
+    out = {"ctas": int(st.shape[1]), "launches": int(st.shape[0]), "l2_scrubbed": flush, "segments": rows,
            "first_entry_to_last_end_us": float(np.mean(first_to_last) / 1e3),
            "event_us": {"mean": float(np.mean(ms) * 1e3), "median": float(np.median(ms) * 1e3)}}
-    print(f"ba_fused_kernel phase clock: {out['launches']} launches x {out['ctas']} CTAs (headline window, L2 scrubbed, resubstituting)")
+    print(f"ba_fused_kernel phase clock: {out['launches']} launches x {out['ctas']} CTAs (headline window, {'L2 scrubbed' if flush else 'warm L2'}, resubstituting)")
     print(f"{'segment':38s} {'mean/CTA us':>12s} {'max/CTA us':>12s}")
     for k, v in rows.items():
         print(f"{k:38s} {v['mean_us']:12.2f} {v['max_us']:12.2f}")
