@@ -12,7 +12,7 @@ Tolerances, and why (fp32 on both sides, different operation order / FMA contrac
 import numpy as np
 import pytest
 
-from helpers import product_ba_from_oracle, rel
+from helpers import check_linearize_parity, check_phase_b, make_case, points_with_in_residual, prior_f, product_ba_from_oracle, rel
 
 pytestmark = pytest.mark.gpu
 
@@ -32,7 +32,14 @@ CONFIGS = [
     dict(nf=8, npts=777, seed=99, hosts="all"),        # max window size, newest frame hosts points too
     dict(nf=7, npts=8000, seed=1234),                  # BASELINE config 4 (all 8000 points on one GPU)
     dict(nf=7, npts=2000, seed=1234, w=512, h=512),    # BASELINE config 5's image shape (TUM-VI 512x512)
+    # helpers.edge_window: depth priors with idepth_zero != idepth, missing / OOB / OUTLIER residuals, points without residuals
+    dict(nf=7, npts=2000, seed=1234, edge=True),
+    dict(nf=7, npts=8000, seed=1234, edge=True),       # several chunks per CTA at P = 16
 ]
+
+
+def cfg_id(c):
+    return f"nf{c['nf']}_n{c['npts']}" + ("_edge" if c.get("edge") else "")
 
 
 def _states_equal_up_to_threshold(o_new, g_new, o_e, th_tol=1e-4):
@@ -40,60 +47,17 @@ def _states_equal_up_to_threshold(o_new, g_new, o_e, th_tol=1e-4):
     return bad
 
 
-@pytest.mark.parametrize("cfg", CONFIGS, ids=lambda c: f"nf{c['nf']}_n{c['npts']}")
+@pytest.mark.parametrize("cfg", CONFIGS, ids=cfg_id)
 @pytest.mark.parametrize("P", [16, 32])
 def test_linearize_accumulate_parity(capi, orc, synth, cfg, P):
-    W = synth.make_window(**cfg)
+    W = make_case(synth, cfg)
     ow = orc.Window(W)
     ba = product_ba_from_oracle(capi, W, ow, chunk_points=P)
     E_o = ow.linearize_all(update_th=False)
     r = ba.linearize()
-    o = ow.res_outputs(False)
-    g = ba.residual_outputs()
-    # ---- states: identical except threshold ties
-    mism = np.nonzero(o["newState"] != g["newState"])[0]
-    for i in mism:
-        eo, TH = o["newEnergyWithOutlier"][i], 512.0
-        assert abs(eo - TH) < 2e-3 * TH or o["newState"][i] == 1 or g["newState"][i] == 1, (i, o["newState"][i], g["newState"][i], eo)
-    assert len(mism) <= max(2, ow.nres // 500)
-    assert r["n_in"] == int((g["newState"] == 0).sum())
-    assert r["n_oob"] == int((g["newState"] == 1).sum())
-    # ---- threshold ties: impose the GPU's classification on the oracle (its Jacobians exist on both sides of the threshold), so that every
-    # comparison below runs UNCONDITIONALLY on the same residual set
-    E_o, nchanged, unfixable = ow.override_new_states(g["newState"])
-    assert unfixable == 0, "an OOB-boundary tie cannot be imposed on the oracle: pick another seed for this config"
-    assert nchanged == len(mism)
-    o = ow.res_outputs(False)
-    assert np.array_equal(o["newState"], g["newState"])
-    # ---- energies
-    ev = o["newState"] != 1
-    np.testing.assert_allclose(g["newEnergy"][ev], o["newEnergy"][ev], rtol=2e-3, atol=0.05)
-    np.testing.assert_allclose(g["newEnergyWithOutlier"][ev], o["newEnergyWithOutlier"][ev], rtol=2e-3, atol=0.05)
-    relerr = np.abs(g["newEnergyWithOutlier"][ev] - o["newEnergyWithOutlier"][ev]) / (np.abs(o["newEnergyWithOutlier"][ev]) + 1.0)
-    assert np.median(relerr) < 2e-4
-    assert abs(r["energy"] - E_o) <= 2e-5 * abs(E_o)
-    np.testing.assert_allclose(g["centerProjectedTo"][ev], o["centerProjectedTo"][ev], rtol=1e-5, atol=2e-4)
-    # ---- commit, then per-residual JpJdF and per-point accumulations
-    ow.apply_res()
-    ba.apply_res()
-    o2 = ow.res_outputs(False)
-    act = o2["isActive"] == 1
-    scale = np.abs(o2["JpJdF"][act]).max()
-    assert np.abs(g["JpJdF"][act] - o2["JpJdF"][act]).max() <= 2e-3 * scale
-    assert np.median(np.abs(g["JpJdF"][act] - o2["JpJdF"][act])) <= 2e-5 * scale
-    a_o = ow.accumulate(1)
-    a_g = ba.accumulate()
-    po, pg = ow.point_outputs(), ba.point_outputs()
-    assert a_g["resInA"] == a_o["resInA"]
-    for k in ("Hdd", "bd", "HdiF", "bdSumF"):
-        np.testing.assert_allclose(pg[k], po[k], rtol=2e-3, atol=2e-4 * np.abs(po[k]).max())
-    assert rel(a_g["HA"], a_o["HA"]) < 1e-5
-    assert rel(a_g["bA"], a_o["bA"]) < 1e-4
-    assert rel(a_g["Hsc"], a_o["Hsc"]) < 1e-5
-    assert rel(a_g["bsc"], a_o["bsc"]) < 1e-4
-    # invariants that hold regardless of ties
-    assert np.abs(a_g["HA"] - a_g["HA"].T).max() <= 1e-9 * np.abs(a_g["HA"]).max()
-    assert np.abs(a_g["Hsc"] - a_g["Hsc"].T).max() <= 1e-9 * np.abs(a_g["Hsc"]).max()
+    g, pg, _ = check_linearize_parity(ow, ba, r, E_o)
+    # ---- phase B in closed form from the launch's own sums (depth prior and its shift to zero included)
+    check_phase_b(pg, points_with_in_residual(W["res_point"], g["newState"], len(W["host"])), prior_f(W), W["idepth"], W["idepth_zero"])
     ba.close()
 
 
@@ -127,6 +91,9 @@ def test_oob_and_prior_states(capi, orc, synth):
     n = len(W["res_point"])
     W["res_state"] = rng.choice([0, 1, 2], n, p=[0.7, 0.2, 0.1]).astype(np.int32)
     W["res_energy"] = rng.uniform(0, 50, n).astype(np.float32)
+    npts = len(W["host"])
+    W["hasDepthPrior"] = (rng.random(npts) < 0.3).astype(np.uint8)
+    W["idepth_zero"] = (W["idepth"] * (1 + 0.02 * rng.standard_normal(npts))).astype(np.float32)
     ow = orc.Window(W)
     ba = product_ba_from_oracle(capi, W, ow)
     E_o = ow.linearize_all(update_th=False)
@@ -138,6 +105,13 @@ def test_oob_and_prior_states(capi, orc, synth):
     E_o, _, unfixable = ow.override_new_states(g["newState"])
     assert unfixable == 0
     assert abs(r["energy"] - E_o) <= 2e-5 * abs(E_o)
+    # the priors enter H = Hdd + priorF and bdSumF = bd + priorF * (idepth - idepth_zero)
+    ow.apply_res(); ba.apply_res()
+    ow.accumulate(1); ba.accumulate()
+    po, pg = ow.point_outputs(), ba.point_outputs()
+    for k in ("HdiF", "bdSumF"):
+        np.testing.assert_allclose(pg[k], po[k], rtol=2e-3, atol=2e-4 * np.abs(po[k]).max())
+    check_phase_b(pg, points_with_in_residual(W["res_point"], g["newState"], npts), prior_f(W), W["idepth"], W["idepth_zero"])
     ba.close()
 
 
@@ -159,20 +133,40 @@ def test_full_gn_iteration_matches_oracle(capi, orc, synth):
     s = 1.0 / np.sqrt(np.diag(Hg) + 10)
     x_g = s * np.linalg.solve(s[:, None] * Hg * s[None, :], s * bg)
     assert rel(x_g, x_o) < 1e-3
+    # the fused step with the GPU-side solution against the oracle's resubstitution of the same x (step = -HdiF * (difference of O(1) sums))
     ba.backup_points()
+    ba.gn_step(x_g, ow.calib()["k8"], ow.precalc(), ow.frame_tables()["frameEnergyTH"])
+    ow.resubstitute(x_g)
+    step_o = ow.point_outputs()["step"]
+    idd, idz = ba.get_idepth()
+    step_g = idd.astype(np.float64) - W["idepth"]
+    np.testing.assert_allclose(step_g, step_o, rtol=2e-3, atol=2e-4 * np.abs(step_o).max() + np.spacing(np.abs(idd)).max())
+    np.testing.assert_array_equal(idd, idz)
     ba.close()
 
 
 def test_batched_windows_identical_to_single_launches(capi, orc, synth):
     """SURVEY §8d batched variant: B windows of different shapes in ONE launch (dmv_ba_batch_gn_step) give, per window, bit-identical
-    results to the window's own launch — first linearisation and a fused GN step (resubstitute + point step inside the launch)."""
+    results to the window's own launch — first linearisation and a fused GN step (resubstitute + point step inside the launch).
+    16-point chunks (the shape the automatic rule picks for these windows); the third window carries depth priors and missing / OOB /
+    OUTLIER residuals."""
+    _batched_vs_single_launches(capi, orc, synth, P=16)
+
+
+def test_batched_windows_identical_to_single_launches_chunk32(capi, orc, synth):
+    """the same with 32-point chunks: the P = 32 batch kernel, the shape ba_fused.cu names for batches"""
+    _batched_vs_single_launches(capi, orc, synth, P=32)
+
+
+def _batched_vs_single_launches(capi, orc, synth, P):
     import dmvio_b200.hostmath as hm
-    cfgs = [dict(nf=7, npts=2000, seed=1234), dict(nf=4, npts=333, seed=5), dict(nf=8, npts=777, seed=99, hosts="all"), dict(nf=2, npts=200, seed=3, hosts="first")]
-    Ws = [synth.make_window(**c) for c in cfgs]
+    cfgs = [dict(nf=7, npts=2000, seed=1234), dict(nf=4, npts=333, seed=5), dict(nf=8, npts=777, seed=99, hosts="all", edge=True),
+            dict(nf=2, npts=200, seed=3, hosts="first")]
+    Ws = [make_case(synth, c) for c in cfgs]
 
     def load(W):
         ow = orc.Window(W)
-        ba = product_ba_from_oracle(capi, W, ow)
+        ba = product_ba_from_oracle(capi, W, ow, chunk_points=P)
         return ba, (ow.calib()["k8"], ow.precalc(), ow.frame_tables()["frameEnergyTH"])
 
     singles, batched = [load(W) for W in Ws], [load(W) for W in Ws]
@@ -191,9 +185,12 @@ def test_batched_windows_identical_to_single_launches(capi, orc, synth):
         assert rb[i]["energy"] == ref[i][0]["energy"] and rb[i]["n_in"] == ref[i][0]["n_in"]
         for k in keys:
             np.testing.assert_array_equal(a[k], ref[i][1][k])
-        for k in ("newState", "newEnergy", "JpJdF"):
+        for k in ("newState", "newEnergy"):
             np.testing.assert_array_equal(g[k], ref[i][2][k])
+        inn = g["newState"] == 0   # JpJdF is defined for IN residuals only (include/dmvio_b200.h)
+        np.testing.assert_array_equal(g["JpJdF"][inn], ref[i][2]["JpJdF"][inn])
         np.testing.assert_array_equal(p["HdiF"], ref[i][3]["HdiF"])
+        np.testing.assert_array_equal(p["bdSumF"], ref[i][3]["bdSumF"])
         HL, bL = hm.prior_system(Ws[i])
         xs.append(hm.solve_reduced(a["HA"], a["bA"], a["Hsc"], a["bsc"], HL, bL, lam=1e-5))
     # ---- a fused GN step

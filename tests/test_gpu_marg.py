@@ -38,11 +38,7 @@ def _case(synth, orc, cfg, frac):
 def test_marginalize_points_parity(capi, orc, synth, cfg, frac, P):
     W, pts = _case(synth, orc, cfg, frac)
     ow = orc.Window(W)
-    ba = product_ba_from_oracle(capi, W, ow, chunk_points=P)
-    ba.set_points(W["host"], W["u"], W["v"], W["idepth"], W["idepth_zero"], W["color"], W["weights"],
-                  priorF=np.where(W["hasDepthPrior"] != 0, 50.0 * 50.0, 0.0).astype(np.float32))
-    ba.set_residuals(W["res_point"], W["res_target"], W["res_state"], W["res_energy"])
-    ba.set_state(ow.calib()["k8"], ow.precalc(), ow.frame_tables()["frameEnergyTH"])
+    ba = product_ba_from_oracle(capi, W, ow, chunk_points=P)   # carries the points' priorF (hasDepthPrior)
     # a committed linearisation exists in real use (the window has just been optimised): the marginalisation must not disturb it
     ba.linearize(); ba.apply_res()
     before = ba.accumulate()
