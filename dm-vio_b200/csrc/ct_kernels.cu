@@ -198,6 +198,7 @@ struct CTTrack {
   float ref_exposure, new_exposure;
   float huber, cutoffTH, affModeA, affModeB;
   double minRes[5];
+  int staged[CT_L];              // ct_track_cluster_kernel: level l's plane is TMA-staged (ct_make_tensor_maps encoded its map)
   double* partial;               // [2][G][CT_NRED]
   unsigned int* bar;             // monotonic arrival counter, zero at launch
   double* out;                   // pinned host: R[9] t[3] a b lastResiduals[5] flow[3] good iterations evaluations status
@@ -685,8 +686,9 @@ __global__ void __launch_bounds__(CTC_THREADS, 1) ct_track_cluster_kernel(const 
   ctc_cluster_sync();  // every CTA's mbarrier exists before the first multicast copy can signal it
   while (!S.done) {
     const int l = S.lvl;
-    // ---- level change: stage the plane with TMA if it fits (one multicast copy issued by CTA 0 lands in every CTA's shared memory)
-    const bool fits = (size_t)T.w[l] * T.h[l] * sizeof(float4) <= (size_t)CTC_PLANE_BYTES;
+    // ---- level change: stage the plane with TMA if the host encoded its map (one multicast copy issued by CTA 0 lands in every CTA's
+    // shared memory); the host decides, so the kernel never issues a copy on a zeroed descriptor
+    const bool fits = T.staged[l] != 0;
     if (fits && staged_lvl != l) {
       const unsigned bytes = (unsigned)(T.w[l] * T.h[l] * sizeof(float4));
       if (tid == 0) asm volatile("mbarrier.arrive.expect_tx.shared::cta.b64 _, [%0], %1;" ::"r"(ctc_smem_u32(&M.mbar)), "r"(bytes) : "memory");
@@ -786,9 +788,10 @@ __global__ void __launch_bounds__(CTC_THREADS, 1) ct_track_cluster_kernel(const 
   ctc_cluster_sync();  // nobody leaves while a peer may still write into its shared memory
   if (rank == 0 && tid == 0) {
     double* o = T.out;
-    for (int i = 0; i < 9; i++) o[i] = S.R[i];
-    for (int i = 0; i < 3; i++) o[9 + i] = S.t[i];
-    o[12] = S.a; o[13] = S.b;
+    const bool ok = (S.status == 0);   // an aborted track returns the input pose, like ct_track_kernel and the reference's early return
+    for (int i = 0; i < 9; i++) o[i] = ok ? S.R[i] : T.R0[i];
+    for (int i = 0; i < 3; i++) o[9 + i] = ok ? S.t[i] : T.t0[i];
+    o[12] = ok ? S.a : T.a0; o[13] = ok ? S.b : T.b0;
     for (int i = 0; i < 5; i++) o[14 + i] = S.lastResiduals[i];
     for (int i = 0; i < 3; i++) o[19 + i] = S.flow[i];
     o[22] = S.good; o[23] = S.iterations; o[24] = S.evaluations; o[25] = S.status; o[26] = S.pevals;
@@ -854,6 +857,7 @@ struct dmv_ct {
   float huber = 9.f;
   int cluster_size = 0;        // CTAs of ct_track_cluster_kernel's cluster (0 = not probed yet, -1 = unavailable: grid version)
   CTMaps* maps = nullptr;      // TMA descriptors of the level planes (host copy; passed as a kernel parameter)
+  int staged[DMV_MAX_PYR_LEVELS] = {0};   // levels whose map ct_make_tensor_maps encoded: the only ones the cluster kernel stages
   long long launches = 0;
   float last_ms[4] = {0, 0, 0, 0};
 };
@@ -1062,7 +1066,8 @@ int dmv_ct_calc_res_gs(dmv_ct* c, int l, const float RKi[9], const float t[3], c
 }
 
 // TMA descriptors of the level planes: a w x h plane of float4 texels = a 2-D tensor of (2w) x h fp64 elements (the widest element type a
-// tensor map knows; 16-byte texels = pairs), one box = the whole plane.  Only levels that fit CTC_PLANE_BYTES are ever copied.
+// tensor map knows; 16-byte texels = pairs), one box = the whole plane.  c->staged[l] records the levels encoded here; the cluster kernel
+// stages exactly those (a plane that fits CTC_PLANE_BYTES but exceeds the 256-element box limit is gathered from L2).
 static int ct_make_tensor_maps(dmv_ct* c) {
   typedef CUresult (*EncodeFn)(CUtensorMap*, CUtensorMapDataType, cuuint32_t, void*, const cuuint64_t*, const cuuint64_t*, const cuuint32_t*, const cuuint32_t*,
                                CUtensorMapInterleave, CUtensorMapSwizzle, CUtensorMapL2promotion, CUtensorMapFloatOOBfill);
@@ -1074,6 +1079,7 @@ static int ct_make_tensor_maps(dmv_ct* c) {
   }
   if (!c->maps) c->maps = new CTMaps();
   std::memset(c->maps, 0, sizeof(CTMaps));
+  for (int l = 0; l < DMV_MAX_PYR_LEVELS; l++) c->staged[l] = 0;
   for (int l = 0; l < c->cfg.levels; l++) {
     const size_t bytes = (size_t)c->w[l] * c->h[l] * sizeof(float4);
     if (bytes > (size_t)CTC_PLANE_BYTES || 2 * c->w[l] > 256 || c->h[l] > 256) continue;   // never staged (box limits: 256 elements per dimension)
@@ -1085,6 +1091,7 @@ static int ct_make_tensor_maps(dmv_ct* c) {
                                                       CU_TENSOR_MAP_INTERLEAVE_NONE, CU_TENSOR_MAP_SWIZZLE_NONE, CU_TENSOR_MAP_L2_PROMOTION_NONE,
                                                       CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
     if (r != CUDA_SUCCESS) return set_error(DMV_ERR_CUDA, "cuTensorMapEncodeTiled failed for level %d (CUresult %d)", l, (int)r);
+    c->staged[l] = 1;
   }
   return DMV_OK;
 }
@@ -1120,11 +1127,19 @@ int dmv_ct_track(dmv_ct* c, const dmv_ct_track_args* in, dmv_ct_track_result* ou
   if (c->cluster_size == 0) {  // probe once: the largest cluster the device schedules for this kernel (16 needs the non-portable opt-in)
     c->cluster_size = -1;
     const char* env = getenv("DMV_CT_GRID");   // A/B switch: DMV_CT_GRID=1 keeps the chip-wide cooperative-grid version
+    // test hook: DMV_CT_CLUSTER=16|8|4 probes only that cluster size, and fails instead of falling back when it cannot be scheduled
+    const char* env_nc = getenv("DMV_CT_CLUSTER");
+    const int want_nc = env_nc ? atoi(env_nc) : 0;
+    if (env_nc && want_nc != 16 && want_nc != 8 && want_nc != 4) {
+      c->cluster_size = 0;
+      return set_error(DMV_ERR_INVALID, "DMV_CT_CLUSTER=%s: expected 16, 8 or 4", env_nc);
+    }
     if (!(env && atoi(env) != 0) && ct_make_tensor_maps(c) == DMV_OK) {
       CK(cudaFuncSetAttribute(ct_track_cluster_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)sizeof(CTCSmem)));
       cudaFuncSetAttribute(ct_track_cluster_kernel, cudaFuncAttributeNonPortableClusterSizeAllowed, 1);
       cudaGetLastError();
       for (int nc : {16, 8, 4}) {
+        if (want_nc && nc != want_nc) continue;
         cudaLaunchConfig_t cfg = {};
         cfg.gridDim = dim3(nc); cfg.blockDim = dim3(CTC_THREADS); cfg.dynamicSmemBytes = sizeof(CTCSmem); cfg.stream = c->stream;
         cudaLaunchAttribute at[1];
@@ -1135,8 +1150,13 @@ int dmv_ct_track(dmv_ct* c, const dmv_ct_track_args* in, dmv_ct_track_result* ou
         cudaGetLastError();
       }
     }
+    if (want_nc && c->cluster_size != want_nc && !(env && atoi(env) != 0)) {
+      c->cluster_size = 0;
+      return set_error(DMV_ERR_INVALID, "DMV_CT_CLUSTER=%d: ct_track_cluster_kernel cannot be scheduled with that cluster size", want_nc);
+    }
   }
   if (c->cluster_size > 0) {
+    for (int l = 0; l < DMV_MAX_PYR_LEVELS; l++) T.staged[l] = c->staged[l];
     cudaLaunchConfig_t cfg = {};
     cfg.gridDim = dim3(c->cluster_size); cfg.blockDim = dim3(CTC_THREADS); cfg.dynamicSmemBytes = sizeof(CTCSmem); cfg.stream = c->stream;
     cudaLaunchAttribute at[1];

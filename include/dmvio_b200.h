@@ -301,7 +301,11 @@ int dmv_ct_calc_res_gs(dmv_ct* ct, int level, const float RKi[9], const float t[
  * doubling, level repeat) runs on the device; the host gets the tracked pose back.  Same semantics as driving dmv_ct_calc_res_gs from the
  * host loop: R,t = lastToNew_out (refToNew, row-major), a,b = aff_g2l_out; on an aborted track (NaN residual or > 1.5*minResForAbort)
  * trackingGood = 0, status = 2 and R,t,a,b are returned unchanged, like the reference's early `return false`.
- * Needs all ceil(n/256) CTAs co-resident (n <= #SMs*256 reference points per level: 132*256 on an H100); otherwise DMV_ERR_INVALID. */
+ * Runs on one thread-block cluster (16, 8 or 4 CTAs, probed once per handle), which tracks any number of reference points.  Only the
+ * cooperative-grid fallback (when no cluster can be scheduled, or DMV_CT_GRID=1) needs all ceil(n/256) CTAs co-resident
+ * (n <= #SMs*256 reference points per level: 132*256 on an H100); it returns DMV_ERR_INVALID otherwise.
+ * Test hook: DMV_CT_CLUSTER=16|8|4 (read at the probe) allows only that cluster size and makes dmv_ct_track return an error instead of
+ * falling back when it cannot be scheduled. */
 typedef struct dmv_ct_track_args {
   double R[9], t[3];          /* in: initial refToNew */
   double a, b;                /* in: initial aff_g2l of the new frame */

@@ -1,5 +1,8 @@
 """CPU tests pinning the oracle's coarse-tracker restatement (CoarseTracker.cpp) by first principles."""
 import numpy as np
+import pytest
+
+import helpers as H
 
 
 def _setup(orc, synth, seed=4321, levels=0):
@@ -79,3 +82,56 @@ def test_tracking_recovers_pose(orc, synth):
     # fp32-faithful accumulation takes the same path
     res32 = ct.track(np.eye(3), np.zeros(3), 0.0, 0.0, precision=0)
     assert np.abs(res32["R"] - res["R"]).max() < 1e-4
+
+
+# scenes where the fp64 reference and the oracle take every decision alike (wide ends an LM level on a near tie that the oracle's
+# sequential fp32 energy sum decides differently; its saturation test at level 2 is also within the bound of 0.6)
+AGREE = ["bench", "aff_free", "aff_fixA", "aff_fixB", "aff_fixAB", "tma0_80x60", "tma0_160x120", "limit", "odd", "stream", "repeat"]
+
+
+@pytest.mark.parametrize("name", AGREE)
+def test_track_ref_matches_oracle(orc, synth, name):
+    """helpers.track_ref (fp64 trackNewestCoarse) against the oracle's trackNewestCoarse: same iterations and good flag, pose within 1e-6,
+    lastResiduals within rtol 1e-4 (the GPU tolerance).  Of track_ref's decisions only accept tests may be undecided by its fp32 bound:
+    every saturation, incNorm and abort test is decided."""
+    sc = H.ct_scene(orc, synth, name)
+    r = H.ct_track_ref(sc)
+    a = sc["args"]
+    ro = H.ct_oracle(orc, sc).track(a["R0"], a["t0"], a["a0"], a["b0"])
+    assert r["iterations"] == ro["iterations"] and bool(r["good"]) == ro["good"] and r["status"] == 0
+    assert np.abs(r["R"] - ro["R"]).max() < 1e-6 and np.abs(r["t"] - ro["t"]).max() < 1e-6
+    assert abs(r["a"] - ro["a"]) < 1e-6 and abs(r["b"] - ro["b"]) < 1e-3
+    np.testing.assert_allclose(r["lastResiduals"], ro["lastResiduals"], rtol=1e-4)
+    assert {u["what"] for u in r["undecided"]} <= {"accept"}, r["undecided"]
+
+
+def test_repeat_scene_doubles_cutoff_and_repeats_level(orc, synth):
+    sc = H.ct_scene(orc, synth, "repeat")
+    log = H.ct_track_ref(sc)["log"]
+    top = sc["levels"] - 1
+    assert log[0]["sat"] > 0.6 and log[1]["kind"] == "double" and log[1]["rep"] == 2.0
+    assert sum(1 for e in log if e["kind"] == "init" and e["lvl"] == top) == 2      # the coarsest level runs twice
+
+
+@pytest.mark.parametrize("name", H.CT_SCENES + ["counts_31"])
+def test_calc_res_ref_matches_oracle(orc, synth, name):
+    """helpers.calc_res_ref against the oracle's calc_res / calc_gs at every pose track_ref logs, within its bound for the oracle's summation
+    order (depth n: the oracle sums E and the flow terms sequentially in fp32)"""
+    sc = H.ct_scene(orc, synth, name)
+    r = H.ct_track_ref(sc)
+    a = sc["args"]
+    oc = H.ct_oracle(orc, sc)
+    for e in r["log"]:
+        l = e["lvl"]
+        RKi, tf, affLL = H.ct_operands(e["R"], e["t"], e["a"], e["b"], sc["Ki"][l], a["ref_a"], a["ref_b"], a["ref_exposure"], a["new_exposure"])
+        n = len(sc["pts"][l]["u"])
+        cut = np.float32(20) * np.float32(e["rep"])
+        c = H.calc_res_ref(sc["pts"][l], sc["planes"][l], sc["k4"][l], sc["Ki"][l], RKi, tf, affLL, a["ref_b"], cut, l, depth=n, R=e["R"])
+        ro = oc.calc_res(l, e["R"], e["t"], e["a"], e["b"], cutoff=float(cut))
+        Ho, bo = oc.calc_gs(l, e["a"], e["b"], 1)
+        assert abs(ro[1] - c["nE"]) <= c["amb"] and abs(ro[0] - c["E"]) <= c["dE"], (l, ro[:2], c["E"], c["nE"], c["dE"])
+        if l == 0:
+            assert abs(ro[2] - c["res6"][2]) <= c["dflow"][0] and abs(ro[4] - c["res6"][4]) <= c["dflow"][1]
+        if c["amb"] == 0:
+            assert ro[1] == c["nE"] and oc.warped().shape[1] == c["npad"]
+            assert (np.abs(Ho - c["H"]) <= c["dH"]).all() and (np.abs(bo - c["b"]) <= c["db"]).all()
