@@ -121,6 +121,11 @@ class CTTrackResult(C.Structure):
                 ("flowIndicators", C.c_double * 3), ("trackingGood", C.c_int), ("iterations", C.c_int), ("evaluations", C.c_int), ("status", C.c_int)]
 
 
+class UndistortConfig(C.Structure):
+    _fields_ = [("wOrg", C.c_int), ("hOrg", C.c_int), ("remapX", vp), ("remapY", vp), ("G", vp), ("nG", C.c_int), ("vignetteInv", vp),
+                ("photometric_mode", C.c_int)]
+
+
 class CIEvalArgs(C.Structure):
     _fields_ = [("level", C.c_int), ("RKi", C.c_float * 9), ("t_d", C.c_double * 3), ("t_log", C.c_double * 3), ("r2new_aff", C.c_float * 2),
                 ("huberTH", C.c_float), ("alphaK", C.c_float), ("alphaW", C.c_float), ("couplingWeight", C.c_float),
@@ -147,6 +152,7 @@ SYMBOLS = [
     "dmv_ct_create", "dmv_ct_destroy", "dmv_ct_set_K", "dmv_ct_set_ref", "dmv_ct_make_coarse_depth", "dmv_ct_get_ref", "dmv_ct_upload_new", "dmv_ct_upload_new_image", "dmv_ct_set_huber",
     "dmv_ci_create", "dmv_ci_destroy", "dmv_ci_set_K", "dmv_ci_upload_first", "dmv_ci_upload_new", "dmv_ci_set_points", "dmv_ci_calc_res_and_gs", "dmv_ci_kernel_launch_count",
     "dmv_ct_calc_res_gs", "dmv_ct_track", "dmv_ip_default_settings", "dmv_ct_init_points", "dmv_ct_trace_points", "dmv_ct_trace_points_multi", "dmv_ct_set_timing", "dmv_ct_last_timing", "dmv_ct_kernel_launch_count", "dmv_ct_last_point_evaluations",
+    "dmv_ct_set_undistort", "dmv_ct_upload_raw_image", "dmv_ct_download_frame",
 ]
 
 
@@ -221,6 +227,9 @@ def lib():
         L.dmv_ct_last_timing.argtypes = [vp, f32p]
         L.dmv_ct_kernel_launch_count.argtypes = [vp, C.POINTER(C.c_longlong)]
         L.dmv_ct_last_point_evaluations.argtypes = [vp, C.POINTER(C.c_double)]
+        L.dmv_ct_set_undistort.argtypes = [vp, C.POINTER(UndistortConfig)]
+        L.dmv_ct_upload_raw_image.argtypes = [vp, vp, C.c_int, C.c_float, C.c_float]
+        L.dmv_ct_download_frame.argtypes = [vp, C.c_int, f32p]
         L.dmv_ci_create.argtypes = [C.POINTER(CTConfig), C.POINTER(vp)]
         L.dmv_ci_destroy.argtypes = [vp]
         L.dmv_ci_set_K.argtypes = [vp, C.c_int, C.c_float, C.c_float, C.c_float, C.c_float]
@@ -513,6 +522,28 @@ class CT:
 
     def set_huber(self, th):
         check(self.L.dmv_ct_set_huber(self.h, th))
+
+    def set_undistort(self, wOrg, hOrg, remapX=None, remapY=None, G=None, vignetteInv=None, photometric_mode=0):
+        """dmv_ct_set_undistort: the per-sequence tables of Undistort (remapX/remapY None = passthrough, G None = no photometric calibration)"""
+        keep = [None if a is None else _c(a, np.float32).reshape(-1) for a in (remapX, remapY, G, vignetteInv)]
+        p = [None if a is None else a.ctypes.data for a in keep]
+        cfg = UndistortConfig(int(wOrg), int(hOrg), p[0], p[1], p[2], 0 if G is None else len(keep[2]), p[3], int(photometric_mode))
+        check(self.L.dmv_ct_set_undistort(self.h, C.byref(cfg)))
+
+    def upload_raw_image(self, raw, exposure=1.0, factor=None):
+        """dmv_ct_upload_raw_image: a uint8 or uint16 frame of the raw size; factor defaults to the reference's readers' (1, or 1/256 for 16 bit)"""
+        raw = np.ascontiguousarray(raw)
+        if raw.dtype not in (np.uint8, np.uint16):
+            raise DmvError("raw frames are uint8 or uint16")
+        if factor is None:
+            factor = 1.0 if raw.itemsize == 1 else 1.0 / 256
+        check(self.L.dmv_ct_upload_raw_image(self.h, raw.ctypes.data, raw.itemsize, float(exposure), float(factor)))
+
+    def download_frame(self, lvl, w, h):
+        """dmv_ct_download_frame: dIp[lvl] as an (h_l, w_l, 3) array (w, h = level-0 size)"""
+        out = np.zeros(((h >> lvl) * (w >> lvl) * 3), np.float32)
+        check(self.L.dmv_ct_download_frame(self.h, lvl, out))
+        return out.reshape(h >> lvl, w >> lvl, 3)
 
     def calc_res_gs(self, lvl, RKi, t, affLL, b0, cutoff, want_gs=True):
         res6 = np.zeros(6); H = np.zeros(64); b = np.zeros(8); n = C.c_int(0)

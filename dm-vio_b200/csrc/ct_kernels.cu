@@ -12,6 +12,7 @@
 #include "inv3.h"
 #include "ip_trace.h"
 #include "ct_depth.h"
+#include "ct_ingest.h"
 #include <cuda.h>
 #include <unordered_map>
 #include <algorithm>
@@ -860,6 +861,13 @@ struct dmv_ct {
   int staged[DMV_MAX_PYR_LEVELS] = {0};   // levels whose map ct_make_tensor_maps encoded: the only ones the cluster kernel stages
   long long launches = 0;
   float last_ms[4] = {0, 0, 0, 0};
+  size_t scratch_bytes = 0;    // capacity of h_scratch
+  // raw-frame ingest (dmv_ct_set_undistort / dmv_ct_upload_raw_image)
+  bool have_undistort = false;
+  int wOrg = 0, hOrg = 0, nG = 0, pmode = 0;
+  float2* d_remap = nullptr;
+  float *d_G = nullptr, *d_vigInv = nullptr;
+  void* d_raw = nullptr;
 };
 
 #define CK(call)                                                                                   \
@@ -871,6 +879,7 @@ struct dmv_ct {
 extern "C" {
 
 static int ct_allocate(dmv_ct* c, const dmv_ct_config* cfg);
+static int ct_build_pyramid(dmv_ct* c);
 
 int dmv_ct_create(const dmv_ct_config* cfg, dmv_ct** out) {
   if (!cfg || !out) return set_error(DMV_ERR_INVALID, "null argument");
@@ -918,7 +927,8 @@ static int ct_allocate(dmv_ct* c, const dmv_ct_config* cfg) {
   CK(cudaMemset(c->d_ticket, 0, sizeof(unsigned int)));
   CK(cudaMalloc(&c->d_out, sizeof(double) * 64));
   CK(cudaMallocHost(&c->h_out, sizeof(double) * 64));
-  CK(cudaMallocHost(&c->h_scratch, sizeof(float) * std::max(npx0 * 3, (size_t)cfg->max_points * 4)));
+  c->scratch_bytes = sizeof(float) * std::max(npx0 * 3, (size_t)cfg->max_points * 4);
+  CK(cudaMallocHost(&c->h_scratch, c->scratch_bytes));
   return DMV_OK;
 }
 
@@ -933,6 +943,7 @@ int dmv_ct_destroy(dmv_ct* c) {
   cudaFreeHost(c->h_out); cudaFreeHost(c->h_scratch); cudaFree(c->d_ip); cudaFreeHost(c->h_ip);
   for (int l = 0; l < DMV_MAX_PYR_LEVELS; l++) { cudaFree(c->cd_idepth[l]); cudaFree(c->cd_ws[l]); cudaFree(c->cd_ws2[l]); }
   cudaFree(c->cd_rowcnt); cudaFree(c->cd_rowoff); cudaFreeHost(c->cd_totals);
+  cudaFree(c->d_remap); cudaFree(c->d_G); cudaFree(c->d_vigInv); cudaFree(c->d_raw);
   if (c->ev[0]) cudaEventDestroy(c->ev[0]);
   if (c->ev[1]) cudaEventDestroy(c->ev[1]);
   if (c->stream) cudaStreamDestroy(c->stream);
@@ -992,6 +1003,16 @@ int dmv_ct_upload_new_image(dmv_ct* c, const float* image) {
   if (c->staging_busy) { CK(cudaStreamSynchronize(c->stream)); c->staging_busy = false; }  // a previous upload may still read the staging buffer
   std::memcpy(c->h_scratch, image, npx * sizeof(float));
   CK(cudaMemcpyAsync(c->d_gray[0], c->h_scratch, npx * sizeof(float), cudaMemcpyHostToDevice, c->stream));
+  const int rc = ct_build_pyramid(c);
+  if (rc != DMV_OK) return rc;
+  // no synchronisation: every consumer (dmv_ct_calc_res_gs / dmv_ct_track) runs on the same stream and synchronises itself; the image
+  // was copied into the handle's pinned staging buffer above, so the caller's buffer is already free
+  c->staging_busy = true;
+  return DMV_OK;
+}
+
+// the pyramid of the frame whose level-0 intensities are in d_gray[0]
+static int ct_build_pyramid(dmv_ct* c) {
   for (int l = 0; l < c->cfg.levels; l++) {
     const int wl = c->w[l], hl = c->h[l];
     if (l > 0) {
@@ -1003,9 +1024,92 @@ int dmv_ct_upload_new_image(dmv_ct* c, const float* image) {
     c->launches++;
   }
   CK(cudaGetLastError());
-  // no synchronisation: every consumer (dmv_ct_calc_res_gs / dmv_ct_track) runs on the same stream and synchronises itself; the image
-  // was copied into the handle's pinned staging buffer above, so the caller's buffer is already free
-  c->staging_busy = true;
+  return DMV_OK;
+}
+
+int dmv_ct_set_undistort(dmv_ct* c, const dmv_undistort_config* u) {
+  if (!c || !u) return set_error(DMV_ERR_INVALID, "null argument");
+  const int w = c->w[0], h = c->h[0];
+  if (u->wOrg < 2 || u->hOrg < 2 || (size_t)u->wOrg * u->hOrg > ((size_t)1 << 28)) return set_error(DMV_ERR_INVALID, "bad raw size %d x %d", u->wOrg, u->hOrg);
+  if (!u->remapX != !u->remapY) return set_error(DMV_ERR_INVALID, "remapX and remapY must both be given or both be NULL");
+  if (!u->remapX && (u->wOrg != w || u->hOrg != h)) return set_error(DMV_ERR_INVALID, "passthrough needs the raw size to equal level 0 (%d x %d)", w, h);
+  if (u->photometric_mode < 0 || u->photometric_mode > 2) return set_error(DMV_ERR_INVALID, "photometric_mode must be 0, 1 or 2");
+  if (u->G && (u->nG < 256 || u->nG > 65536)) return set_error(DMV_ERR_INVALID, "nG = %d: the response map has 256 to 65536 entries", u->nG);
+  if (u->G && u->photometric_mode == 2 && !u->vignetteInv) return set_error(DMV_ERR_INVALID, "photometric_mode 2 needs vignetteInv");
+  const size_t npx = (size_t)w * h, nraw = (size_t)u->wOrg * u->hOrg;
+  std::vector<float2> remap;
+  if (u->remapX) {  // every sample the kernel reads must lie inside the raw image (the reference's constructor guarantees it, L920-941)
+    remap.resize(npx);
+    const float xmax = (float)(u->wOrg - 1), ymax = (float)(u->hOrg - 1);
+    for (size_t i = 0; i < npx; i++) {
+      const float x = u->remapX[i], y = u->remapY[i];
+      if (!(x < 0) && !(x >= 0 && x < xmax && y >= 0 && y < ymax))
+        return set_error(DMV_ERR_INVALID, "remap entry %zu = (%g, %g) lies outside [0, %d) x [0, %d)", i, x, y, u->wOrg - 1, u->hOrg - 1);
+      remap[i] = make_float2(x, y);
+    }
+  }
+  CK(cudaSetDevice(c->device));
+  CK(cudaStreamSynchronize(c->stream));  // kernels in flight may read the old tables or the staging buffer
+  c->staging_busy = false;
+  c->have_undistort = false;
+  cudaFree(c->d_remap); cudaFree(c->d_G); cudaFree(c->d_vigInv); cudaFree(c->d_raw);
+  c->d_remap = nullptr; c->d_G = nullptr; c->d_vigInv = nullptr; c->d_raw = nullptr;
+  if (nraw * 2 > c->scratch_bytes) {
+    cudaFreeHost(c->h_scratch);
+    c->h_scratch = nullptr;
+    c->scratch_bytes = 0;
+    CK(cudaMallocHost(&c->h_scratch, nraw * 2));
+    c->scratch_bytes = nraw * 2;
+  }
+  CK(cudaMalloc(&c->d_raw, nraw * 2));
+  if (u->remapX) {
+    CK(cudaMalloc(&c->d_remap, npx * sizeof(float2)));
+    CK(cudaMemcpy(c->d_remap, remap.data(), npx * sizeof(float2), cudaMemcpyHostToDevice));
+  }
+  if (u->G) {
+    CK(cudaMalloc(&c->d_G, (size_t)u->nG * sizeof(float)));
+    CK(cudaMemcpy(c->d_G, u->G, (size_t)u->nG * sizeof(float), cudaMemcpyHostToDevice));
+  }
+  if (u->G && u->vignetteInv) {
+    CK(cudaMalloc(&c->d_vigInv, nraw * sizeof(float)));
+    CK(cudaMemcpy(c->d_vigInv, u->vignetteInv, nraw * sizeof(float), cudaMemcpyHostToDevice));
+  }
+  c->wOrg = u->wOrg; c->hOrg = u->hOrg; c->nG = u->G ? u->nG : 0; c->pmode = u->photometric_mode;
+  c->have_undistort = true;
+  return DMV_OK;
+}
+
+int dmv_ct_upload_raw_image(dmv_ct* c, const void* raw, int bpp, float exposure, float factor) {
+  if (!c || !raw) return set_error(DMV_ERR_INVALID, "null argument");
+  if (bpp != 1 && bpp != 2) return set_error(DMV_ERR_INVALID, "bytes_per_px must be 1 or 2");
+  if (!c->have_undistort) return set_error(DMV_ERR_INVALID, "dmv_ct_set_undistort first");
+  // PhotometricUndistorter::processFrame L222: the calibrated branch needs a valid calibration, exposure_time > 0 and mode != 0
+  const bool use_G = c->d_G && exposure > 0 && c->pmode != 0;
+  if (use_G && c->nG < (bpp == 1 ? 256 : 65536)) return set_error(DMV_ERR_INVALID, "a %d-entry response map does not cover %d-bit pixels", c->nG, 8 * bpp);
+  CK(cudaSetDevice(c->device));
+  const size_t bytes = (size_t)c->wOrg * c->hOrg * bpp;
+  if (c->staging_busy) { CK(cudaStreamSynchronize(c->stream)); c->staging_busy = false; }
+  std::memcpy(c->h_scratch, raw, bytes);
+  CK(cudaMemcpyAsync(c->d_raw, c->h_scratch, bytes, cudaMemcpyHostToDevice, c->stream));
+  IngestTables t;
+  t.npx = c->w[0] * c->h[0]; t.wOrg = c->wOrg; t.remap = c->d_remap; t.G = c->d_G; t.vigInv = c->d_vigInv; t.mode = c->pmode;
+  ingest_launch(t, c->d_raw, bpp, use_G, factor, c->d_gray[0], c->stream);
+  c->launches++;
+  const int rc = ct_build_pyramid(c);
+  if (rc != DMV_OK) return rc;
+  c->staging_busy = true;  // asynchronous like dmv_ct_upload_new_image
+  return DMV_OK;
+}
+
+int dmv_ct_download_frame(dmv_ct* c, int l, float* dIp) {
+  if (!c || !dIp || l < 0 || l >= c->cfg.levels) return set_error(DMV_ERR_INVALID, "bad level / pointer");
+  CK(cudaSetDevice(c->device));
+  const size_t npx = (size_t)c->w[l] * c->h[l];
+  if (c->staging_busy) { CK(cudaStreamSynchronize(c->stream)); c->staging_busy = false; }
+  // float4 (I, dx, dy, 0) -> 3 floats per pixel into the pinned staging buffer (it holds w*h*3 floats of level 0)
+  CK(cudaMemcpy2DAsync(c->h_scratch, 3 * sizeof(float), c->d_img[l], sizeof(float4), 3 * sizeof(float), npx, cudaMemcpyDeviceToHost, c->stream));
+  CK(cudaStreamSynchronize(c->stream));
+  std::memcpy(dIp, c->h_scratch, npx * 3 * sizeof(float));
   return DMV_OK;
 }
 

@@ -33,6 +33,12 @@ class CoarseTracker {
   // newFrame: raw image (pyramid built on the device) and its exposure
   bool setNewFrame(const float* image_wh, float ab_exposure);
   bool setNewFramePyramid(const float* const* dIp, float ab_exposure);
+  // Raw frames (coarse_tracker_ingest.cpp): the per-frame part of Undistort::undistort<T> runs on the device (dmv_ct_set_undistort /
+  // dmv_ct_upload_raw_image).  setUndistort once per sequence with the host-built tables; uploadRawImage replaces setNewFrame with the
+  // camera's frame; downloadFrame reads dIp[level] back (keyframes: pixel selection, initialisation).
+  bool setUndistort(const dmv_undistort_config& cfg);
+  bool uploadRawImage(const void* raw, int bytes_per_px, float exposure, float factor, float ab_exposure);
+  bool downloadFrame(int level, float* dIp_aos3);
   // CoarseTracker.cpp:L539-770 (visual-only branch L639-683)
   bool trackNewestCoarse(SE3& lastToNew_out, AffLight& aff_g2l_out, int coarsestLvl, const double minResForAbort[5]);
 

@@ -73,6 +73,11 @@ void dmvh_ct_set_device_lm(void* ct, int on);
 double dmvh_ct_point_evaluations(void* ct); /* CoarseTracker::pointEvaluations of the last track (measurement) */ /* 1 (default): LM loop on the device (dmv_ct_track); 0: host loop */
 int dmvh_ct_track(void* ct, double R[9], double t[3], double* a, double* b, int coarsestLvl, const double minResForAbort[5],
                   double lastResiduals[5], double flow[3], int* iterations, long long* evaluations);
+/* raw-frame ingest (host/coarse_tracker_ingest.cpp): CoarseTracker::setUndistort / uploadRawImage / downloadFrame */
+int dmvh_ct_set_undistort(void* ct, int wOrg, int hOrg, const float* remapX, const float* remapY, const float* G, int nG, const float* vignetteInv,
+                          int photometric_mode);
+int dmvh_ct_upload_raw_image(void* ct, const void* raw, int bytes_per_px, float exposure, float factor, float ab_exposure);
+int dmvh_ct_download_frame(void* ct, int level, float* dIp_aos3);
 
 /* CoarseInitializer adapter (host/coarse_initializer.h): trackFrame on the host, calcResAndGS on the device */
 void* dmvh_ci_create(int w, int h, int levels, int max_points, int device, const double calib_value_scaled[4]);

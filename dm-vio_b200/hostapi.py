@@ -293,6 +293,35 @@ class CoarseTracker:
         if self.L.dmvh_ct_set_new_image(self.h, _c(img, np.float32).reshape(-1), exposure) != 0:
             raise capi.DmvError("dmvh_ct_set_new_image failed")
 
+    def _ingest(self):
+        # bound here rather than in _bind: the CPU build of the adapters over the oracle stand-in has no ingest path
+        L = self.L
+        L.dmvh_ct_set_undistort.argtypes = [vp, C.c_int, C.c_int, vp, vp, vp, C.c_int, vp, C.c_int]
+        L.dmvh_ct_upload_raw_image.argtypes = [vp, vp, C.c_int, C.c_float, C.c_float, C.c_float]
+        L.dmvh_ct_download_frame.argtypes = [vp, C.c_int, f32p]
+        return L
+
+    def set_undistort(self, wOrg, hOrg, remapX=None, remapY=None, G=None, vignetteInv=None, photometric_mode=0):
+        """CoarseTracker::setUndistort (dmv_ct_set_undistort)"""
+        keep = [None if a is None else _c(a, np.float32).reshape(-1) for a in (remapX, remapY, G, vignetteInv)]
+        p = [None if a is None else a.ctypes.data for a in keep]
+        if self._ingest().dmvh_ct_set_undistort(self.h, int(wOrg), int(hOrg), p[0], p[1], p[2], 0 if G is None else len(keep[2]), p[3],
+                                                int(photometric_mode)) != 0:
+            raise capi.DmvError("dmvh_ct_set_undistort failed")
+
+    def upload_raw_image(self, raw, exposure=1.0, factor=None, ab_exposure=1.0):
+        """CoarseTracker::uploadRawImage: the new frame from the camera's raw bytes"""
+        raw = np.ascontiguousarray(raw)
+        factor = (1.0 if raw.itemsize == 1 else 1.0 / 256) if factor is None else factor
+        if self._ingest().dmvh_ct_upload_raw_image(self.h, raw.ctypes.data, raw.itemsize, float(exposure), float(factor), float(ab_exposure)) != 0:
+            raise capi.DmvError("dmvh_ct_upload_raw_image failed")
+
+    def download_frame(self, lvl, w, h):
+        out = np.zeros((h >> lvl) * (w >> lvl) * 3, np.float32)
+        if self._ingest().dmvh_ct_download_frame(self.h, lvl, out) != 0:
+            raise capi.DmvError("dmvh_ct_download_frame failed")
+        return out.reshape(h >> lvl, w >> lvl, 3)
+
     def track(self, R, t, a, b, coarsest=None, minRes=None, device_lm=True):
         self.L.dmvh_ct_set_device_lm(self.h, int(device_lm))
         R = _c(R, np.float64).reshape(-1).copy(); t = _c(t, np.float64).copy()

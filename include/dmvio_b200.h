@@ -289,6 +289,34 @@ int dmv_ct_upload_new_image(dmv_ct* ct, const float* image_wh);
 /* settings read by calcRes: setting_huberTH */
 int dmv_ct_set_huber(dmv_ct* ct, float huberTH);
 
+/* Raw-frame ingest == the per-frame part of Undistort::undistort<T> (util/Undistort.cpp:L385-482) with
+ * PhotometricUndistorter::processFrame (L213-252) on the device.  The tables are built once per sequence on the host, as the
+ * reference builds them (camera model, makeOptimalK_*, G, vignetteMapInv), and uploaded by dmv_ct_set_undistort.
+ *   remapX / remapY: w*h each (w, h = the handle's level 0); x < 0 marks a pixel outside the raw image (output 0), every other
+ *                    entry must satisfy 0 <= x < wOrg-1 and 0 <= y < hOrg-1.  Both NULL = passthrough (requires wOrg = w, hOrg = h).
+ *   G / nG:          the response map as PhotometricUndistorter holds it (256 <= nG <= 65536), or NULL = no photometric calibration.
+ *                    A raw upload that applies G (exposure > 0, photometric_mode != 0) needs nG >= 256 (8-bit) / 65536 (16-bit).
+ *   vignetteInv:     wOrg*hOrg (vignetteMapInv), required with photometric_mode 2 and G; may be NULL otherwise.
+ *   photometric_mode = setting_photometricCalibration (0, 1, 2).
+ * The benchmark-only distortions (benchmark_varNoise, benchmark_varBlurNoise) are not supported. */
+typedef struct dmv_undistort_config {
+  int wOrg, hOrg;
+  const float* remapX;
+  const float* remapY;
+  const float* G;
+  int nG;
+  const float* vignetteInv;
+  int photometric_mode;
+} dmv_undistort_config;
+int dmv_ct_set_undistort(dmv_ct* ct, const dmv_undistort_config* cfg);
+/* One raw frame (wOrg*hOrg pixels of bytes_per_px = 1 (uint8) or 2 (uint16)) -> the level-0 intensity plane, then the whole pyramid, like
+ * dmv_ct_upload_new_image with the image Undistort::undistort<T>(raw, exposure, 0, factor) returns; bit-identical.  factor multiplies the raw
+ * value when the photometric map is off (no G, exposure <= 0 or photometric_mode 0): 1 for 8-bit, 1/256 as the reference's 16-bit reader.
+ * Asynchronous like dmv_ct_upload_new_image (the frame goes through the handle's pinned staging buffer). */
+int dmv_ct_upload_raw_image(dmv_ct* ct, const void* raw, int bytes_per_px, float exposure, float factor);
+/* read-back of the resident frame's dIp[level] (w_l*h_l*3 floats AoS: I, dx, dy), e.g. for pixel selection on keyframes */
+int dmv_ct_download_frame(dmv_ct* ct, int level, float* dIp_aos3);
+
 /* CoarseTracker::calcRes (L361-517) fused with calcGSSSE (L299-356) for one pose:
  *   RKi = R * Ki[lvl] (row-major 3x3 float), t (3), affLL = AffLight::fromToVecExposure(...) (2),
  *   a_gs = affLL[0] (first argument `a` of calcGSSSE), b0 = lastRef_aff_g2l.b, cutoffTH.
