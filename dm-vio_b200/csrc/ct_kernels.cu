@@ -3,7 +3,7 @@
 //   ct_res_gs_kernel   CoarseTracker::calcRes (CoarseTracker.cpp:L361-517) fused with calcGSSSE (L299-356): one thread per
 //                      reference point: project, 4-tap float4 gather from the new frame's level plane, Huber residual,
 //                      energy / saturation counters / flow indicators and the 45 unique entries of the weighted 9x9
-//                      outer product.  Warp-shuffle + shared-memory block reduction, per-block fp64 partials, and the last
+//                      outer product.  Block reduction (ct_block_sum), per-block fp64 partials, and the last
 //                      block to finish (threadfence + ticket) folds the partials in a fixed order -> deterministic, one launch.
 //                      The buf_warped_* lists of the reference are never materialised.
 //   pyr_down_kernel / grad_kernel   FrameHessian::makeImages (HessianBlocks.cpp:L128-191) on the device.
@@ -32,71 +32,72 @@ struct CTParams {
   int w, h, n, lvl, want_gs;
 };
 
-// one reference point: CoarseTracker::calcRes (L399-483) + its row of calcGSSSE (L316-336); v[] = this point's contribution
-__device__ __forceinline__ void ct_eval_point(const CTParams& P, int i, const float* __restrict__ pc_u, const float* __restrict__ pc_v,
-                                              const float* __restrict__ pc_id, const float* __restrict__ pc_col, const float4* __restrict__ img,
-                                              float v[CT_NRED]) {
-#pragma unroll
-  for (int k = 0; k < CT_NRED; k++) v[k] = 0.f;
-  if (i < P.n) {
-    const float id = pc_id[i], x = pc_u[i], y = pc_v[i];
-    const float p0 = P.RKi[0] * x + P.RKi[1] * y + P.RKi[2] + P.t[0] * id;
-    const float p1 = P.RKi[3] * x + P.RKi[4] * y + P.RKi[5] + P.t[1] * id;
-    const float p2 = P.RKi[6] * x + P.RKi[7] * y + P.RKi[8] + P.t[2] * id;
-    const float u = p0 / p2, vv = p1 / p2;
-    const float Ku = P.fx * u + P.cx, Kv = P.fy * vv + P.cy;
-    const float new_idepth = id / p2;
-    if (P.lvl == 0 && (i & 31) == 0) {  // flow indicators (L416-447)
-      const float k0 = P.Ki[0] * x + P.Ki[1] * y + P.Ki[2], k1 = P.Ki[3] * x + P.Ki[4] * y + P.Ki[5], k2 = P.Ki[6] * x + P.Ki[7] * y + P.Ki[8];
-      const float T0 = k0 + P.t[0] * id, T1 = k1 + P.t[1] * id, T2 = k2 + P.t[2] * id;
-      const float M0 = k0 - P.t[0] * id, M1 = k1 - P.t[1] * id, M2 = k2 - P.t[2] * id;
-      const float q0 = P.RKi[0] * x + P.RKi[1] * y + P.RKi[2] - P.t[0] * id;
-      const float q1 = P.RKi[3] * x + P.RKi[4] * y + P.RKi[5] - P.t[1] * id;
-      const float q2 = P.RKi[6] * x + P.RKi[7] * y + P.RKi[8] - P.t[2] * id;
-      const float KuT = P.fx * (T0 / T2) + P.cx, KvT = P.fy * (T1 / T2) + P.cy;
-      const float KuT2 = P.fx * (M0 / M2) + P.cx, KvT2 = P.fy * (M1 / M2) + P.cy;
-      const float Ku3 = P.fx * (q0 / q2) + P.cx, Kv3 = P.fy * (q1 / q2) + P.cy;
-      v[49] = (KuT - x) * (KuT - x) + (KvT - y) * (KvT - y) + (KuT2 - x) * (KuT2 - x) + (KvT2 - y) * (KvT2 - y);
-      v[50] = (Ku - x) * (Ku - x) + (Kv - y) * (Kv - y) + (Ku3 - x) * (Ku3 - x) + (Kv3 - y) * (Kv3 - y);
-      v[51] = 2.f;
-    }
-    if (Ku > 2.f && Kv > 2.f && Ku < (float)(P.w - 3) && Kv < (float)(P.h - 3) && new_idepth > 0.f) {
-      const int ix = (int)Ku, iy = (int)Kv;
-      const float dx = Ku - ix, dy = Kv - iy, dxdy = dx * dy;
+// one reference point (x, y, id, refColor): CoarseTracker::calcRes (L399-483) + its row of calcGSSSE (L316-336), added into v[]; the 4 taps
+// come from the level plane in shared memory (SMEM: staged by TMA, plane_s) or from global memory (img)
+template <bool SMEM>
+__device__ __forceinline__ void ct_eval_accumulate(const CTParams& P, int i, const float x, const float y, const float id, const float refColor,
+                                                   const float4* __restrict__ img, const float4* plane_s, float v[64]) {
+  const float p0 = P.RKi[0] * x + P.RKi[1] * y + P.RKi[2] + P.t[0] * id;
+  const float p1 = P.RKi[3] * x + P.RKi[4] * y + P.RKi[5] + P.t[1] * id;
+  const float p2 = P.RKi[6] * x + P.RKi[7] * y + P.RKi[8] + P.t[2] * id;
+  const float u = p0 / p2, vv = p1 / p2;
+  const float Ku = P.fx * u + P.cx, Kv = P.fy * vv + P.cy;
+  const float new_idepth = id / p2;
+  if (P.lvl == 0 && (i & 31) == 0) {  // flow indicators (CoarseTracker.cpp:L416-447)
+    const float k0 = P.Ki[0] * x + P.Ki[1] * y + P.Ki[2], k1 = P.Ki[3] * x + P.Ki[4] * y + P.Ki[5], k2 = P.Ki[6] * x + P.Ki[7] * y + P.Ki[8];
+    const float T0 = k0 + P.t[0] * id, T1 = k1 + P.t[1] * id, T2 = k2 + P.t[2] * id;
+    const float M0 = k0 - P.t[0] * id, M1 = k1 - P.t[1] * id, M2 = k2 - P.t[2] * id;
+    const float q0 = P.RKi[0] * x + P.RKi[1] * y + P.RKi[2] - P.t[0] * id;
+    const float q1 = P.RKi[3] * x + P.RKi[4] * y + P.RKi[5] - P.t[1] * id;
+    const float q2 = P.RKi[6] * x + P.RKi[7] * y + P.RKi[8] - P.t[2] * id;
+    const float KuT = P.fx * (T0 / T2) + P.cx, KvT = P.fy * (T1 / T2) + P.cy;
+    const float KuT2 = P.fx * (M0 / M2) + P.cx, KvT2 = P.fy * (M1 / M2) + P.cy;
+    const float Ku3 = P.fx * (q0 / q2) + P.cx, Kv3 = P.fy * (q1 / q2) + P.cy;
+    v[49] += (KuT - x) * (KuT - x) + (KvT - y) * (KvT - y) + (KuT2 - x) * (KuT2 - x) + (KvT2 - y) * (KvT2 - y);
+    v[50] += (Ku - x) * (Ku - x) + (Kv - y) * (Kv - y) + (Ku3 - x) * (Ku3 - x) + (Kv3 - y) * (Kv3 - y);
+    v[51] += 2.f;
+  }
+  if (Ku > 2.f && Kv > 2.f && Ku < (float)(P.w - 3) && Kv < (float)(P.h - 3) && new_idepth > 0.f) {
+    const int ix = (int)Ku, iy = (int)Kv;
+    const float dx = Ku - ix, dy = Kv - iy, dxdy = dx * dy;
+    float4 tl, tr, bl, br;
+    if constexpr (SMEM) {
+      const float4* bp = plane_s + iy * P.w + ix;
+      tl = bp[0]; tr = bp[1]; bl = bp[P.w]; br = bp[P.w + 1];
+    } else {
       const float4* bp = img + (size_t)iy * P.w + ix;
-      const float4 tl = __ldg(bp), tr = __ldg(bp + 1), bl = __ldg(bp + P.w), br = __ldg(bp + P.w + 1);
-      const float w11 = dxdy, w10 = dy - dxdy, w01 = dx - dxdy, w00 = 1 - dx - dy + dxdy;
-      const float h0 = w11 * br.x + w10 * bl.x + w01 * tr.x + w00 * tl.x;
-      const float h1 = w11 * br.y + w10 * bl.y + w01 * tr.y + w00 * tl.y;
-      const float h2 = w11 * br.z + w10 * bl.z + w01 * tr.z + w00 * tl.z;
-      if (isfinite(h0)) {
-        const float refColor = pc_col[i];
-        const float residual = h0 - (P.affa * refColor + P.affb);
-        const float ar = fabsf(residual);
-        const float hw = ar < P.huber ? 1.f : P.huber / ar;
-        if (ar > P.cutoff) {
-          v[45] = P.maxEnergy; v[46] = 1.f; v[47] = 1.f;
-        } else {
-          v[45] = hw * residual * residual * (2.f - hw); v[46] = 1.f; v[48] = 1.f;
-          if (P.want_gs) {  // calcGSSSE row (L316-336) and Accumulator9::updateSSE_eighted (MatrixAccumulators.h:L1091-1166)
-            const float gx = h1 * P.fx, gy = h2 * P.fy;
-            float J[9];
-            J[0] = new_idepth * gx;
-            J[1] = new_idepth * gy;
-            J[2] = 0.f - new_idepth * (u * gx + vv * gy);
-            J[3] = 0.f - ((u * vv) * gx + gy * (1.f + vv * vv));
-            J[4] = (u * vv) * gy + gx * (1.f + u * u);
-            J[5] = u * gy - vv * gx;
-            J[6] = P.a_gs * (P.b0 - refColor);
-            J[7] = -1.f;
-            J[8] = residual;
-            int e = 0;
+      tl = __ldg(bp); tr = __ldg(bp + 1); bl = __ldg(bp + P.w); br = __ldg(bp + P.w + 1);
+    }
+    const float w11 = dxdy, w10 = dy - dxdy, w01 = dx - dxdy, w00 = 1 - dx - dy + dxdy;
+    const float h0 = w11 * br.x + w10 * bl.x + w01 * tr.x + w00 * tl.x;
+    const float h1 = w11 * br.y + w10 * bl.y + w01 * tr.y + w00 * tl.y;
+    const float h2 = w11 * br.z + w10 * bl.z + w01 * tr.z + w00 * tl.z;
+    if (isfinite(h0)) {
+      const float residual = h0 - (P.affa * refColor + P.affb);
+      const float ar = fabsf(residual);
+      const float hw = ar < P.huber ? 1.f : P.huber / ar;
+      if (ar > P.cutoff) {
+        v[45] += P.maxEnergy; v[46] += 1.f; v[47] += 1.f;
+      } else {
+        v[45] += hw * residual * residual * (2.f - hw); v[46] += 1.f; v[48] += 1.f;
+        if (P.want_gs) {  // calcGSSSE row (L316-336) and Accumulator9::updateSSE_eighted (MatrixAccumulators.h:L1091-1166)
+          const float gx = h1 * P.fx, gy = h2 * P.fy;
+          float J[9];
+          J[0] = new_idepth * gx;
+          J[1] = new_idepth * gy;
+          J[2] = 0.f - new_idepth * (u * gx + vv * gy);
+          J[3] = 0.f - ((u * vv) * gx + gy * (1.f + vv * vv));
+          J[4] = (u * vv) * gy + gx * (1.f + u * u);
+          J[5] = u * gy - vv * gx;
+          J[6] = P.a_gs * (P.b0 - refColor);
+          J[7] = -1.f;
+          J[8] = residual;
+          int e = 0;
 #pragma unroll
-            for (int r = 0; r < 9; r++) {
-              const float Jw = J[r] * hw;
+          for (int r = 0; r < 9; r++) {
+            const float Jw = J[r] * hw;
 #pragma unroll
-              for (int c = r; c < 9; c++) v[e++] = Jw * J[c];
-            }
+            for (int c = r; c < 9; c++) v[e++] += Jw * J[c];
           }
         }
       }
@@ -104,26 +105,31 @@ __device__ __forceinline__ void ct_eval_point(const CTParams& P, int i, const fl
   }
 }
 
-// block reduction: warp shuffles, then the 8 warp partials through shared memory; thread k < CT_NRED returns the block's sum of v[k] in fp64
-__device__ __forceinline__ double ct_block_reduce(const float v[CT_NRED], float (*s_red)[CT_NRED]) {
+// block reduction of the 53 sums of a block of NW warps (v[53..63] = 0 pads; v is overwritten).  Per warp a transposing butterfly: 62
+// shuffles, after which lane L holds the warp sums of entries 2L and 2L+1.  It pairs lanes at distance 16, 8, 4, 2, 1, the addition tree
+// of a per-entry xor reduction (53 x 5 shuffles), and gives the same bits.  Then thread k < CT_NRED returns the sum of entry k over the
+// warps, in fp64 and in warp order.
+template <int NW>
+__device__ __forceinline__ double ct_block_sum(float v[64], float (*red)[64]) {
+  static_assert(CT_NRED <= 64, "");
   const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
 #pragma unroll
-  for (int k = 0; k < CT_NRED; k++) {
-    float a = v[k];
-    a += __shfl_xor_sync(0xffffffffu, a, 16);
-    a += __shfl_xor_sync(0xffffffffu, a, 8);
-    a += __shfl_xor_sync(0xffffffffu, a, 4);
-    a += __shfl_xor_sync(0xffffffffu, a, 2);
-    a += __shfl_xor_sync(0xffffffffu, a, 1);
-    if (lane == 0) s_red[warp][k] = a;
+  for (int st = 0; st < 5; st++) {
+    const int hstep = 32 >> st, m = 16 >> st;
+    const bool up = (lane & m) != 0;
+#pragma unroll
+    for (int k = 0; k < 32; k++)
+      if (k < hstep) v[k] = (up ? v[k + hstep] : v[k]) + __shfl_xor_sync(0xffffffffu, up ? v[k] : v[k + hstep], m);
   }
+  red[warp][2 * lane] = v[0];
+  red[warp][2 * lane + 1] = v[1];
   __syncthreads();
-  double s = 0.0;
+  double sm = 0.0;
   if (threadIdx.x < CT_NRED) {
 #pragma unroll
-    for (int wv = 0; wv < CT_THREADS / 32; wv++) s += (double)s_red[wv][threadIdx.x];
+    for (int wv = 0; wv < NW; wv++) sm += (double)red[wv][threadIdx.x];
   }
-  return s;
+  return sm;
 }
 
 // fold of the per-CTA fp64 partials in a FIXED order with the loads in flight together: thread (q, k) adds quarter q of the CTAs for
@@ -153,10 +159,12 @@ __global__ void __launch_bounds__(CT_THREADS) ct_res_gs_kernel(CTParams P, const
                                                                const float4* __restrict__ img, double* __restrict__ partial,
                                                                unsigned int* __restrict__ ticket, double* __restrict__ out) {
   const int i = blockIdx.x * blockDim.x + threadIdx.x;
-  float v[CT_NRED];
-  ct_eval_point(P, i, pc_u, pc_v, pc_id, pc_col, img, v);
-  __shared__ float s_red[CT_THREADS / 32][CT_NRED];
-  const double bs = ct_block_reduce(v, s_red);
+  float v[64];
+#pragma unroll
+  for (int k = 0; k < 64; k++) v[k] = 0.f;
+  if (i < P.n) ct_eval_accumulate<false>(P, i, pc_u[i], pc_v[i], pc_id[i], pc_col[i], img, nullptr, v);
+  __shared__ float s_red[CT_THREADS / 32][64];
+  const double bs = ct_block_sum<CT_THREADS / 32>(v, s_red);
   if (threadIdx.x < CT_NRED) partial[(size_t)blockIdx.x * CT_NRED + threadIdx.x] = bs;
   // ---- last block folds the per-block partials in block order
   __shared__ bool s_last;
@@ -179,16 +187,16 @@ __global__ void __launch_bounds__(CT_THREADS) ct_res_gs_kernel(CTParams P, const
 }
 
 // ---------------------------------------------------------------------------------------------------------------------
-// ct_track_kernel — CoarseTracker::trackNewestCoarse (CoarseTracker.cpp:L539-770, visual-only branch L639-683) as ONE persistent
-// launch: the Levenberg-Marquardt loop over all pyramid levels runs on the device.  G = ceil(max_l n_l / 256) co-resident CTAs
-// (cooperative launch); one evaluation = every CTA evaluates its points (calcRes + calcGSSSE row, as ct_res_gs_kernel), per-CTA
-// fp64 partials, a grid barrier, then EVERY CTA folds the partials in CTA order and its thread 0 advances the same scalar state
-// machine in double (8x8 LDLT, SE3 exp, accept/reject, level schedule) - identical inputs, identical decisions, so no second
-// barrier and no broadcast.  Replaces ~21 launch + sync round trips per frame by one launch.
+// The state machine of CoarseTracker::trackNewestCoarse (CoarseTracker.cpp:L539-770, visual-only branch L639-683), which lets
+// ct_track_cluster_kernel run the whole Levenberg-Marquardt loop over all pyramid levels in ONE launch instead of ~21 launch + sync
+// round trips per frame.  CTTrack holds the launch's inputs; CTLM is the scalar state, one copy per CTA in shared memory.  After each
+// evaluation every CTA holds the same folded sums, and warp 0 advances its copy in double (ct_advance_warp: accept/reject, level
+// schedule, damped 8x8 system, LDL^T, SE3 exp, the operands of the next evaluation).  Identical inputs give identical decisions in every
+// CTA, so no broadcast is needed.
 // ---------------------------------------------------------------------------------------------------------------------
 constexpr int CT_L = DMV_MAX_PYR_LEVELS;
 struct CTTrack {
-  int levels, coarsest, G;
+  int levels, coarsest;
   int n[CT_L], w[CT_L], h[CT_L];
   float fx[CT_L], fy[CT_L], cx[CT_L], cy[CT_L];
   float Ki[CT_L][9];
@@ -199,10 +207,8 @@ struct CTTrack {
   float ref_exposure, new_exposure;
   float huber, cutoffTH, affModeA, affModeB;
   double minRes[5];
-  int staged[CT_L];              // ct_track_cluster_kernel: level l's plane is TMA-staged (ct_make_tensor_maps encoded its map)
-  double* partial;               // [2][G][CT_NRED]
-  unsigned int* bar;             // monotonic arrival counter, zero at launch
-  double* out;                   // pinned host: R[9] t[3] a b lastResiduals[5] flow[3] good iterations evaluations status
+  int staged[CT_L];              // level l's plane is TMA-staged (ct_make_tensor_maps encoded its map)
+  double* out;                  // pinned host: R[9] t[3] a b lastResiduals[5] flow[3] good iterations evaluations status
 };
 
 struct CTLM {  // the scalar state of trackNewestCoarse, one copy per CTA (shared memory), advanced by thread 0
@@ -221,14 +227,6 @@ struct CTLM {  // the scalar state of trackNewestCoarse, one copy per CTA (share
 };
 enum { CT_PH_INIT = 0, CT_PH_LM = 1 };
 
-// Hl.ldlt().solve(-b) for the 8x8 system (L639-665): plain LDL^T (ct_factor_warp / ct_propose_post below).  A parameter that is not
-// optimised (setting_affineOptModeA/B < 0: the reference solves the 6x6 / 7x7 sub-system) is padded with an identity row/column and a zero
-// right-hand side: the extra terms are exact zeros, the other components come out bit-identical.
-// operands of calcRes for a pose (CoarseTracker.cpp:L377-379): RKi = R.cast<float>() * Ki[lvl], t.cast<float>(), affLL.cast<float>()
-__device__ __forceinline__ void ct_request(const CTTrack& T, CTLM& S, const double R[9], const double t[3], double a, double b) {
-  (void)T; (void)R; (void)t; (void)a; (void)b;
-  S.need_request = 1;   // evaluate at the current pose: the warp forms the operands (ct_pose_request_warp)
-}
 // Vec6 of calcRes (L508-516) and H, b of calcGSSSE (L341-355) from the 53 folded sums, one output per thread (tid < 78)
 __device__ __forceinline__ void ct_finish_parallel(const double* o, double* res6, double* H, double* b, int tid) {
   const int npad = ((int)o[48] + 3) & ~3;
@@ -256,9 +254,12 @@ __device__ __forceinline__ void ct_finish_parallel(const double* o, double* res6
 __device__ void ct_begin_level(const CTTrack& T, CTLM& S) {
   S.rep = 1.f;
   S.phase = CT_PH_INIT;
-  ct_request(T, S, S.R, S.t, S.a, S.b);
+  S.need_request = 1;   // evaluate at the current pose
 }
-// one LM trial step from the current linearisation (L605-683), in three parts: lane 0 sets up the damped system, the WARP factorises it
+// Hl.ldlt().solve(-b) for the 8x8 system (L639-665): plain LDL^T (ct_factor_warp / ct_propose_post below).  A parameter that is not
+// optimised (setting_affineOptModeA/B < 0: the reference solves the 6x6 / 7x7 sub-system) is padded with an identity row/column and a zero
+// right-hand side: the extra terms are exact zeros, the other components come out bit-identical.
+// one LM trial step from the current linearisation (L605-683), in three parts: the warp sets up the damped system and factorises it
 // (row i of L in lane i: the 8^3/3 multiply-adds and the 28 divisions of the scalar version collapse to 8 dependent column steps), lane 0
 // substitutes and updates the pose.  Every element sees the same operations in the same order as the scalar LDL^T: bit-identical result.
 __device__ void ct_propose_pre(const CTTrack& T, CTLM& S) {  // lane 0: bookkeeping only; the damped system is built by the warp (ct_build_system_warp)
@@ -354,8 +355,8 @@ __device__ void ct_propose_post(const CTTrack& T, CTLM& S) {
   S.need_solve = 0;
   S.need_request = 2;   // evaluate at the candidate exp(incs) * (R, t)
 }
-// SE3::exp(incs) * (R, t) -> (Rn, tn) and the operands of the next calcRes, spread over the lanes of warp 0: every output element is formed
-// by exactly the expression of the scalar code (ct_se3_exp_mul / ct_request), only by a different lane.
+// SE3::exp(incs) * (R, t) -> (Rn, tn) and the operands of the next calcRes, spread over the lanes of warp 0: each lane forms one output
+// element with the same expression in double a single thread would use.
 __device__ __forceinline__ void ct_pose_request_warp(const CTTrack& T, CTLM& S, const bool from_candidate) {
   const int lane = threadIdx.x & 31;
   if (from_candidate) {
@@ -406,8 +407,6 @@ __device__ __forceinline__ void ct_pose_request_warp(const CTTrack& T, CTLM& S, 
     S.pevals += (double)T.n[S.lvl];
   }
 }
-// the scalar state machine step, executed by warp 0 of every CTA
-__device__ __forceinline__ void ct_advance_warp(const CTTrack& T, CTLM& S);
 __device__ void ct_end_level(const CTTrack& T, CTLM& S) {  // L722-745
   const int lvl = S.lvl;
   const double* resOld = S.res[S.cur];
@@ -438,7 +437,7 @@ __device__ void ct_advance(const CTTrack& T, CTLM& S) {
   const double* res = S.res[nw];
   if (S.phase == CT_PH_INIT) {  // L566-578: first evaluation of a level, cutoff doubling while too many residuals saturate
     S.cur = nw;                 // this evaluation becomes the current linearisation (resOld, H, b)
-    if (res[5] > 0.6 && (S.rep < 50 || res[5] > 0.99)) { S.rep *= 2; ct_request(T, S, S.R, S.t, S.a, S.b); return; }
+    if (res[5] > 0.6 && (S.rep < 50 || res[5] > 0.99)) { S.rep *= 2; S.need_request = 1; return; }
     S.lambda = 0.01f;
     S.iteration = 0;
     if (S.iteration >= maxIterations[S.lvl]) { ct_end_level(T, S); return; }
@@ -465,6 +464,7 @@ __device__ void ct_advance(const CTTrack& T, CTLM& S) {
   if (!(incNorm > 1e-3) || S.iteration >= maxIterations[S.lvl]) { ct_end_level(T, S); return; }
   ct_propose_pre(T, S);
 }
+// one step of the state machine, executed by warp 0 of every CTA
 __device__ __forceinline__ void ct_advance_warp(const CTTrack& T, CTLM& S) {
   const int lane = threadIdx.x & 31;
   if (lane == 0) { S.need_request = 0; ct_advance(T, S); }
@@ -480,91 +480,15 @@ __device__ __forceinline__ void ct_advance_warp(const CTTrack& T, CTLM& S) {
   if (S.need_request) ct_pose_request_warp(T, S, S.need_request == 2);
 }
 
-__global__ void __launch_bounds__(CT_THREADS) ct_track_kernel(const __grid_constant__ CTTrack T) {
-  __shared__ float s_red[CT_THREADS / 32][CT_NRED];
-  __shared__ double s_sum[CT_NRED];
-  __shared__ double s_q[4][CT_NRED];
-  __shared__ CTLM S;
-  const int tid = threadIdx.x;
-  const int G = T.G;
-  unsigned int epoch = 0;
-  int par = 0;
-  if (tid == 0) {
-    for (int i = 0; i < 9; i++) S.R[i] = T.R0[i];
-    for (int i = 0; i < 3; i++) S.t[i] = T.t0[i];
-    S.a = T.a0; S.b = T.b0;
-    for (int i = 0; i < 5; i++) S.lastResiduals[i] = __longlong_as_double(0x7ff8000000000000ll);  // NAN
-    for (int i = 0; i < 3; i++) S.flow[i] = 1000;
-    S.haveRepeated = 0; S.iterations = 0; S.evaluations = 0; S.done = 0; S.good = 0; S.status = 0; S.cur = 0; S.need_solve = 0; S.pevals = 0;
-    S.lvl = T.coarsest;
-    ct_begin_level(T, S);
-  }
-  __syncthreads();
-  if (tid < 32) ct_pose_request_warp(T, S, false);
-  __syncthreads();
-  while (!S.done) {
-    // ---- one evaluation: calcRes + calcGSSSE at the requested pose
-    CTParams P;
-    const int l = S.lvl;
-#pragma unroll
-    for (int i = 0; i < 9; i++) { P.RKi[i] = S.RKi[i]; P.Ki[i] = T.Ki[l][i]; }
-#pragma unroll
-    for (int i = 0; i < 3; i++) P.t[i] = S.tf[i];
-    P.fx = T.fx[l]; P.fy = T.fy[l]; P.cx = T.cx[l]; P.cy = T.cy[l];
-    P.affa = S.affLL[0]; P.affb = S.affLL[1]; P.a_gs = S.affLL[0]; P.b0 = (float)T.ref_b;
-    P.cutoff = S.cutoff; P.huber = T.huber; P.maxEnergy = 2 * T.huber * S.cutoff - T.huber * T.huber;
-    P.w = T.w[l]; P.h = T.h[l]; P.n = T.n[l]; P.lvl = l; P.want_gs = 1;
-    float v[CT_NRED];
-    ct_eval_point(P, blockIdx.x * CT_THREADS + tid, T.u[l], T.v[l], T.id[l], T.col[l], T.img[l], v);
-    const double bs = ct_block_reduce(v, s_red);
-    if (tid < CT_NRED) T.partial[((size_t)par * G + blockIdx.x) * CT_NRED + tid] = bs;
-    // ---- grid barrier (all G CTAs are co-resident: cooperative launch)
-    __syncthreads();
-    if (tid == 0) {
-      __threadfence();
-      epoch += (unsigned)G;
-      atomicAdd(T.bar, 1u);
-      unsigned long long t_start;
-      asm volatile("mov.u64 %0, %globaltimer;" : "=l"(t_start));
-      while (*((volatile unsigned int*)T.bar) < epoch) {
-        unsigned long long t_now;
-        asm volatile("mov.u64 %0, %globaltimer;" : "=l"(t_now));
-        if (t_now - t_start > 200000000ull) { S.done = 1; S.good = 0; S.status = 1; break; }  // 0.2 s: never hang the GPU on a lost CTA
-      }
-      __threadfence();
-    }
-    __syncthreads();
-    if (S.status == 1) break;
-    // ---- every CTA folds the partials in CTA order (bit-identical sums everywhere) and advances the same state machine
-    ct_fold(T.partial + (size_t)par * G * CT_NRED, G, s_q, s_sum);
-    par ^= 1;
-    __syncthreads();
-    ct_finish_parallel(s_sum, S.res[S.cur ^ 1], S.H[S.cur ^ 1], S.bb[S.cur ^ 1], tid);
-    __syncthreads();
-    if (tid < 32) ct_advance_warp(T, S);
-    __syncthreads();
-  }
-  if (blockIdx.x == 0 && tid == 0) {
-    double* o = T.out;
-    const bool ok = (S.status == 0);
-    for (int i = 0; i < 9; i++) o[i] = ok ? S.R[i] : T.R0[i];
-    for (int i = 0; i < 3; i++) o[9 + i] = ok ? S.t[i] : T.t0[i];
-    o[12] = ok ? S.a : T.a0; o[13] = ok ? S.b : T.b0;
-    for (int i = 0; i < 5; i++) o[14 + i] = S.lastResiduals[i];
-    for (int i = 0; i < 3; i++) o[19 + i] = S.flow[i];
-    o[22] = S.good; o[23] = S.iterations; o[24] = S.evaluations; o[25] = S.status; o[26] = S.pevals;
-  }
-}
-
 // ---------------------------------------------------------------------------------------------------------------------
-// ct_track_cluster_kernel — the same trackNewestCoarse state machine on ONE THREAD-BLOCK CLUSTER (sm_90+ hardware feature):
+// ct_track_cluster_kernel — the trackNewestCoarse state machine above on ONE THREAD-BLOCK CLUSTER (sm_90+ hardware feature):
 //   * the CTAs of the cluster exchange their fp64 partials through DISTRIBUTED SHARED MEMORY (st.shared::cluster into every peer's
 //     slot) and meet at the hardware cluster barrier (barrier.cluster.arrive/wait): no global-memory partials, no atomics, no spinning
-//     on an L2 counter — the per-evaluation synchronisation of the 39-CTA grid version (~4 us) shrinks to a few hundred ns;
+//     on an L2 counter — a few hundred ns per evaluation (~4 us through a chip-wide software grid barrier);
 //   * pyramid levels whose float4 plane fits in shared memory (80x60 at 640x480: 76.8 KB; 64x64 at 512^2; 40x30) are staged ONCE per
 //     level by TMA (cp.async.bulk.tensor.2d, multicast to every CTA of the cluster, completion on an mbarrier) and every Levenberg-
 //     Marquardt evaluation of that level gathers its 4 taps per point from shared memory instead of L2;
-//   * the block reduction of the 53 sums per point is a transposing butterfly (62 shuffles per warp instead of 265).
+//   * the block reduction of the 53 sums is ct_block_sum's transposing butterfly, as in ct_res_gs_kernel.
 // Every CTA folds the cluster's partials in rank order and advances the same scalar state machine: identical decisions everywhere.
 // A sequential LM chain is latency-bound: fewer, closer SMs with a hardware barrier beat a chip-wide software barrier (DESIGN.md §5).
 // ---------------------------------------------------------------------------------------------------------------------
@@ -590,81 +514,11 @@ __device__ __forceinline__ void ctc_cluster_sync() {
 }
 __device__ __forceinline__ unsigned ctc_smem_u32(const void* p) { return (unsigned)__cvta_generic_to_shared(p); }
 
-// one reference point against a plane in SHARED memory (same arithmetic as ct_eval_point; the taps come from the staged copy)
-template <bool SMEM>
-__device__ __forceinline__ void ctc_eval_accumulate(const CTParams& P, int i, const float x, const float y, const float id, const float refColor,
-                                                    const float4* __restrict__ img, const float4* plane_s, float v[CT_NRED]) {
-  const float p0 = P.RKi[0] * x + P.RKi[1] * y + P.RKi[2] + P.t[0] * id;
-  const float p1 = P.RKi[3] * x + P.RKi[4] * y + P.RKi[5] + P.t[1] * id;
-  const float p2 = P.RKi[6] * x + P.RKi[7] * y + P.RKi[8] + P.t[2] * id;
-  const float u = p0 / p2, vv = p1 / p2;
-  const float Ku = P.fx * u + P.cx, Kv = P.fy * vv + P.cy;
-  const float new_idepth = id / p2;
-  if (P.lvl == 0 && (i & 31) == 0) {  // flow indicators (CoarseTracker.cpp:L416-447)
-    const float k0 = P.Ki[0] * x + P.Ki[1] * y + P.Ki[2], k1 = P.Ki[3] * x + P.Ki[4] * y + P.Ki[5], k2 = P.Ki[6] * x + P.Ki[7] * y + P.Ki[8];
-    const float T0 = k0 + P.t[0] * id, T1 = k1 + P.t[1] * id, T2 = k2 + P.t[2] * id;
-    const float M0 = k0 - P.t[0] * id, M1 = k1 - P.t[1] * id, M2 = k2 - P.t[2] * id;
-    const float q0 = P.RKi[0] * x + P.RKi[1] * y + P.RKi[2] - P.t[0] * id;
-    const float q1 = P.RKi[3] * x + P.RKi[4] * y + P.RKi[5] - P.t[1] * id;
-    const float q2 = P.RKi[6] * x + P.RKi[7] * y + P.RKi[8] - P.t[2] * id;
-    const float KuT = P.fx * (T0 / T2) + P.cx, KvT = P.fy * (T1 / T2) + P.cy;
-    const float KuT2 = P.fx * (M0 / M2) + P.cx, KvT2 = P.fy * (M1 / M2) + P.cy;
-    const float Ku3 = P.fx * (q0 / q2) + P.cx, Kv3 = P.fy * (q1 / q2) + P.cy;
-    v[49] += (KuT - x) * (KuT - x) + (KvT - y) * (KvT - y) + (KuT2 - x) * (KuT2 - x) + (KvT2 - y) * (KvT2 - y);
-    v[50] += (Ku - x) * (Ku - x) + (Kv - y) * (Kv - y) + (Ku3 - x) * (Ku3 - x) + (Kv3 - y) * (Kv3 - y);
-    v[51] += 2.f;
-  }
-  if (Ku > 2.f && Kv > 2.f && Ku < (float)(P.w - 3) && Kv < (float)(P.h - 3) && new_idepth > 0.f) {
-    const int ix = (int)Ku, iy = (int)Kv;
-    const float dx = Ku - ix, dy = Kv - iy, dxdy = dx * dy;
-    float4 tl, tr, bl, br;
-    if constexpr (SMEM) {
-      const float4* bp = plane_s + iy * P.w + ix;
-      tl = bp[0]; tr = bp[1]; bl = bp[P.w]; br = bp[P.w + 1];
-    } else {
-      const float4* bp = img + (size_t)iy * P.w + ix;
-      tl = __ldg(bp); tr = __ldg(bp + 1); bl = __ldg(bp + P.w); br = __ldg(bp + P.w + 1);
-    }
-    const float w11 = dxdy, w10 = dy - dxdy, w01 = dx - dxdy, w00 = 1 - dx - dy + dxdy;
-    const float h0 = w11 * br.x + w10 * bl.x + w01 * tr.x + w00 * tl.x;
-    const float h1 = w11 * br.y + w10 * bl.y + w01 * tr.y + w00 * tl.y;
-    const float h2 = w11 * br.z + w10 * bl.z + w01 * tr.z + w00 * tl.z;
-    if (isfinite(h0)) {
-      const float residual = h0 - (P.affa * refColor + P.affb);
-      const float ar = fabsf(residual);
-      const float hw = ar < P.huber ? 1.f : P.huber / ar;
-      if (ar > P.cutoff) {
-        v[45] += P.maxEnergy; v[46] += 1.f; v[47] += 1.f;
-      } else {
-        v[45] += hw * residual * residual * (2.f - hw); v[46] += 1.f; v[48] += 1.f;
-        const float gx = h1 * P.fx, gy = h2 * P.fy;
-        float J[9];
-        J[0] = new_idepth * gx;
-        J[1] = new_idepth * gy;
-        J[2] = 0.f - new_idepth * (u * gx + vv * gy);
-        J[3] = 0.f - ((u * vv) * gx + gy * (1.f + vv * vv));
-        J[4] = (u * vv) * gy + gx * (1.f + u * u);
-        J[5] = u * gy - vv * gx;
-        J[6] = P.a_gs * (P.b0 - refColor);
-        J[7] = -1.f;
-        J[8] = residual;
-        int e = 0;
-#pragma unroll
-        for (int r = 0; r < 9; r++) {
-          const float Jw = J[r] * hw;
-#pragma unroll
-          for (int c = r; c < 9; c++) v[e++] += Jw * J[c];
-        }
-      }
-    }
-  }
-}
-
 __global__ void __launch_bounds__(CTC_THREADS, 1) ct_track_cluster_kernel(const __grid_constant__ CTTrack T, const __grid_constant__ CTMaps maps) {
   extern __shared__ __align__(128) unsigned char ctc_raw[];
   CTCSmem& M = *reinterpret_cast<CTCSmem*>(ctc_raw);
   CTLM& S = M.S;
-  const int tid = threadIdx.x, lane = tid & 31, warp = tid >> 5;
+  const int tid = threadIdx.x;
   const unsigned rank = ctc_rank(), NC = ctc_size();
   int par = 0, staged_lvl = -1, cached_lvl = -1;
   unsigned mphase = 0;
@@ -737,40 +591,22 @@ __global__ void __launch_bounds__(CTC_THREADS, 1) ct_track_cluster_kernel(const 
     for (int k = 0; k < CTC_SLOTS; k++) {
       const int i = first + k * stride;
       if (i < P.n) {
-        if (fits) ctc_eval_accumulate<true>(P, i, pts[k].x, pts[k].y, pts[k].z, pts[k].w, T.img[l], reinterpret_cast<const float4*>(M.plane), v);
-        else ctc_eval_accumulate<false>(P, i, pts[k].x, pts[k].y, pts[k].z, pts[k].w, T.img[l], nullptr, v);
+        if (fits) ct_eval_accumulate<true>(P, i, pts[k].x, pts[k].y, pts[k].z, pts[k].w, T.img[l], reinterpret_cast<const float4*>(M.plane), v);
+        else ct_eval_accumulate<false>(P, i, pts[k].x, pts[k].y, pts[k].z, pts[k].w, T.img[l], nullptr, v);
       }
     }
     for (int i = first + CTC_SLOTS * stride; i < P.n; i += stride) {  // more points than register slots: stream the rest
-      if (fits) ctc_eval_accumulate<true>(P, i, __ldg(T.u[l] + i), __ldg(T.v[l] + i), __ldg(T.id[l] + i), __ldg(T.col[l] + i), T.img[l], reinterpret_cast<const float4*>(M.plane), v);
-      else ctc_eval_accumulate<false>(P, i, __ldg(T.u[l] + i), __ldg(T.v[l] + i), __ldg(T.id[l] + i), __ldg(T.col[l] + i), T.img[l], nullptr, v);
+      if (fits) ct_eval_accumulate<true>(P, i, __ldg(T.u[l] + i), __ldg(T.v[l] + i), __ldg(T.id[l] + i), __ldg(T.col[l] + i), T.img[l], reinterpret_cast<const float4*>(M.plane), v);
+      else ct_eval_accumulate<false>(P, i, __ldg(T.u[l] + i), __ldg(T.v[l] + i), __ldg(T.id[l] + i), __ldg(T.col[l] + i), T.img[l], nullptr, v);
     }
-    // ---- warp: transposing butterfly, lane L ends with the warp sums of entries 2L, 2L+1
-    {
-      static_assert(CT_NRED <= 64, "");
-#pragma unroll
-      for (int st2 = 0; st2 < 5; st2++) {
-        const int hstep = 32 >> st2, m = 16 >> st2;
-        const bool up = (lane & m) != 0;
-#pragma unroll
-        for (int k = 0; k < 32; k++)
-          if (k < hstep) v[k] = (up ? v[k + hstep] : v[k]) + __shfl_xor_sync(0xffffffffu, up ? v[k] : v[k + hstep], m);
-      }
-      // entry index of v[k] in lane L: 32 b4 + 16 b3 + 8 b2 + 4 b1 + 2 b0 + k = 2 * bitrev-free L' ... = 2 L + k with L's bits in natural order
-      M.red[warp][2 * lane] = v[0];
-      M.red[warp][2 * lane + 1] = v[1];
-    }
-    __syncthreads();
     // ---- CTA: fp64 sum over the warps, pushed into EVERY CTA's exchange slot through distributed shared memory
+    const double bs = ct_block_sum<CTC_THREADS / 32>(v, M.red);
     if (tid < CT_NRED) {
-      double sm = 0.0;
-#pragma unroll
-      for (int wv = 0; wv < CTC_THREADS / 32; wv++) sm += (double)M.red[wv][tid];
       const unsigned local = ctc_smem_u32(&M.xch[par][rank][tid]);
       for (unsigned c = 0; c < NC; c++) {
         unsigned remote;
         asm volatile("mapa.shared::cluster.u32 %0, %1, %2;" : "=r"(remote) : "r"(local), "r"(c));
-        asm volatile("st.shared::cluster.f64 [%0], %1;" ::"r"(remote), "d"(sm) : "memory");
+        asm volatile("st.shared::cluster.f64 [%0], %1;" ::"r"(remote), "d"(bs) : "memory");
       }
     }
     ctc_cluster_sync();  // release / acquire at cluster scope: every CTA's partials are visible in every CTA's shared memory
@@ -789,7 +625,7 @@ __global__ void __launch_bounds__(CTC_THREADS, 1) ct_track_cluster_kernel(const 
   ctc_cluster_sync();  // nobody leaves while a peer may still write into its shared memory
   if (rank == 0 && tid == 0) {
     double* o = T.out;
-    const bool ok = (S.status == 0);   // an aborted track returns the input pose, like ct_track_kernel and the reference's early return
+    const bool ok = (S.status == 0);   // an aborted track returns the input pose, like the reference's early return
     for (int i = 0; i < 9; i++) o[i] = ok ? S.R[i] : T.R0[i];
     for (int i = 0; i < 3; i++) o[9 + i] = ok ? S.t[i] : T.t0[i];
     o[12] = ok ? S.a : T.a0; o[13] = ok ? S.b : T.b0;
@@ -845,7 +681,6 @@ struct dmv_ct {
   int n[DMV_MAX_PYR_LEVELS];
   double* d_partial = nullptr;
   unsigned int* d_ticket = nullptr;
-  unsigned int* d_bar = nullptr;   // grid-barrier counter of ct_track_kernel
   double* d_out = nullptr;
   double* h_out = nullptr;
   float* h_scratch = nullptr;
@@ -856,7 +691,7 @@ struct dmv_ct {
   float* h_ip = nullptr;
   int ip_cap = 0;
   float huber = 9.f;
-  int cluster_size = 0;        // CTAs of ct_track_cluster_kernel's cluster (0 = not probed yet, -1 = unavailable: grid version)
+  int cluster_size = 0;        // CTAs of ct_track_cluster_kernel's cluster (0 = not probed yet, -1 = none schedulable: dmv_ct_track fails)
   CTMaps* maps = nullptr;      // TMA descriptors of the level planes (host copy; passed as a kernel parameter)
   int staged[DMV_MAX_PYR_LEVELS] = {0};   // levels whose map ct_make_tensor_maps encoded: the only ones the cluster kernel stages
   long long launches = 0;
@@ -921,8 +756,7 @@ static int ct_allocate(dmv_ct* c, const dmv_ct_config* cfg) {
   const size_t npx0 = (size_t)cfg->w * cfg->h;
   CK(cudaMalloc(&c->d_stage, npx0 * 3 * sizeof(float)));
   const int maxBlocks = (cfg->max_points + CT_THREADS - 1) / CT_THREADS;
-  CK(cudaMalloc(&c->d_partial, sizeof(double) * CT_NRED * maxBlocks * 2));  // x2: ct_track_kernel double-buffers the per-CTA partials
-  CK(cudaMalloc(&c->d_bar, sizeof(unsigned int)));
+  CK(cudaMalloc(&c->d_partial, sizeof(double) * CT_NRED * maxBlocks));  // ct_res_gs_kernel's per-block partials
   CK(cudaMalloc(&c->d_ticket, sizeof(unsigned int)));
   CK(cudaMemset(c->d_ticket, 0, sizeof(unsigned int)));
   CK(cudaMalloc(&c->d_out, sizeof(double) * 64));
@@ -939,7 +773,7 @@ int dmv_ct_destroy(dmv_ct* c) {
   for (int l = 0; l < DMV_MAX_PYR_LEVELS; l++) {
     cudaFree(c->d_img[l]); cudaFree(c->d_gray[l]); cudaFree(c->d_u[l]); cudaFree(c->d_v[l]); cudaFree(c->d_id[l]); cudaFree(c->d_col[l]);
   }
-  cudaFree(c->d_stage); cudaFree(c->d_partial); cudaFree(c->d_ticket); cudaFree(c->d_bar); cudaFree(c->d_out);
+  cudaFree(c->d_stage); cudaFree(c->d_partial); cudaFree(c->d_ticket); cudaFree(c->d_out);
   cudaFreeHost(c->h_out); cudaFreeHost(c->h_scratch); cudaFree(c->d_ip); cudaFreeHost(c->h_ip);
   for (int l = 0; l < DMV_MAX_PYR_LEVELS; l++) { cudaFree(c->cd_idepth[l]); cudaFree(c->cd_ws[l]); cudaFree(c->cd_ws2[l]); }
   cudaFree(c->cd_rowcnt); cudaFree(c->cd_rowoff); cudaFreeHost(c->cd_totals);
@@ -1208,7 +1042,6 @@ int dmv_ct_track(dmv_ct* c, const dmv_ct_track_args* in, dmv_ct_track_result* ou
   CTTrack T;
   std::memset(&T, 0, sizeof(T));
   T.levels = c->cfg.levels; T.coarsest = in->coarsestLvl;
-  int maxn = 1;
   for (int l = 0; l < c->cfg.levels; l++) {
     if (!c->haveK[l]) return set_error(DMV_ERR_STATE, "dmv_ct_set_K(level) first");
     T.n[l] = c->n[l]; T.w[l] = c->w[l]; T.h[l] = c->h[l];
@@ -1216,29 +1049,24 @@ int dmv_ct_track(dmv_ct* c, const dmv_ct_track_args* in, dmv_ct_track_result* ou
     const float Kl[9] = {c->fx[l], 0.f, c->cx[l], 0.f, c->fy[l], c->cy[l], 0.f, 0.f, 1.f};
     inv3_cofactor(Kl, T.Ki[l]);
     T.u[l] = c->d_u[l]; T.v[l] = c->d_v[l]; T.id[l] = c->d_id[l]; T.col[l] = c->d_col[l]; T.img[l] = c->d_img[l];
-    if (l <= in->coarsestLvl) maxn = std::max(maxn, c->n[l]);
   }
-  T.G = (maxn + CT_THREADS - 1) / CT_THREADS;
-  int dev_sms = 0;
-  CK(cudaDeviceGetAttribute(&dev_sms, cudaDevAttrMultiProcessorCount, c->device));
   for (int i = 0; i < 9; i++) T.R0[i] = in->R[i];
   for (int i = 0; i < 3; i++) T.t0[i] = in->t[i];
   T.a0 = in->a; T.b0 = in->b; T.ref_a = in->ref_a; T.ref_b = in->ref_b;
   T.ref_exposure = in->ref_exposure; T.new_exposure = in->new_exposure;
   T.huber = c->huber; T.cutoffTH = in->coarseCutoffTH; T.affModeA = in->affineOptModeA; T.affModeB = in->affineOptModeB;
   for (int i = 0; i < 5; i++) T.minRes[i] = in->minResForAbort[i];
-  T.partial = c->d_partial; T.bar = c->d_bar; T.out = c->h_out;
+  T.out = c->h_out;
   if (c->cluster_size == 0) {  // probe once: the largest cluster the device schedules for this kernel (16 needs the non-portable opt-in)
     c->cluster_size = -1;
-    const char* env = getenv("DMV_CT_GRID");   // A/B switch: DMV_CT_GRID=1 keeps the chip-wide cooperative-grid version
-    // test hook: DMV_CT_CLUSTER=16|8|4 probes only that cluster size, and fails instead of falling back when it cannot be scheduled
+    // test hook: DMV_CT_CLUSTER=16|8|4 probes only that cluster size
     const char* env_nc = getenv("DMV_CT_CLUSTER");
     const int want_nc = env_nc ? atoi(env_nc) : 0;
     if (env_nc && want_nc != 16 && want_nc != 8 && want_nc != 4) {
       c->cluster_size = 0;
       return set_error(DMV_ERR_INVALID, "DMV_CT_CLUSTER=%s: expected 16, 8 or 4", env_nc);
     }
-    if (!(env && atoi(env) != 0) && ct_make_tensor_maps(c) == DMV_OK) {
+    if (ct_make_tensor_maps(c) == DMV_OK) {
       CK(cudaFuncSetAttribute(ct_track_cluster_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)sizeof(CTCSmem)));
       cudaFuncSetAttribute(ct_track_cluster_kernel, cudaFuncAttributeNonPortableClusterSizeAllowed, 1);
       cudaGetLastError();
@@ -1254,25 +1082,21 @@ int dmv_ct_track(dmv_ct* c, const dmv_ct_track_args* in, dmv_ct_track_result* ou
         cudaGetLastError();
       }
     }
-    if (want_nc && c->cluster_size != want_nc && !(env && atoi(env) != 0)) {
+    if (want_nc && c->cluster_size != want_nc) {
       c->cluster_size = 0;
       return set_error(DMV_ERR_INVALID, "DMV_CT_CLUSTER=%d: ct_track_cluster_kernel cannot be scheduled with that cluster size", want_nc);
     }
   }
-  if (c->cluster_size > 0) {
-    for (int l = 0; l < DMV_MAX_PYR_LEVELS; l++) T.staged[l] = c->staged[l];
-    cudaLaunchConfig_t cfg = {};
-    cfg.gridDim = dim3(c->cluster_size); cfg.blockDim = dim3(CTC_THREADS); cfg.dynamicSmemBytes = sizeof(CTCSmem); cfg.stream = c->stream;
-    cudaLaunchAttribute at[1];
-    at[0].id = cudaLaunchAttributeClusterDimension; at[0].val.clusterDim.x = c->cluster_size; at[0].val.clusterDim.y = 1; at[0].val.clusterDim.z = 1;
-    cfg.attrs = at; cfg.numAttrs = 1;
-    CK(cudaLaunchKernelEx(&cfg, ct_track_cluster_kernel, T, *c->maps));
-  } else {
-    if (T.G > dev_sms) return set_error(DMV_ERR_INVALID, "%d reference points need %d co-resident CTAs, the device has %d SMs: use dmv_ct_calc_res_gs", maxn, T.G, dev_sms);
-    CK(cudaMemsetAsync(c->d_bar, 0, sizeof(unsigned int), c->stream));
-    void* args[] = {&T};
-    CK(cudaLaunchCooperativeKernel((void*)ct_track_kernel, dim3(T.G), dim3(CT_THREADS), args, 0, c->stream));  // co-residency of all CTAs guaranteed
-  }
+  if (c->cluster_size < 0)
+    return set_error(DMV_ERR_INVALID, "dmv_ct_track needs a thread-block cluster of 16, 8 or 4 CTAs and TMA tensor maps, which this device "
+                                      "cannot provide: drive dmv_ct_calc_res_gs from the host LM loop instead");
+  for (int l = 0; l < DMV_MAX_PYR_LEVELS; l++) T.staged[l] = c->staged[l];
+  cudaLaunchConfig_t cfg = {};
+  cfg.gridDim = dim3(c->cluster_size); cfg.blockDim = dim3(CTC_THREADS); cfg.dynamicSmemBytes = sizeof(CTCSmem); cfg.stream = c->stream;
+  cudaLaunchAttribute at[1];
+  at[0].id = cudaLaunchAttributeClusterDimension; at[0].val.clusterDim.x = c->cluster_size; at[0].val.clusterDim.y = 1; at[0].val.clusterDim.z = 1;
+  cfg.attrs = at; cfg.numAttrs = 1;
+  CK(cudaLaunchKernelEx(&cfg, ct_track_cluster_kernel, T, *c->maps));
   c->launches++;
   CK(cudaStreamSynchronize(c->stream));
   c->staging_busy = false;
@@ -1283,7 +1107,6 @@ int dmv_ct_track(dmv_ct* c, const dmv_ct_track_args* in, dmv_ct_track_result* ou
   for (int i = 0; i < 5; i++) out->lastResiduals[i] = o[14 + i];
   for (int i = 0; i < 3; i++) out->flowIndicators[i] = o[19 + i];
   out->trackingGood = (int)o[22]; out->iterations = (int)o[23]; out->evaluations = (int)o[24]; out->status = (int)o[25];
-  if (out->status == 1) return set_error(DMV_ERR_CUDA, "ct_track_kernel: grid barrier timed out");
   return DMV_OK;
 }
 

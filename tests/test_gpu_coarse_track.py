@@ -1,6 +1,7 @@
-"""dmv_ct_track (trackNewestCoarse in one launch) against the fp64 reference in helpers.py (calc_res_ref / track_ref), in all four
-configurations: ct_track_cluster_kernel with clusters of 16, 8 and 4 CTAs (DMV_CT_CLUSTER) and the cooperative-grid ct_track_kernel
-(DMV_CT_GRID=1).  The environment is read when a handle first tracks, so every test builds a fresh handle after setting it.
+"""dmv_ct_track (trackNewestCoarse in one launch) against the fp64 reference in helpers.py (calc_res_ref / track_ref), in four
+configurations of ct_track_cluster_kernel: clusters of 16, 8 and 4 CTAs forced by the DMV_CT_CLUSTER test hook, and "default", the
+hook unset, where the handle probes 16, 8 and 4 as it does for a user.  The environment is read when a handle first tracks, so every test
+builds a fresh handle after setting it.
 
 Bounds: calc_res_ref's first-order fp32 bound (see its docstring).  It decides every saturation, incNorm and abort test of the scenes, but
 not the accept tests at the end of an LM level (energy ratios within 1e-3 of 1 against bounds of 1e-3 to 1e-2), so no scene is decidable in
@@ -14,7 +15,7 @@ import helpers as H
 
 pytestmark = pytest.mark.gpu
 
-CONFIGS = ["nc16", "nc8", "nc4", "grid"]
+CONFIGS = ["nc16", "nc8", "nc4", "default"]
 TRAJ = ["bench", "aff_free", "aff_fixA", "aff_fixB", "aff_fixAB", "tma0_80x60", "tma0_160x120", "limit", "odd", "stream", "repeat"]
 LINEAR = TRAJ + ["wide", "counts_1", "counts_31", "counts_513"]
 _SC, _REF = {}, {}
@@ -48,11 +49,8 @@ def ref(sc):
 
 
 def handle(capi, sc, cfg, monkeypatch, pts=None):
-    monkeypatch.delenv("DMV_CT_GRID", raising=False)
     monkeypatch.delenv("DMV_CT_CLUSTER", raising=False)
-    if cfg == "grid":
-        monkeypatch.setenv("DMV_CT_GRID", "1")
-    else:
+    if cfg != "default":
         monkeypatch.setenv("DMV_CT_CLUSTER", cfg[2:])
     pts = sc["pts"] if pts is None else pts
     g = capi.CT(sc["w"], sc["h"], sc["levels"], max_points=max(65536, max(len(p["u"]) for p in pts)))
@@ -125,10 +123,15 @@ def test_track_against_fp64_reference(capi, orc, synth, monkeypatch, name, cfg):
     g.close()
 
 
+HOST_LOOP = ["bench", "tma0_80x60", "tma0_160x120", "limit", "odd", "repeat"]
+
+
 @pytest.mark.parametrize("name", LINEAR)
 def test_configurations_agree_with_each_other(capi, orc, synth, monkeypatch, name):
-    """check 3: the four kernels give the same counts, and so does the host-loop adapter on the bench scene.  The grid kernel gathers every
-    level from L2, so on odd, wide and the tma0 scenes this also compares the staged planes with the unstaged ones."""
+    """check 3: the four configurations give the same counts, and so does the host-loop adapter (hostapi.CoarseTracker, device_lm=False)
+    on the HOST_LOOP scenes: those built from makeCoarseDepthL0 with the adapter's photometric and affine settings (the aff_* scenes
+    change them).  The host loop evaluates with ct_res_gs_kernel, which gathers every level
+    from L2, so on the tma0, limit and odd scenes this also compares the TMA-staged planes with the unstaged ones."""
     sc = scene(orc, synth, name)
     rs = []
     for cfg in CONFIGS:
@@ -138,13 +141,13 @@ def test_configurations_agree_with_each_other(capi, orc, synth, monkeypatch, nam
     for r in rs[1:]:
         for k in ("iterations", "evaluations", "good", "status"):
             assert r[k] == rs[0][k], (k, [x[k] for x in rs])
-    if name == "bench":
+    if name in HOST_LOOP:
         import dmvio_b200.hostapi as hostapi
-        T = sc["T"]
+        T, a = sc["T"], sc["args"]
         h = hostapi.CoarseTracker(T["w"], T["h"], T["K"], sc["levels"])
         h.set_ref(T["Ku"], T["Kv"], T["new_idepth"], T["HdiF"], T["pyr_ref"])
         h.set_new_image(T["img_new"])
-        rh = h.track(np.eye(3), np.zeros(3), 0.0, 0.0, device_lm=False)
+        rh = h.track(a["R0"], a["t0"], a["a0"], a["b0"], device_lm=False)
         assert rh["iterations"] == rs[0]["iterations"] and rh["evaluations"] == rs[0]["evaluations"] and rh["good"] == bool(rs[0]["good"])
         h.close()
 
@@ -204,18 +207,14 @@ def test_abort_contract(capi, orc, synth, monkeypatch, cfg, name, where):
     g.close()
 
 
-def test_grid_limit(capi, orc, synth, monkeypatch):
-    """check 6: more than #SMs*256 points on a level is DMV_ERR_INVALID on the grid kernel; the cluster kernel tracks it"""
+def test_more_points_than_one_wave_of_ctas(capi, orc, synth, monkeypatch):
+    """check 6: a level of #SMs*256 + 1 points, more than one 256-point CTA per SM would cover, is tracked by a cluster of 16"""
     import torch
     n = torch.cuda.get_device_properties(0).multi_processor_count * 256 + 1
     sc = H.ct_scene(orc, synth, "points_big", npts=n)
-    g = handle(capi, sc, "grid", monkeypatch)
-    with pytest.raises(capi.DmvError):
-        track(g, sc)
-    g.close()
     g = handle(capi, sc, "nc16", monkeypatch)
     r = track(g, sc)
-    check_final_linearisation(sc, r, level0_rep(H.ct_track_ref(sc)["log"]), "grid-limit nc16")
+    check_final_linearisation(sc, r, level0_rep(H.ct_track_ref(sc)["log"]), "points_big nc16")
     g.close()
 
 
