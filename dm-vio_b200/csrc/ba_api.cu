@@ -42,6 +42,7 @@ int dmv_ba_fill_descriptor(dmv_ba* b) {
   W.c_st = b->d_st_new[c2]; W.c_jpjd = b->d_jpjd[c2]; W.c_pout = b->d_pout[c2];
   W.step = b->d_step;
   W.part = b->d_part; W.wg = b->d_wg; W.hdig = b->d_hdig;
+  W.ditem = b->d_dtab; W.nditems = b->nditems;
   W.bar = b->d_bar;
   W.result = b->d_result[t];
   W.result_host = nullptr;
@@ -146,6 +147,7 @@ static int ba_allocate(dmv_ba* b, const dmv_ba_config* cfg) {
   CK(cudaMalloc(&b->d_step, sizeof(float) * mp));
   CK(cudaMemset(b->d_step, 0, sizeof(float) * mp));
   CK(cudaMalloc(&b->d_part, sizeof(double) * PART_STRIDE * (size_t)b->max_chunks));
+  CK(cudaMalloc(&b->d_dtab, sizeof(int4) * 2 * DITEMS_MAX));
   CK(cudaMalloc(&b->d_wg, sizeof(float4) * (size_t)maxT0 * mp));
   CK(cudaMalloc(&b->d_hdig, sizeof(float) * mp));
   CK(cudaMalloc(&b->d_hdi_solve, sizeof(float) * mp));
@@ -175,7 +177,7 @@ int dmv_ba_destroy(dmv_ba* b) {
     cudaFree(b->d_pout[k]); cudaFree(b->d_result[k]); cudaFreeHost(b->h_result[k]);
   }
   cudaFree(b->d_step); cudaFree(b->d_resub_sums); cudaFree(b->d_flush);
-  cudaFree(b->d_part); cudaFree(b->d_wg); cudaFree(b->d_hdig); cudaFree(b->d_hdi_solve); cudaFree(b->d_bar);
+  cudaFree(b->d_part); cudaFree(b->d_dtab); cudaFree(b->d_wg); cudaFree(b->d_hdig); cudaFree(b->d_hdi_solve); cudaFree(b->d_bar);
   cudaFreeHost(b->h_up); cudaFreeHost(b->h_adj); cudaFreeHost(b->h_scratch); cudaFreeHost(b->h_en_newest);
   for (int i = 0; i < 4; i++) if (b->ev[i]) cudaEventDestroy(b->ev[i]);
   if (b->nccl_comm) dmv::nccl_destroy(b->nccl_comm);
@@ -289,6 +291,35 @@ int dmv_ba_set_points(dmv_ba* b, int npts, const int32_t* host, const float* u, 
     b->nchunks = c;
   }
   if (b->nchunks > b->max_chunks) return set_error(DMV_ERR_INVALID, "too many chunks");
+  {  // phase D items of this window shape (ba_fused.cu: fused_reduce), uploaded ahead of the point data below
+    const int nf = b->nf, N = b->N, nch = b->nchunks;
+    const int* cb = b->chunk_beg;
+    std::vector<int4>& t = b->h_dtab;
+    t.clear();
+    // one offset over [lo, hi): split at DSEG chunks into the two segments of an item (the same partials, summed in the same order)
+    auto one = [&](int off, int d0, int d1, int lo, int hi) {
+      const int mid = std::min(hi, lo + DSEG);
+      t.push_back(make_int4(off, off, d0, d1));
+      t.push_back(make_int4(lo, mid, mid, hi));
+    };
+    for (int a = 0; a < nf; a++)  // off-diagonal blocks H[a, c], a < c: partials of host a's chunks (slot c), then of host c's (slot a)
+      for (int c = a + 1; c < nf; c++)
+        for (int ij = 0; ij < 64; ij++) {
+          const int i = ij >> 3, j = ij & 7;
+          t.push_back(make_int4(c * PART_SLOT + i * 8 + j, a * PART_SLOT + j * 8 + i, (4 + 8 * a + i) * N + 4 + 8 * c + j, (4 + 8 * c + j) * N + 4 + 8 * a + i));
+          t.push_back(make_int4(cb[a], cb[a + 1], cb[c], cb[c + 1]));
+        }
+    for (int a = 0; a < nf; a++)
+      for (int ij = 0; ij < 64; ij++) one(a * PART_SLOT + 64 + ij, (4 + 8 * a + (ij >> 3)) * N + 4 + 8 * a + (ij & 7), -1, 0, nch);
+    for (int a = 0; a < nf; a++)
+      for (int ic = 0; ic < 32; ic++) one(a * PART_SLOT + 128 + ic, (4 + 8 * a + (ic >> 2)) * N + (ic & 3), (ic & 3) * N + 4 + 8 * a + (ic >> 2), 0, nch);
+    for (int e = 0; e < nf * 8; e++) one((e >> 3) * PART_SLOT + 160 + (e & 7), N * N + 4 + e, -1, 0, nch);
+    for (int e = 0; e < 16; e++) one(PART_CC + e, (e >> 2) * N + (e & 3), -1, 0, nch);
+    for (int e = 0; e < 4; e++) one(PART_CC + 16 + e, N * N + e, -1, 0, nch);
+    for (int e = 0; e < ACC_MISC - 1; e++) one(PART_MISC + e, N * N + N + b->ntiles * 16 + e, -1, 0, nch);  // the error-flag slot is written on error only
+    b->nditems = (int)t.size() / 2;
+    CK(cudaMemcpyAsync(b->d_dtab, t.data(), sizeof(int4) * t.size(), cudaMemcpyHostToDevice, b->stream));
+  }
   // one pinned staging block, the copies queued back to back, ONE synchronisation (was: seven blocking copies from pageable memory)
   float* s = b->h_scratch;   // >= 8 * MAXF * mp floats
   const size_t n = (size_t)npts;

@@ -78,6 +78,7 @@ int dmv_ba_batch_gn_step(dmv_ba_batch* B, const double* const* x, const dmv_ba_s
     dmv_ba* b = B->h[i];
     if (b->P != B->P) return set_error(DMV_ERR_STATE, "window %d uses %d-point chunks, window 0 %d: create the handles of a batch with an explicit chunk_points", i, b->P, B->P);
     if (!st[i]) return set_error(DMV_ERR_INVALID, "state %d is null", i);
+    if (b->xchg_on) return set_error(DMV_ERR_STATE, "window %d is sharded with the in-kernel peer exchange: the batched kernel has none", i);
     if (b->npts < 1) return set_error(DMV_ERR_STATE, "window %d: points not set", i);
     if (!b->have_adj) return set_error(DMV_ERR_STATE, "window %d: dmv_ba_set_adjoints first", i);
     const double* xi = x ? x[i] : nullptr;

@@ -26,6 +26,11 @@ constexpr int PART_SLOT = 168;
 constexpr int PART_CC = MAXF * PART_SLOT;
 constexpr int PART_MISC = PART_CC + 20;
 constexpr int PART_STRIDE = PART_MISC + ACC_MISC;
+// Phase D of ba_fused_kernel: one item per result entry of H_top / b_top / the counters = the fixed-order sum over up to two chunk ranges
+// of one partial-blob offset each, written to d0 (and its mirror d1 >= 0).  A range of more than DSEG chunks is split at DSEG so that
+// the common case is one round trip of 2 x 6 loads per lane.
+constexpr int DSEG = 96;
+constexpr int DITEMS_MAX = MAXF * (MAXF - 1) / 2 * 64 + MAXF * (64 + 32 + 8) + 16 + 4 + (ACC_MISC - 1);
 
 // per-iteration parameter block
 struct BAIter {
@@ -97,6 +102,8 @@ struct BAWinDev {
   float* step;               // [p]
   // scratch of one launch (never read by the host)
   double* part;              // [chunk][PART_STRIDE] partial blobs
+  const int4* ditem;         // [nditems][2] phase D items of the window's shape (DItem, built by dmv_ba_set_points)
+  int nditems;
   float4* wg;                // [4-column group][mp] Schur vectors w_p, transposed
   float* hdig;               // [p] HdiF
   unsigned int* bar;         // grid-barrier arrival counter (monotonic)

@@ -839,14 +839,13 @@ __device__ __forceinline__ void fused_chunk(const BAWinDev& W, const BAIter& it,
     }
   }
   }
-  {  // counters: warp sums
-    float es = e_sum, fin = (float)n_in, foob = (float)n_oob, fout = (float)n_outl;
+  {  // counters: warp sums (the integer ones in one exact REDUX each)
+    float es = e_sum;
+    const float fin = (float)__reduce_add_sync(0xffffffffu, (unsigned)n_in), foob = (float)__reduce_add_sync(0xffffffffu, (unsigned)n_oob),
+                fout = (float)__reduce_add_sync(0xffffffffu, (unsigned)n_outl);
 #pragma unroll
     for (int m = 1; m < 32; m <<= 1) {
       es += __shfl_xor_sync(0xffffffffu, es, m);
-      fin += __shfl_xor_sync(0xffffffffu, fin, m);
-      foob += __shfl_xor_sync(0xffffffffu, foob, m);
-      fout += __shfl_xor_sync(0xffffffffu, fout, m);
       rs_step2 += __shfl_xor_sync(0xffffffffu, rs_step2, m);
       rs_nid += __shfl_xor_sync(0xffffffffu, rs_nid, m);
       rs_cnt += __shfl_xor_sync(0xffffffffu, rs_cnt, m);
@@ -1012,127 +1011,116 @@ __device__ __forceinline__ void fused_chunk(const BAWinDev& W, const BAIter& it,
   clk_stamp<CLK>(clk, 5);
 }
 
-// phases D / E for one window: the work is split over `ncta` CTAs, this one acting as CTA `vcta`
-template <int P, int LPR, bool CLK = false>
-__device__ __forceinline__ void fused_reduce(const BAWinDev& W, FusedSmem<P, LPR>& S, bool ok, const int vcta, const int ncta,
-                                             unsigned long long* clk = nullptr) {
-  const int nf = W.nf, N = W.N, mp = W.mp;
-  const int tid = threadIdx.x, nthreads = blockDim.x;
-  const int warp = tid >> 5, lane = tid & 31, nwarps = nthreads >> 5;
+// Two configurations: chunk_points = 16 -> (P = 16, LPR = 4): 448 threads, 4 lanes per residual (the latency-oriented default for ONE window);
+//                     chunk_points = 32 -> (P = 32, LPR = 1): 224 threads, one thread per residual (fewest instructions: batches / large windows)
+template <int P> struct FusedCfgOf { static constexpr int LPR = (P == 16) ? 4 : 1, TPB = (P == 16) ? 448 : 224; };
 
+// ---------------------------------------------------------------------------------------------------------------------------
+// phases D / E.  Everything below runs once per CTA behind the grid barrier, with a cold instruction cache: the code is kept short
+// (item table instead of a decode, the long-segment sum out of line, no exchange code unless XCH).
+// ---------------------------------------------------------------------------------------------------------------------------
+// phase D item (table built by dmv_ba_set_points): a = {off0, off1, d0, d1}, b = {lo0, hi0, lo1, hi1}: the entry is the sum of the partials
+// at offset off0 of chunks [lo0, hi0), then at off1 of chunks [lo1, hi1), written to d0 and, if d1 >= 0, to its mirror d1.  Past the end of
+// the table: empty ranges, nothing written.
+struct DItem { int4 a, b; };
+__device__ __forceinline__ DItem load_ditem(const BAWinDev& W, int item) {
+  DItem d{make_int4(0, 0, 0, -1), make_int4(0, 0, 0, 0)};
+  if (item < W.nditems) { d.a = __ldg(W.ditem + 2 * item); d.b = __ldg(W.ditem + 2 * item + 1); }
+  return d;
+}
+// the item of this thread's 16-lane group on phase D's first trip (items are dealt from the last CTA down): the kernel loads it before
+// the grid barrier, whose spin hides the load
+template <int P>
+__device__ __forceinline__ DItem first_ditem(const BAWinDev& W, int vcta, int ncta) {
+  return load_ditem(W, (ncta - 1 - vcta) * (FusedCfgOf<P>::TPB / 16) + (threadIdx.x >> 4));
+}
+// a segment of more than DSEG chunks (windows of more than ~1500 points per host frame): 12 partials per lane in flight per trip.  Every
+// lane adds its chunks lo + gl, lo + gl + 16, ... in ascending order, as the one-trip form does (the added zeros change no sum)
+__device__ __noinline__ double dsum_long(const double* __restrict__ part, const int4 a, const int4 b, const int gl) {
+  double sum = 0.0;
+#pragma unroll 1
+  for (int seg = 0; seg < 2; seg++) {
+    const int lo = seg ? b.z : b.x, hi = seg ? b.w : b.y;
+    const double* __restrict__ src = part + (seg ? a.y : a.x);
+#pragma unroll 1
+    for (int c0 = lo + gl; c0 < hi; c0 += 192) {
+      double v[12];
+#pragma unroll
+      for (int u = 0; u < 12; u++) v[u] = (c0 + 16 * u < hi) ? __ldcg(src + (size_t)(c0 + 16 * u) * PART_STRIDE) : 0.0;
+#pragma unroll
+      for (int u = 0; u < 12; u++) sum += v[u];
+    }
+  }
+  return sum;
+}
+
+// phases D / E for one window: the work is split over `ncta` CTAs, this one acting as CTA `vcta`; `it` = first_ditem(W, vcta, ncta).
+// XCH = true (sharded window, W.xc.nranks > 1): every result entry is also pushed to the peers and, after phase E, the peers' values are
+// pulled and added in rank order.
+template <int P, int LPR, bool CLK, bool XCH>
+__device__ __forceinline__ void fused_reduce(const BAWinDev& W, FusedSmem<P, LPR>& S, bool ok, const int vcta, const int ncta, DItem it,
+                                             unsigned long long* clk = nullptr) {
+  constexpr int NT = FusedCfgOf<P>::TPB, NWARPS = NT / 32, GPC = NT / 16;  // the launch's fixed block size
+  const int N = W.N, mp = W.mp;
+  const int tid = threadIdx.x, warp = tid >> 5, lane = tid & 31;
   const int nH = N * N + N;
   double* __restrict__ R = W.result;
   double* __restrict__ RH = W.result_host;
-  const bool xch = W.xc.nranks > 1;
   const double* __restrict__ part = W.part;
 
   // ---------------------------------------------------------------- phase D: H_top / b_top / counters, 16 lanes per result entry
-  // item list: [unordered frame pairs a<b: 64 entries each][diagonal blocks: nf x 64][H[.,C]: nf x 32][b: nf x 8][CC 16][bC 4][counters 7]
-  // Usually one pass over the items (16-lane groups in the grid >= items), every lane sums <= 12 chunk partials per segment whose loads
-  // are all in flight together, then a 4-step butterfly.  Fixed order => bit-reproducible.
-  const int npair = nf * (nf - 1) / 2;
-  const int n_off = npair * 64, n_diag = nf * 64, n_c = nf * 32, n_b = nf * 8;
-  const int nitems = n_off + n_diag + n_c + n_b + 16 + 4 + (ACC_MISC - 1);  // the last counter slot is the error flag: written on error only
-  const int grp = tid >> 4, gl = tid & 15, groups_per_cta = nthreads >> 4;
-  const int nch = W.nchunks;
-  // with the peer exchange on: pass 0 (sum + push) -> phase E (Gram tiles + push) -> pass 1 (pull) -> phase E pull: the NVLink round trip of
-  // the H_top entries overlaps the Gram computation
-  // items are dealt from the LAST CTA down: the first CTAs carry the second Schur tile of phase E (tile vcta + ncta), so the two tails
-  // land on different CTAs
+  // Usually one trip (16-lane groups in the grid >= items): every lane sums <= 12 chunk partials whose loads are all in flight together,
+  // then a 4-step butterfly.  Fixed order => bit-reproducible.  Items are dealt from the LAST CTA down: the first CTAs carry the second
+  // Schur tile of phase E (tile vcta + ncta), so the two tails land on different CTAs.
+  const int nitems = W.nditems, grp = tid >> 4, gl = tid & 15;
   const int dcta = ncta - 1 - vcta;
-  auto phase_d = [&](const int pass) {
-    for (int base = dcta * groups_per_cta; base < nitems; base += ncta * groups_per_cta) {  // CTA-uniform trip count (shuffles below)
-      const int item = base + grp;
-      const bool act = item < nitems;
-      // decode: up to two (offset, chunk range) segments and up to two destinations
-      int off0 = 0, lo0 = 0, hi0 = act ? nch : 0, off1 = 0, lo1 = 0, hi1 = 0, d0 = 0, d1 = -1;
-      int e = act ? item : nitems - 1;
-      if (e < n_off) {
-        const int q = e >> 6, ij = e & 63, i = ij >> 3, j = ij & 7;
-        int a = 0, rem = q;
-        while (rem >= nf - 1 - a) { rem -= nf - 1 - a; a++; }
-        const int b = a + 1 + rem;
-        off0 = b * PART_SLOT + i * 8 + j; lo0 = W.chunk_beg[a]; hi0 = act ? W.chunk_beg[a + 1] : lo0;
-        off1 = a * PART_SLOT + j * 8 + i; lo1 = W.chunk_beg[b]; hi1 = act ? W.chunk_beg[b + 1] : lo1;
-        d0 = (4 + 8 * a + i) * N + 4 + 8 * b + j; d1 = (4 + 8 * b + j) * N + 4 + 8 * a + i;
-      } else if ((e -= n_off) < n_diag) {
-        const int a = e >> 6, ij = e & 63;
-        off0 = a * PART_SLOT + 64 + ij;
-        d0 = (4 + 8 * a + (ij >> 3)) * N + 4 + 8 * a + (ij & 7);
-      } else if ((e -= n_diag) < n_c) {
-        const int a = e >> 5, ic = e & 31;
-        off0 = a * PART_SLOT + 128 + ic;
-        d0 = (4 + 8 * a + (ic >> 2)) * N + (ic & 3); d1 = (ic & 3) * N + 4 + 8 * a + (ic >> 2);
-      } else if ((e -= n_c) < n_b) {
-        off0 = (e >> 3) * PART_SLOT + 160 + (e & 7);
-        d0 = N * N + 4 + e;
-      } else if ((e -= n_b) < 16) {
-        off0 = PART_CC + e; d0 = (e >> 2) * N + (e & 3);
-      } else if ((e -= 16) < 4) {
-        off0 = PART_CC + 16 + e; d0 = N * N + e;
-      } else {
-        e -= 4;
-        off0 = PART_MISC + e; d0 = nH + W.ntiles * 16 + e;
-      }
-      if (pass == 0) {
-        double sum = 0.0;
-        if (hi0 - lo0 <= 96 && hi1 - lo1 <= 96) {  // both segments in one round trip: <= 6 partials per lane each, summed in the same order
-          double v[12];
-#pragma unroll
-          for (int u = 0; u < 12; u++) {
-            const int c = (u < 6 ? lo0 : lo1) + gl + 16 * (u % 6);
-            v[u] = (c < (u < 6 ? hi0 : hi1)) ? __ldcg(part + (u < 6 ? off0 : off1) + (size_t)c * PART_STRIDE) : 0.0;
-          }
-#pragma unroll
-          for (int u = 0; u < 12; u++) sum += v[u];
-        } else {
 #pragma unroll 1
-          for (int seg = 0; seg < 2; seg++) {
-            const int lo = seg ? lo1 : lo0, hi = seg ? hi1 : hi0;
-            const double* __restrict__ src = part + (seg ? off1 : off0);
-            for (int c0 = lo + gl; c0 < hi; c0 += 192) {
-              double v[12];
+  for (int base = dcta * GPC; base < nitems; base += ncta * GPC) {  // CTA-uniform trip count (shuffles below)
+    double sum = 0.0;
+    if (it.b.y - it.b.x <= DSEG && it.b.w - it.b.z <= DSEG) {  // both segments in one round trip: <= 6 partials per lane each
+      double v[12];
 #pragma unroll
-              for (int u = 0; u < 12; u++) v[u] = (c0 + 16 * u < hi) ? __ldcg(src + (size_t)(c0 + 16 * u) * PART_STRIDE) : 0.0;
-#pragma unroll
-              for (int u = 0; u < 12; u++) sum += v[u];
-            }
-          }
-        }
-        sum += __shfl_xor_sync(0xffffffffu, sum, 8);
-        sum += __shfl_xor_sync(0xffffffffu, sum, 4);
-        sum += __shfl_xor_sync(0xffffffffu, sum, 2);
-        sum += __shfl_xor_sync(0xffffffffu, sum, 1);
-        if (gl == 0 && act) {
-          if (xch) { R[d0] = sum; xchg_push(W.xc, d0, sum); }
-          else { R[d0] = sum; if (d1 >= 0) R[d1] = sum; if (RH) { RH[d0] = sum; if (d1 >= 0) RH[d1] = sum; } }
-        }
-      } else {  // warp-collective: both 16-lane groups of the warp wait together
-        const double sum = xchg_pull_sum_group(W.xc, d0, (gl == 0 && act) ? R[d0] : 0.0, act, ok);
-        if (gl == 0 && act) {
-          R[d0] = sum; if (d1 >= 0) R[d1] = sum;
-          if (RH) { RH[d0] = sum; if (d1 >= 0) RH[d1] = sum; }
-        }
+      for (int u = 0; u < 12; u++) {
+        const int c = (u < 6 ? it.b.x : it.b.z) + gl + 16 * (u % 6);
+        v[u] = (c < (u < 6 ? it.b.y : it.b.w)) ? __ldcg(part + (u < 6 ? it.a.x : it.a.y) + (size_t)c * PART_STRIDE) : 0.0;
       }
+#pragma unroll
+      for (int u = 0; u < 12; u++) sum += v[u];
+    } else {
+      sum = dsum_long(part, it.a, it.b, gl);
     }
-    };
-  phase_d(0);
+    sum += __shfl_xor_sync(0xffffffffu, sum, 8);
+    sum += __shfl_xor_sync(0xffffffffu, sum, 4);
+    sum += __shfl_xor_sync(0xffffffffu, sum, 2);
+    sum += __shfl_xor_sync(0xffffffffu, sum, 1);
+    if (gl == 0 && base + grp < nitems) {
+      const int d0 = it.a.z, d1 = it.a.w;
+      R[d0] = sum;
+      if constexpr (XCH) xchg_push(W.xc, d0, sum);
+      else { if (d1 >= 0) R[d1] = sum; if (RH) { RH[d0] = sum; if (d1 >= 0) RH[d1] = sum; } }
+    }
+    it = load_ditem(W, base + ncta * GPC + grp);
+  }
   clk_stamp<CLK>(clk, 7);
 
   // ---------------------------------------------------------------- phase E: [H_sc | b_sc] = sum_p HdiF w_p w_p^T as 4x4 tiles over ALL points
-  // of the window: a CTA takes tiles vcta, vcta + ncta (both in ONE pass over the points when the grid has fewer CTAs than tiles)
+  // of the window: a CTA takes tiles vcta, vcta + ncta (the second when the grid has fewer CTAs than tiles) in ONE pass over the points
   {
-    const int T = W.T, npts = W.npts;
-    for (int tile0 = vcta; tile0 < W.ntiles; tile0 += 2 * ncta) {
-      const int tile1 = tile0 + ncta;
-      const bool two = tile1 < W.ntiles;
-      int ti0 = 0, rem = tile0;
-      while (rem >= T - ti0) { rem -= T - ti0; ti0++; }
-      const int tj0 = ti0 + rem;
-      int ti1 = 0;
-      rem = two ? tile1 : tile0;
-      while (rem >= T - ti1) { rem -= T - ti1; ti1++; }
-      const int tj1 = ti1 + rem;
+    const int npts = W.npts, ntiles = W.ntiles, T = W.T;
+#pragma unroll 1
+    for (int tile0 = vcta; tile0 < ntiles; tile0 += 2 * ncta) {
+      const bool two = tile0 + ncta < ntiles;  // CTA-uniform
+      // (ti, tj) of tile t in the row-major upper triangle of T x T tiles: row i starts at off(i) = i T - i (i - 1) / 2
+      const float4* __restrict__ wt[2][2];
+#pragma unroll
+      for (int q = 0; q < 2; q++) {
+        const int t = two ? tile0 + q * ncta : tile0, T2 = 2 * T + 1;
+        int ti = (int)(0.5f * ((float)T2 - sqrtf((float)(T2 * T2 - 8 * t))));
+        ti -= (ti * T - ti * (ti - 1) / 2 > t) ? 1 : 0;           // the approximate square root: one step either way at most
+        ti += ((ti + 1) * T - (ti + 1) * ti / 2 <= t) ? 1 : 0;
+        wt[q][0] = W.wg + (size_t)ti * mp;
+        wt[q][1] = W.wg + (size_t)(ti + t - (ti * T - ti * (ti - 1) / 2)) * mp;
+      }
       float a[2][4][4];
 #pragma unroll
       for (int q = 0; q < 2; q++)
@@ -1140,14 +1128,12 @@ __device__ __forceinline__ void fused_reduce(const BAWinDev& W, FusedSmem<P, LPR
         for (int i = 0; i < 4; i++)
 #pragma unroll
           for (int j = 0; j < 4; j++) a[q][i][j] = 0.f;
-      const float4* __restrict__ wi0 = W.wg + (size_t)ti0 * mp;
-      const float4* __restrict__ wj0 = W.wg + (size_t)tj0 * mp;
-      const float4* __restrict__ wi1 = W.wg + (size_t)ti1 * mp;
-      const float4* __restrict__ wj1 = W.wg + (size_t)tj1 * mp;
+      // per-thread fp32 sums over p = tid, tid + NT, ...: both tiles in one pass, the loads of 4 points in flight (with 36 points per thread
+      // at 8000 points, fewer points in flight cost more latency than the shorter code saves)
 #pragma unroll 4
-      for (int p = tid; p < npts; p += nthreads) {
+      for (int p = tid; p < npts; p += (int)blockDim.x) {
         const float sc = __ldcg(W.hdig + p);
-        const float4 wi = __ldcg(wi0 + p), wj = __ldcg(wj0 + p);
+        const float4 wi = __ldcg(wt[0][0] + p), wj = __ldcg(wt[0][1] + p);
         const float si[4] = {sc * wi.x, sc * wi.y, sc * wi.z, sc * wi.w};
         const float vj[4] = {wj.x, wj.y, wj.z, wj.w};
 #pragma unroll
@@ -1155,7 +1141,7 @@ __device__ __forceinline__ void fused_reduce(const BAWinDev& W, FusedSmem<P, LPR
 #pragma unroll
           for (int j = 0; j < 4; j++) a[0][i][j] += si[i] * vj[j];
         if (two) {  // CTA-uniform
-          const float4 xi = __ldcg(wi1 + p), xj = __ldcg(wj1 + p);
+          const float4 xi = __ldcg(wt[1][0] + p), xj = __ldcg(wt[1][1] + p);
           const float ti[4] = {sc * xi.x, sc * xi.y, sc * xi.z, sc * xi.w};
           const float uj[4] = {xj.x, xj.y, xj.z, xj.w};
 #pragma unroll
@@ -1164,10 +1150,7 @@ __device__ __forceinline__ void fused_reduce(const BAWinDev& W, FusedSmem<P, LPR
             for (int j = 0; j < 4; j++) a[1][i][j] += ti[i] * uj[j];
         }
       }
-      // per-thread fp32 sums over <= npts / nthreads points; transposing warp butterfly in fp32 (31 exchanges for the 32 values: lane L ends with
-      // the warp's sum of value L over its <= 160 points; half the instructions of the fp64 form, and this straight-line code is fetched
-      // once per CTA, where instruction fetch is the stall), then fp64 across the warps in a fixed order through shared memory
-      {
+      {  // transposing warp butterfly in fp32 (31 exchanges for the 32 values: lane L ends with the warp's sum of value L)
         float d[32];
 #pragma unroll
         for (int qq = 0; qq < 2; qq++)
@@ -1184,24 +1167,36 @@ __device__ __forceinline__ void fused_reduce(const BAWinDev& W, FusedSmem<P, LPR
         S.red[warp][lane] = (double)d[0];   // lane L: value index 16 b4 + 8 b3 + 4 b2 + 2 b1 + b0 = L
       }
       __syncthreads();
-      if (tid < 32) {  // the whole first warp (the exchange below is warp-collective)
+      if (tid < 32) {  // the whole first warp (the exchange below is warp-collective): fp64 across the warps in a fixed order
         const bool own = tid < 16 || two;
-        double d = 0.0;
-        for (int wv = 0; wv < nwarps; wv++) d += S.red[wv][tid];
-        const int idx = nH + (tid < 16 ? tile0 : tile1) * 16 + (tid & 15);
+        double s = 0.0;
+#pragma unroll
+        for (int wv = 0; wv < NWARPS; wv++) s += S.red[wv][tid];
+        const int idx = nH + (tid < 16 ? tile0 : tile0 + ncta) * 16 + (tid & 15);
         if (own) {
-          R[idx] = d;
-          if (xch) xchg_push(W.xc, idx, d);
-          else if (RH) RH[idx] = d;
+          R[idx] = s;
+          if constexpr (XCH) xchg_push(W.xc, idx, s);
+          else if (RH) RH[idx] = s;
         }
       }
       __syncthreads();
     }
   }
   clk_stamp<CLK>(clk, 8);
-  if (xch) {
-    phase_d(1);
-    if (tid < 32) {  // pull of the Gram tiles: same (tile, lane) ownership as above, so R[idx] is this lane's own earlier store
+  if constexpr (XCH) {  // the peers' values: phase D entries, then the Gram tiles (their pushes overlapped the Gram computation)
+#pragma unroll 1
+    for (int base = dcta * GPC; base < nitems; base += ncta * GPC) {  // warp-collective: both 16-lane groups of the warp wait together
+      const bool act = base + grp < nitems;
+      const DItem e = load_ditem(W, base + grp);
+      const int d0 = e.a.z, d1 = e.a.w;
+      const double sum = xchg_pull_sum_group(W.xc, d0, (gl == 0 && act) ? R[d0] : 0.0, act, ok);
+      if (gl == 0 && act) {
+        R[d0] = sum; if (d1 >= 0) R[d1] = sum;
+        if (RH) { RH[d0] = sum; if (d1 >= 0) RH[d1] = sum; }
+      }
+    }
+    if (tid < 32) {  // same (tile, lane) ownership as above, so R[idx] is this lane's own earlier store
+#pragma unroll 1
       for (int tile0 = vcta; tile0 < W.ntiles; tile0 += 2 * ncta) {
         const int tile1 = tile0 + ncta;
         const bool own = tid < 16 || tile1 < W.ntiles;
@@ -1224,12 +1219,9 @@ __device__ __forceinline__ void fused_reduce(const BAWinDev& W, FusedSmem<P, LPR
 // residuals are re-linearised from scratch (PointFrameResidual::resetOOB; FullSystem.cpp:L826-838), EFResidual::fixLinearizationF
 // (EnergyFunctionalStructs.cpp:L88-114) turns resF into res_toZeroF, and the accumulation is AccumulatedTopHessian::addPoint<2> +
 // AccumulatedSCHessian::addPoint(p, shiftPriorToZero = false) with priorF * idepthFixPriorMargFac (EnergyFunctional.cpp:L678-742).
-// Two configurations: chunk_points = 16 -> (P = 16, LPR = 4): 448 threads, 4 lanes per residual (the latency-oriented default for ONE window);
-//                     chunk_points = 32 -> (P = 32, LPR = 1): 224 threads, one thread per residual (fewest instructions: batches / large windows)
-template <int P> struct FusedCfgOf { static constexpr int LPR = (P == 16) ? 4 : 1, TPB = (P == 16) ? 448 : 224; };
-
-// CLK = true: the phase clock (clk_stamp) into clk[gridDim.x][NCLK]; measurement only, launched by launch_fused_kernel_clocked alone
-template <int P, bool MARG, bool CLK = false>
+// The two chunk shapes: FusedCfgOf.  CLK = true: the phase clock (clk_stamp) into clk[gridDim.x][NCLK]; measurement only, launched by
+// launch_fused_kernel_clocked alone.  XCH = true: the sharded window's peer exchange (W.xc.nranks > 1); the single-GPU kernels carry none.
+template <int P, bool MARG, bool CLK, bool XCH>
 __global__ void __launch_bounds__(FusedCfgOf<P>::TPB, 1)
     ba_fused_kernel(const __grid_constant__ BAWinDev W, const __grid_constant__ BAIter it, unsigned long long* clk) {
   constexpr int LPR = FusedCfgOf<P>::LPR;
@@ -1238,14 +1230,16 @@ __global__ void __launch_bounds__(FusedCfgOf<P>::TPB, 1)
   clk_stamp<CLK>(clk, 0);
 #pragma unroll 1
   for (int chunk = blockIdx.x; chunk < W.nchunks; chunk += gridDim.x) fused_chunk<P, LPR, MARG, CLK>(W, it, S, chunk, clk);
+  const DItem d = first_ditem<P>(W, blockIdx.x, gridDim.x);
   const bool ok = grid_barrier(W.bar, W.bar_target);  // every chunk of the window is done
   clk_stamp<CLK>(clk, 6);
-  fused_reduce<P, LPR, CLK>(W, S, ok, blockIdx.x, gridDim.x, clk);
+  fused_reduce<P, LPR, CLK, XCH>(W, S, ok, blockIdx.x, gridDim.x, d, clk);
 }
 
 // Batched variant (SURVEY.md §8d): B independent windows in ONE launch.  Descriptors and per-iteration tables come from global memory;
 // work items = (window, chunk) pairs dealt round-robin to the resident CTAs; after the grid barrier every window's reduction is spread
-// over all CTAs, rotated per window so that the Schur tiles of different windows land on different CTAs.
+// over all CTAs, rotated per window so that the Schur tiles of different windows land on different CTAs.  Sharded windows are refused by
+// dmv_ba_batch_gn_step: no exchange code here.
 template <int P>
 __global__ void __launch_bounds__(FusedCfgOf<P>::TPB, P == 32 ? 2 : 1)
     ba_fused_batch_kernel(const BAWinDev* __restrict__ gW, const BAIter* __restrict__ gIt, const __grid_constant__ BABatchHdr hdr) {
@@ -1258,9 +1252,16 @@ __global__ void __launch_bounds__(FusedCfgOf<P>::TPB, P == 32 ? 2 : 1)
     while (w + 1 < hdr.B && item >= hdr.prefix[w + 1]) w++;
     fused_chunk<P, LPR, false>(gW[w], gIt[w], S, item - hdr.prefix[w]);
   }
+  // each window's first phase D item is loaded one window ahead (the first before the grid barrier): no table round trip per window
+  DItem next = first_ditem<P>(gW[0], (int)(blockIdx.x % gridDim.x), gridDim.x);
   const bool ok = grid_barrier(hdr.bar, hdr.bar_target);
 #pragma unroll 1
-  for (int w = 0; w < hdr.B; w++) fused_reduce<P, LPR>(gW[w], S, ok, (int)((blockIdx.x + (unsigned)w * 41u) % gridDim.x), gridDim.x);
+  for (int w = 0; w < hdr.B; w++) {
+    const int v = (int)((blockIdx.x + (unsigned)w * 41u) % gridDim.x);
+    const DItem cur = next;
+    if (w + 1 < hdr.B) next = first_ditem<P>(gW[w + 1], (int)((blockIdx.x + (unsigned)(w + 1) * 41u) % gridDim.x), gridDim.x);
+    fused_reduce<P, LPR, false, false>(gW[w], S, ok, v, gridDim.x, cur);
+  }
 }
 
 // ---------------------------------------------------------------------------------------------------------------------------
@@ -1270,7 +1271,7 @@ __global__ void __launch_bounds__(FusedCfgOf<P>::TPB, P == 32 ? 2 : 1)
 struct FusedCfg { bool done = false; int max_ctas = 0; };
 static std::mutex g_cfg_mutex;
 
-template <int P, bool MARG, bool CLK = false>
+template <int P, bool MARG, bool CLK, bool XCH>
 static cudaError_t launch_cfg(BAWinDev& W, const BAIter& it, cudaStream_t s, unsigned* bar_count, unsigned long long* clk = nullptr) {
   static FusedCfg cfg[64];
   constexpr int TPB = FusedCfgOf<P>::TPB;
@@ -1284,10 +1285,10 @@ static cudaError_t launch_cfg(BAWinDev& W, const BAIter& it, cudaStream_t s, uns
     std::lock_guard<std::mutex> lk(g_cfg_mutex);
     FusedCfg& c = cfg[dev & 63];
     if (!c.done) {
-      e = cudaFuncSetAttribute(ba_fused_kernel<P, MARG, CLK>, cudaFuncAttributeMaxDynamicSharedMemorySize, smem);
+      e = cudaFuncSetAttribute(ba_fused_kernel<P, MARG, CLK, XCH>, cudaFuncAttributeMaxDynamicSharedMemorySize, smem);
       if (e != cudaSuccess) return e;
       int per_sm = 0, sms = 0;
-      e = cudaOccupancyMaxActiveBlocksPerMultiprocessor(&per_sm, ba_fused_kernel<P, MARG, CLK>, TPB, smem);
+      e = cudaOccupancyMaxActiveBlocksPerMultiprocessor(&per_sm, ba_fused_kernel<P, MARG, CLK, XCH>, TPB, smem);
       if (e != cudaSuccess) return e;
       e = cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, dev);
       if (e != cudaSuccess) return e;
@@ -1300,7 +1301,7 @@ static cudaError_t launch_cfg(BAWinDev& W, const BAIter& it, cudaStream_t s, uns
   *bar_count += (unsigned)grid;   // monotonic arrival counter: every CTA of this launch adds one
   W.bar_target = *bar_count;
   void* args[3] = {(void*)&W, (void*)&it, (void*)&clk};
-  return cudaLaunchCooperativeKernel((const void*)ba_fused_kernel<P, MARG, CLK>, dim3(grid), dim3(threads), args, (size_t)smem, s);
+  return cudaLaunchCooperativeKernel((const void*)ba_fused_kernel<P, MARG, CLK, XCH>, dim3(grid), dim3(threads), args, (size_t)smem, s);
 }
 
 template <int P>
@@ -1341,16 +1342,22 @@ cudaError_t launch_fused_batch_kernel(int P, const BAWinDev* gW, const BAIter* g
   return (P == 32) ? launch_batch_cfg<32>(gW, gIt, hdr, max_nf, s, bar_count) : launch_batch_cfg<16>(gW, gIt, hdr, max_nf, s, bar_count);
 }
 
+// the instantiation of the window's shape: peer exchange only on a sharded window
+template <int P, bool MARG, bool CLK = false>
+static cudaError_t launch_xch(BAWinDev& W, const BAIter& it, cudaStream_t s, unsigned* bar_count, unsigned long long* clk = nullptr) {
+  return (W.xc.nranks > 1) ? launch_cfg<P, MARG, CLK, true>(W, it, s, bar_count, clk) : launch_cfg<P, MARG, CLK, false>(W, it, s, bar_count, clk);
+}
+
 // W.bar_target is filled in here; *bar_count is the handle's running arrival count
 cudaError_t launch_fused_kernel(BAWinDev& W, const BAIter& it, bool marg, cudaStream_t s, unsigned* bar_count) {
-  if (W.P == 32) return marg ? launch_cfg<32, true>(W, it, s, bar_count) : launch_cfg<32, false>(W, it, s, bar_count);
-  return marg ? launch_cfg<16, true>(W, it, s, bar_count) : launch_cfg<16, false>(W, it, s, bar_count);
+  if (W.P == 32) return marg ? launch_xch<32, true>(W, it, s, bar_count) : launch_xch<32, false>(W, it, s, bar_count);
+  return marg ? launch_xch<16, true>(W, it, s, bar_count) : launch_xch<16, false>(W, it, s, bar_count);
 }
 
 // the linearisation launch with the phase clock (measurement only): clk holds >= grid x NCLK stamps, *grid receives the CTA count
 cudaError_t launch_fused_kernel_clocked(BAWinDev& W, const BAIter& it, cudaStream_t s, unsigned* bar_count, unsigned long long* clk, int* grid) {
   const unsigned before = *bar_count;
-  const cudaError_t e = (W.P == 32) ? launch_cfg<32, false, true>(W, it, s, bar_count, clk) : launch_cfg<16, false, true>(W, it, s, bar_count, clk);
+  const cudaError_t e = (W.P == 32) ? launch_xch<32, false, true>(W, it, s, bar_count, clk) : launch_xch<16, false, true>(W, it, s, bar_count, clk);
   *grid = (int)(*bar_count - before);
   return e;
 }

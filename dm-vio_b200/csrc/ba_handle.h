@@ -53,6 +53,9 @@ struct dmv_ba {
   double* d_result[2] = {nullptr, nullptr};
   float* d_step = nullptr;
   double* d_part = nullptr;        // [max_chunks][PART_STRIDE] per-chunk partial blobs (scratch of one launch)
+  int4* d_dtab = nullptr;          // phase D items [DITEMS_MAX][2] of the current window shape (dmv_ba_set_points)
+  std::vector<int4> h_dtab;
+  int nditems = 0;
   float4* d_wg = nullptr;          // [WG_GROUPS][mp] Schur vectors, transposed (scratch)
   float* d_hdig = nullptr;         // [mp] HdiF (scratch)
   float* d_hdi_solve = nullptr;    // [mp] HdiF of the linearisation the last dmv_ba_accumulate returned (PointHessian::idepth_hessian)
