@@ -149,7 +149,7 @@ SYMBOLS = [
     "dmv_ba_resubstitute", "dmv_ba_backup_points", "dmv_ba_restore_points", "dmv_ba_get_idepth", "dmv_ba_gn_step", "dmv_nccl_unique_id",
     "dmv_ba_comm_init", "dmv_ba_activate_points", "dmv_ba_marginalize_points", "dmv_ba_drop_residuals", "dmv_ba_reset_oob", "dmv_ba_p2p_export", "dmv_ba_p2p_import", "dmv_ba_last_timing", "dmv_ba_bench_device", "dmv_ba_bench_phases", "dmv_ba_kernel_launch_count", "dmv_ba_io_bytes", "dmv_ba_set_timing", "dmv_ba_bench_e2e",
     "dmv_ba_batch_create", "dmv_ba_batch_destroy", "dmv_ba_batch_gn_step", "dmv_ba_batch_set_timing", "dmv_ba_batch_last_kernel_ms", "dmv_ba_batch_bench",
-    "dmv_ct_create", "dmv_ct_destroy", "dmv_ct_set_K", "dmv_ct_set_ref", "dmv_ct_make_coarse_depth", "dmv_ct_get_ref", "dmv_ct_upload_new", "dmv_ct_upload_new_image", "dmv_ct_set_huber",
+    "dmv_ct_create", "dmv_ct_destroy", "dmv_ct_set_K", "dmv_ct_set_ref", "dmv_ct_make_coarse_depth", "dmv_ct_set_ref_from_ba", "dmv_ct_get_ref", "dmv_ct_upload_new", "dmv_ct_upload_new_image", "dmv_ct_set_huber",
     "dmv_ci_create", "dmv_ci_destroy", "dmv_ci_set_K", "dmv_ci_upload_first", "dmv_ci_upload_new", "dmv_ci_set_points", "dmv_ci_calc_res_and_gs", "dmv_ci_kernel_launch_count",
     "dmv_ct_calc_res_gs", "dmv_ct_track", "dmv_ip_default_settings", "dmv_ct_init_points", "dmv_ct_trace_points", "dmv_ct_trace_points_multi", "dmv_ct_set_timing", "dmv_ct_last_timing", "dmv_ct_kernel_launch_count", "dmv_ct_last_point_evaluations",
     "dmv_ct_set_undistort", "dmv_ct_upload_raw_image", "dmv_ct_download_frame",
@@ -214,6 +214,7 @@ def lib():
         L.dmv_ct_set_K.argtypes = [vp, C.c_int, C.c_float, C.c_float, C.c_float, C.c_float]
         L.dmv_ct_set_ref.argtypes = [vp, C.c_int, C.c_int, f32p, f32p, f32p, f32p]
         L.dmv_ct_make_coarse_depth.argtypes = [vp, C.c_int, f32p, f32p, f32p, f32p, i32p]
+        L.dmv_ct_set_ref_from_ba.argtypes = [vp, vp, i32p]
         L.dmv_ct_get_ref.argtypes = [vp, C.c_int, C.POINTER(C.c_int), vp, vp, vp, vp]
         L.dmv_ct_upload_new.argtypes = [vp, C.c_int, f32p]
         L.dmv_ct_upload_new_image.argtypes = [vp, f32p]
@@ -577,6 +578,13 @@ class CT:
         """makeCoarseDepthL0 on the device with the resident frame as the reference; returns pc_n per level"""
         pc_n = np.zeros(8, np.int32)
         check(self.L.dmv_ct_make_coarse_depth(self.h, len(Ku), _c(Ku, np.float32), _c(Kv, np.float32), _c(new_idepth, np.float32), _c(HdiF, np.float32), pc_n))
+        return pc_n
+
+    def set_ref_from_ba(self, ba):
+        """setCoarseTrackingRef + makeCoarseDepthL0 from a BA handle on the same device (dmv_ct_set_ref_from_ba): the window's newest frame becomes
+        the reference.  ba: a BA, or a raw dmv_ba* (e.g. hostapi.WindowBA.ba_handle()).  Returns pc_n per level."""
+        pc_n = np.zeros(8, np.int32)
+        check(self.L.dmv_ct_set_ref_from_ba(self.h, ba.h if isinstance(ba, BA) else ba, pc_n))
         return pc_n
 
     def get_ref(self, lvl):

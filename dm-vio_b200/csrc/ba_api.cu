@@ -1,6 +1,8 @@
 // C-ABI of the bundle-adjustment handle (include/dmvio_b200.h).  Host-side plumbing only: buffer ownership, the
 // [target][point] residual-slot layout, tentative/committed double buffering, one stream + pinned staging per handle.
 #include "ba_handle.h"
+#include "ct_depth.h"
+#include "remove_outliers.h"
 #include "ip_trace.h"
 #include <algorithm>
 #include <cstdlib>
@@ -242,6 +244,41 @@ int dmv_ba_adopt_frame(dmv_ba* b, int slot, dmv_ct* ct) {
   CK(cudaStreamWaitEvent(b->stream, b->ev[0], 0));
   CK(cudaMemcpyAsync(b->d_img[slot], plane, sizeof(float4) * (size_t)w * h, cudaMemcpyDeviceToDevice, b->stream));
   CK(cudaStreamSynchronize(b->stream));
+  return DMV_OK;
+}
+
+// library-internal: what dmv_ct_set_ref_from_ba (ct_kernels.cu) reads from the window — the committed linearisation's residuals into the newest
+// frame (slot (nf-1)*mp + p: state, centerProjectedTo), the HdiF of the last dmv_ba_accumulate and the newest frame's level-0 plane.  Nothing is
+// copied: the caller orders its stream behind this handle's with an event.  The fold order is the reference's at setCoarseTrackingRef, i.e.
+// after FullSystem::removeOutliers: which points still have residuals is host bookkeeping here (res_slot), so the reorder is replayed on the host
+// and only the moved points go to the device (as (from, to) pairs; none when every point kept a residual).
+extern "C" __attribute__((visibility("hidden"))) int dmv_ba_ref_source(dmv_ba* b, dmv::CDFromBA* out) {
+  if (!b || !out) return set_error(DMV_ERR_INVALID, "null argument");
+  if (b->nranks > 1)
+    return set_error(DMV_ERR_STATE, "sharded BA handle (%d ranks): its points are one rank's share; build the reference on the host from the gathered outputs", b->nranks);
+  if (b->nf < 2 || b->npts < 1) return set_error(DMV_ERR_STATE, "window / points not set");
+  if (!b->have_committed) return set_error(DMV_ERR_STATE, "no committed linearisation (the tail's linearize + apply_res first)");
+  if (b->hdi_solve_n != b->npts) return set_error(DMV_ERR_STATE, "no dmv_ba_accumulate since the points were set: HdiF of the last solve is unknown");
+  const int c = 1 - b->tent;
+  const size_t ns = (size_t)MAXF * b->mp, base = (size_t)(b->nf - 1) * b->mp;
+  out->device = b->device; out->w = b->cfg.w; out->h = b->cfg.h; out->npts = b->npts;
+  out->st = b->d_st_new[c] + base;
+  out->cu = b->d_cpt[c] + base; out->cv = b->d_cpt[c] + ns + base; out->cid = b->d_cpt[c] + 2 * ns + base;
+  out->hdi = b->d_hdi_solve;
+  out->img = b->d_img[b->slots[b->nf - 1]];
+  out->stream = b->stream;
+  std::vector<char> alive(b->npts, 0);
+  for (int s : b->res_slot) alive[s % b->mp] = 1;
+  b->ref_moves.clear();
+  for (int h = 0; h < b->nf; h++) {
+    const int beg = b->host_start[h];
+    const std::vector<int> order = dmv::remove_outliers_order(beg, b->host_start[h + 1], alive);
+    for (int k = 0; k < (int)order.size(); k++)
+      if (order[k] != beg + k) { b->ref_moves.push_back(order[k]); b->ref_moves.push_back(beg + k); }
+  }
+  out->n_moves = (int)b->ref_moves.size() / 2;
+  out->moves_host = b->ref_moves.data();
+  out->moves = nullptr;
   return DMV_OK;
 }
 

@@ -80,6 +80,7 @@ struct dmv_ba {
   std::vector<int> res_slot;   // residual index -> slot (t*mp+p)
   std::vector<uint8_t> h_st_in;
   std::vector<float> h_en_in;
+  std::vector<int> ref_moves;  // dmv_ba_ref_source: FullSystem::removeOutliers' reorder as (from, to) point pairs
   bool st_in_clean = false;    // every existing residual's INPUT state on the device is IN with zero energy (dmv_ba_reset_oob becomes a flag flip)
   bool no_zero_copy = false;   // DMV_NO_ZERO_COPY=1: D2H copy node instead of in-kernel writes to the pinned result (A/B experiment)
   bool timing = false;         // record CUDA events around the kernels of every call (dmv_ba_set_timing)

@@ -686,7 +686,11 @@ struct dmv_ct {
   float* h_scratch = nullptr;
   // device-side makeCoarseDepthL0 (ct_depth.cu)
   float *cd_idepth[DMV_MAX_PYR_LEVELS] = {nullptr}, *cd_ws[DMV_MAX_PYR_LEVELS] = {nullptr}, *cd_ws2[DMV_MAX_PYR_LEVELS] = {nullptr};
-  int *cd_rowcnt = nullptr, *cd_rowoff = nullptr, *cd_totals = nullptr;  // cd_totals: pinned host, device-visible
+  int *cd_rowcnt = nullptr, *cd_rowoff = nullptr, *cd_totals = nullptr;  // cd_totals: pinned host, device-visible; [DMV_MAX_PYR_LEVELS] = bad point
+  // the device fold of dmv_ct_set_ref_from_ba: sort scratch for up to rb_cap points, and the event that orders this stream behind the BA's
+  CDSortScratch rb = {{nullptr, nullptr}, {nullptr, nullptr}, nullptr, 0, nullptr, nullptr, nullptr};
+  int rb_cap = 0;
+  cudaEvent_t ev_ba = nullptr;
   float* d_ip = nullptr;   // immature-point arrays (dmv_ct_trace_points)
   float* h_ip = nullptr;
   int ip_cap = 0;
@@ -714,7 +718,7 @@ struct dmv_ct {
 extern "C" {
 
 static int ct_allocate(dmv_ct* c, const dmv_ct_config* cfg);
-static int ct_build_pyramid(dmv_ct* c);
+static int ct_build_pyramid(dmv_ct* c, int first_level);
 
 int dmv_ct_create(const dmv_ct_config* cfg, dmv_ct** out) {
   if (!cfg || !out) return set_error(DMV_ERR_INVALID, "null argument");
@@ -777,6 +781,9 @@ int dmv_ct_destroy(dmv_ct* c) {
   cudaFreeHost(c->h_out); cudaFreeHost(c->h_scratch); cudaFree(c->d_ip); cudaFreeHost(c->h_ip);
   for (int l = 0; l < DMV_MAX_PYR_LEVELS; l++) { cudaFree(c->cd_idepth[l]); cudaFree(c->cd_ws[l]); cudaFree(c->cd_ws2[l]); }
   cudaFree(c->cd_rowcnt); cudaFree(c->cd_rowoff); cudaFreeHost(c->cd_totals);
+  for (int k = 0; k < 2; k++) { cudaFree(c->rb.key[k]); cudaFree(c->rb.ord[k]); }
+  cudaFree(c->rb.temp); cudaFree(c->rb.bad); cudaFree(c->rb.moves); cudaFreeHost(c->rb.h_moves);
+  if (c->ev_ba) cudaEventDestroy(c->ev_ba);
   cudaFree(c->d_remap); cudaFree(c->d_G); cudaFree(c->d_vigInv); cudaFree(c->d_raw);
   if (c->ev[0]) cudaEventDestroy(c->ev[0]);
   if (c->ev[1]) cudaEventDestroy(c->ev[1]);
@@ -837,7 +844,7 @@ int dmv_ct_upload_new_image(dmv_ct* c, const float* image) {
   if (c->staging_busy) { CK(cudaStreamSynchronize(c->stream)); c->staging_busy = false; }  // a previous upload may still read the staging buffer
   std::memcpy(c->h_scratch, image, npx * sizeof(float));
   CK(cudaMemcpyAsync(c->d_gray[0], c->h_scratch, npx * sizeof(float), cudaMemcpyHostToDevice, c->stream));
-  const int rc = ct_build_pyramid(c);
+  const int rc = ct_build_pyramid(c, 0);
   if (rc != DMV_OK) return rc;
   // no synchronisation: every consumer (dmv_ct_calc_res_gs / dmv_ct_track) runs on the same stream and synchronises itself; the image
   // was copied into the handle's pinned staging buffer above, so the caller's buffer is already free
@@ -845,9 +852,10 @@ int dmv_ct_upload_new_image(dmv_ct* c, const float* image) {
   return DMV_OK;
 }
 
-// the pyramid of the frame whose level-0 intensities are in d_gray[0]
-static int ct_build_pyramid(dmv_ct* c) {
-  for (int l = 0; l < c->cfg.levels; l++) {
+// the pyramid of the frame whose level-0 intensities are in d_gray[0] (first_level 0), or whose level-0 plane d_img[0] is already in place
+// (first_level 1: dmv_ct_set_ref_from_ba copies it from the BA handle)
+static int ct_build_pyramid(dmv_ct* c, int first_level) {
+  for (int l = first_level; l < c->cfg.levels; l++) {
     const int wl = c->w[l], hl = c->h[l];
     if (l > 0) {
       dim3 grid((wl + 127) / 128, hl);
@@ -929,7 +937,7 @@ int dmv_ct_upload_raw_image(dmv_ct* c, const void* raw, int bpp, float exposure,
   t.npx = c->w[0] * c->h[0]; t.wOrg = c->wOrg; t.remap = c->d_remap; t.G = c->d_G; t.vigInv = c->d_vigInv; t.mode = c->pmode;
   ingest_launch(t, c->d_raw, bpp, use_G, factor, c->d_gray[0], c->stream);
   c->launches++;
-  const int rc = ct_build_pyramid(c);
+  const int rc = ct_build_pyramid(c, 0);
   if (rc != DMV_OK) return rc;
   c->staging_busy = true;  // asynchronous like dmv_ct_upload_new_image
   return DMV_OK;
@@ -1115,23 +1123,49 @@ void dmv_ip_default_settings(dmv_ip_settings* s) {
   s->trace_minImprovementFactor = 2.f; s->huberTH = 9.f; s->trace_GNIterations = 3; s->minTraceTestRadius = 2;
 }
 
+// working planes of the device makeCoarseDepthL0, allocated on first use
+static int ct_cd_allocate(dmv_ct* c) {
+  if (c->cd_totals) return DMV_OK;
+  for (int l = 0; l < c->cfg.levels; l++) {
+    const size_t npx = (size_t)c->w[l] * c->h[l];
+    CK(cudaMalloc(&c->cd_idepth[l], npx * sizeof(float)));
+    CK(cudaMalloc(&c->cd_ws[l], npx * sizeof(float)));
+    CK(cudaMalloc(&c->cd_ws2[l], npx * sizeof(float)));
+  }
+  CK(cudaMalloc(&c->cd_rowcnt, sizeof(int) * c->h[0]));
+  CK(cudaMalloc(&c->cd_rowoff, sizeof(int) * c->h[0]));
+  CK(cudaMallocHost(&c->cd_totals, sizeof(int) * (DMV_MAX_PYR_LEVELS + 1)));
+  return DMV_OK;
+}
+static CDLevels ct_cd_levels(const dmv_ct* c) {
+  CDLevels Lv;
+  Lv.levels = c->cfg.levels; Lv.cap = c->cfg.max_points;
+  for (int l = 0; l < c->cfg.levels; l++) {
+    Lv.w[l] = c->w[l]; Lv.h[l] = c->h[l];
+    Lv.idepth[l] = c->cd_idepth[l]; Lv.ws[l] = c->cd_ws[l]; Lv.ws2[l] = c->cd_ws2[l]; Lv.img[l] = c->d_img[l];
+    Lv.pc_u[l] = c->d_u[l]; Lv.pc_v[l] = c->d_v[l]; Lv.pc_id[l] = c->d_id[l]; Lv.pc_col[l] = c->d_col[l];
+  }
+  Lv.rowcnt = c->cd_rowcnt; Lv.rowoff = c->cd_rowoff; Lv.totals = c->cd_totals;
+  return Lv;
+}
+// pc_n of every level from the compaction's totals (after the stream synchronisation); a level over capacity is an error
+static int ct_cd_take_counts(dmv_ct* c, int32_t* pc_n_out) {
+  for (int l = 0; l < c->cfg.levels; l++) {
+    if (c->cd_totals[l] > c->cfg.max_points) return set_error(DMV_ERR_INVALID, "level %d: %d reference points exceed max_points %d", l, c->cd_totals[l], c->cfg.max_points);
+    c->n[l] = c->cd_totals[l];
+    if (pc_n_out) pc_n_out[l] = c->n[l];
+  }
+  return DMV_OK;
+}
+
 // CoarseTracker::setCoarseTrackingRef -> makeCoarseDepthL0 (CoarseTracker.cpp:L138-295) on the device (ct_depth.cu); the reference frame is
 // the one resident in the handle (last dmv_ct_upload_new_image / dmv_ct_upload_new of every level)
 int dmv_ct_make_coarse_depth(dmv_ct* c, int n, const float* Ku, const float* Kv, const float* new_idepth, const float* HdiF, int32_t* pc_n_out) {
   if (!c || n < 0 || (n > 0 && (!Ku || !Kv || !new_idepth || !HdiF))) return set_error(DMV_ERR_INVALID, "null argument");
   CK(cudaSetDevice(c->device));
   const int L = c->cfg.levels, w0 = c->w[0], h0 = c->h[0];
-  if (!c->cd_totals) {
-    for (int l = 0; l < L; l++) {
-      const size_t npx = (size_t)c->w[l] * c->h[l];
-      CK(cudaMalloc(&c->cd_idepth[l], npx * sizeof(float)));
-      CK(cudaMalloc(&c->cd_ws[l], npx * sizeof(float)));
-      CK(cudaMalloc(&c->cd_ws2[l], npx * sizeof(float)));
-    }
-    CK(cudaMalloc(&c->cd_rowcnt, sizeof(int) * h0));
-    CK(cudaMalloc(&c->cd_rowoff, sizeof(int) * h0));
-    CK(cudaMallocHost(&c->cd_totals, sizeof(int) * DMV_MAX_PYR_LEVELS));
-  }
+  int rc = ct_cd_allocate(c);
+  if (rc != DMV_OK) return rc;
   // ---- the splat's only order-dependent part on the host: points hitting the same pixel are folded in input order (L144-160)
   if (n > c->ip_cap) {
     if (c->d_ip) cudaFree(c->d_ip);
@@ -1160,24 +1194,65 @@ int dmv_ct_make_coarse_depth(dmv_ct* c, int n, const float* Ku, const float* Kv,
     }
   }
   CK(cudaMemcpyAsync(c->d_ip, c->h_ip, sizeof(float) * 3 * cap, cudaMemcpyHostToDevice, c->stream));
-  CDLevels Lv;
-  Lv.levels = L; Lv.cap = c->cfg.max_points;
-  for (int l = 0; l < L; l++) {
-    Lv.w[l] = c->w[l]; Lv.h[l] = c->h[l];
-    Lv.idepth[l] = c->cd_idepth[l]; Lv.ws[l] = c->cd_ws[l]; Lv.ws2[l] = c->cd_ws2[l]; Lv.img[l] = c->d_img[l];
-    Lv.pc_u[l] = c->d_u[l]; Lv.pc_v[l] = c->d_v[l]; Lv.pc_id[l] = c->d_id[l]; Lv.pc_col[l] = c->d_col[l];
-  }
-  Lv.rowcnt = c->cd_rowcnt; Lv.rowoff = c->cd_rowoff; Lv.totals = c->cd_totals;
+  const CDLevels Lv = ct_cd_levels(c);
   cd_launch(Lv, nu, reinterpret_cast<const int*>(c->d_ip), c->d_ip + cap, c->d_ip + 2 * cap, c->stream);
   c->launches += 2 + 4 * L;
   CK(cudaGetLastError());
   CK(cudaStreamSynchronize(c->stream));
-  for (int l = 0; l < L; l++) {
-    if (c->cd_totals[l] > c->cfg.max_points) return set_error(DMV_ERR_INVALID, "level %d: %d reference points exceed max_points %d", l, c->cd_totals[l], c->cfg.max_points);
-    c->n[l] = c->cd_totals[l];
-    if (pc_n_out) pc_n_out[l] = c->n[l];
+  return ct_cd_take_counts(c, pc_n_out);
+}
+
+// CoarseTracker::setCoarseTrackingRef fed straight from a BA handle on the same device (ct_depth.cu: cd_launch_from_ba).  The points' IN
+// residuals into the window's newest frame are folded on the device; the frame's level-0 plane is copied from the BA slot and the coarser levels
+// are built as dmv_ct_upload_new_image builds them.  Ordered behind the BA stream by an event; one synchronisation at the end (pc_n).
+extern "C" __attribute__((visibility("hidden"))) int dmv_ba_ref_source(dmv_ba* b, CDFromBA* out);
+int dmv_ct_set_ref_from_ba(dmv_ct* c, dmv_ba* ba, int32_t* pc_n_out) {
+  if (!c || !ba) return set_error(DMV_ERR_INVALID, "null argument");
+  CDFromBA B;
+  int rc = dmv_ba_ref_source(ba, &B);
+  if (rc != DMV_OK) return rc;
+  if (B.device != c->device) return set_error(DMV_ERR_INVALID, "the BA handle lives on device %d, the tracker handle on %d", B.device, c->device);
+  if (B.w != c->w[0] || B.h != c->h[0]) return set_error(DMV_ERR_INVALID, "image size mismatch (BA %dx%d vs tracker %dx%d)", B.w, B.h, c->w[0], c->h[0]);
+  CK(cudaSetDevice(c->device));
+  if ((rc = ct_cd_allocate(c)) != DMV_OK) return rc;
+  if (!c->ev_ba) CK(cudaEventCreateWithFlags(&c->ev_ba, cudaEventDisableTiming));
+  if (B.npts > c->rb_cap) {
+    CK(cudaStreamSynchronize(c->stream));   // kernels in flight may still use the old scratch
+    for (int k = 0; k < 2; k++) { cudaFree(c->rb.key[k]); cudaFree(c->rb.ord[k]); c->rb.key[k] = nullptr; c->rb.ord[k] = nullptr; }
+    cudaFree(c->rb.temp); c->rb.temp = nullptr;
+    cudaFree(c->rb.moves); c->rb.moves = nullptr;
+    cudaFreeHost(c->rb.h_moves); c->rb.h_moves = nullptr;
+    c->rb_cap = 0;
+    const int cap = std::max(B.npts, 2048);
+    for (int k = 0; k < 2; k++) { CK(cudaMalloc(&c->rb.key[k], sizeof(unsigned) * cap)); CK(cudaMalloc(&c->rb.ord[k], sizeof(int) * cap)); }
+    CK(cudaMalloc(&c->rb.moves, sizeof(int) * 2 * cap));
+    CK(cudaMallocHost(&c->rb.h_moves, sizeof(int) * 2 * cap));
+    c->rb.temp_bytes = cd_sort_temp_bytes(cap);
+    CK(cudaMalloc(&c->rb.temp, std::max<size_t>(c->rb.temp_bytes, 16)));
+    if (!c->rb.bad) CK(cudaMalloc(&c->rb.bad, sizeof(int)));
+    c->rb_cap = cap;
   }
-  return DMV_OK;
+  CK(cudaEventRecord(c->ev_ba, B.stream));         // the BA's last linearisation / accumulate / frame upload
+  CK(cudaStreamWaitEvent(c->stream, c->ev_ba, 0));
+  CK(cudaMemcpyAsync(c->d_img[0], B.img, sizeof(float4) * (size_t)c->w[0] * c->h[0], cudaMemcpyDeviceToDevice, c->stream));
+  if ((rc = ct_build_pyramid(c, 1)) != DMV_OK) return rc;
+  if (B.n_moves > 0) {   // the previous call ended in a synchronisation: the pinned staging is free
+    std::memcpy(c->rb.h_moves, B.moves_host, sizeof(int) * 2 * (size_t)B.n_moves);
+    CK(cudaMemcpyAsync(c->rb.moves, c->rb.h_moves, sizeof(int) * 2 * (size_t)B.n_moves, cudaMemcpyHostToDevice, c->stream));
+    B.moves = c->rb.moves;
+  }
+  int kernels = 0;
+  CK(cd_launch_from_ba(ct_cd_levels(c), B, c->rb, c->stream, &kernels));
+  c->launches += kernels;   // the pyramid counted itself; the radix sort's own launches are not counted
+  CK(cudaMemcpyAsync(c->cd_totals + DMV_MAX_PYR_LEVELS, c->rb.bad, sizeof(int), cudaMemcpyDeviceToHost, c->stream));
+  CK(cudaGetLastError());
+  CK(cudaStreamSynchronize(c->stream));
+  const int bad = c->cd_totals[DMV_MAX_PYR_LEVELS];
+  if (bad < B.npts) {  // the lists were rebuilt from an inconsistent window: leave no reference to track against
+    for (int l = 0; l < c->cfg.levels; l++) c->n[l] = 0;
+    return set_error(DMV_ERR_INVALID, "point %d: its IN residual into the newest frame projects outside the image", bad);
+  }
+  return ct_cd_take_counts(c, pc_n_out);
 }
 
 // pc_u / pc_v / pc_idepth / pc_color of a level as they sit on the device (tests; any pointer may be NULL); returns pc_n[level] in *n

@@ -30,6 +30,11 @@ class CoarseTracker {
   // splat / pooling / dilation / compaction run there and the pc_* lists never leave the GPU.  Bit-identical lists.
   bool setCoarseTrackingRefOnDevice(int n, const float* Ku, const float* Kv, const float* new_idepth, const float* HdiF, const float* ref_image_wh,
                                     AffLight lastRef_aff_g2l, float lastRef_ab_exposure);
+  // Same, fed straight from the window on the device (coarse_tracker_window.cpp, dmv_ct_set_ref_from_ba): FullSystem::makeKeyFrame's
+  // removeOutliers + setCoarseTrackingRef(frameHessians) (FullSystem.cpp:L1438-1458) after finishOptimize and before the window is
+  // re-uploaded (the fold follows removeOutliers' point order).  The reference keyframe is the window's newest frame; its IN residuals, the last solve's HdiF and its level-0 plane never leave the GPU.  Unsharded
+  // windows only.  Refuses (false, error()) a window whose lastResiduals bookkeeping disagrees with the residuals it holds into the newest frame.
+  bool setCoarseTrackingRefFromWindow(const WindowBA& W, AffLight lastRef_aff_g2l, float lastRef_ab_exposure);
   // newFrame: raw image (pyramid built on the device) and its exposure
   bool setNewFrame(const float* image_wh, float ab_exposure);
   bool setNewFramePyramid(const float* const* dIp, float ab_exposure);

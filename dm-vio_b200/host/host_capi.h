@@ -78,6 +78,16 @@ int dmvh_ct_set_undistort(void* ct, int wOrg, int hOrg, const float* remapX, con
                           int photometric_mode);
 int dmvh_ct_upload_raw_image(void* ct, const void* raw, int bytes_per_px, float exposure, float factor, float ab_exposure);
 int dmvh_ct_download_frame(void* ct, int level, float* dIp_aos3);
+/* the keyframe hand-off from the window (host/coarse_tracker_window.cpp): CoarseTracker::setCoarseTrackingRefFromWindow (dmv_ct_set_ref_from_ba) */
+int dmvh_ct_set_ref_from_window(void* ct, void* win, double ref_a, double ref_b, float ref_exposure);
+const char* dmvh_ct_error(void* ct);   /* CoarseTracker::error() */
+/* the window's dmv_ba handle (for the C ABI directly) */
+void* dmvh_window_ba_handle(void* win);
+/* makeCoarseDepthL0's inputs as the host path gathers them from the window, in its fold order (WindowBA::coarseTrackingRefInputs): writes at
+ * most cap entries (point: index in the window's point list, may be NULL), returns the count (or -1, dmvh_window_error says why) */
+int dmvh_window_coarse_ref_inputs(void* win, float* Ku, float* Kv, float* new_idepth, float* HdiF, int32_t* point, int cap);
+/* per point: lastResiduals[0..1] target frameIDs and states (the inverse of dmvh_window_set_last_residuals) */
+void dmvh_window_get_last_residuals(void* win, int32_t* target_frameID2, int32_t* state2);
 
 /* CoarseInitializer adapter (host/coarse_initializer.h): trackFrame on the host, calcResAndGS on the device */
 void* dmvh_ci_create(int w, int h, int levels, int max_points, int device, const double calib_value_scaled[4]);

@@ -3,6 +3,7 @@
 #include "marg_frame.h"
 #include "nullspace.h"
 #include "../csrc/inv3.h"
+#include "../csrc/remove_outliers.h"
 #include <algorithm>
 #include <chrono>
 #include <cmath>
@@ -723,6 +724,37 @@ void WindowBA::syncResidualStates() {
   }
 }
 void WindowBA::getIdepths(float* idepth) { fetchPointFloats(0, idepth); }
+
+int WindowBA::coarseTrackingRefInputs(float* Ku, float* Kv, float* nid, float* HdiF, int32_t* point, int cap) {
+  err_.clear();
+  const int np = (int)points.size(), newest = nf() - 1;
+  if (newest < 0 || np == 0) return 0;
+  std::vector<float> hdi(np);
+  if (!fetchPointFloats(1, hdi.data())) { fail("dmv_ba_get_solve_HdiF"); return -1; }
+  std::vector<int> res_of_point(np, -1);   // the point's residual into the newest frame
+  std::vector<char> alive(np, 0);          // the point still has a residual (FullSystem::removeOutliers keeps it)
+  for (int i = 0; i < (int)activeResiduals.size(); i++) {
+    alive[activeResiduals[i].point] = 1;
+    if (activeResiduals[i].target == newest) res_of_point[activeResiduals[i].point] = i;
+  }
+  const int tid = frameHessians[newest].frameID;
+  int n = 0;
+  for (int b = 0; b < np;) {
+    int e = b;
+    while (e < np && points[e].host == points[b].host) e++;
+    for (int p : dmv::remove_outliers_order(b, e, alive)) {
+      const PointHessian& ph = points[p];
+      if (ph.lastResiduals_target[0] != tid || ph.lastResiduals_state[0] != 0 || res_of_point[p] < 0) continue;
+      if (n == cap) { err_ = "coarseTrackingRefInputs: more than " + std::to_string(cap) + " entries"; return -1; }
+      const PointFrameResidual& r = activeResiduals[res_of_point[p]];
+      Ku[n] = r.centerProjectedTo[0]; Kv[n] = r.centerProjectedTo[1]; nid[n] = r.centerProjectedTo[2]; HdiF[n] = hdi[p];
+      if (point) point[n] = p;
+      n++;
+    }
+    b = e;
+  }
+  return n;
+}
 
 // ---- sharding
 void WindowBA::rebuildResidualMaps() {

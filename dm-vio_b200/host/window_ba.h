@@ -175,10 +175,18 @@ class WindowBA {
   bool p2pSetup();                                         // export -> allgather of the 64-byte handles -> import
   int rank() const { return rank_; }
   int nranks() const { return nranks_; }
+  // the device handle, for consumers that read the window on the device (CoarseTracker::setCoarseTrackingRefFromWindow)
+  dmv_ba* handle() const { return ba_; }
 
   // ---- results
   void syncResidualStates();           // pulls state_NewState / energies / centerProjectedTo of the last linearisation from the device
   void getIdepths(float* idepth);      // current device depths
+  // makeCoarseDepthL0's inputs as the host path collects them (CoarseTracker.cpp:L144-158) for the newest frame: per point whose
+  // lastResiduals[0] targets it and is IN, that residual's centerProjectedTo, the point's HdiF of the last solve (downloaded) and its index in
+  // `points`.  The order is makeCoarseDepthL0's: `points` after FullSystem::removeOutliers' swap-with-back removal of the points without
+  // residuals (csrc/remove_outliers.h), which makeKeyFrame runs right before setCoarseTrackingRef.  Writes at most cap entries (point may be
+  // null) and returns their number, or -1 with error() set (more than cap entries; a failed download — sharded windows need the allgather).
+  int coarseTrackingRefInputs(float* Ku, float* Kv, float* new_idepth, float* HdiF, int32_t* point, int cap);
   void getFrameStates(double* state10) const;
   double lastGpuMs() const;
 

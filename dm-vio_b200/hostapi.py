@@ -251,6 +251,37 @@ class WindowBA:
         self.npts, self.nres = npl.value, nrl.value
         return dict(resInM=rc, HM=HM, bM=bM, npts=npl.value, nres=nrl.value)
 
+    def _window_ref(self):
+        # bound here rather than in _bind: the CPU build of the adapters over the oracle stand-in has no device hand-off
+        L = self.L
+        L.dmvh_window_ba_handle.restype = vp
+        L.dmvh_window_ba_handle.argtypes = [vp]
+        L.dmvh_window_coarse_ref_inputs.argtypes = [vp, f32p, f32p, f32p, f32p, i32p, C.c_int]
+        L.dmvh_window_get_last_residuals.argtypes = [vp, i32p, i32p]
+        return L
+
+    def ba_handle(self):
+        """the window's dmv_ba* (for capi.CT.set_ref_from_ba)"""
+        return self._window_ref().dmvh_window_ba_handle(self.h)
+
+    def coarse_ref_inputs(self, with_points=False):
+        """WindowBA::coarseTrackingRefInputs: (Ku, Kv, new_idepth, HdiF) of the points whose lastResiduals[0] is IN in the newest frame, in
+        makeCoarseDepthL0's order (after removeOutliers' swap-with-back), as the host path downloads them for dmv_ct_make_coarse_depth;
+        with_points: the points' indices as a fifth array"""
+        a = [np.zeros(max(1, self.npts), np.float32) for _ in range(4)]
+        pt = np.zeros(max(1, self.npts), np.int32)
+        n = self._window_ref().dmvh_window_coarse_ref_inputs(self.h, *a, pt, len(pt))
+        if n < 0:
+            raise capi.DmvError(self.L.dmvh_window_error(self.h).decode())
+        out = tuple(x[:n].copy() for x in a)
+        return out + (pt[:n].copy(),) if with_points else out
+
+    def last_residuals(self):
+        """per point (target frameID, state) of lastResiduals[0..1], each (npts, 2)"""
+        t, s = np.zeros((self.npts, 2), np.int32), np.zeros((self.npts, 2), np.int32)
+        self._window_ref().dmvh_window_get_last_residuals(self.h, t.reshape(-1), s.reshape(-1))
+        return t, s
+
     def states(self):
         st = np.zeros((self.nf, 10)); idd = np.zeros(self.npts, np.float32); th = np.zeros(self.nf, np.float32)
         self.L.dmvh_window_get_states(self.h, st.reshape(-1), idd, th)
@@ -288,6 +319,17 @@ class CoarseTracker:
         if rc != 0:
             raise capi.DmvError("dmvh_ct_set_ref_device failed")
         return [self.L.dmvh_ct_pc_n(self.h, l) for l in range(self.levels)]
+
+    def set_ref_from_ba(self, ba, ref_a=0.0, ref_b=0.0, ref_exposure=1.0):
+        """CoarseTracker::setCoarseTrackingRefFromWindow: the reference is the newest keyframe of the WindowBA `ba`, built on the device from
+        the window's committed residuals, last-solve HdiF and level-0 plane.  Returns pc_n per level."""
+        L = self.L
+        L.dmvh_ct_set_ref_from_window.argtypes = [vp, vp, C.c_double, C.c_double, C.c_float]
+        if L.dmvh_ct_set_ref_from_window(self.h, ba.h, float(ref_a), float(ref_b), float(ref_exposure)) != 0:
+            L.dmvh_ct_error.restype = C.c_char_p
+            L.dmvh_ct_error.argtypes = [vp]
+            raise capi.DmvError(L.dmvh_ct_error(self.h).decode())
+        return [L.dmvh_ct_pc_n(self.h, l) for l in range(self.levels)]
 
     def set_new_image(self, img, exposure=1.0):
         if self.L.dmvh_ct_set_new_image(self.h, _c(img, np.float32).reshape(-1), exposure) != 0:

@@ -280,6 +280,24 @@ int dmv_ct_set_ref(dmv_ct* ct, int level, int n, const float* pc_u, const float*
  * dmv_ct_upload_new of every level); afterwards a new frame may be uploaded for tracking.  pc_n_out (levels entries, may be NULL) = pc_n[].
  * Bit-identical lists (values and order) to the CPU code. */
 int dmv_ct_make_coarse_depth(dmv_ct* ct, int n, const float* Ku, const float* Kv, const float* new_idepth, const float* HdiF, int32_t* pc_n_out);
+/* CoarseTracker::setCoarseTrackingRef (CoarseTracker.cpp:L524-538) + makeCoarseDepthL0 (L138-295) fed directly from a BA handle on the same
+ * device, nothing crossing PCIe: the reference keyframe is the newest frame of the BA window (frame nf-1 of dmv_ba_set_window).
+ *   - points: a point contributes exactly when its residual into that frame is still present (not removed by dmv_ba_drop_residuals) and
+ *     ended the committed linearisation IN — ph->lastResiduals[0] IN after the tail's linearizeAll(true) (FullSystemOptimize.cpp:L175-203);
+ *     its committed centerProjectedTo and the HdiF of the last dmv_ba_accumulate (dmv_ba_get_solve_HdiF) are used;
+ *   - order: colliding splats are folded in makeCoarseDepthL0's order (CoarseTracker.cpp:L144-146): the frameHessians x fh->pointHessians
+ *     order of the last dmv_ba_set_points, after FullSystem::removeOutliers (FullSystemOptimize.cpp:L680-697), which makeKeyFrame runs just
+ *     before (FullSystem.cpp:L1438): in each host frame a point left without residuals is replaced by the host's last point (swap-with-back).
+ *     The call applies that reorder itself; the handle must not have been re-uploaded since the tail;
+ *   - frame: the BA slot's level-0 plane becomes the handle's level 0 and the coarser levels are built as dmv_ct_upload_new_image builds them,
+ *     so afterwards the keyframe is the handle's resident frame, as after dmv_ct_upload_new_image + dmv_ct_make_coarse_depth.
+ * Ordered behind everything queued on the BA handle (no host synchronisation needed in between); returns after one synchronisation.
+ * pc_n_out as dmv_ct_make_coarse_depth.  Bit-identical lists (values and order) to dmv_ct_make_coarse_depth fed with the same residuals.
+ * Errors: DMV_ERR_INVALID for handles on different devices, different image sizes, or a projection outside the image (the lowest such point
+ * is reported; every level's list is then emptied); the capacity error of dmv_ct_make_coarse_depth; DMV_ERR_STATE without a committed
+ * linearisation, without a dmv_ba_accumulate since dmv_ba_set_points, or on a sharded handle (its points are one rank's share: build the
+ * reference on the host from the gathered outputs there). */
+int dmv_ct_set_ref_from_ba(dmv_ct* ct, dmv_ba* ba, int32_t* pc_n_out);
 /* download pc_u / pc_v / pc_idepth / pc_color of one level (any pointer may be NULL; *n = pc_n[level]) */
 int dmv_ct_get_ref(dmv_ct* ct, int level, int* n, float* pc_u, float* pc_v, float* pc_idepth, float* pc_color);
 /* newFrame->dIp[level] (w_l*h_l*3 floats AoS) */
