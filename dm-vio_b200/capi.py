@@ -110,6 +110,18 @@ class CTConfig(C.Structure):
     _fields_ = [("w", C.c_int), ("h", C.c_int), ("levels", C.c_int), ("max_points", C.c_int), ("device", C.c_int)]
 
 
+class PSSettings(C.Structure):
+    _fields_ = [("minGradHistCut", C.c_float), ("minGradHistAdd", C.c_float), ("gradDownweightPerLevel", C.c_float),
+                ("selectDirectionDistribution", C.c_int), ("gammaWeightsPixelSelect", C.c_int)]
+
+
+class NewTracesArgs(C.Structure):
+    _fields_ = [("density", C.c_float), ("recursionsLeft", C.c_int), ("thFactor", C.c_float), ("B", C.c_void_p), ("settings", C.c_void_p),
+                ("potential", C.POINTER(C.c_int)), ("cap", C.c_int), ("n", C.POINTER(C.c_int)), ("numPointsTotal", C.POINTER(C.c_int)),
+                ("u", C.c_void_p), ("v", C.c_void_p), ("type", C.c_void_p), ("color8", C.c_void_p), ("weights8", C.c_void_p), ("gradH4", C.c_void_p),
+                ("energyTH", C.c_void_p), ("map", C.c_void_p)]
+
+
 class CTTrackArgs(C.Structure):
     _fields_ = [("R", C.c_double * 9), ("t", C.c_double * 3), ("a", C.c_double), ("b", C.c_double), ("ref_a", C.c_double), ("ref_b", C.c_double),
                 ("ref_exposure", C.c_float), ("new_exposure", C.c_float), ("coarseCutoffTH", C.c_float), ("affineOptModeA", C.c_float),
@@ -152,7 +164,7 @@ SYMBOLS = [
     "dmv_ct_create", "dmv_ct_destroy", "dmv_ct_set_K", "dmv_ct_set_ref", "dmv_ct_make_coarse_depth", "dmv_ct_set_ref_from_ba", "dmv_ct_get_ref", "dmv_ct_upload_new", "dmv_ct_upload_new_image", "dmv_ct_set_huber",
     "dmv_ci_create", "dmv_ci_destroy", "dmv_ci_set_K", "dmv_ci_upload_first", "dmv_ci_upload_new", "dmv_ci_set_points", "dmv_ci_calc_res_and_gs", "dmv_ci_kernel_launch_count",
     "dmv_ct_calc_res_gs", "dmv_ct_track", "dmv_ip_default_settings", "dmv_ct_init_points", "dmv_ct_trace_points", "dmv_ct_trace_points_multi", "dmv_ct_set_timing", "dmv_ct_last_timing", "dmv_ct_kernel_launch_count", "dmv_ct_last_point_evaluations",
-    "dmv_ct_set_undistort", "dmv_ct_upload_raw_image", "dmv_ct_download_frame",
+    "dmv_ct_set_undistort", "dmv_ct_upload_raw_image", "dmv_ct_download_frame", "dmv_ps_default_settings", "dmv_ct_make_new_traces",
 ]
 
 
@@ -231,6 +243,9 @@ def lib():
         L.dmv_ct_set_undistort.argtypes = [vp, C.POINTER(UndistortConfig)]
         L.dmv_ct_upload_raw_image.argtypes = [vp, vp, C.c_int, C.c_float, C.c_float]
         L.dmv_ct_download_frame.argtypes = [vp, C.c_int, f32p]
+        L.dmv_ps_default_settings.restype = None
+        L.dmv_ps_default_settings.argtypes = [C.POINTER(PSSettings)]
+        L.dmv_ct_make_new_traces.argtypes = [vp, C.POINTER(NewTracesArgs)]
         L.dmv_ci_create.argtypes = [C.POINTER(CTConfig), C.POINTER(vp)]
         L.dmv_ci_destroy.argtypes = [vp]
         L.dmv_ci_set_K.argtypes = [vp, C.c_int, C.c_float, C.c_float, C.c_float, C.c_float]
@@ -497,6 +512,7 @@ class CT:
         self.h = vp()
         check(self.L.dmv_ct_create(C.byref(cfg), C.byref(self.h)))
         self.levels = levels
+        self.size = (w, h)
 
     def close(self):
         if self.h:
@@ -593,6 +609,36 @@ class CT:
         a = [np.zeros(n.value, np.float32) for _ in range(4)]
         check(self.L.dmv_ct_get_ref(self.h, lvl, C.byref(n), *[x.ctypes.data for x in a]))
         return dict(u=a[0], v=a[1], idepth=a[2], color=a[3])
+
+    def make_new_traces(self, potential, density=1500.0, recursionsLeft=1, thFactor=1.0, B=None, settings=None, cap=16384, want_map=False):
+        """FullSystem::makeNewTraces on the resident frame (dmv_ct_make_new_traces).  potential: the selector's currentPotential before the call.
+        cap: point capacity (the default is ten times the default density; an overflow raises DmvError and sets last_needed).
+        Returns dict(points (u, v, type, color, weights, gradH, energyTH), numPointsTotal, potential (after), map (if want_map))."""
+        W, H = self.size
+        cap = int(cap)
+        pot, n, npt = C.c_int(int(potential)), C.c_int(0), C.c_int(0)
+        P = dict(u=np.zeros(max(cap, 1), np.int32), v=np.zeros(max(cap, 1), np.int32), type=np.zeros(max(cap, 1), np.float32),
+                 color=np.zeros((max(cap, 1), 8), np.float32), weights=np.zeros((max(cap, 1), 8), np.float32), gradH=np.zeros((max(cap, 1), 4), np.float32),
+                 energyTH=np.zeros(max(cap, 1), np.float32))
+        m = np.zeros(W * H, np.float32) if want_map else None
+        Bk = None if B is None else _c(B, np.float32)
+        S = None
+        if settings is not None:
+            S = PSSettings()
+            self.L.dmv_ps_default_settings(C.byref(S))
+            for k, val in settings.items():
+                setattr(S, k, val)
+        a = NewTracesArgs(float(density), int(recursionsLeft), float(thFactor), None if Bk is None else Bk.ctypes.data,
+                          None if S is None else C.addressof(S), C.pointer(pot), cap, C.pointer(n), C.pointer(npt), P["u"].ctypes.data, P["v"].ctypes.data,
+                          P["type"].ctypes.data, P["color"].ctypes.data, P["weights"].ctypes.data, P["gradH"].ctypes.data, P["energyTH"].ctypes.data,
+                          None if m is None else m.ctypes.data)
+        rc = self.L.dmv_ct_make_new_traces(self.h, C.byref(a))
+        self.last_needed, self.last_potential = n.value, pot.value
+        check(rc)
+        out = dict(points={k: P[k][:n.value] for k in P}, numPointsTotal=npt.value, potential=pot.value)
+        if want_map:
+            out["map"] = m.reshape(H, W)
+        return out
 
     def init_points(self, u, v):
         """ImmaturePoint constructor on the resident frame; same dict layout as oracle.orc.ip_init."""

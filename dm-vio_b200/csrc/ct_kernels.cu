@@ -13,6 +13,7 @@
 #include "ip_trace.h"
 #include "ct_depth.h"
 #include "ct_ingest.h"
+#include "ps_select.h"
 #include <cuda.h>
 #include <unordered_map>
 #include <algorithm>
@@ -707,6 +708,8 @@ struct dmv_ct {
   float2* d_remap = nullptr;
   float *d_G = nullptr, *d_vigInv = nullptr;
   void* d_raw = nullptr;
+  // dmv_ct_make_new_traces (ps_select.cu): allocated on first use
+  PSScratch ps;
 };
 
 #define CK(call)                                                                                   \
@@ -785,6 +788,7 @@ int dmv_ct_destroy(dmv_ct* c) {
   cudaFree(c->rb.temp); cudaFree(c->rb.bad); cudaFree(c->rb.moves); cudaFreeHost(c->rb.h_moves);
   if (c->ev_ba) cudaEventDestroy(c->ev_ba);
   cudaFree(c->d_remap); cudaFree(c->d_G); cudaFree(c->d_vigInv); cudaFree(c->d_raw);
+  ps_free(c->ps);
   if (c->ev[0]) cudaEventDestroy(c->ev[0]);
   if (c->ev[1]) cudaEventDestroy(c->ev[1]);
   if (c->stream) cudaStreamDestroy(c->stream);
@@ -1291,7 +1295,7 @@ int dmv_ct_init_points(dmv_ct* c, int n, const int32_t* u, const int32_t* v, flo
   std::memcpy(hb, u, 4 * (size_t)n); std::memcpy(hb + cap, v, 4 * (size_t)n);
   CK(cudaMemcpyAsync(d, hb, sizeof(float) * 2 * cap, cudaMemcpyHostToDevice, c->stream));
   IPInitArgs A;
-  A.n = n; A.w = c->w[0];
+  A.n = n; A.w = c->w[0]; A.n_dev = nullptr;
   A.outlierTHSumComponent = 50.f * 50.f; A.outlierTH = 12.f * 12.f; A.overallEnergyTHWeight = 1.f;  // util/settings.cpp:L111-114, L159
   A.u = reinterpret_cast<const int*>(d); A.v = reinterpret_cast<const int*>(d + cap);
   A.color = d + 2 * cap; A.weights = d + 10 * cap; A.gradH = d + 18 * cap; A.energyTH = d + 22 * cap; A.ok = reinterpret_cast<int*>(d + 23 * cap);
@@ -1383,6 +1387,64 @@ int dmv_ct_trace_points(dmv_ct* c, const dmv_ip_points* p, const float KRKi[9], 
   float tab[14];
   std::memcpy(tab, KRKi, 36); std::memcpy(tab + 9, Kt, 12); std::memcpy(tab + 12, aff, 8);
   return dmv_ct_trace_points_multi(c, 1, p, tab, settings);
+}
+
+void dmv_ps_default_settings(dmv_ps_settings* s) {
+  if (!s) return;
+  s->minGradHistCut = 0.5f; s->minGradHistAdd = 7.f; s->gradDownweightPerLevel = 0.75f;   // util/settings.cpp:L144, L167-170
+  s->selectDirectionDistribution = 1; s->gammaWeightsPixelSelect = 1;
+}
+
+// FullSystem::makeNewTraces on the resident frame (ps_select.cu)
+int dmv_ct_make_new_traces(dmv_ct* c, const dmv_new_traces_args* a) {
+  if (!c || !a) return set_error(DMV_ERR_INVALID, "null argument");
+  if (c->cfg.levels < 3) return set_error(DMV_ERR_INVALID, "pixel selection reads levels 0-2: the handle has %d", c->cfg.levels);
+  const int w = c->w[0], h = c->h[0];
+  if (w % 16 || h % 16) return set_error(DMV_ERR_INVALID, "pixel selection needs w and h divisible by 16 (%d x %d)", w, h);
+  if (!a->potential || !a->n || !a->numPointsTotal || a->cap < 0 || (a->cap > 0 && (!a->u || !a->v || !a->type || !a->color8 || !a->weights8 || !a->gradH4 || !a->energyTH)))
+    return set_error(DMV_ERR_INVALID, "null argument");
+  if (*a->potential < 1) return set_error(DMV_ERR_INVALID, "potential %d < 1", *a->potential);
+  if (!(a->density > 0.f) || !std::isfinite(a->density)) return set_error(DMV_ERR_INVALID, "density must be finite and > 0");
+  if (!(a->thFactor > 0.f) || !std::isfinite(a->thFactor)) return set_error(DMV_ERR_INVALID, "thFactor must be finite and > 0");
+  if (a->recursionsLeft < 0 || a->recursionsLeft > 8) return set_error(DMV_ERR_INVALID, "recursionsLeft must be in 0..8");
+  dmv_ps_settings st;
+  if (a->settings) st = *a->settings; else dmv_ps_default_settings(&st);
+  if (!(st.minGradHistCut < 0.99f) || !std::isfinite(st.minGradHistCut) || !std::isfinite(st.minGradHistAdd) || !std::isfinite(st.gradDownweightPerLevel))
+    return set_error(DMV_ERR_INVALID, "bad dmv_ps_settings");
+  CK(cudaSetDevice(c->device));
+  if (c->ps.w != w || c->ps.h != h) CK(ps_alloc(c->ps, w, h));
+  const int out_cap = std::min(a->cap, w * h);
+  CK(ps_ensure_out(c->ps, std::max(out_cap, 1)));
+  if (c->staging_busy) { CK(cudaStreamSynchronize(c->stream)); c->staging_busy = false; }
+  float B[256];
+  for (int i = 0; i < 256; i++) B[i] = a->B ? a->B[i] : (float)i;   // CalibHessian's constructor: B[i] = i
+  CK(cudaMemcpyAsync(c->ps.B, B, sizeof(B), cudaMemcpyHostToDevice, c->stream));
+  PSArgs A;
+  A.w = w; A.h = h;
+  for (int l = 0; l < 3; l++) A.img[l] = c->d_img[l];
+  A.s = st; A.density = a->density; A.thFactor = a->thFactor; A.recursionsLeft = a->recursionsLeft; A.potential = *a->potential;
+  A.out_cap = out_cap;
+  int kernels = 0;
+  CK(ps_launch(A, c->ps, c->stream, &kernels));
+  c->launches += kernels;
+  if (a->map) CK(cudaMemcpyAsync(a->map, c->ps.map, sizeof(float) * (size_t)w * h, cudaMemcpyDeviceToHost, c->stream));
+  CK(cudaStreamSynchronize(c->stream));
+  PSState S;
+  std::memcpy(&S, c->ps.h_out, sizeof(S));
+  *a->n = S.n_points;
+  // on overflow the selector's state stays as it was, so a retry with a larger cap continues from the same potential
+  if (S.n_points > a->cap) return set_error(DMV_ERR_INVALID, "%d new points exceed cap %d", S.n_points, a->cap);
+  *a->potential = S.ideal;
+  *a->numPointsTotal = S.numHaveSub;
+  const size_t n = (size_t)S.n_points, O = out_cap;
+  const float* o = c->ps.h_out + sizeof(PSState) / sizeof(float);
+  std::memcpy(a->u, o, 4 * n); std::memcpy(a->v, o + O, 4 * n); std::memcpy(a->type, o + 2 * O, 4 * n);
+  for (size_t i = 0; i < n; i++)
+    for (int k = 0; k < 8; k++) { a->color8[8 * i + k] = o[(3 + k) * O + i]; a->weights8[8 * i + k] = o[(11 + k) * O + i]; }
+  for (size_t i = 0; i < n; i++)
+    for (int k = 0; k < 4; k++) a->gradH4[4 * i + k] = o[(19 + k) * O + i];
+  std::memcpy(a->energyTH, o + 23 * O, 4 * n);
+  return DMV_OK;
 }
 
 // library-internal: the resident level-0 float4 plane of the coarse-tracker handle (dmv_ba_adopt_frame copies it device-to-device)

@@ -257,7 +257,7 @@ __global__ void __launch_bounds__(128) ip_trace_kernel(const __grid_constant__ I
 // (the reference then leaves energyTH = NaN and the caller drops the point)
 __global__ void __launch_bounds__(128) ip_init_kernel(const __grid_constant__ IPInitArgs A) {
   const int i = blockIdx.x * blockDim.x + threadIdx.x;
-  if (i >= A.n) return;
+  if (i >= A.n || (A.n_dev && i >= *A.n_dev)) return;
   const int u = A.u[i], v = A.v[i];
   float g0 = 0, g1 = 0, g2 = 0, g3 = 0;
   bool ok = true;

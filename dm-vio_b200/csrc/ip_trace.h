@@ -17,6 +17,7 @@ struct IPTraceArgs {
 };
 struct IPInitArgs {
   int n, w;
+  const int* n_dev;   // non-null: the point count is read there (written by an earlier kernel on the stream); n bounds it and sizes the grid
   float outlierTHSumComponent, outlierTH, overallEnergyTHWeight;
   const int *u, *v;
   float *color, *weights, *gradH, *energyTH;

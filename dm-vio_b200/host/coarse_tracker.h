@@ -44,6 +44,12 @@ class CoarseTracker {
   bool setUndistort(const dmv_undistort_config& cfg);
   bool uploadRawImage(const void* raw, int bytes_per_px, float exposure, float factor, float ab_exposure);
   bool downloadFrame(int level, float* dIp_aos3);
+  // FullSystem::makeNewTraces on the resident keyframe (coarse_tracker_select.cpp, dmv_ct_make_new_traces): PixelSelector::makeMaps with the
+  // caller's currentPotential (in/out; FullSystem's one selector outlives the tracker swap), then the ImmaturePoint constructor per selected
+  // pixel.  Outputs as dmv_new_traces_args; false (error()) on overflow with *n = the count needed.
+  bool makeNewTraces(int& currentPotential, float density, int recursionsLeft, float thFactor, const float* B, const dmv_ps_settings* settings, int cap,
+                     int* n, int* numPointsTotal, int32_t* u, int32_t* v, float* type, float* color8, float* weights8, float* gradH4, float* energyTH,
+                     float* map);
   // CoarseTracker.cpp:L539-770 (visual-only branch L639-683)
   bool trackNewestCoarse(SE3& lastToNew_out, AffLight& aff_g2l_out, int coarsestLvl, const double minResForAbort[5]);
 

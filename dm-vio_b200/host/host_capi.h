@@ -78,6 +78,11 @@ int dmvh_ct_set_undistort(void* ct, int wOrg, int hOrg, const float* remapX, con
                           int photometric_mode);
 int dmvh_ct_upload_raw_image(void* ct, const void* raw, int bytes_per_px, float exposure, float factor, float ab_exposure);
 int dmvh_ct_download_frame(void* ct, int level, float* dIp_aos3);
+/* new immature points of the resident keyframe (host/coarse_tracker_select.cpp): CoarseTracker::makeNewTraces (dmv_ct_make_new_traces);
+ * settings5 = {minGradHistCut, minGradHistAdd, gradDownweightPerLevel, selectDirectionDistribution, gammaWeightsPixelSelect} or NULL */
+int dmvh_ct_make_new_traces(void* ct, int* potential, float density, int recursionsLeft, float thFactor, const float* B, const float* settings5, int cap,
+                            int* n, int* numPointsTotal, int32_t* u, int32_t* v, float* type, float* color8, float* weights8, float* gradH4,
+                            float* energyTH, float* map);
 /* the keyframe hand-off from the window (host/coarse_tracker_window.cpp): CoarseTracker::setCoarseTrackingRefFromWindow (dmv_ct_set_ref_from_ba) */
 int dmvh_ct_set_ref_from_window(void* ct, void* win, double ref_a, double ref_b, float ref_exposure);
 const char* dmvh_ct_error(void* ct);   /* CoarseTracker::error() */

@@ -292,6 +292,7 @@ class CoarseTracker:
     def __init__(self, w, h, K, levels, max_points=65536, device=0):
         self.L = lib()
         self.levels = levels
+        self.size = (w, h)
         self.h = self.L.dmvh_ct_create(w, h, levels, max_points, device, _c(K, np.float64))
 
     def close(self):
@@ -363,6 +364,25 @@ class CoarseTracker:
         if self._ingest().dmvh_ct_download_frame(self.h, lvl, out) != 0:
             raise capi.DmvError("dmvh_ct_download_frame failed")
         return out.reshape(h >> lvl, w >> lvl, 3)
+
+    def make_new_traces(self, potential, density=1500.0, recursionsLeft=1, thFactor=1.0, B=None, cap=16384):
+        """CoarseTracker::makeNewTraces on the resident keyframe -> dict(points, numPointsTotal, potential) as capi.CT.make_new_traces
+        (cap: point capacity, ten times the default density by default)"""
+        L = self.L
+        # bound here rather than in _bind: the CPU build of the adapters over the oracle stand-in has no pixel-selection path
+        L.dmvh_ct_make_new_traces.argtypes = [vp, C.POINTER(C.c_int), C.c_float, C.c_int, C.c_float, vp, vp, C.c_int, C.POINTER(C.c_int),
+                                              C.POINTER(C.c_int)] + [vp] * 8
+        cap = int(cap)
+        m = max(cap, 1)
+        P = dict(u=np.zeros(m, np.int32), v=np.zeros(m, np.int32), type=np.zeros(m, np.float32), color=np.zeros((m, 8), np.float32),
+                 weights=np.zeros((m, 8), np.float32), gradH=np.zeros((m, 4), np.float32), energyTH=np.zeros(m, np.float32))
+        pot, n, npt = C.c_int(int(potential)), C.c_int(0), C.c_int(0)
+        Bk = None if B is None else _c(B, np.float32)
+        if L.dmvh_ct_make_new_traces(self.h, C.byref(pot), float(density), int(recursionsLeft), float(thFactor), None if Bk is None else Bk.ctypes.data, None,
+                                     cap, C.byref(n), C.byref(npt), *[P[k].ctypes.data for k in ("u", "v", "type", "color", "weights", "gradH", "energyTH")],
+                                     None) != 0:
+            raise capi.DmvError("dmvh_ct_make_new_traces failed")
+        return dict(points={k: P[k][:n.value] for k in P}, numPointsTotal=npt.value, potential=pot.value)
 
     def track(self, R, t, a, b, coarsest=None, minRes=None, device_lm=True):
         self.L.dmvh_ct_set_device_lm(self.h, int(device_lm))

@@ -411,6 +411,45 @@ int dmv_ct_trace_points(dmv_ct* ct, const dmv_ip_points* pts, const float KRKi[9
  * sets[k] = the points hosted by keyframe k, tables14 = per host [KRKi 9 | Kt 3 | aff 2]; one upload, one launch, one download. */
 int dmv_ct_trace_points_multi(dmv_ct* ct, int nsets, const dmv_ip_points* sets, const float* tables14, const dmv_ip_settings* settings);
 
+/* ------------------------------------------------------------------------------------------------
+ * New immature points of a keyframe  ==  FullSystem::makeNewTraces (FullSystem.cpp:L1640-1667): PixelSelector::makeMaps
+ * (FullSystem/PixelSelector2.cpp:L158-307) on the handle's RESIDENT frame (the one last given to dmv_ct_upload_new_image /
+ * dmv_ct_upload_raw_image / dmv_ct_upload_new, or made resident by dmv_ct_set_ref_from_ba), then the raster loop over
+ * [3, w-4) x [3, h-4) with the ImmaturePoint constructor of dmv_ct_init_points, keeping the points whose energyTH is finite.
+ * Bit-identical to the reference's CPU code: selection map, point order, types and constructor fields.
+ * ------------------------------------------------------------------------------------------------ */
+typedef struct dmv_ps_settings {      /* util/settings.cpp:L144, L167-170 */
+  float minGradHistCut;               /* 0.5 (must be < 0.99: the reference reads unset histogram bins above) */
+  float minGradHistAdd;               /* 7 */
+  float gradDownweightPerLevel;       /* 0.75 */
+  int selectDirectionDistribution;    /* 1 */
+  int gammaWeightsPixelSelect;        /* 1: absSquaredGrad *= getBGradOnly(I)^2 (HessianBlocks.cpp:L184-188) */
+} dmv_ps_settings;
+void dmv_ps_default_settings(dmv_ps_settings* s);
+typedef struct dmv_new_traces_args {
+  float density;                /* makeMaps' numWant: setting_desiredImmatureDensity = 1500 (finite, > 0) */
+  int recursionsLeft;           /* 1 (0..8) */
+  float thFactor;               /* 1 (CoarseInitializer::setFirst passes 2; finite, > 0) */
+  const float* B;               /* CalibHessian::B[256] as FullSystem::setGammaFunction leaves it; NULL = identity */
+  const dmv_ps_settings* settings;  /* NULL = defaults */
+  int* potential;               /* in/out: PixelSelector::currentPotential (3 at construction; >= 1).  The caller's state: FullSystem owns
+                                   one PixelSelector while its two coarse trackers swap roles */
+  int cap;                      /* capacity of every per-point output */
+  int* n;                       /* out: points created; on overflow the count needed (and DMV_ERR_INVALID: *potential and *numPointsTotal
+                                   are then left unchanged, so a retry with a larger cap gives the same result) */
+  int* numPointsTotal;          /* out: makeMaps' return value (numHaveSub) */
+  int32_t *u, *v;               /* out, makeNewTraces' push_back order */
+  float* type;                  /* out: the selectionMap value, 1 / 2 / 4 */
+  float *color8, *weights8, *gradH4, *energyTH;   /* out: as dmv_ct_init_points */
+  float* map;                   /* optional (w*h): selectionMap as makeMaps leaves it */
+} dmv_new_traces_args;
+/* PixelSelector's randomPattern (srand(3141592), rand() & 0xFF over w*h entries, L43-47) is generated once per handle, on first use, by a
+ * restatement of glibc's rand(); the caller's rand() state is not touched.  The scratch (about 170 bytes of device memory per level-0 pixel, and 96 bytes of
+ * pinned host memory per point of min(cap, w*h)) is allocated on first use, so dmv_ct_create is unchanged.  Ordered on the handle's stream; returns after one synchronisation (makeMaps' recursion is decided on the device).
+ * Errors: DMV_ERR_INVALID for levels < 3, w or h not a multiple of 16, bad arguments (including *potential < 1), or more than cap points
+ * (*n = the count needed); DMV_ERR_CUDA. */
+int dmv_ct_make_new_traces(dmv_ct* ct, const dmv_new_traces_args* a);
+
 /* enable/disable the CUDA-event timing of dmv_ct_calc_res_gs (off by default); dmv_ct_last_timing()[0] = kernel milliseconds */
 int dmv_ct_set_timing(dmv_ct* ct, int enable);
 int dmv_ct_last_timing(dmv_ct* ct, float ms[4]);
