@@ -56,6 +56,12 @@ class IPPoints(C.Structure):
                                                               "lastTraceStatus", "lastTraceUV2", "lastTracePixelInterval")]
 
 
+class IPSettings(C.Structure):
+    """dmv_ip_settings (include/dmvio_b200.h); ip_default_settings() fills it as dmv_ip_default_settings does"""
+    _fields_ = [(k, C.c_float) for k in ("maxPixSearch", "trace_stepsize", "trace_GNThreshold", "trace_extraSlackOnTH", "trace_slackInterval",
+                                          "trace_minImprovementFactor", "huberTH")] + [("trace_GNIterations", C.c_int), ("minTraceTestRadius", C.c_int)]
+
+
 class BABatch:
     """dmv_ba_batch: B independent windows (BA handles on one device) linearised by ONE launch (include/dmvio_b200.h)."""
 
@@ -245,6 +251,8 @@ def lib():
         L.dmv_ct_download_frame.argtypes = [vp, C.c_int, f32p]
         L.dmv_ps_default_settings.restype = None
         L.dmv_ps_default_settings.argtypes = [C.POINTER(PSSettings)]
+        L.dmv_ip_default_settings.restype = None
+        L.dmv_ip_default_settings.argtypes = [C.POINTER(IPSettings)]
         L.dmv_ct_make_new_traces.argtypes = [vp, C.POINTER(NewTracesArgs)]
         L.dmv_ci_create.argtypes = [C.POINTER(CTConfig), C.POINTER(vp)]
         L.dmv_ci_destroy.argtypes = [vp]
@@ -499,6 +507,13 @@ class BA:
         check(self.L.dmv_ba_p2p_import(self.h, nranks, rank, C.cast(buf, vp)))
 
 
+def ip_default_settings():
+    """an IPSettings filled by dmv_ip_default_settings"""
+    S = IPSettings()
+    lib().dmv_ip_default_settings(C.byref(S))
+    return S
+
+
 def nccl_unique_id():
     buf = C.create_string_buffer(128)
     check(lib().dmv_nccl_unique_id(C.cast(buf, vp)))
@@ -653,9 +668,9 @@ class CT:
                  status=np.full(n, 5, np.int32), lastTraceUV=np.zeros((n, 2), np.float32), lastTracePixelInterval=np.zeros(n, np.float32))
         return P
 
-    def trace_points(self, P, KRKi, Kt, aff):
+    def trace_points(self, P, KRKi, Kt, aff, settings=None):
         """ImmaturePoint::traceOn for the points of one host frame (dict of arrays as oracle.orc.ip_init returns) against the resident newest
-        frame; returns a dict with the updated in/out fields (P itself is not modified)."""
+        frame; returns a dict with the updated in/out fields (P itself is not modified).  settings: an IPSettings, or None (NULL: defaults)."""
         n = len(P["u"])
         keep = {k: _c(P[k], np.float32) for k in ("u", "v", "color", "weights", "gradH", "energyTH")}
         out = {"idepth_min": np.array(P["idepth_min"], np.float32, copy=True), "idepth_max": np.array(P["idepth_max"], np.float32, copy=True),
@@ -663,14 +678,15 @@ class CT:
                "lastTraceUV": np.array(P["lastTraceUV"], np.float32, copy=True), "lastTracePixelInterval": np.array(P["lastTracePixelInterval"], np.float32, copy=True)}
         pts = IPPoints(n, *[a.ctypes.data for a in (keep["u"], keep["v"], keep["color"], keep["weights"], keep["gradH"], keep["energyTH"], out["idepth_min"],
                                                      out["idepth_max"], out["quality"], out["status"], out["lastTraceUV"], out["lastTracePixelInterval"])])
-        check(self.L.dmv_ct_trace_points(self.h, C.byref(pts), _c(KRKi, np.float32).reshape(-1), _c(Kt, np.float32), _c(aff, np.float32), None))
+        check(self.L.dmv_ct_trace_points(self.h, C.byref(pts), _c(KRKi, np.float32).reshape(-1), _c(Kt, np.float32), _c(aff, np.float32),
+                                              None if settings is None else C.byref(settings)))
         Q = dict(P)
         Q.update(out)
         return Q
 
-    def trace_points_multi(self, sets):
+    def trace_points_multi(self, sets, settings=None):
         """sets = [(P, KRKi, Kt, aff), ...]: the immature points of several host keyframes in ONE launch (dmv_ct_trace_points_multi);
-        returns the list of updated dicts."""
+        returns the list of updated dicts.  settings: an IPSettings, or None (NULL: defaults)."""
         ns = len(sets)
         arr = (IPPoints * ns)()
         keeps, outs = [], []
@@ -684,7 +700,7 @@ class CT:
                                                                       out["idepth_max"], out["quality"], out["status"], out["lastTraceUV"], out["lastTracePixelInterval"])])
             tab[k, :9] = np.asarray(KRKi, np.float32).reshape(-1); tab[k, 9:12] = Kt; tab[k, 12:14] = aff
             keeps.append(keep); outs.append(out)
-        check(self.L.dmv_ct_trace_points_multi(self.h, ns, C.addressof(arr), tab.reshape(-1), None))
+        check(self.L.dmv_ct_trace_points_multi(self.h, ns, C.addressof(arr), tab.reshape(-1), None if settings is None else C.byref(settings)))
         res = []
         for (P, _, _, _), out in zip(sets, outs):
             Q = dict(P); Q.update(out); res.append(Q)

@@ -300,11 +300,14 @@ __global__ void __launch_bounds__(128) ip_init_kernel(const __grid_constant__ IP
 // ---------------------------------------------------------------------------------------------------------------------
 struct IPResState { int state, newState; double energy, newEnergy; };
 
-// linearizeResidual for (point, target f) by the point's 8 lanes; every lane returns the same value and updates its copy of (Hdd, bd, rs)
+// linearizeResidual for (point, target f) by the point's 8 lanes; every lane returns the same value and updates its copy of (Hdd, bd, rs).
+// Every group of the warp calls it for every f < nf: the 4 points of a warp may have different hosts, and the shuffles and the ballot below
+// name all 32 lanes, so a group whose host is f runs them too, adds nothing and returns 0 without touching rs.
 __device__ __forceinline__ double ip_linearize_group(const IPActArgs& A, const int host, const int f, const float pu, const float pv, const float colL,
                                                      const float wL, const float energyTH, const float outlierTHSlack, IPResState& rs, float& Hdd, float& bd,
                                                      const float idepth, const int lane) {
-  const bool skip = (rs.state == 1);   // an OOB residual stays OOB (uniform within the group; the warp's other groups still need this group's lanes in the shuffles)
+  const bool own = (f != host);        // f == host: no residual (the group only takes part in the warp's shuffles)
+  const bool skip = !own || (rs.state == 1);   // an OOB residual stays OOB (uniform within the group; the warp's other groups still need this group's lanes in the shuffles)
   const int idx = lane & 7, base = lane & ~7;
   const float* R = A.RT + (size_t)(host * A.nf + f) * 12;
   const float* t = R + 9;
@@ -340,6 +343,7 @@ __device__ __forceinline__ double ip_linearize_group(const IPActArgs& A, const i
     const float sE = __shfl_sync(0xffffffffu, tE, base + k), sH = __shfl_sync(0xffffffffu, tH, base + k), sb = __shfl_sync(0xffffffffu, tb, base + k);
     if (k < first_bad && !skip) { energyLeft += sE; Hdd += sH; bd += sb; }
   }
+  if (!own) return 0.0;
   if (skip || first_bad < 8) { rs.newState = 1; return rs.energy; }
   if (energyLeft > energyTH * outlierTHSlack) { energyLeft = energyTH * outlierTHSlack; rs.newState = 2; }
   else rs.newState = 0;
@@ -366,10 +370,13 @@ __global__ void __launch_bounds__(128) ip_activate_kernel(const __grid_constant_
   int status_out = 0;
 #pragma unroll
   for (int f = 0; f < DMV_MAX_FRAMES; f++) {
-    if (f < nf && f != host) {
-      lastEnergy = (float)((double)lastEnergy + ip_linearize_group(A, host, f, pu, pv, colL, wL, energyTH, 1000.f, res[f], lastHdd, lastbd, currentIdepth, lane));
-      res[f].state = res[f].newState;
-      res[f].energy = res[f].newEnergy;
+    if (f < nf) {   // warp-uniform; f == host is decided per group inside (the call holds warp-wide shuffles)
+      const double e = ip_linearize_group(A, host, f, pu, pv, colL, wL, energyTH, 1000.f, res[f], lastHdd, lastbd, currentIdepth, lane);
+      if (f != host) {
+        lastEnergy = (float)((double)lastEnergy + e);
+        res[f].state = res[f].newState;
+        res[f].energy = res[f].newEnergy;
+      }
     }
   }
   float idepth_out = currentIdepth;
@@ -383,9 +390,12 @@ __global__ void __launch_bounds__(128) ip_activate_kernel(const __grid_constant_
     const float newIdepth = currentIdepth - step;
     float newHdd = 0, newbd = 0, newEnergy = 0;
 #pragma unroll
-    for (int f = 0; f < DMV_MAX_FRAMES; f++)
-      if (f < nf && f != host)
-        newEnergy = (float)((double)newEnergy + ip_linearize_group(A, host, f, pu, pv, colL, wL, energyTH, 1.f, res[f], newHdd, newbd, newIdepth, lane));
+    for (int f = 0; f < DMV_MAX_FRAMES; f++) {
+      if (f < nf) {
+        const double e = ip_linearize_group(A, host, f, pu, pv, colL, wL, energyTH, 1.f, res[f], newHdd, newbd, newIdepth, lane);
+        if (f != host) newEnergy = (float)((double)newEnergy + e);
+      }
+    }
     if (done) continue;
     if (!isfinite(lastEnergy) || newHdd < A.minIdepthH_act) { idepth_out = currentIdepth; status_out = 0; done = true; continue; }
     if (newEnergy < lastEnergy) {

@@ -104,6 +104,7 @@ def _declare(L):
                                   i32p, f32p, i32p]
     L.orc_ip_init.argtypes = [C.c_int, f32p, C.c_int, C.c_int, i32p, i32p, f32p, f32p, f32p, f32p, u8p]
     L.orc_ip_trace.argtypes = [C.c_int, f32p, C.c_int, C.c_int, f32p, f32p, f32p, f32p, f32p, f32p, f32p, f32p, f32p, f32p, f32p, f32p, i32p, f32p, f32p]
+    L.orc_ip_trace_diag.argtypes = L.orc_ip_trace.argtypes + [i32p]
     L.orc_se3_exp.argtypes = [f64p, f64p, f64p]
     L.orc_se3_log.argtypes = [f64p, f64p, f64p]
     return L
@@ -412,16 +413,34 @@ def ip_init(dI_host, w, h, u, v, _fn=None):
     return P
 
 
-def ip_trace(P, dI, w, h, KRKi, Kt, aff, _fn=None):
-    """ImmaturePoint::traceOn for every point of P against the frame dI; returns the updated state (P is not modified)."""
+# per-point columns of ip_trace(..., diag=True)["diag"] (oracle/orc_trace.h IPD_*): what each traceOn call went through
+IP_DIAG_KEYS = ("numSteps", "bestIdx", "nTied", "maxTiedIdx", "gnIts", "gnBreak", "nonfiniteSearch", "nonfiniteGN", "exit")
+# values of the "exit" column (oracle/orc_trace.h IPX_*): the return traceOn took
+IPX = dict(STICKY_OOB=0, UMIN_OOB=1, UMAX_OOB=2, DEPTH_RANGE=3, SKIPPED=4, BADCONDITION=5, NONFINITE_DIR=6, GN_OOB=7, OUTLIER=8, OUTLIER_TWICE=9,
+           BAD_INTERVAL=10, GOOD=11)
+
+
+def ip_trace(P, dI, w, h, KRKi, Kt, aff, _fn=None, diag=False):
+    """ImmaturePoint::traceOn for every point of P against the frame dI; returns the updated state (P is not modified).
+    diag=True also returns Q["diag"], (n, len(IP_DIAG_KEYS)) int32: the search's step count, best step and ties, the GN iterations, the
+    non-finite samples met and the return taken, per point (same arithmetic: the state fields are those of diag=False)."""
     c = lambda a, t: np.ascontiguousarray(a, t)
     out = {k: np.array(P[k], copy=True) for k in IP_STATE_KEYS}
-    fn = _fn or (lambda *a: lib().orc_ip_trace(*a))
-    fn(len(P["u"]), c(dI, np.float32).reshape(-1), w, h, c(KRKi, np.float32).reshape(-1), c(Kt, np.float32), c(aff, np.float32), P["u"], P["v"],
+    n = len(P["u"])
+    dg = np.zeros((n, len(IP_DIAG_KEYS)), np.int32)
+    if diag:
+        assert _fn is None, "diagnostics come from the oracle's own traceOn"
+        fn = lambda *a: lib().orc_ip_trace_diag(*a, dg.reshape(-1))
+    else:
+        fn = _fn or (lambda *a: lib().orc_ip_trace(*a))
+    fn(n, c(dI, np.float32).reshape(-1), w, h, c(KRKi, np.float32).reshape(-1), c(Kt, np.float32), c(aff, np.float32), P["u"], P["v"],
        P["color"], P["weights"], P["gradH"], P["energyTH"], out["idepth_min"], out["idepth_max"], out["quality"], out["status"], out["lastTraceUV"],
        out["lastTracePixelInterval"])
     Q = dict(P)
+    Q.pop("diag", None)
     Q.update(out)
+    if diag:
+        Q["diag"] = dg
     return Q
 
 

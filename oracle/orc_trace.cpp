@@ -59,10 +59,15 @@ bool initImmature(ImmaturePt& p, const float* dI, int w, int u, int v, const Tra
   return true;
 }
 
-int traceOn(ImmaturePt& P, const float* dI, int w, int h, const float KRKi[9], const float Kt[3], const float aff[2], const TraceSettings& s) {
-  if (P.lastTraceStatus == IPS_OOB) return P.lastTraceStatus;  // L79
+int traceOn(ImmaturePt& P, const float* dI, int w, int h, const float KRKi[9], const float Kt[3], const float aff[2], const TraceSettings& s,
+            int32_t* diag) {
+  int32_t scratch[IPD_N];
+  int32_t* D = diag ? diag : scratch;
+  for (int k = 0; k < IPD_N; k++) D[k] = 0;
+  D[IPD_BEST_IDX] = -1; D[IPD_MAX_TIED_IDX] = -1;
+  if (P.lastTraceStatus == IPS_OOB) { D[IPD_EXIT] = IPX_STICKY_OOB; return P.lastTraceStatus; }  // L79
   const float maxPixSearch = (w + h) * s.maxPixSearch;
-  auto oob = [&]() { P.lastTraceUV[0] = -1; P.lastTraceUV[1] = -1; P.lastTracePixelInterval = 0; return P.lastTraceStatus = IPS_OOB; };
+  auto oob = [&](int exit) { D[IPD_EXIT] = exit; P.lastTraceUV[0] = -1; P.lastTraceUV[1] = -1; P.lastTracePixelInterval = 0; return P.lastTraceStatus = IPS_OOB; };
   // ---- project min and max (L98-176)
   float pr[3];
   for (int i = 0; i < 3; i++) pr[i] = (KRKi[3 * i] * P.u + KRKi[3 * i + 1] * P.v) + KRKi[3 * i + 2] * 1.0f;
@@ -80,15 +85,16 @@ int traceOn(ImmaturePt& P, const float* dI, int w, int h, const float KRKi[9], c
     maxRotPatY = std::max(absY, maxRotPatY);
   }
   const int boundU = std::max(4, maxRotPatX + 2), boundV = std::max(4, maxRotPatY + 2);
-  if (!(uMin > boundU && vMin > boundV && uMin < w - boundU - 1 && vMin < h - boundV - 1)) return oob();
+  if (!(uMin > boundU && vMin > boundV && uMin < w - boundU - 1 && vMin < h - boundV - 1)) return oob(IPX_UMIN_OOB);
   float dist, uMax, vMax, ptpMax[3];
   if (std::isfinite(P.idepth_max)) {
     for (int i = 0; i < 3; i++) ptpMax[i] = pr[i] + Kt[i] * P.idepth_max;
     uMax = ptpMax[0] / ptpMax[2]; vMax = ptpMax[1] / ptpMax[2];
-    if (!(uMax > boundU && vMax > boundV && uMax < w - boundU - 1 && vMax < h - boundV - 1)) return oob();
+    if (!(uMax > boundU && vMax > boundV && uMax < w - boundU - 1 && vMax < h - boundV - 1)) return oob(IPX_UMAX_OOB);
     dist = (uMin - uMax) * (uMin - uMax) + (vMin - vMax) * (vMin - vMax);
     dist = sqrtf(dist);
     if (dist < s.trace_slackInterval) {
+      D[IPD_EXIT] = IPX_SKIPPED;
       P.lastTraceUV[0] = (uMax + uMin) * 0.5f; P.lastTraceUV[1] = (vMax + vMin) * 0.5f;
       P.lastTracePixelInterval = dist;
       return P.lastTraceStatus = IPS_SKIPPED;
@@ -101,9 +107,9 @@ int traceOn(ImmaturePt& P, const float* dI, int w, int h, const float KRKi[9], c
     const float d = 1.0f / sqrtf(ddx * ddx + ddy * ddy);
     uMax = uMin + dist * ddx * d;
     vMax = vMin + dist * ddy * d;
-    if (!(uMax > boundU && vMax > boundV && uMax < w - boundU - 1 && vMax < h - boundV - 1)) return oob();
+    if (!(uMax > boundU && vMax > boundV && uMax < w - boundU - 1 && vMax < h - boundV - 1)) return oob(IPX_UMAX_OOB);
   }
-  if (!(P.idepth_min < 0 || (ptpMin[2] > 0.75 && ptpMin[2] < 1.5))) return oob();  // L179-185 (double literals: compared in double)
+  if (!(P.idepth_min < 0 || (ptpMin[2] > 0.75 && ptpMin[2] < 1.5))) return oob(IPX_DEPTH_RANGE);  // L179-185 (double literals: compared in double)
   // ---- error bounds (L188-206)
   float dx = s.trace_stepsize * (uMax - uMin);
   float dy = s.trace_stepsize * (vMax - vMin);
@@ -112,6 +118,7 @@ int traceOn(ImmaturePt& P, const float* dI, int w, int h, const float KRKi[9], c
   const float b = (dy * g[0] + (-dx) * g[2]) * dy + (dy * g[1] + (-dx) * g[3]) * (-dx);
   float errorInPixel = 0.2f + 0.2f * (a + b) / a;
   if (errorInPixel * s.trace_minImprovementFactor > dist && std::isfinite(P.idepth_max)) {
+    D[IPD_EXIT] = IPX_BADCONDITION;
     P.lastTraceUV[0] = (uMax + uMin) * 0.5f; P.lastTraceUV[1] = (vMax + vMin) * 0.5f;
     P.lastTracePixelInterval = dist;
     return P.lastTraceStatus = IPS_BADCONDITION;
@@ -129,7 +136,7 @@ int traceOn(ImmaturePt& P, const float* dI, int w, int h, const float KRKi[9], c
   const float randShift = uMin * 1000 - floorf(uMin * 1000);
   float ptx = uMin - randShift * dx;
   float pty = vMin - randShift * dy;
-  if (!std::isfinite(dx) || !std::isfinite(dy)) { P.lastTracePixelInterval = 0; P.lastTraceUV[0] = -1; P.lastTraceUV[1] = -1; return P.lastTraceStatus = IPS_OOB; }
+  if (!std::isfinite(dx) || !std::isfinite(dy)) { D[IPD_EXIT] = IPX_NONFINITE_DIR; P.lastTracePixelInterval = 0; P.lastTraceUV[0] = -1; P.lastTraceUV[1] = -1; return P.lastTraceStatus = IPS_OOB; }
   float errors[100];
   float bestU = 0, bestV = 0, bestEnergy = 1e10;
   int bestIdx = -1;
@@ -138,7 +145,7 @@ int traceOn(ImmaturePt& P, const float* dI, int w, int h, const float KRKi[9], c
     float energy = 0;
     for (int idx = 0; idx < 8; idx++) {
       const float hitColor = interp31(dI, (float)(ptx + rot[idx][0]), (float)(pty + rot[idx][1]), w);
-      if (!std::isfinite(hitColor)) { energy += 1e5; continue; }
+      if (!std::isfinite(hitColor)) { energy += 1e5; D[IPD_NONFINITE_SEARCH]++; continue; }
       const float residual = hitColor - (float)(aff[0] * P.color[idx] + aff[1]);
       const float hw = fabs(residual) < s.huberTH ? 1 : s.huberTH / fabs(residual);
       energy += hw * residual * residual * (2 - hw);
@@ -148,6 +155,10 @@ int traceOn(ImmaturePt& P, const float* dI, int w, int h, const float KRKi[9], c
     ptx += dx;
     pty += dy;
   }
+  D[IPD_NUM_STEPS] = numSteps;
+  D[IPD_BEST_IDX] = bestIdx;
+  for (int i = 0; i < numSteps; i++)
+    if (bestIdx >= 0 && errors[i] == bestEnergy) { D[IPD_N_TIED]++; D[IPD_MAX_TIED_IDX] = i; }
   float secondBest = 1e10;
   for (int i = 0; i < numSteps; i++)
     if ((i < bestIdx - s.minTraceTestRadius || i > bestIdx + s.minTraceTestRadius) && errors[i] < secondBest) secondBest = errors[i];
@@ -157,14 +168,15 @@ int traceOn(ImmaturePt& P, const float* dI, int w, int h, const float KRKi[9], c
   float uBak = bestU, vBak = bestV, gnstepsize = 1, stepBack = 0;
   if (s.trace_GNIterations > 0) bestEnergy = 1e5;
   for (int it = 0; it < s.trace_GNIterations; it++) {
+    D[IPD_GN_ITS]++;
     float H = 1, bb = 0, energy = 0;
     for (int idx = 0; idx < 8; idx++) {
       const float posU = (float)(bestU + rot[idx][0]);
       const float posV = (float)(bestV + rot[idx][1]);
-      if (posU < 0 || posV < 0 || posU >= w - 1 || posV >= h - 1) return oob();
+      if (posU < 0 || posV < 0 || posU >= w - 1 || posV >= h - 1) return oob(IPX_GN_OOB);
       float hit[3];
       interp33(dI, posU, posV, w, hit);
-      if (!std::isfinite((float)hit[0])) { energy += 1e5; continue; }
+      if (!std::isfinite((float)hit[0])) { energy += 1e5; D[IPD_NONFINITE_GN]++; continue; }
       const float residual = hit[0] - (aff[0] * P.color[idx] + aff[1]);
       const float dResdDist = dx * hit[1] + dy * hit[2];
       const float hw = fabs(residual) < s.huberTH ? 1 : s.huberTH / fabs(residual);
@@ -188,13 +200,14 @@ int traceOn(ImmaturePt& P, const float* dI, int w, int h, const float KRKi[9], c
       bestV += step * dy;
       bestEnergy = energy;
     }
-    if (fabsf(stepBack) < s.trace_GNThreshold) break;
+    if (fabsf(stepBack) < s.trace_GNThreshold) { D[IPD_GN_BREAK] = 1; break; }
   }
   // ---- energy-based outlier (L360-376)
   if (!(bestEnergy < P.energyTH * s.trace_extraSlackOnTH)) {
     P.lastTracePixelInterval = 0;
     P.lastTraceUV[0] = -1; P.lastTraceUV[1] = -1;
-    if (P.lastTraceStatus == IPS_OUTLIER) return P.lastTraceStatus = IPS_OOB;
+    if (P.lastTraceStatus == IPS_OUTLIER) { D[IPD_EXIT] = IPX_OUTLIER_TWICE; return P.lastTraceStatus = IPS_OOB; }
+    D[IPD_EXIT] = IPX_OUTLIER;
     return P.lastTraceStatus = IPS_OUTLIER;
   }
   // ---- new interval (L380-402)
@@ -207,10 +220,12 @@ int traceOn(ImmaturePt& P, const float* dI, int w, int h, const float KRKi[9], c
   }
   if (P.idepth_min > P.idepth_max) std::swap(P.idepth_min, P.idepth_max);
   if (!std::isfinite(P.idepth_min) || !std::isfinite(P.idepth_max) || (P.idepth_max < 0)) {
+    D[IPD_EXIT] = IPX_BAD_INTERVAL;
     P.lastTracePixelInterval = 0;
     P.lastTraceUV[0] = -1; P.lastTraceUV[1] = -1;
     return P.lastTraceStatus = IPS_OUTLIER;
   }
+  D[IPD_EXIT] = IPX_GOOD;
   P.lastTracePixelInterval = 2 * errorInPixel;
   P.lastTraceUV[0] = bestU; P.lastTraceUV[1] = bestV;
   return P.lastTraceStatus = IPS_GOOD;
@@ -234,9 +249,9 @@ int orc_ip_init(int n, const float* dI, int w, int h, const int32_t* u, const in
   }
   return good;
 }
-void orc_ip_trace(int n, const float* dI, int w, int h, const float* KRKi, const float* Kt, const float* aff, const float* u, const float* v,
-                  const float* color8, const float* weights8, const float* gradH4, const float* energyTH, float* idepth_min, float* idepth_max,
-                  float* quality, int32_t* status, float* uv2, float* interval) {
+static void ip_trace_all(int n, const float* dI, int w, int h, const float* KRKi, const float* Kt, const float* aff, const float* u, const float* v,
+                         const float* color8, const float* weights8, const float* gradH4, const float* energyTH, float* idepth_min, float* idepth_max,
+                         float* quality, int32_t* status, float* uv2, float* interval, int32_t* diag) {
   TraceSettings s;
   for (int i = 0; i < n; i++) {
     ImmaturePt p;
@@ -244,10 +259,20 @@ void orc_ip_trace(int n, const float* dI, int w, int h, const float* KRKi, const
     std::memcpy(p.color, color8 + 8 * i, 32); std::memcpy(p.weights, weights8 + 8 * i, 32); std::memcpy(p.gradH, gradH4 + 4 * i, 16);
     p.energyTH = energyTH[i]; p.idepth_min = idepth_min[i]; p.idepth_max = idepth_max[i]; p.quality = quality[i];
     p.lastTraceStatus = status[i]; p.lastTraceUV[0] = uv2[2 * i]; p.lastTraceUV[1] = uv2[2 * i + 1]; p.lastTracePixelInterval = interval[i];
-    traceOn(p, dI, w, h, KRKi, Kt, aff, s);
+    traceOn(p, dI, w, h, KRKi, Kt, aff, s, diag ? diag + (size_t)IPD_N * i : nullptr);
     idepth_min[i] = p.idepth_min; idepth_max[i] = p.idepth_max; quality[i] = p.quality; status[i] = p.lastTraceStatus;
     uv2[2 * i] = p.lastTraceUV[0]; uv2[2 * i + 1] = p.lastTraceUV[1]; interval[i] = p.lastTracePixelInterval;
   }
+}
+void orc_ip_trace(int n, const float* dI, int w, int h, const float* KRKi, const float* Kt, const float* aff, const float* u, const float* v,
+                  const float* color8, const float* weights8, const float* gradH4, const float* energyTH, float* idepth_min, float* idepth_max,
+                  float* quality, int32_t* status, float* uv2, float* interval) {
+  ip_trace_all(n, dI, w, h, KRKi, Kt, aff, u, v, color8, weights8, gradH4, energyTH, idepth_min, idepth_max, quality, status, uv2, interval, nullptr);
+}
+void orc_ip_trace_diag(int n, const float* dI, int w, int h, const float* KRKi, const float* Kt, const float* aff, const float* u, const float* v,
+                       const float* color8, const float* weights8, const float* gradH4, const float* energyTH, float* idepth_min, float* idepth_max,
+                       float* quality, int32_t* status, float* uv2, float* interval, int32_t* diag) {
+  ip_trace_all(n, dI, w, h, KRKi, Kt, aff, u, v, color8, weights8, gradH4, energyTH, idepth_min, idepth_max, quality, status, uv2, interval, diag);
 }
 }
 

@@ -28,8 +28,37 @@ struct ImmaturePt {  // the fields of ImmaturePoint that the constructor writes 
 
 // ImmaturePoint constructor: colours, weights, gradH, energyTH from the host's level-0 [I,dx,dy]; returns false if a colour is not finite
 bool initImmature(ImmaturePt& p, const float* dI_host, int w, int u, int v, const TraceSettings& s);
-// ImmaturePoint::traceOn; dI = frame->dI (w*h*3), KRKi row-major 3x3; returns lastTraceStatus
-int traceOn(ImmaturePt& p, const float* dI, int w, int h, const float KRKi[9], const float Kt[3], const float aff[2], const TraceSettings& s);
+// What one traceOn call went through (test coverage only; the arithmetic is the same with or without it).  diag[IPD_*]:
+enum {
+  IPD_NUM_STEPS = 0,   // numSteps of the discrete search after the clamp at 99 (0: no search)
+  IPD_BEST_IDX,        // bestIdx of the search (-1: no search)
+  IPD_N_TIED,          // steps whose energy equals the best energy exactly (the best step included)
+  IPD_MAX_TIED_IDX,    // the largest such step index
+  IPD_GN_ITS,          // Gauss-Newton iterations executed
+  IPD_GN_BREAK,        // 1 if the GN loop left by its |stepBack| < trace_GNThreshold break, 0 if it ran out of iterations (or never ran)
+  IPD_NONFINITE_SEARCH,// non-finite samples in the search (each added 1e5 to a step's energy)
+  IPD_NONFINITE_GN,    // non-finite samples in the GN iterations (each added 1e5)
+  IPD_EXIT,            // the return taken: IPX_*
+  IPD_N
+};
+enum {
+  IPX_STICKY_OOB = 0,  // entered OOB, returned at once
+  IPX_UMIN_OOB,        // uMin outside the image
+  IPX_UMAX_OOB,        // uMax outside the image
+  IPX_DEPTH_RANGE,     // idepth_min >= 0 and ptpMin[2] outside (0.75, 1.5)
+  IPX_SKIPPED,         // interval shorter than trace_slackInterval
+  IPX_BADCONDITION,    // errorInPixel * trace_minImprovementFactor > dist
+  IPX_NONFINITE_DIR,   // dx or dy not finite
+  IPX_GN_OOB,          // a GN pattern sample outside [0, w-1) x [0, h-1)
+  IPX_OUTLIER,         // energy test failed, previous status not OUTLIER -> OUTLIER
+  IPX_OUTLIER_TWICE,   // energy test failed, previous status OUTLIER -> OOB
+  IPX_BAD_INTERVAL,    // new depth interval not finite or idepth_max < 0 -> OUTLIER
+  IPX_GOOD,
+  IPX_N
+};
+// ImmaturePoint::traceOn; dI = frame->dI (w*h*3), KRKi row-major 3x3; returns lastTraceStatus.  diag: NULL or IPD_N ints.
+int traceOn(ImmaturePt& p, const float* dI, int w, int h, const float KRKi[9], const float Kt[3], const float aff[2], const TraceSettings& s,
+            int32_t* diag = nullptr);
 
 }  // namespace orc
 
@@ -40,6 +69,10 @@ int orc_ip_init(int n, const float* dI_host, int w, int h, const int32_t* u, con
 void orc_ip_trace(int n, const float* dI, int w, int h, const float* KRKi9, const float* Kt3, const float* aff2, const float* u, const float* v,
                   const float* color8, const float* weights8, const float* gradH4, const float* energyTH, float* idepth_min, float* idepth_max,
                   float* quality, int32_t* status, float* lastTraceUV2, float* lastTracePixelInterval);
+// orc_ip_trace plus diag[n * IPD_N] (see IPD_* / IPX_*)
+void orc_ip_trace_diag(int n, const float* dI, int w, int h, const float* KRKi9, const float* Kt3, const float* aff2, const float* u, const float* v,
+                       const float* color8, const float* weights8, const float* gradH4, const float* energyTH, float* idepth_min, float* idepth_max,
+                       float* quality, int32_t* status, float* lastTraceUV2, float* lastTracePixelInterval, int32_t* diag);
 }
 
 extern "C" {

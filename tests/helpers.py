@@ -929,3 +929,158 @@ def ci_poison(first, new, pts0, st, k4, synth):
     j = inside[len(inside) // 2]
     new[int(Kv[j]), int(Ku[j]), 0] = np.nan
     return first, new
+
+
+# ---------------------------------------------------------------------------------------------------------------------------------
+# Immature-point tracing scenes past one warp round of the search (tests/test_ref_pin_ip.py, tests/test_gpu_ip_edges.py)
+# ---------------------------------------------------------------------------------------------------------------------------------
+def ip_num_steps(w, h):
+    """the discrete search's step count for a fresh point (idepth_max = NaN: dist = maxPixSearch), before the clamp at 99"""
+    return int(np.float32(1.9999) + np.float32(w + h) * np.float32(0.027))
+
+
+def ip_scene(synth, w, h, seed, poses, quantize=False, nan_boxes=None):
+    """A textured plane at depth 2 seen by frame 0 (identity) and by one frame per pose xi (6,); the dict carries what
+    hostmath.trace_tables reads (K as make_window, state 0: aff = (1, 0)) and the level-0 planes dI.
+
+    The fresh search runs from the point at infinity (uMin = the host pixel) towards the plane; with a translation (t, 0, t) the plane's
+    disparity f t (1 - x/f) / (2 + t) sweeps [0, 2 f t / (2 + t)] across the image, so choosing f t ~ numSteps puts best steps in every
+    lane round.  quantize: 8-bit frames after a contrast stretch, with wide bands clipped to 0 (exact ties: a point whose pattern lies in
+    such a band matches every step of the band with energy 0).  nan_boxes: {frame: [(x0, y0, x1, y1), ...]} NaN rectangles."""
+    rng = np.random.default_rng(seed)
+    K = (0.5 * w, 0.5 * w, 0.5 * w - 0.5, 0.5 * h - 0.5)
+    tex = synth.make_texture(rng, size=1024)
+    nf = 1 + len(poses)
+    R_eval, t_eval = np.zeros((nf, 3, 3)), np.zeros((nf, 3))
+    images, dI = [], []
+    for k in range(nf):
+        R, t = synth.se3_exp(np.zeros(6) if k == 0 else np.asarray(poses[k - 1], np.float64))
+        R_eval[k], t_eval[k] = R, t
+        img, _ = synth.render_plane(tex, K, R, t, w, h, 2.0, texel_per_unit=0.5 * K[0] / 2.0)
+        if quantize:
+            img = np.clip(np.round(3.0 * (img - 0.5 * 255) + 100.0), 0, 255).astype(np.float32)
+        d = synth.make_pyramid(img, 1)[0]
+        for (x0, y0, x1, y1) in (nan_boxes or {}).get(k, ()):
+            d[y0:y1, x0:x1, :] = np.nan
+        images.append(img)
+        dI.append(d.reshape(-1).copy())
+    return dict(w=w, h=h, nf=nf, K=np.array(K, np.float64), images=images, dI=dI, R_eval=R_eval, t_eval=t_eval, state=np.zeros((nf, 10)),
+                exposure=np.ones(nf, np.float32))
+
+
+def ip_points(rng, w, h, n, margin=6):
+    """n distinct integer pixels at least `margin` from the border (the ImmaturePoint pattern stays inside)"""
+    sel = rng.choice((w - 2 * margin) * (h - 2 * margin), n, replace=False)
+    return (margin + sel % (w - 2 * margin)).astype(np.int32), (margin + sel // (w - 2 * margin)).astype(np.int32)
+
+
+# shapes whose fresh search reaches lane rounds past the first: numSteps = 46, 55, 82, 99 (105 before the clamp)
+IP_ROUND_SHAPES = [(848, 800, 11), (1280, 720, 12), (1920, 1080, 13), (2560, 1280, 14)]
+IP_TRACE_SEQ = (1, 2, 1)   # fresh points, refinement against another frame, re-tracing (traceNewCoarse on successive frames)
+
+
+def ip_poses(w, h):
+    """frame 1: translation (t, 0, t) with f t = numSteps, so best steps fall in every round the search has; frame 2: a smaller motion
+    (the refinement: short segments, numSteps <= 10 for most points)"""
+    t = ip_num_steps(w, h) / (0.5 * w)
+    return [np.array([t, 0, t, 0.002, -0.003, 0.001]), np.array([-0.3 * t, 0.2 * t, 0.2 * t, 0.001, 0.002, -0.001])]
+
+
+def ip_round_case(synth, orc, w, h, seed, n=1500, quantize=False, nan_boxes=None):
+    S = ip_scene(synth, w, h, seed, ip_poses(w, h), quantize=quantize, nan_boxes=nan_boxes)
+    u, v = ip_points(np.random.default_rng(seed), w, h, n)
+    return S, orc.ip_init(S["dI"][0], w, h, u, v)
+
+
+# NaN rectangles at the same place in both traced frames: segments and GN patterns cross them (the +1e5 branches), and points that fail
+# the energy test against frame 1 fail it again against frame 2 (OUTLIER, then OOB)
+IP_NAN_BOXES = [(500, 250, 700, 450), (900, 0, 903, 720), (0, 600, 1280, 602)]   # a block, a column and a row
+
+
+def ip_status_case(synth, orc, n=2000, seed=21):
+    w, h = 1280, 720
+    return ip_round_case(synth, orc, w, h, seed, n, nan_boxes={1: IP_NAN_BOXES, 2: IP_NAN_BOXES})
+
+
+def ip_gn_oob_case(w=640, h=480, theta=-0.03, n=2000):
+    """Points whose Gauss-Newton refinement walks a pattern sample off the left border (traceOn's OOB return inside the GN loop).
+
+    Where it can happen: uMin > boundU = max(4, maxRotPatX + 2) and the first search position is uMin - randShift dx > uMin - 1; each GN
+    iteration moves at most 0.5 px and the bound test runs before the update, so the last test is at >= uMin - randShift - 1, and a pattern
+    sample at >= uMin - randShift - 1 - |rot|.  With |rot| < 2 that stays > 1: only |rot| > 2 (KRKi[0][0] > 1, a rotation about y of the
+    sign of theta) and uMin within 2 - |rot| + randShift - 1 of 4 can reach posU < 0.  Here KRKi is K Ry(theta) K^-1 (|rot| = 2 KRKi[0][0]
+    ~ 2.04), the search runs along +x (Kt = K (0.05, 0, 0)), the frame is a ramp I = 2 x, and the points' colours are that ramp 3 px left of
+    the pattern, so the search picks step 0 and every GN step is -0.5.  The host positions u sweep uMin over [3.99, 4.05] in n steps: the oracle's diag
+    tells which of them exit by GN OOB.  Returns (P, dI, w, h, KRKi, Kt, aff)."""
+    f, cx, cy = 0.5 * w, 0.5 * w - 0.5, 0.5 * h - 0.5
+    K = np.array([[f, 0, cx], [0, f, cy], [0, 0, 1]], np.float64)
+    c, s = np.cos(theta), np.sin(theta)
+    R = np.array([[c, 0, s], [0, 1, 0], [-s, 0, c]])
+    KRKi = (K @ R @ np.linalg.inv(K)).astype(np.float32)
+    Kt = (K @ np.array([0.05, 0, 0])).astype(np.float32)
+    xs = np.arange(w, dtype=np.float32)
+    d = np.zeros((h, w, 3), np.float32)
+    d[:, :, 0] = 2 * xs[None, :]
+    d[:, :, 1] = 2
+    v = np.full(n, 0.5 * h, np.float32)
+    Ki = np.linalg.inv(KRKi.astype(np.float64))
+    u = np.array([(Ki @ np.array([um, 0.5 * h, 1.0]))[0] / (Ki @ np.array([um, 0.5 * h, 1.0]))[2] for um in np.linspace(3.99, 4.05, n)], np.float32)
+    pat = np.array([[0, -2], [-1, -1], [1, -1], [-2, 0], [0, 0], [2, 0], [-1, 1], [0, 2]], np.float32)
+    rotx = KRKi[0, 0] * pat[:, 0] + KRKi[0, 1] * pat[:, 1]
+    uMin = (KRKi[0, 0] * u + KRKi[0, 1] * v + KRKi[0, 2]) / (KRKi[2, 0] * u + KRKi[2, 1] * v + KRKi[2, 2])
+    P = dict(u=u, v=v, color=(2 * (uMin[:, None] - 3 + rotx[None, :])).astype(np.float32), weights=np.ones((n, 8), np.float32),
+             gradH=np.tile(np.array([32, 0, 0, 32], np.float32), (n, 1)), energyTH=np.full(n, 1152, np.float32),
+             idepth_min=np.zeros(n, np.float32), idepth_max=np.full(n, np.nan, np.float32), quality=np.full(n, 10000, np.float32),
+             status=np.full(n, 5, np.int32), lastTraceUV=np.zeros((n, 2), np.float32), lastTracePixelInterval=np.zeros(n, np.float32))
+    return P, d.reshape(-1), w, h, KRKi, Kt, np.array([1, 0], np.float32)
+
+
+def activation_edge_case(synth, orc, nf, n, seed, nan_frames=(), flat=True):
+    """activation_case's window and points, with hosts in every frame (the newest included), points down to 3 px from the border (their
+    patterns leave the image in some targets part-way through: the sums keep the samples before the first bad one), NaN blocks in the
+    level-0 planes of nan_frames, and a flat block (I = 128, no gradient) at the same place in every frame: points there have Hdd = 0,
+    below setting_minIdepthH_act (status 0)."""
+    W = synth.make_window(nf=nf, npts=50, seed=seed, trans=0.06, rot=0.01, hosts="all")
+    w, h = W["w"], W["h"]
+    for f in range(nf):
+        d = W["dI"][f].reshape(h, w, 3)
+        d[200:280, 280:360] = (128.0, 0.0, 0.0)
+        if f in nan_frames:
+            d[60:120, 440:520] = np.nan
+    rng = np.random.default_rng(seed)
+    host = np.sort(np.concatenate([np.arange(nf), rng.integers(0, nf, n - nf)])).astype(np.int32)
+    edge = rng.random(n) < 0.3
+    u = np.where(edge, rng.choice(np.r_[3:12, w - 12:w - 4], n), rng.integers(3, w - 4, n))
+    v = rng.integers(3, h - 4, n)
+    flat_pts = rng.random(n) < 0.05
+    u = np.where(flat_pts, rng.integers(305, 335, n), u); v = np.where(flat_pts, rng.integers(225, 255, n), v)
+    parts = [orc.ip_init(W["dI"][hh], w, h, u[host == hh], v[host == hh]) for hh in range(nf)]
+    P = {k: np.concatenate([p[k] for p in parts]) for k in parts[0]}
+    idt = (0.5 * (1 + 0.02 * rng.standard_normal(n))).astype(np.float32)
+    wide = rng.random(n) < 0.5
+    P["idepth_min"] = (idt * np.where(wide, 0.7, 0.97)).astype(np.float32)
+    P["idepth_max"] = (idt * np.where(wide, 1.4, 1.03)).astype(np.float32)
+    bad = rng.random(n) < 0.03
+    P["idepth_min"][bad] *= 3; P["idepth_max"][bad] *= 3
+    return W, host, P
+
+
+def activation_partial_oob(W, RT, calib6, host, P, status, idepth, res_state, margin=0.5):
+    """(point, target) pairs of activated points whose residual is OOB with its first pattern sample inside the image and a later one
+    outside, each by more than `margin` px at the point's final inverse depth (projectPoint in float64)"""
+    nf, w, h = W["nf"], W["w"], W["h"]
+    fx, fy, cx, cy, fxi, fyi = (float(x) for x in calib6)
+    pat = np.array([[0, -2], [-1, -1], [1, -1], [-2, 0], [0, 0], [2, 0], [-1, 1], [0, 2]], np.float64)
+    RT = np.asarray(RT, np.float64).reshape(nf * nf, 12)
+    out = []
+    for i, f in zip(*np.nonzero((np.asarray(res_state) == 1) & (np.asarray(status) == 1)[:, None])):
+        M = RT[host[i] * nf + f]
+        R, t = M[:9].reshape(3, 3), M[9:]
+        Kp = np.stack([(P["u"][i] + pat[:, 0] - cx) * fxi, (P["v"][i] + pat[:, 1] - cy) * fyi, np.ones(8)])
+        q = R @ Kp + t[:, None] * float(idepth[i])
+        Ku, Kv = q[0] / q[2] * fx + cx, q[1] / q[2] * fy + cy
+        inside = (Ku > 1.1 + margin) & (Kv > 1.1 + margin) & (Ku < w - 3 - margin) & (Kv < h - 3 - margin)
+        outside = (Ku < 1.1 - margin) | (Kv < 1.1 - margin) | (Ku > w - 3 + margin) | (Kv > h - 3 + margin)
+        if inside[0] and outside[1:].any():
+            out.append((i, f))
+    return out

@@ -37,7 +37,7 @@ def test_trace_bit_exact(capi, orc, synth, cfg):
             np.testing.assert_array_equal(Qg[k], Qo[k], err_msg=f"frame {new}: {k}")
         seen += np.bincount(Qo["status"], minlength=6)
         st = Qo
-    assert seen[0] > 0 and seen[1] > 0
+    assert (seen[:5] > 0).all(), seen   # GOOD, OOB, OUTLIER, SKIPPED, BADCONDITION all exercised
     g.close()
 
 
