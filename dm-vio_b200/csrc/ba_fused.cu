@@ -477,7 +477,11 @@ __device__ __forceinline__ void fused_chunk(const BAWinDev& W, const BAIter& it,
     // and the residual's part of the point's Schur vector
     float jp[8] = {0.f, 0.f, 0.f, 0.f, 0.f, 0.f, 0.f, 0.f}, Hdd = 0.f, bd = 0.f, Hcd0 = 0.f, Hcd1 = 0.f, Hcd2 = 0.f, Hcd3 = 0.f;
     if (in) {
-      if constexpr (!MARG) geo_jac(pc, Kl0, Kl1, cu, cv, drescale, new_idepth, fx, fy, fxi, fyi, x, y, ddx, ddy);
+      // evaluated here in the marginalisation launch too, although its res_toZeroF already needed them above: only here does the compiler
+      // see that x[5], y[4] are 0 and x[6], x[7], x[9], y[6], y[7] negations, and it contracts jp's products into FMAs accordingly.  Fed
+      // from the earlier evaluation, jp was contracted differently and rounded differently, so the launch's Schur vectors (Msc, Mbsc)
+      // differed in the last bits from the plain launch's on the same residuals.  The plain kernels compile to the same code as before.
+      geo_jac(pc, Kl0, Kl1, cu, cv, drescale, new_idepth, fx, fy, fxi, fyi, x, y, ddx, ddy);
       const float J0 = s.JI00 * ddx + s.JI10 * ddy, J1 = s.JI10 * ddx + s.JI11 * ddy;  // JIdx2 * Jpdd
 #pragma unroll
       for (int k = 0; k < 6; k++) jp[k] = x[4 + k] * J0 + y[4 + k] * J1;
@@ -749,7 +753,7 @@ __device__ __forceinline__ void fused_chunk(const BAWinDev& W, const BAIter& it,
     // ---- takeDataF, per-point terms, Schur-vector rows (split over the lanes)
     float jp[8] = {0.f, 0.f, 0.f, 0.f, 0.f, 0.f, 0.f, 0.f}, Hdd = 0.f, bd = 0.f, Hcd0 = 0.f, Hcd1 = 0.f, Hcd2 = 0.f, Hcd3 = 0.f;
     if (in) {
-      if constexpr (!MARG) geo_jac(pc, Kl0, Kl1, cu, cv, drescale, new_idepth, fx, fy, fxi, fyi, x, y, ddx, ddy);
+      geo_jac(pc, Kl0, Kl1, cu, cv, drescale, new_idepth, fx, fy, fxi, fyi, x, y, ddx, ddy);  // also when MARG: see phase A (LPR = 1)
       const float J0 = s.JI00 * ddx + s.JI10 * ddy, J1 = s.JI10 * ddx + s.JI11 * ddy;
 #pragma unroll
       for (int k = 0; k < 6; k++) jp[k] = x[4 + k] * J0 + y[4 + k] * J1;

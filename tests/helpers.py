@@ -91,10 +91,106 @@ def check_phase_b(pg, good, priorF, idepth, idepth_zero):
     assert not pg["HdiF"][~good].any() and not pg["bdSumF"][~good].any()
 
 
-def check_linearize_parity(ow, ba, r, E_o):
+EPS32 = float(np.finfo(np.float32).eps)
+EPS64 = float(np.finfo(np.float64).eps)
+# check_system tau of the GPU-vs-oracle comparisons (check_linearize_parity, tests/test_gpu_marg.py).  The two sides differ by per-residual
+# rounding (rtol <= 2e-3), so 4e-3 is a hard ceiling.  Worst ratios measured on an H100 (SXM, 80 GB) over every config of
+# tests/test_gpu_ba.py and tests/test_gpu_ba_step.py at both chunk shapes: H_A 3.7e-6, b_A 1.5e-5, H_sc 5.5e-6, b_sc 1.7e-5;
+# tests/test_gpu_marg.py: M 4.6e-6, Mb 4.3e-6, Msc 8.6e-6, Mbsc 3.0e-6; the oracle's own faithful-float system against its fp64 one:
+# <= 7.7e-7.  tau = ~10x the worst.
+SYSTEM_TAU = 2e-4
+FRAME_PARAMS = ("trans x", "trans y", "trans z", "rot x", "rot y", "rot z", "a", "b")   # order of a frame's 8 parameters in the system
+
+
+def system_entry_name(i):
+    """row / column i of a window system [camera 4 | frame 0 (8) | frame 1 (8) | ...] in words"""
+    return f"camera {i}" if i < 4 else f"frame {(i - 4) // 8} {FRAME_PARAMS[(i - 4) % 8]}"
+
+
+def check_system(H, b, H_ref, b_ref, R, tau, what="system"):
+    """Per-entry check of an accumulated system (H, b) against a reference (H_ref, b_ref), each entry on its own Jacobi scale.
+
+    The systems are sums of Gram terms (sum J^T J with right-hand side sum J^T r, or sum HdiF v v^T with sum HdiF bdSum v), so by
+    Cauchy-Schwarz the absolute sum behind H_ij is at most sqrt(H_ii H_jj) and that behind b_i at most sqrt(H_ii R), R a bound of the
+    summed squared residuals (sum of the IN residuals' energies, sum HdiF bdSumF^2, sum res_toZeroF^2).  With d = diag(H_ref):
+      |H_ij - H_ref_ij| <= tau sqrt(d_i d_j),   |b_i - b_ref_i| <= tau sqrt(d_i R),
+    and where d_i = 0 the entries of row / column i are exactly 0 on both sides.  A failure names the entry (camera, or frame + parameter).
+    Returns the worst ratios |error| / sqrt(...) of H and of b (what tau must exceed)."""
+    H, b, Hr, br = (np.asarray(a, np.float64) for a in (H, b, H_ref, b_ref))
+    d = np.diag(Hr)
+    assert np.all(d >= 0), f"{what}: negative reference diagonal at {system_entry_name(int(np.argmin(d)))}"
+    s = np.sqrt(d)
+    ratios = []
+    for name, got, ref, scale in (("H", H, Hr, np.outer(s, s)), ("b", b, br, s * np.sqrt(max(float(R), 0.0)))):
+        zero = scale == 0
+        nz = zero & ((got != 0) | (ref != 0))
+        if nz.any():
+            idx = np.unravel_index(int(np.argmax(nz)), nz.shape)
+            where = ", ".join(system_entry_name(int(i)) for i in idx)
+            raise AssertionError(f"{what}: {name}[{where}] = {got[idx]:.6e} / reference {ref[idx]:.6e} where the reference diagonal is 0")
+        ratio = np.abs(got - ref) / np.where(zero, 1.0, scale)
+        worst = np.unravel_index(int(np.argmax(ratio)), ratio.shape)
+        where = ", ".join(system_entry_name(int(i)) for i in worst)
+        assert ratio[worst] <= tau, (f"{what}: {name}[{where}] = {got[worst]:.9e}, reference {ref[worst]:.9e}: |error| = "
+                                     f"{ratio[worst]:.3e} x its Jacobi scale {scale[worst]:.3e} > tau = {tau:.1e}")
+        ratios.append(float(ratio[worst]))
+    return tuple(ratios)
+
+
+def energy_bound(newState, newEnergy):
+    """R of check_system for a top system: the sum of newEnergy over the IN residuals.  It bounds sum resF^2: a pixel's energy is
+    w^2 hw r^2 (2 - hw) and its resF^2 = w^2 hw r^2, with Huber's 2 - hw >= 1."""
+    return float(np.asarray(newEnergy, np.float64)[np.asarray(newState) == RES_IN].sum())
+
+
+def schur_bound(HdiF, bdSumF):
+    """R of check_system for a Schur system: sum_p HdiF bdSumF^2"""
+    return float((np.asarray(HdiF, np.float64) * np.asarray(bdSumF, np.float64) ** 2).sum())
+
+
+def schur_vectors(W, state, JpJdF, Hcd, adH, adT):
+    """The points' Schur vectors v_p in R^N (N = 8 nf + 4) from fp32 committed outputs, in fp64, and the same sums over absolute values:
+      v_p[0:4] = Hcd_p;  every IN residual (host h, target t) adds adHostF[h + t nf] @ JpJdF to frame block h and
+      diag(adTargetF[h + t nf]) o JpJdF to frame block t (adjoints rounded to fp32 and indexed as dmv_ba_set_adjoints reads them)."""
+    nf, npts = W["nf"], len(W["host"])
+    N = 8 * nf + 4
+    AH = np.asarray(adH).astype(np.float32).astype(np.float64)
+    AT = np.einsum("ikk->ik", np.asarray(adT)).astype(np.float32).astype(np.float64)
+    V, Va = np.zeros((npts, N)), np.zeros((npts, N))
+    V[:, :4] = np.asarray(Hcd, np.float32)
+    Va[:, :4] = np.abs(V[:, :4])
+    inn = np.asarray(state) == RES_IN
+    rp, rt = np.asarray(W["res_point"])[inn], np.asarray(W["res_target"])[inn]
+    J = np.asarray(JpJdF, np.float32)[inn].astype(np.float64)
+    rh = np.asarray(W["host"])[rp]
+    for h in range(nf):
+        for t in range(nf):
+            m = (rh == h) & (rt == t)
+            if h == t or not m.any():
+                continue
+            p, Jm = rp[m], J[m]
+            A, dT = AH[h + t * nf], AT[h + t * nf]
+            np.add.at(V, (p[:, None], 4 + 8 * h + np.arange(8)[None, :]), Jm @ A.T)
+            np.add.at(Va, (p[:, None], 4 + 8 * h + np.arange(8)[None, :]), np.abs(Jm) @ np.abs(A).T)
+            np.add.at(V, (p[:, None], 4 + 8 * t + np.arange(8)[None, :]), Jm * dT)
+            np.add.at(Va, (p[:, None], 4 + 8 * t + np.arange(8)[None, :]), np.abs(Jm * dT))
+    return V, Va
+
+
+def schur_reference(W, state, JpJdF, Hcd, HdiF, bdSumF, adH, adT):
+    """H_sc = sum_p HdiF_p v_p v_p^T, b_sc = sum_p HdiF_p bdSumF_p v_p in fp64 (schur_vectors), and Habs / babs: the same sums over the
+    absolute value of every product (|v_p| taken term by term).  Returns Hsc, bsc, Habs, babs."""
+    V, Va = schur_vectors(W, state, JpJdF, Hcd, adH, adT)
+    hd = np.asarray(HdiF, np.float32).astype(np.float64)
+    bs = np.asarray(bdSumF, np.float32).astype(np.float64)
+    return (V * hd[:, None]).T @ V, V.T @ (hd * bs), (Va * np.abs(hd)[:, None]).T @ Va, Va.T @ np.abs(hd * bs)
+
+
+def check_linearize_parity(ow, ba, r, E_o, tau=None):
     """A GPU linearisation (result r, still tentative) against the oracle's (energy E_o of ow.linearize_all), then both committed and
-    accumulated.  Tolerances and their reasons: tests/test_gpu_ba.py's docstring.  Returns the GPU's (residual outputs, point outputs,
-    accumulated system)."""
+    accumulated.  Tolerances and their reasons: tests/test_gpu_ba.py's docstring; the accumulated systems are compared entry by entry
+    (check_system, tau = SYSTEM_TAU by default).  Returns the GPU's (residual outputs, point outputs, accumulated system); the worst
+    check_system ratios are in the system's "ratios" entry."""
     o = ow.res_outputs(False)
     g = ba.residual_outputs()
     # ---- states: identical except threshold ties
@@ -138,6 +234,12 @@ def check_linearize_parity(ow, ba, r, E_o):
     assert rel(a_g["bA"], a_o["bA"]) < 1e-4
     assert rel(a_g["Hsc"], a_o["Hsc"]) < 1e-5
     assert rel(a_g["bsc"], a_o["bsc"]) < 1e-4
+    # ---- entry by entry: whole-matrix ratios only see the largest blocks (the camera block holds ~5e-5 of ||H_A||_F)
+    tau = SYSTEM_TAU if tau is None else tau
+    a_g["ratios"] = (check_system(a_g["HA"], a_g["bA"], a_o["HA"], a_o["bA"], energy_bound(o["newState"], o["newEnergy"]), tau, "top system")
+                     + check_system(a_g["Hsc"], a_g["bsc"], a_o["Hsc"], a_o["bsc"], schur_bound(po["HdiF"], po["bdSumF"]), tau, "Schur system"))
+    print(f"check_system vs oracle: worst |error| / Jacobi scale: HA {a_g['ratios'][0]:.2e} bA {a_g['ratios'][1]:.2e} "
+          f"Hsc {a_g['ratios'][2]:.2e} bsc {a_g['ratios'][3]:.2e}")
     # invariants that hold regardless of ties
     assert np.abs(a_g["HA"] - a_g["HA"].T).max() <= 1e-9 * np.abs(a_g["HA"]).max()
     assert np.abs(a_g["Hsc"] - a_g["Hsc"].T).max() <= 1e-9 * np.abs(a_g["Hsc"]).max()

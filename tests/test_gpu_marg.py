@@ -3,11 +3,13 @@ the reference's compiled fixLinearizationF / marginalizePointsF (tests/test_ref_
 
 Tolerances: the same reasoning as tests/test_gpu_ba.py — per-residual vectors (res_toZeroF) rtol 2e-3 of their scale with a small median
 error, the summed systems ||d||_F/||.||_F <= 1e-5 (H) and 2e-4 (b: signed sums; res_toZeroF adds one more cancellation than resF) against
-the fp64-accumulating oracle."""
+the fp64-accumulating oracle, and entry by entry (helpers.check_system at SYSTEM_TAU) with R = sum res_toZeroF^2 for both systems: it
+bounds sum J^T rtz by Cauchy-Schwarz, and per point HdiF bd^2 <= bd^2 / Hdd <= the point's sum rtz^2, so it bounds sum_p HdiF bd^2 too.
+This window has idepth_zero != idepth: the only test of the depth-delta term of res_toZeroF."""
 import numpy as np
 import pytest
 
-from helpers import product_ba_from_oracle, rel
+from helpers import SYSTEM_TAU, check_system, product_ba_from_oracle, rel
 
 pytestmark = pytest.mark.gpu
 
@@ -67,6 +69,10 @@ def test_marginalize_points_parity(capi, orc, synth, cfg, frac, P):
     assert rel(g["M"], o["M"]) < 1e-5 and rel(g["Msc"], o["Msc"]) < 1e-5
     assert rel(g["H"], o["H"]) < 1e-5
     assert rel(g["Mb"], o["Mb"]) < 2e-4 and rel(g["Mbsc"], o["Mbsc"]) < 2e-4 and rel(g["b"], o["b"]) < 2e-4
+    R = float((o["rtz"].astype(np.float64) ** 2).sum())
+    r = (check_system(g["M"], g["Mb"], o["M"], o["Mb"], R, SYSTEM_TAU, "marginalisation M, Mb")
+         + check_system(g["Msc"], g["Mbsc"], o["Msc"], o["Mbsc"], R, SYSTEM_TAU, "marginalisation Msc, Mbsc"))
+    print(f"check_system vs oracle: worst |error| / Jacobi scale: M {r[0]:.2e} Mb {r[1]:.2e} Msc {r[2]:.2e} Mbsc {r[3]:.2e}")
     assert np.allclose(g["M"], g["M"].T) and np.allclose(g["Msc"], g["Msc"].T, rtol=1e-12, atol=0)
     ba.close()
 
