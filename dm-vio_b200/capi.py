@@ -46,6 +46,13 @@ class BAActivateArgs(C.Structure):
                [("minObs", C.c_int)] + [(k, C.c_void_p) for k in ("status", "idepth", "res_state")]
 
 
+class BASelectArgs(C.Structure):
+    _fields_ = [("nf", C.c_int), ("newest", C.c_int), ("tables12", vp), ("flagged", vp), ("n_active", C.c_int)] + \
+               [(k, vp) for k in ("act_u", "act_v", "act_idepth_scaled", "act_host", "imm_offset", "u", "v", "idepth_min", "idepth_max", "lastTraceStatus",
+                                  "lastTracePixelInterval", "quality", "my_type")] + \
+               [("currentMinActDist", C.c_float), ("minTraceQuality", C.c_float), ("cap", C.c_int)] + [(k, vp) for k in ("n_opt", "action", "opt_idx", "map", "stats")]
+
+
 class BAMargArgs(C.Structure):
     _fields_ = [("n", C.c_int32), ("point", C.c_void_p), ("adHTdeltaF", C.c_void_p), ("cDeltaF", C.c_float * 4), ("idepthFixPriorMargFac", C.c_float)] + \
                [(k, C.c_void_p) for k in ("M", "Mb", "Msc", "Mbsc", "resInM", "ngoodRes", "res_toZeroF", "isLinearized")]
@@ -165,7 +172,7 @@ SYMBOLS = [
     "dmv_ba_set_window", "dmv_ba_set_points", "dmv_ba_set_residuals", "dmv_ba_set_adjoints", "dmv_ba_set_state", "dmv_ba_linearize",
     "dmv_ba_get_residual_outputs", "dmv_ba_get_target_energies", "dmv_ba_apply_res", "dmv_ba_accumulate", "dmv_ba_get_point_outputs", "dmv_ba_get_solve_HdiF",
     "dmv_ba_resubstitute", "dmv_ba_backup_points", "dmv_ba_restore_points", "dmv_ba_get_idepth", "dmv_ba_gn_step", "dmv_nccl_unique_id",
-    "dmv_ba_comm_init", "dmv_ba_activate_points", "dmv_ba_marginalize_points", "dmv_ba_drop_residuals", "dmv_ba_reset_oob", "dmv_ba_p2p_export", "dmv_ba_p2p_import", "dmv_ba_last_timing", "dmv_ba_bench_device", "dmv_ba_bench_phases", "dmv_ba_kernel_launch_count", "dmv_ba_io_bytes", "dmv_ba_set_timing", "dmv_ba_bench_e2e",
+    "dmv_ba_comm_init", "dmv_ba_activate_points", "dmv_ba_select_activation", "dmv_ba_marginalize_points", "dmv_ba_drop_residuals", "dmv_ba_reset_oob", "dmv_ba_p2p_export", "dmv_ba_p2p_import", "dmv_ba_last_timing", "dmv_ba_bench_device", "dmv_ba_bench_phases", "dmv_ba_kernel_launch_count", "dmv_ba_io_bytes", "dmv_ba_set_timing", "dmv_ba_bench_e2e",
     "dmv_ba_batch_create", "dmv_ba_batch_destroy", "dmv_ba_batch_gn_step", "dmv_ba_batch_set_timing", "dmv_ba_batch_last_kernel_ms", "dmv_ba_batch_bench",
     "dmv_ct_create", "dmv_ct_destroy", "dmv_ct_set_K", "dmv_ct_set_ref", "dmv_ct_make_coarse_depth", "dmv_ct_set_ref_from_ba", "dmv_ct_get_ref", "dmv_ct_upload_new", "dmv_ct_upload_new_image", "dmv_ct_set_huber",
     "dmv_ci_create", "dmv_ci_destroy", "dmv_ci_set_K", "dmv_ci_upload_first", "dmv_ci_upload_new", "dmv_ci_set_points", "dmv_ci_calc_res_and_gs", "dmv_ci_kernel_launch_count",
@@ -207,6 +214,7 @@ def lib():
         L.dmv_nccl_unique_id.argtypes = [vp]
         L.dmv_ba_comm_init.argtypes = [vp, C.c_int, C.c_int, vp]
         L.dmv_ba_activate_points.argtypes = [vp, C.POINTER(BAActivateArgs)]
+        L.dmv_ba_select_activation.argtypes = [vp, C.POINTER(BASelectArgs)]
         L.dmv_ba_marginalize_points.argtypes = [vp, C.POINTER(BAMargArgs)]
         L.dmv_ba_drop_residuals.argtypes = [vp, C.c_int, i32p]
         L.dmv_ba_reset_oob.argtypes = [vp]
@@ -466,6 +474,28 @@ class BA:
         args = BAActivateArgs(n, *[a.ctypes.data for a in keep], int(minObs), status.ctypes.data, idepth.ctypes.data, rs.ctypes.data)
         check(self.L.dmv_ba_activate_points(self.h, C.byref(args)))
         return status, idepth, rs
+
+    def select_activation(self, nf, newest, tables12, flagged, act_u, act_v, act_idepth_scaled, act_host, imm_offset, imm, min_act_dist,
+                          min_trace_quality=3.0, cap=None, want_map=True):
+        """FullSystem::activatePointsMT up to activatePointsMT_Reductor (dmv_ba_select_activation): imm = dict of the immature points' u, v,
+        idepth_min, idepth_max, status, interval, quality, type, grouped by host as imm_offset says.  Returns (action: 0 keep / 1 delete /
+        2 optimise, toOptimize indexes, level-1 map (h/2, w/2) or None, stats dict: undecided candidates, floods run, rounds of the chain)."""
+        off = _c(imm_offset, np.int32)
+        n = int(off[-1])
+        keep = [_c(tables12, np.float32), _c(flagged, np.uint8), _c(act_u, np.float32), _c(act_v, np.float32), _c(act_idepth_scaled, np.float32),
+                _c(act_host, np.int32), off] + [_c(imm[k], t) for k, t in (("u", np.float32), ("v", np.float32), ("idepth_min", np.float32),
+                ("idepth_max", np.float32), ("status", np.int32), ("interval", np.float32), ("quality", np.float32), ("type", np.float32))]
+        cap = n if cap is None else int(cap)
+        action, opt = np.zeros(max(n, 1), np.int32), np.zeros(max(cap, 1), np.int32)
+        m = np.zeros((self.hh // 2, self.w // 2), np.float32) if want_map else None
+        n_opt, stats = C.c_int(0), np.zeros(3, np.int32)
+        a = BASelectArgs(int(nf), int(newest), keep[0].ctypes.data, keep[1].ctypes.data, len(keep[2]), *[k.ctypes.data for k in keep[2:]],
+                         float(min_act_dist), float(min_trace_quality), cap, C.addressof(n_opt), action.ctypes.data, opt.ctypes.data,
+                         m.ctypes.data if want_map else None, stats.ctypes.data)
+        rc = self.L.dmv_ba_select_activation(self.h, C.byref(a))
+        if rc != 0:
+            raise DmvError(f"dmvio_b200 error {rc}: {lib().dmv_last_error().decode()}", n_opt.value)
+        return action[:n], opt[:n_opt.value].copy(), m, dict(undecided=int(stats[0]), floods=int(stats[1]), rounds=int(stats[2]))
 
     def reset_oob(self):
         check(self.L.dmv_ba_reset_oob(self.h))

@@ -184,6 +184,7 @@ int dmv_ba_destroy(dmv_ba* b) {
   for (int i = 0; i < 4; i++) if (b->ev[i]) cudaEventDestroy(b->ev[i]);
   if (b->nccl_comm) dmv::nccl_destroy(b->nccl_comm);
   cudaFree(b->d_act); cudaFreeHost(b->h_act);
+  cudaFree(b->d_sel); cudaFreeHost(b->h_sel);
   cudaFree(b->d_marg); cudaFree(b->d_marg_mask); cudaFree(b->d_marg_rtz); cudaFree(b->d_marg_result);
   cudaFreeHost(b->h_marg_result);
   for (int r = 0; r < XCHG_MAXR; r++)

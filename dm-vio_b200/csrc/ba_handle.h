@@ -100,6 +100,9 @@ struct dmv_ba {
   float* d_act = nullptr;      // point-activation staging (dmv_ba_activate_points)
   float* h_act = nullptr;
   int act_cap = 0;
+  float* d_sel = nullptr;      // activation-selection staging and scratch (dmv_ba_select_activation, ip_select.cu)
+  float* h_sel = nullptr;
+  size_t sel_words = 0;
   // peer-memory exchange (inside ba_fused_kernel)
   void* xchg_own = nullptr;                 // this rank's inbox (cudaMalloc, exported through CUDA IPC)
   void* xchg_map[XCHG_MAXR] = {nullptr};    // every rank's inbox as mapped here ([rank] == xchg_own)

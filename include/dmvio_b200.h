@@ -180,6 +180,45 @@ typedef struct dmv_ba_activate_args {
 } dmv_ba_activate_args;
 int dmv_ba_activate_points(dmv_ba* ba, const dmv_ba_activate_args* a);
 
+/* Which immature points to activate: the part of FullSystem::activatePointsMT (FullSystem.cpp:L642-717) from coarseDistanceMap->makeK up to,
+ * not including, activatePointsMT_Reductor.  CoarseDistanceMap::makeDistanceMap (CoarseTracker.cpp:L931-967) projects the active points into
+ * the newest frame at pyramid level 1 and grows the distance map over (w/2) x (h/2) cells (growDistBFS, L979-1073); then the immature points of
+ * every other frame are deleted, kept, or accepted by the map, each accepted point flooding the map again (addIntoDistFinal, L1076-1082).
+ * All arrays are the caller's host memory.  Active points: any order; those hosted by the newest frame are skipped, as the reference skips
+ * that frame.  Immature points: grouped by host frame in frame order, host->immaturePoints order inside a group (imm_offset[f] .. imm_offset[f+1]);
+ * the newest frame's group is skipped (action keep).  tables12: per frame [KRKi 9 row-major | Kt 3], computed in float as the reference does:
+ * K[1] * R * Ki[0] and K[1] * t of newest->PRE_worldToCam * host->PRE_camToWorld.  lastTraceStatus: ImmaturePointStatus (dmv_ip_points).
+ * Results are BIT-IDENTICAL to the reference's CPU code.  No BA state is read or changed; only the handle's device, stream and image size
+ * are used.  Scratch (8 bytes per level-1 cell, 52 per immature point and 16 per active point, on the device and again in pinned host
+ * memory) is allocated on first use and grown when a call needs more.  Returns after one synchronisation.
+ * Errors: DMV_ERR_INVALID for bad arguments, or more accepted points than cap (*n_opt = the count needed; action is still written);
+ * DMV_ERR_CUDA. */
+enum { DMV_ACT_KEEP = 0, DMV_ACT_DELETE = 1, DMV_ACT_OPTIMIZE = 2 };
+typedef struct dmv_ba_select_args {
+  int nf;                       /* frames of the window (1 .. DMV_MAX_FRAMES) */
+  int newest;                   /* index of frameHessians.back() */
+  const float* tables12;        /* nf * 12 */
+  const uint8_t* flagged;       /* nf: FrameHessian::flaggedForMarginalization */
+  int n_active;
+  const float *act_u, *act_v, *act_idepth_scaled;
+  const int32_t* act_host;
+  const int32_t* imm_offset;    /* nf + 1, imm_offset[0] = 0 */
+  const float *u, *v, *idepth_min, *idepth_max;
+  const int32_t* lastTraceStatus;
+  const float *lastTracePixelInterval, *quality, *my_type;
+  float currentMinActDist;      /* as FullSystem::activatePointsMT leaves it after its update from ef->nPoints (L607-629) */
+  float minTraceQuality;        /* setting_minTraceQuality = 3 */
+  int cap;                      /* capacity of opt_idx */
+  int* n_opt;                   /* out: size of toOptimize (on overflow the count needed) */
+  int32_t* action;              /* out, imm_offset[nf] entries: DMV_ACT_KEEP / DMV_ACT_DELETE / DMV_ACT_OPTIMIZE */
+  int32_t* opt_idx;             /* out: indexes of the accepted points in toOptimize order */
+  float* map;                   /* optional ((w/2)*(h/2)): fwdWarpedIDDistFinal after the loop */
+  int* stats;                   /* optional out [3]: candidates the map before the loop could not decide (the only ones whose decision
+                                   waits for earlier floods), floods run (floods no later decision needs are skipped unless map is
+                                   requested), rounds of the chain (its serial depth) */
+} dmv_ba_select_args;
+int dmv_ba_select_activation(dmv_ba* ba, const dmv_ba_select_args* a);
+
 /* PointFrameResidual::resetOOB for every residual of the window, as FullSystem::optimize does when it collects activeResiduals
  * (FullSystem/FullSystemOptimize.cpp:L431-448; FullSystem/Residuals.h:L91-98): state IN, energy 0.  Discards the tentative and the committed
  * linearisation (the next dmv_ba_linearize / dmv_ba_gn_step starts from these states). */
