@@ -1,56 +1,47 @@
 """TEST INFRASTRUCTURE ONLY — bindings and cases of the activation-selection oracles (dmv_ba_select_activation).
 
-  restate(case)   liborc_activation.so: the CPU restatement of makeDistanceMap, growDistBFS, addIntoDistFinal and activatePointsMT's
-                  selection loop (orc_activation.cpp, built by activation.mk)
+  restate(case)   liborc.so: the CPU restatement of makeDistanceMap, growDistBFS, addIntoDistFinal and activatePointsMT's selection loop
+                  (orc_activation.cpp)
   reference(case) _ref/libactivation_ref.so: the REFERENCE's own CoarseDistanceMap around a line-for-line mirror of the loop
-                  (ref_activation.cpp, ref_build_activation.sh); also returns the [KRKi | Kt] tables it computed
+                  (ref_activation.cpp, built by ref_build.sh); also returns the [KRKi | Kt] tables it computed
   make_case(...)  seeded windows shared by the CPU pin, the golden fixture, the device tests and tools/bench_activation.py"""
 import ctypes as C
-import os
+import functools
 
 import numpy as np
 
-_HERE = os.path.dirname(os.path.abspath(__file__))
-ORC_PATH = os.path.join(_HERE, "liborc_activation.so")
-REF_PATH = os.path.join(_HERE, "_ref", "libactivation_ref.so")
-f32p = np.ctypeslib.ndpointer(np.float32, flags="C_CONTIGUOUS")
-f64p = np.ctypeslib.ndpointer(np.float64, flags="C_CONTIGUOUS")
-i32p = np.ctypeslib.ndpointer(np.int32, flags="C_CONTIGUOUS")
-u8p = np.ctypeslib.ndpointer(np.uint8, flags="C_CONTIGUOUS")
-_ORC = None
-_REF = None
+from . import orc, ref
+from .orc import f32p, f64p, i32p, u8p
+
+REF_LIB = "libactivation_ref.so"
 
 IMM_KEYS = ("u", "v", "idepth_min", "idepth_max", "status", "interval", "quality", "type")
 KEEP, DELETE, OPTIMIZE = 0, 1, 2
 MIN_TRACE_QUALITY = 3.0  # setting_minTraceQuality
 
 
+@functools.cache
 def orc_lib():
-    global _ORC
-    if _ORC is None:
-        L = C.CDLL(ORC_PATH)
-        L.orc_act_select.restype = C.c_int
-        L.orc_act_select.argtypes = [C.c_int, C.c_int, C.c_int, C.c_int, f32p, u8p, C.c_int, f32p, f32p, f32p, i32p, i32p, f32p, f32p, f32p, f32p, i32p,
-                                     f32p, f32p, f32p, C.c_float, C.c_float, i32p, i32p, f32p]
-        L.orc_act_grow.argtypes = [C.c_int, C.c_int, f32p, C.c_int, i32p]
-        _ORC = L
-    return _ORC
+    L = orc.lib()
+    L.orc_act_select.restype = C.c_int
+    L.orc_act_select.argtypes = [C.c_int, C.c_int, C.c_int, C.c_int, f32p, u8p, C.c_int, f32p, f32p, f32p, i32p, i32p, f32p, f32p, f32p, f32p, i32p,
+                                 f32p, f32p, f32p, C.c_float, C.c_float, i32p, i32p, f32p]
+    L.orc_act_grow.argtypes = [C.c_int, C.c_int, f32p, C.c_int, i32p]
+    return L
 
 
 def ref_available():
-    return os.path.exists(REF_PATH)
+    return ref.built(REF_LIB)
 
 
+@functools.cache
 def ref_lib():
-    global _REF
-    if _REF is None:
-        L = C.CDLL(REF_PATH, mode=C.RTLD_LOCAL)
-        L.ref_act_select.restype = C.c_int
-        L.ref_act_select.argtypes = [C.c_int, C.c_int, f64p, C.c_int, C.c_int, f64p, f64p, u8p, C.c_int, f32p, f32p, f32p, i32p, i32p, f32p, f32p, f32p,
-                                     f32p, i32p, f32p, f32p, f32p, C.c_float, C.c_float, i32p, i32p, f32p, f32p]
-        L.ref_act_grow.argtypes = [C.c_int, C.c_int, f32p, C.c_int, i32p]
-        _REF = L
-    return _REF
+    L = ref.open_ref(REF_LIB)
+    L.ref_act_select.restype = C.c_int
+    L.ref_act_select.argtypes = [C.c_int, C.c_int, f64p, C.c_int, C.c_int, f64p, f64p, u8p, C.c_int, f32p, f32p, f32p, i32p, i32p, f32p, f32p, f32p,
+                                 f32p, i32p, f32p, f32p, f32p, C.c_float, C.c_float, i32p, i32p, f32p, f32p]
+    L.ref_act_grow.argtypes = [C.c_int, C.c_int, f32p, C.c_int, i32p]
+    return L
 
 
 def _n(case):

@@ -1,7 +1,7 @@
 // TEST INFRASTRUCTURE ONLY — CPU restatement of the selection half of FullSystem::activatePointsMT (reference FullSystem.cpp:L642-717):
 // CoarseDistanceMap::makeDistanceMap (CoarseTracker.cpp:L931-967), growDistBFS (L979-1073), addIntoDistFinal (L1076-1082) and the loop over the
 // immature points of every other frame, serial and in the reference's order.  The oracle of dmv_ba_select_activation; pinned to the
-// reference's compiled CoarseDistanceMap by ref_activation.cpp (tests/test_ref_pin_activation.py).  Built by activation.mk with the reference's
+// reference's compiled CoarseDistanceMap by ref_activation.cpp (tests/test_ref_pin_activation.py).  Built into liborc.so with the reference's
 // flags (-O3, no -march).  Arguments as dmv_ba_select_args (include/dmvio_b200.h); actions 0 keep, 1 delete, 2 optimise.
 #include <cmath>
 #include <cstdint>

@@ -2,7 +2,7 @@
 // FullSystem::makeNewTraces (FullSystem.cpp:L1640-1667), the oracle of dmv_ct_make_new_traces.  select() stays the reference's literal
 // serial loop; it additionally counts the "mixed" pot-blocks it meets (a level-0 candidate under some of the 16 directions but not all),
 // the blocks the device resolves on its serial chain.  The ImmaturePoint constructor is the existing restatement (orc.ip_init, applied in
-// oracle/select.py).  Built into liborc_select.so by select.mk with the reference's flags.
+// oracle/select.py).  Built into liborc.so with the reference's flags.
 #include <algorithm>
 #include <cmath>
 #include <cstdint>

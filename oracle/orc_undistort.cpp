@@ -1,7 +1,7 @@
 // TEST INFRASTRUCTURE ONLY — CPU restatement of the per-frame part of Undistort::undistort<T> (src/dso/util/Undistort.cpp:L385-482)
 // with PhotometricUndistorter::processFrame (L213-252), on the same tables the reference builds once per sequence (remapX / remapY,
 // G, vignetteMapInv).  Same two passes and operation order as the reference: the photometric map over the whole raw image, then the
-// bilinear remap.  Built with the reference's flags (-O3, no -march: scalar SSE2, no FMA) by oracle/undistort.mk.
+// bilinear remap.  Built with the reference's flags (-O3, no -march: scalar SSE2, no FMA) into oracle/liborc.so.
 #include <cstring>
 #include <vector>
 

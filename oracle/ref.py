@@ -2,8 +2,10 @@
 compiled from /root/reference by oracle/ref_build.sh behind the C harness oracle/ref_harness.cpp.
 
 It exposes the same Window interface as oracle/orc.py (the CPU restatement), so tests/test_ref_pin.py can run both on the
-same seeded inputs: that comparison is what pins the oracle to the reference.  Only tests/ may import this."""
+same seeded inputs: that comparison is what pins the oracle to the reference.  built() and open_ref() find and open every library
+under oracle/_ref; select.py, activation.py and undistort.py load theirs through them.  Only tests/ may import this."""
 import ctypes as C
+import functools
 import os
 import subprocess
 
@@ -12,8 +14,21 @@ import numpy as np
 from . import orc
 
 _HERE = os.path.dirname(os.path.abspath(__file__))
-LIB_PATH = os.environ.get("DMV_REF_LIB", os.path.join(_HERE, "_ref", "libdso_ref.so"))  # DMV_REF_LIB: tools/eigen_order_sensitivity.py
+REF_DIR = os.path.join(_HERE, "_ref")
+LIB_PATH = os.environ.get("DMV_REF_LIB", os.path.join(REF_DIR, "libdso_ref.so"))  # DMV_REF_LIB: tools/eigen_order_sensitivity.py
 _LIB = None
+
+
+def built(name):
+    """whether oracle/_ref/<name> exists: ref_build.sh makes it where the reference sources are present"""
+    return os.path.exists(os.path.join(REF_DIR, name))
+
+
+@functools.cache
+def open_ref(name):
+    """oracle/_ref/<name> (or an absolute path), opened once and RTLD_LOCAL: every reference library keeps its own copy of the reference's
+    process-global settings"""
+    return C.CDLL(os.path.join(REF_DIR, name), mode=C.RTLD_LOCAL)
 
 
 def available():
@@ -41,7 +56,7 @@ def lib():
     if _LIB is None:
         if not os.path.exists(LIB_PATH):
             build()
-        L = C.CDLL(LIB_PATH)
+        L = open_ref(LIB_PATH)
         vp = C.c_void_p
         f32p, f64p, i32p, u8p = orc.f32p, orc.f64p, orc.i32p, orc.u8p
         L.ref_win_create.restype = vp

@@ -1,8 +1,8 @@
 // TEST INFRASTRUCTURE ONLY — C entry points that drive the REFERENCE's own compiled CoarseDistanceMap (FullSystem/CoarseTracker.cpp: makeK,
 // makeDistanceMap, addIntoDistFinal) for tests/test_ref_pin_activation.py and tests/golden/make_golden_activation.py.  The selection loop
 // of FullSystem::activatePointsMT (FullSystem.cpp:L642-717) is a FullSystem member, which cannot be compiled here, so it is mirrored line for
-// line around the reference's objects, as ref_harness.cpp's ref_win_activate mirrors optimizeImmaturePoint.  Built by ref_build_activation.sh
-// into a library of its own, linked with the reference objects ref_build.sh compiles and ref_harness.o.
+// line around the reference's objects, as ref_harness.cpp's ref_win_activate mirrors optimizeImmaturePoint.  Built by ref_build.sh
+// into a library of its own, linked with the reference objects it compiles and ref_harness.o.
 #include <cmath>
 #include <cstdint>
 #include <cstring>

@@ -1,6 +1,6 @@
 // TEST INFRASTRUCTURE ONLY — C entry points that drive the REFERENCE's own compiled PixelSelector (FullSystem/PixelSelector2.cpp), its
 // FrameHessian::makeImages and its ImmaturePoint constructor, for tests/test_ref_pin_select.py and tests/golden/make_golden_select.py.
-// Built by ref_build_select.sh into a library of its own, linked with the reference objects ref_build.sh compiles and ref_harness.o.
+// Built by ref_build.sh into a library of its own, linked with the reference objects it compiles and ref_harness.o.
 #include <cmath>
 #include <cstdint>
 #include <cstring>

@@ -1,5 +1,5 @@
 // TEST INFRASTRUCTURE ONLY — C harness around the REFERENCE's own Undistort (src/dso/util/Undistort.cpp, compiled from where it lies by
-// oracle/ref_build_undistort.sh).  The test writes the calibration and response files; the vignette image comes from memory through the
+// oracle/ref_build.sh).  The test writes the calibration and response files; the vignette image comes from memory through the
 // two IOWrap readers defined here (the reference reads it with OpenCV).  Exposes Undistort::undistort<T> and the tables it built, so the
 // restatement (orc_undistort.cpp) and the device path can be fed the very same remap, G and vignetteMapInv.
 #include <Eigen/Core>

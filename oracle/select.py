@@ -1,47 +1,58 @@
 """TEST INFRASTRUCTURE ONLY — bindings and cases of the pixel-selection oracles (dmv_ct_make_new_traces).
 
-  restate(...)   liborc_select.so: the CPU restatement of PixelSelector::makeMaps and makeNewTraces' loop (orc_select.cpp, built by select.mk);
-                 the ImmaturePoint constructor is orc.ip_init
-  Ref            _ref/libselect_ref.so: the REFERENCE's own PixelSelector / makeImages / ImmaturePoint (ref_select.cpp, ref_build_select.sh)
+  restate(...)   liborc.so: the CPU restatement of PixelSelector::makeMaps and makeNewTraces' loop (orc_select.cpp); the ImmaturePoint
+                 constructor is orc.ip_init
+  Ref            _ref/libselect_ref.so: the REFERENCE's own PixelSelector / makeImages / ImmaturePoint (ref_select.cpp, built by ref_build.sh)
   CASES          seeded keyframes and arguments shared by the CPU pin, the golden fixture and the device tests"""
 import ctypes as C
-import os
+import functools
 
 import numpy as np
 
-from . import orc
+from . import orc, ref
+from .orc import f32p, f64p, i32p, u8p
 
-_HERE = os.path.dirname(os.path.abspath(__file__))
-ORC_PATH = os.path.join(_HERE, "liborc_select.so")
-REF_PATH = os.path.join(_HERE, "_ref", "libselect_ref.so")
+REF_LIB = "libselect_ref.so"
 vp = C.c_void_p
-f32p = np.ctypeslib.ndpointer(np.float32, flags="C_CONTIGUOUS")
-i32p = np.ctypeslib.ndpointer(np.int32, flags="C_CONTIGUOUS")
-u8p = np.ctypeslib.ndpointer(np.uint8, flags="C_CONTIGUOUS")
-f64p = np.ctypeslib.ndpointer(np.float64, flags="C_CONTIGUOUS")
-_ORC = None
-_REF = None
 
 DEFAULTS = dict(minGradHistCut=0.5, minGradHistAdd=7.0, gradDownweightPerLevel=0.75, selectDirectionDistribution=1, gammaWeightsPixelSelect=1)
 POINT_KEYS = ("u", "v", "type", "color", "weights", "gradH", "energyTH")
 
 
+@functools.cache
 def orc_lib():
-    global _ORC
-    if _ORC is None:
-        L = C.CDLL(ORC_PATH)
-        L.orc_sel_random_pattern.argtypes = [C.c_uint, C.c_int, u8p]
-        L.orc_sel_make_maps.restype = C.c_int
-        L.orc_sel_make_maps.argtypes = [C.c_int, C.c_int, f32p, f32p, f32p, f32p, f32p, i32p, C.c_float, C.c_int, C.c_float, C.POINTER(C.c_int), f32p,
-                                        C.POINTER(C.c_longlong), C.POINTER(C.c_float)]
-        L.orc_sel_trace_pixels.restype = C.c_int
-        L.orc_sel_trace_pixels.argtypes = [C.c_int, C.c_int, f32p, i32p, i32p, f32p]
-        _ORC = L
-    return _ORC
+    L = orc.lib()
+    L.orc_sel_random_pattern.argtypes = [C.c_uint, C.c_int, u8p]
+    L.orc_sel_make_maps.restype = C.c_int
+    L.orc_sel_make_maps.argtypes = [C.c_int, C.c_int, f32p, f32p, f32p, f32p, f32p, i32p, C.c_float, C.c_int, C.c_float, C.POINTER(C.c_int), f32p,
+                                    C.POINTER(C.c_longlong), C.POINTER(C.c_float)]
+    L.orc_sel_trace_pixels.restype = C.c_int
+    L.orc_sel_trace_pixels.argtypes = [C.c_int, C.c_int, f32p, i32p, i32p, f32p]
+    return L
+
+
+@functools.cache
+def ref_lib():
+    L = ref.open_ref(REF_LIB)
+    L.ref_sel_settings.argtypes = [C.c_float, C.c_float, C.c_float, C.c_int, C.c_int]
+    L.ref_sel_frame_create.restype = vp
+    L.ref_sel_frame_create.argtypes = [C.c_int, C.c_int, f64p, f32p, vp]
+    L.ref_sel_frame_destroy.argtypes = [vp]
+    L.ref_sel_frame_dI.argtypes = [vp, C.c_int, f32p]
+    L.ref_sel_create.restype = vp
+    L.ref_sel_create.argtypes = [C.c_int, C.c_int]
+    L.ref_sel_destroy.argtypes = [vp]
+    L.ref_sel_get_potential.argtypes = [vp]
+    L.ref_sel_set_potential.argtypes = [vp, C.c_int]
+    L.ref_sel_make_maps.restype = C.c_int
+    L.ref_sel_make_maps.argtypes = [vp, vp, f32p, C.c_float, C.c_int, C.c_float]
+    L.ref_sel_new_traces.restype = C.c_int
+    L.ref_sel_new_traces.argtypes = [vp, f32p, i32p, i32p, f32p, f32p, f32p, f32p, f32p]
+    return L
 
 
 def ref_available():
-    return os.path.exists(REF_PATH)
+    return ref.built(REF_LIB)
 
 
 def random_pattern(n, seed=3141592):
@@ -97,25 +108,7 @@ class Ref:
     """the reference's PixelSelector (persistent: currentPotential carries over between calls), keyframes built by its makeImages"""
 
     def __init__(self, w, h):
-        global _REF
-        if _REF is None:
-            L = C.CDLL(REF_PATH)
-            L.ref_sel_settings.argtypes = [C.c_float, C.c_float, C.c_float, C.c_int, C.c_int]
-            L.ref_sel_frame_create.restype = vp
-            L.ref_sel_frame_create.argtypes = [C.c_int, C.c_int, f64p, f32p, vp]
-            L.ref_sel_frame_destroy.argtypes = [vp]
-            L.ref_sel_frame_dI.argtypes = [vp, C.c_int, f32p]
-            L.ref_sel_create.restype = vp
-            L.ref_sel_create.argtypes = [C.c_int, C.c_int]
-            L.ref_sel_destroy.argtypes = [vp]
-            L.ref_sel_get_potential.argtypes = [vp]
-            L.ref_sel_set_potential.argtypes = [vp, C.c_int]
-            L.ref_sel_make_maps.restype = C.c_int
-            L.ref_sel_make_maps.argtypes = [vp, vp, f32p, C.c_float, C.c_int, C.c_float]
-            L.ref_sel_new_traces.restype = C.c_int
-            L.ref_sel_new_traces.argtypes = [vp, f32p, i32p, i32p, f32p, f32p, f32p, f32p, f32p]
-            _REF = L
-        self.L = _REF
+        self.L = ref_lib()
         self.w, self.h = w, h
         self.ps = self.L.ref_sel_create(w, h)
         self.frames = []   # kept alive until close(): makeMaps caches its histogram by FrameHessian address

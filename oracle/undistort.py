@@ -1,22 +1,20 @@
 """TEST INFRASTRUCTURE ONLY — ctypes bindings of the Undistort oracles and the inputs the ingest tests share.
 
-  restate(...)   liborc_undistort.so: the CPU restatement of Undistort::undistort<T> (orc_undistort.cpp, built by undistort.mk)
-  Ref            _ref/libundistort_ref.so: the REFERENCE's own Undistort (ref_undistort.cpp, built by ref_build_undistort.sh)
+  restate(...)   liborc.so: the CPU restatement of Undistort::undistort<T> (orc_undistort.cpp)
+  Ref            _ref/libundistort_ref.so: the REFERENCE's own Undistort (ref_undistort.cpp, built by ref_build.sh)
   the calibration / response / vignette inputs of the cases, and table builders that need no reference (synthetic_remap, G_from_file,
   vignette_inv), so that the device tests run where the reference is absent."""
 import ctypes as C
+import functools
 import os
-import subprocess
 import tempfile
 
 import numpy as np
 
-_HERE = os.path.dirname(os.path.abspath(__file__))
-ORC_PATH = os.path.join(_HERE, "liborc_undistort.so")
-REF_PATH = os.path.join(_HERE, "_ref", "libundistort_ref.so")
+from . import orc, ref
+
+REF_LIB = "libundistort_ref.so"
 vp = C.c_void_p
-_ORC = None
-_REF = None
 
 # (calibration file text, raw size) of the cases: EuRoC-like RadTan crop, TUM-VI-like EquiDistant, FOV, Pinhole passthrough
 CAMERAS = {
@@ -83,16 +81,12 @@ def raw_frame(wOrg, hOrg, bpp, seed):
     return np.clip(img, 0, top).astype(np.uint8 if bpp == 1 else np.uint16)
 
 
-def orc():
-    global _ORC
-    if _ORC is None:
-        if not os.path.exists(ORC_PATH):
-            subprocess.check_call(["make", "-s", "-C", _HERE, "-f", "undistort.mk"])
-        L = C.CDLL(ORC_PATH)
-        L.orc_undistort.argtypes = [C.c_int] * 4 + [vp] * 4 + [C.c_int, vp, C.c_int, C.c_float, C.c_float, vp]
-        L.orc_undistort.restype = None
-        _ORC = L
-    return _ORC
+@functools.cache
+def orc_lib():
+    L = orc.lib()
+    L.orc_undistort.argtypes = [C.c_int] * 4 + [vp] * 4 + [C.c_int, vp, C.c_int, C.c_float, C.c_float, vp]
+    L.orc_undistort.restype = None
+    return L
 
 
 def _p(a):
@@ -106,33 +100,31 @@ def restate(w, h, raw, remapX, remapY, G, vigInv, mode, exposure, factor):
     c = lambda a: None if a is None else np.ascontiguousarray(a, np.float32)
     keep = [c(remapX), c(remapY), c(G), c(vigInv)]
     out = np.zeros((h, w), np.float32)
-    orc().orc_undistort(w, h, wOrg, hOrg, *[_p(a) for a in keep], int(mode), raw.ctypes.data, raw.itemsize, float(exposure), float(factor), out.ctypes.data)
+    orc_lib().orc_undistort(w, h, wOrg, hOrg, *[_p(a) for a in keep], int(mode), raw.ctypes.data, raw.itemsize, float(exposure), float(factor), out.ctypes.data)
     return out
 
 
 def ref_available():
-    return os.path.exists(REF_PATH)
+    return ref.built(REF_LIB)
 
 
-def _ref():
-    global _REF
-    if _REF is None:
-        L = C.CDLL(REF_PATH)
-        L.refu_create.restype = vp
-        L.refu_create.argtypes = [C.c_char_p, C.c_char_p, vp, C.c_int, C.c_int, C.c_int, C.c_int]
-        L.refu_destroy.argtypes = [vp]
-        L.refu_info.argtypes = [vp, vp, vp]
-        L.refu_tables.argtypes = [vp, vp, vp, vp, vp]
-        L.refu_undistort.argtypes = [vp, vp, C.c_int, C.c_float, C.c_float, C.c_int, vp]
-        _REF = L
-    return _REF
+@functools.cache
+def ref_lib():
+    L = ref.open_ref(REF_LIB)
+    L.refu_create.restype = vp
+    L.refu_create.argtypes = [C.c_char_p, C.c_char_p, vp, C.c_int, C.c_int, C.c_int, C.c_int]
+    L.refu_destroy.argtypes = [vp]
+    L.refu_info.argtypes = [vp, vp, vp]
+    L.refu_tables.argtypes = [vp, vp, vp, vp, vp]
+    L.refu_undistort.argtypes = [vp, vp, C.c_int, C.c_float, C.c_float, C.c_int, vp]
+    return L
 
 
 class Ref:
     """the reference's Undistort::getUndistorterForFile on a calibration text, nG response entries and an 8-bit vignette (None: none)"""
 
     def __init__(self, calib_text, nG, vignette, mode):
-        L = _ref()
+        L = ref_lib()
         self.mode = mode
         with tempfile.TemporaryDirectory() as d:
             cf, gf = os.path.join(d, "camera.txt"), os.path.join(d, "pcalib.txt")
@@ -150,18 +142,18 @@ class Ref:
     def tables(self):
         rx, ry = np.zeros(self.w * self.h_, np.float32), np.zeros(self.w * self.h_, np.float32)
         G, vi = np.zeros(65536, np.float32), np.zeros(self.wOrg * self.hOrg, np.float32)
-        _ref().refu_tables(self.h, rx.ctypes.data, ry.ctypes.data, G.ctypes.data, vi.ctypes.data)
+        ref_lib().refu_tables(self.h, rx.ctypes.data, ry.ctypes.data, G.ctypes.data, vi.ctypes.data)
         return rx, ry, G, vi
 
     def undistort(self, raw, exposure, factor):
         raw = np.ascontiguousarray(raw)
         out = np.zeros((self.h_, self.w), np.float32)
-        _ref().refu_undistort(self.h, raw.ctypes.data, raw.itemsize, float(exposure), float(factor), self.mode, out.ctypes.data)
+        ref_lib().refu_undistort(self.h, raw.ctypes.data, raw.itemsize, float(exposure), float(factor), self.mode, out.ctypes.data)
         return out
 
     def close(self):
         if self.h:
-            _ref().refu_destroy(self.h)
+            ref_lib().refu_destroy(self.h)
             self.h = None
 
 

@@ -1,5 +1,5 @@
 """Regenerates tests/golden/golden_activation.npz from the REFERENCE's own CoarseDistanceMap (oracle/_ref/libactivation_ref.so, built by
-oracle/ref_build_activation.sh): per case of oracle.activation.CASES, the [KRKi | Kt] tables the reference computed, the actions, toOptimize
+oracle/ref_build.sh): per case of oracle.activation.CASES, the [KRKi | Kt] tables the reference computed, the actions, toOptimize
 and the final distance map.  The inputs are regenerated from the cases' seeds.  Run from the repository root:
     python tests/golden/make_golden_activation.py"""
 import os

@@ -1,6 +1,7 @@
 """Writes tests/golden/golden_select.npz from the reference's compiled PixelSelector, makeImages and ImmaturePoint constructor
-(oracle/_ref/libselect_ref.so): per case of oracle/select.py the points makeNewTraces creates, numPointsTotal and the potential after the call,
-and for the keyframe sequence on one persistent selector the same per keyframe.  The keyframes are regenerated from their seeds.
+(oracle/_ref/libselect_ref.so, built by oracle/ref_build.sh): per case of oracle/select.py the points makeNewTraces creates, numPointsTotal and
+the potential after the call, and for the keyframe sequence on one persistent selector the same per keyframe.  The keyframes are regenerated
+from their seeds.
     python tests/golden/make_golden_select.py"""
 import os
 import sys

@@ -1,5 +1,6 @@
-"""Writes tests/golden/golden_undistort.npz from the reference's compiled Undistort (oracle/_ref/libundistort_ref.so): the reduced-size cameras
-of oracle/undistort.py, their remap tables, the raw frames and the reference's output for every photometric case.
+"""Writes tests/golden/golden_undistort.npz from the reference's compiled Undistort (oracle/_ref/libundistort_ref.so, built by
+oracle/ref_build.sh): the reduced-size cameras of oracle/undistort.py, their remap tables, the raw frames and the reference's output for every
+photometric case.
     python tests/golden/make_golden_undistort.py"""
 import os
 import sys
