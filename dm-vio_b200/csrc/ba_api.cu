@@ -3,7 +3,6 @@
 #include "ba_handle.h"
 #include "ct_depth.h"
 #include "remove_outliers.h"
-#include "ip_trace.h"
 #include <algorithm>
 #include <cstdlib>
 #include <cstring>
@@ -248,7 +247,7 @@ int dmv_ba_adopt_frame(dmv_ba* b, int slot, dmv_ct* ct) {
   return DMV_OK;
 }
 
-// library-internal: what dmv_ct_set_ref_from_ba (ct_kernels.cu) reads from the window — the committed linearisation's residuals into the newest
+// library-internal: what dmv_ct_set_ref_from_ba (ct_depth.cu) reads from the window — the committed linearisation's residuals into the newest
 // frame (slot (nf-1)*mp + p: state, centerProjectedTo), the HdiF of the last dmv_ba_accumulate and the newest frame's level-0 plane.  Nothing is
 // copied: the caller orders its stream behind this handle's with an event.  The fold order is the reference's at setCoarseTrackingRef, i.e.
 // after FullSystem::removeOutliers: which points still have residuals is host bookkeeping here (res_slot), so the reorder is replayed on the host
@@ -921,56 +920,6 @@ extern "C" int dmv_ba_p2p_import(dmv_ba* b, int nranks, int rank, const void* ip
   b->nranks = nranks; b->rank = rank;
   b->xchg_on = nranks > 1;
   b->xchg_seq = 0;
-  return DMV_OK;
-}
-
-// FullSystem::optimizeImmaturePoint for a batch of immature points (ip_trace.cu: ip_activate_kernel)
-extern "C" int dmv_ba_activate_points(dmv_ba* b, const dmv_ba_activate_args* a) {
-  if (!b || !a) return set_error(DMV_ERR_INVALID, "null argument");
-  if (b->nf < 2 || !b->have_state) return set_error(DMV_ERR_STATE, "dmv_ba_set_window + dmv_ba_set_state first");
-  if (a->n < 0 || (a->n > 0 && (!a->host || !a->u || !a->v || !a->color8 || !a->weights8 || !a->energyTH || !a->idepth_min || !a->idepth_max || !a->RT ||
-                                !a->status || !a->idepth || !a->res_state)))
-    return set_error(DMV_ERR_INVALID, "incomplete dmv_ba_activate_args");
-  if (a->n == 0) return DMV_OK;
-  const int n = a->n, nf = b->nf;
-  for (int i = 0; i < n; i++)
-    if (a->host[i] < 0 || a->host[i] >= nf) return set_error(DMV_ERR_INVALID, "point %d: host %d out of range", i, a->host[i]);
-  CK(cudaSetDevice(b->device));
-  if (n > b->act_cap) {
-    cudaFree(b->d_act); cudaFreeHost(b->h_act);
-    b->act_cap = std::max(n, 2048);
-    const size_t words = (size_t)MAXF * MAXF * 14 + (size_t)(24 + MAXF) * b->act_cap;
-    CK(cudaMalloc(&b->d_act, sizeof(float) * words));
-    CK(cudaMallocHost(&b->h_act, sizeof(float) * words));
-  }
-  const size_t cap = b->act_cap;
-  float* hb = b->h_act;
-  float* d = b->d_act;
-  // layout (words): RT[64*12] | aff[64*2] | host | u | v | color*8 | weights*8 | energyTH | idmin | idmax | status | idepth | res_state*MAXF
-  const size_t o_rt = 0, o_aff = (size_t)MAXF * MAXF * 12, o_host = (size_t)MAXF * MAXF * 14, o_u = o_host + cap, o_v = o_u + cap, o_col = o_v + cap,
-               o_wgt = o_col + 8 * cap, o_eth = o_wgt + 8 * cap, o_min = o_eth + cap, o_max = o_min + cap, o_st = o_max + cap, o_id = o_st + cap, o_rs = o_id + cap;
-  std::memcpy(hb + o_rt, a->RT, sizeof(float) * 12 * nf * nf);
-  const BAIter& it = b->h_up->it;
-  for (int k = 0; k < nf * nf; k++) { hb[o_aff + 2 * k] = it.precalc[k][24]; hb[o_aff + 2 * k + 1] = it.precalc[k][25]; }  // PRE_aff_mode
-  std::memcpy(hb + o_host, a->host, 4 * (size_t)n); std::memcpy(hb + o_u, a->u, 4 * (size_t)n); std::memcpy(hb + o_v, a->v, 4 * (size_t)n);
-  std::memcpy(hb + o_col, a->color8, 32 * (size_t)n); std::memcpy(hb + o_wgt, a->weights8, 32 * (size_t)n); std::memcpy(hb + o_eth, a->energyTH, 4 * (size_t)n);
-  std::memcpy(hb + o_min, a->idepth_min, 4 * (size_t)n); std::memcpy(hb + o_max, a->idepth_max, 4 * (size_t)n);
-  CK(cudaMemcpyAsync(d, hb, sizeof(float) * o_st, cudaMemcpyHostToDevice, b->stream));
-  IPActArgs A;
-  A.n = n; A.nf = nf; A.w = b->cfg.w; A.h = b->cfg.h; A.minObs = a->minObs; A.GNIts = 3;  // setting_GNItsOnPointActivation
-  A.fxl = it.calib[0]; A.fyl = it.calib[1]; A.cxl = it.calib[2]; A.cyl = it.calib[3]; A.fxli = it.calib[4]; A.fyli = it.calib[5];
-  A.huberTH = b->prm.huberTH; A.minIdepthH_act = 100.f;                                      // setting_minIdepthH_act
-  for (int f = 0; f < MAXF; f++) A.img[f] = f < nf ? b->d_img[b->slots[f]] : nullptr;
-  A.RT = d + o_rt; A.aff = d + o_aff; A.host = reinterpret_cast<const int*>(d + o_host);
-  A.u = d + o_u; A.v = d + o_v; A.color = d + o_col; A.weights = d + o_wgt; A.energyTH = d + o_eth; A.idepth_min = d + o_min; A.idepth_max = d + o_max;
-  A.status = reinterpret_cast<int*>(d + o_st); A.idepth = d + o_id; A.res_state = reinterpret_cast<int*>(d + o_rs);
-  launch_ip_activate(A, b->stream);
-  b->launches++;
-  CK(cudaGetLastError());
-  CK(cudaMemcpyAsync(hb + o_st, d + o_st, sizeof(float) * (2 * cap + (size_t)nf * n), cudaMemcpyDeviceToHost, b->stream));
-  CK(cudaStreamSynchronize(b->stream));
-  std::memcpy(a->status, hb + o_st, 4 * (size_t)n); std::memcpy(a->idepth, hb + o_id, 4 * (size_t)n);
-  std::memcpy(a->res_state, hb + o_rs, 4 * (size_t)n * nf);
   return DMV_OK;
 }
 

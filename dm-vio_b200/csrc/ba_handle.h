@@ -1,4 +1,5 @@
-// Internal layout of the BA handle (shared by ba_api.cu and the measurement-only entry points in ba_bench.cu).
+// Internal layout of the BA handle (shared by ba_api.cu, the entry points beside their kernels in ip_trace.cu and ip_select.cu, and the
+// measurement-only entry points in ba_bench.cu).
 #pragma once
 #include "../../include/dmvio_b200.h"
 #include "ba_device.cuh"
@@ -11,8 +12,6 @@ cudaError_t launch_fused_kernel(BAWinDev& W, const BAIter& it, bool marg, cudaSt
 cudaError_t launch_fused_kernel_clocked(BAWinDev& W, const BAIter& it, cudaStream_t s, unsigned* bar_count, unsigned long long* clk, int* grid);
 cudaError_t launch_fused_batch_kernel(int P, const BAWinDev* gW, const BAIter* gIt, BABatchHdr& hdr, int max_nf, cudaStream_t s, unsigned* bar_count);
 void launch_resub_kernel(const BAWinDev& W, const BAIter& it, int apply, double* sums, cudaStream_t s);
-void launch_repack(const float* src, float4* dst, int n, cudaStream_t s);
-void launch_make_dI(const float* img, float4* dst, int w, int h, cudaStream_t s);
 void launch_l2_flush(float4* buf, size_t n, cudaStream_t s);
 }  // namespace dmv
 
@@ -110,13 +109,6 @@ struct dmv_ba {
   bool xchg_on = false;
   unsigned int xchg_seq = 0;
 };
-
-
-#define CK(call)                                                                                   \
-  do {                                                                                             \
-    cudaError_t _e = (call);                                                                       \
-    if (_e != cudaSuccess) return dmv::set_error(DMV_ERR_CUDA, "%s failed: %s", #call, cudaGetErrorString(_e)); \
-  } while (0)
 
 // shared by the product path and the benches (library-internal: hidden from the dynamic symbol table)
 #define DMV_INTERNAL extern "C" __attribute__((visibility("hidden")))

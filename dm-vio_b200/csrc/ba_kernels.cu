@@ -1,6 +1,5 @@
 // Small sm_90a kernels of the bundle-adjustment path next to ba_fused_kernel (ba_fused.cu):
 //   ba_resub_kernel     stand-alone EnergyFunctional::resubstituteFPt + point part of doStepFromBackup (the hot loop uses the fused prologue)
-//   repack_aos3_kernel / make_dI_kernel   image ingestion (float4 texels)
 //   l2_flush_kernel     larger-than-L2 scrub used by the bench between timed iterations
 #include "ba_common.cuh"
 
@@ -41,27 +40,6 @@ __global__ void __launch_bounds__(128) ba_resub_kernel(const __grid_constant__ B
   }
 }
 
-// ---------------------------------------------------------------------------------------------------------------
-// image planes: AoS3 -> float4 texels, and level-0 [I,dx,dy] construction (HessianBlocks.cpp:L169-179)
-// ---------------------------------------------------------------------------------------------------------------
-__global__ void repack_aos3_kernel(const float* __restrict__ src, float4* __restrict__ dst, int n) {
-  const int i = blockIdx.x * blockDim.x + threadIdx.x;
-  if (i < n) dst[i] = make_float4(src[3 * i], src[3 * i + 1], src[3 * i + 2], 0.f);
-}
-
-__global__ void make_dI_kernel(const float* __restrict__ img, float4* __restrict__ dst, int w, int h) {
-  const int idx = blockIdx.x * blockDim.x + threadIdx.x;
-  if (idx >= w * h) return;
-  float dx = 0.f, dy = 0.f;
-  if (idx >= w && idx < w * (h - 1)) {  // the reference's flat loop: row ends wrap into the neighbouring rows
-    dx = 0.5f * (img[idx + 1] - img[idx - 1]);
-    dy = 0.5f * (img[idx + w] - img[idx - w]);
-    if (!isfinite(dx)) dx = 0.f;
-    if (!isfinite(dy)) dy = 0.f;
-  }
-  dst[idx] = make_float4(img[idx], dx, dy, 0.f);
-}
-
 // larger-than-L2 scrub used by the bench between timed iterations
 __global__ void l2_flush_kernel(float4* buf, size_t n) {
   size_t i = (size_t)blockIdx.x * blockDim.x + threadIdx.x;
@@ -75,8 +53,6 @@ __global__ void l2_flush_kernel(float4* buf, size_t n) {
 void launch_resub_kernel(const BAWinDev& W, const BAIter& it, int apply, double* sums, cudaStream_t s) {
   ba_resub_kernel<<<(W.npts + 127) / 128, 128, 0, s>>>(W, it, apply, sums);
 }
-void launch_repack(const float* src, float4* dst, int n, cudaStream_t s) { repack_aos3_kernel<<<(n + 255) / 256, 256, 0, s>>>(src, dst, n); }
-void launch_make_dI(const float* img, float4* dst, int w, int h, cudaStream_t s) { make_dI_kernel<<<(w * h + 255) / 256, 256, 0, s>>>(img, dst, w, h); }
 void launch_l2_flush(float4* buf, size_t n, cudaStream_t s) { l2_flush_kernel<<<132 * 8, 256, 0, s>>>(buf, n); }
 
 }  // namespace dmv

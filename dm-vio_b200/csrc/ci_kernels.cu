@@ -205,11 +205,6 @@ __global__ void __launch_bounds__(CI_THREADS) ci_res_gs_kernel(const __grid_cons
   }
 }
 
-__global__ void ci_repack_kernel(const float* __restrict__ src, float4* __restrict__ dst, int n) {
-  const int i = blockIdx.x * blockDim.x + threadIdx.x;
-  if (i < n) dst[i] = make_float4(src[3 * i], src[3 * i + 1], src[3 * i + 2], 0.f);
-}
-
 }  // namespace dmv
 
 using namespace dmv;
@@ -234,13 +229,9 @@ struct dmv_ci {
   long long launches = 0;
 };
 
-#define CK(call)                                                                                   \
-  do {                                                                                             \
-    cudaError_t _e = (call);                                                                       \
-    if (_e != cudaSuccess) return dmv::set_error(DMV_ERR_CUDA, "%s failed: %s", #call, cudaGetErrorString(_e)); \
-  } while (0)
-
 extern "C" {
+
+static int ci_allocate(dmv_ci* c, const dmv_ci_config* cfg);
 
 int dmv_ci_create(const dmv_ci_config* cfg, dmv_ci** out) {
   if (!cfg || !out) return set_error(DMV_ERR_INVALID, "null argument");
@@ -249,10 +240,20 @@ int dmv_ci_create(const dmv_ci_config* cfg, dmv_ci** out) {
   int ndev = 0;
   if (cudaGetDeviceCount(&ndev) != cudaSuccess || ndev < 1) return set_error(DMV_ERR_NO_DEVICE, "no CUDA device: dmvio_b200 has no CPU path");
   if (cfg->device < 0 || cfg->device >= ndev) return set_error(DMV_ERR_INVALID, "device %d out of range", cfg->device);
+  CK(cudaSetDevice(cfg->device));
   dmv_ci* c = new dmv_ci();
+  const int rc = ci_allocate(c, cfg);
+  if (rc != DMV_OK) {  // allocation failed half-way: release what exists, keep the failing call's error message
+    dmv_ci_destroy(c);
+    return rc;
+  }
+  *out = c;
+  return DMV_OK;
+}
+
+static int ci_allocate(dmv_ci* c, const dmv_ci_config* cfg) {
   c->cfg = *cfg;
   c->device = cfg->device;
-  CK(cudaSetDevice(c->device));
   CK(cudaStreamCreateWithFlags(&c->stream, cudaStreamNonBlocking));
   const size_t mp = (size_t)cfg->max_points;
   for (int l = 0; l < cfg->levels; l++) {
@@ -275,7 +276,6 @@ int dmv_ci_create(const dmv_ci_config* cfg, dmv_ci** out) {
   CK(cudaMallocHost(&c->h_out, sizeof(double) * CI_NRED));
   CK(cudaMalloc(&c->d_ticket, sizeof(unsigned int)));
   CK(cudaMemset(c->d_ticket, 0, sizeof(unsigned int)));
-  *out = c;
   return DMV_OK;
 }
 
@@ -301,7 +301,7 @@ static int ci_upload(dmv_ci* c, int l, const float* dIp, float4* dst) {
   const size_t npx = (size_t)c->w[l] * c->h[l];
   CK(cudaSetDevice(c->device));
   CK(cudaMemcpyAsync(c->d_stage, dIp, sizeof(float) * 3 * npx, cudaMemcpyHostToDevice, c->stream));
-  ci_repack_kernel<<<(unsigned)((npx + 255) / 256), 256, 0, c->stream>>>(c->d_stage, dst, (int)npx);
+  launch_repack(c->d_stage, dst, (int)npx, c->stream);
   CK(cudaGetLastError());
   CK(cudaStreamSynchronize(c->stream));   // pageable source + shared staging buffer
   return DMV_OK;

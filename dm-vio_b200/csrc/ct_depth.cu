@@ -9,12 +9,41 @@
 //   * compaction = per-row counts, an exclusive scan over the rows, ballot-prefix writes: row-major order like the reference's loops.
 // Fed from a BA handle (dmv_ct_set_ref_from_ba) the fold runs here too: a stable radix sort of (pixel, point index) puts the points that
 // hit one pixel next to each other in input order, and one thread per pixel adds its run in that order — the reference's sequential +=.
-#include "../../include/dmvio_b200.h"
-#include "common_host.h"
+#include "ct_handle.h"
 #include "ct_depth.h"
 #include <cub/device/device_radix_sort.cuh>
+#include <cstring>
+#include <unordered_map>
 
 namespace dmv {
+
+// the handle's share (dmv_ct::cd), allocated on first use
+struct CDScratch {
+  float *idepth[DMV_MAX_PYR_LEVELS] = {nullptr}, *ws[DMV_MAX_PYR_LEVELS] = {nullptr}, *ws2[DMV_MAX_PYR_LEVELS] = {nullptr};
+  int *rowcnt = nullptr, *rowoff = nullptr;   // scratch rows of the compaction
+  int* totals = nullptr;    // pinned host, device-visible: pc_n of every level, then [DMV_MAX_PYR_LEVELS] = bad
+  // the device fold of dmv_ct_set_ref_from_ba, for up to sort_cap points: radix-sort keys / ordinals (double-buffered) and CUB's temporary
+  // storage, the moves, and the event that orders the tracker's stream behind the BA's
+  unsigned* key[2] = {nullptr, nullptr};
+  int* ord[2] = {nullptr, nullptr};
+  void* temp = nullptr;
+  size_t temp_bytes = 0;
+  int* bad = nullptr;       // lowest point index whose projection leaves the image (>= npts: none)
+  int* moves = nullptr;     // device copy of CDFromBA::moves_host (2 * sort_cap ints)
+  int* h_moves = nullptr;   // its pinned staging
+  int sort_cap = 0;
+  cudaEvent_t ev_ba = nullptr;
+};
+
+void cd_free(CDScratch* S) {
+  if (!S) return;
+  for (int l = 0; l < DMV_MAX_PYR_LEVELS; l++) { cudaFree(S->idepth[l]); cudaFree(S->ws[l]); cudaFree(S->ws2[l]); }
+  cudaFree(S->rowcnt); cudaFree(S->rowoff); cudaFreeHost(S->totals);
+  for (int k = 0; k < 2; k++) { cudaFree(S->key[k]); cudaFree(S->ord[k]); }
+  cudaFree(S->temp); cudaFree(S->bad); cudaFree(S->moves); cudaFreeHost(S->h_moves);
+  if (S->ev_ba) cudaEventDestroy(S->ev_ba);
+  delete S;
+}
 
 __global__ void cd_scatter_kernel(int n, const int* __restrict__ pix, const float* __restrict__ idw, const float* __restrict__ wsum, float* idepth0, float* ws0) {
   const int i = blockIdx.x * blockDim.x + threadIdx.x;
@@ -112,40 +141,37 @@ __global__ void cd_write_kernel(const float* __restrict__ ws, const float* __res
   }
 }
 
-static void cd_clear(const CDLevels& L, cudaStream_t s) {
-  cudaMemsetAsync(L.idepth[0], 0, sizeof(float) * L.w[0] * L.h[0], s);
-  cudaMemsetAsync(L.ws[0], 0, sizeof(float) * L.w[0] * L.h[0], s);
+static void cd_clear(const dmv_ct* c) {
+  cudaMemsetAsync(c->cd->idepth[0], 0, sizeof(float) * c->w[0] * c->h[0], c->stream);
+  cudaMemsetAsync(c->cd->ws[0], 0, sizeof(float) * c->w[0] * c->h[0], c->stream);
 }
 
-// everything after the level-0 splat: pooling, dilation, compaction
-static int cd_reduce(const CDLevels& L, cudaStream_t s) {
+// everything after the level-0 splat: pooling, dilation, compaction into the handle's pc_* lists
+static int cd_reduce(dmv_ct* c) {
+  const CDScratch& S = *c->cd;
+  const cudaStream_t s = c->stream;
   int k = 0;
-  for (int l = 1; l < L.levels; l++) {
-    dim3 grid((L.w[l] + 127) / 128, L.h[l]);
-    cd_pool_kernel<<<grid, 128, 0, s>>>(L.idepth[l - 1], L.ws[l - 1], L.idepth[l], L.ws[l], L.w[l], L.h[l], L.w[l - 1]);
+  for (int l = 1; l < c->cfg.levels; l++) {
+    dim3 grid((c->w[l] + 127) / 128, c->h[l]);
+    cd_pool_kernel<<<grid, 128, 0, s>>>(S.idepth[l - 1], S.ws[l - 1], S.idepth[l], S.ws[l], c->w[l], c->h[l], c->w[l - 1]);
     k++;
   }
-  for (int l = 0; l < L.levels; l++) {
-    const int npx = L.w[l] * L.h[l];
-    cd_dilate_kernel<<<(npx + 255) / 256, 256, 0, s>>>(L.ws[l], L.ws2[l], L.idepth[l], L.w[l], L.h[l], l < 2 ? 1 : 0);
+  for (int l = 0; l < c->cfg.levels; l++) {
+    const int npx = c->w[l] * c->h[l];
+    cd_dilate_kernel<<<(npx + 255) / 256, 256, 0, s>>>(S.ws[l], S.ws2[l], S.idepth[l], c->w[l], c->h[l], l < 2 ? 1 : 0);
     k++;
-    const int nrows = L.h[l] - 4;
+    const int nrows = c->h[l] - 4;
     if (nrows > 0) {
-      cd_rowcount_kernel<<<(nrows + 7) / 8, 256, 0, s>>>(L.ws2[l], L.idepth[l], L.img[l], L.w[l], L.h[l], L.rowcnt);
-      cd_scan_kernel<<<1, 1024, 0, s>>>(L.rowcnt, L.rowoff, nrows, L.totals + l);
-      cd_write_kernel<<<(nrows + 7) / 8, 256, 0, s>>>(L.ws2[l], L.idepth[l], L.img[l], L.w[l], L.h[l], L.rowoff, L.cap, L.pc_u[l], L.pc_v[l], L.pc_id[l], L.pc_col[l]);
+      cd_rowcount_kernel<<<(nrows + 7) / 8, 256, 0, s>>>(S.ws2[l], S.idepth[l], c->d_img[l], c->w[l], c->h[l], S.rowcnt);
+      cd_scan_kernel<<<1, 1024, 0, s>>>(S.rowcnt, S.rowoff, nrows, S.totals + l);
+      cd_write_kernel<<<(nrows + 7) / 8, 256, 0, s>>>(S.ws2[l], S.idepth[l], c->d_img[l], c->w[l], c->h[l], S.rowoff, c->cfg.max_points, c->d_u[l],
+                                                      c->d_v[l], c->d_id[l], c->d_col[l]);
       k += 3;
     } else {
-      cudaMemsetAsync(L.totals + l, 0, sizeof(int), s);
+      cudaMemsetAsync(S.totals + l, 0, sizeof(int), s);
     }
   }
   return k;
-}
-
-void cd_launch(const CDLevels& L, int n_unique, const int* d_pix, const float* d_idw, const float* d_wsum, cudaStream_t s) {
-  cd_clear(L, s);
-  if (n_unique > 0) cd_scatter_kernel<<<(n_unique + 255) / 256, 256, 0, s>>>(n_unique, d_pix, d_idw, d_wsum, L.idepth[0], L.ws[0]);
-  cd_reduce(L, s);
 }
 
 // one entry per window point: key = the level-0 pixel u + w0 * v of its IN residual into the reference frame (CoarseTracker.cpp:L148-153),
@@ -195,22 +221,26 @@ __global__ void cd_fold_kernel(int n, const unsigned* __restrict__ key, const in
   ws0[k] = ws;
 }
 
-size_t cd_sort_temp_bytes(int cap) {
+static size_t cd_sort_temp_bytes(int cap) {
   size_t bytes = 0;
   cub::DeviceRadixSort::SortPairs(nullptr, bytes, (const unsigned*)nullptr, (unsigned*)nullptr, (const int*)nullptr, (int*)nullptr, cap, 0, 32);
   return bytes;
 }
 
-cudaError_t cd_launch_from_ba(const CDLevels& L, const CDFromBA& B, const CDSortScratch& S, cudaStream_t s, int* kernels) {
-  const unsigned npx = (unsigned)(L.w[0] * L.h[0]);
+// the same lists as dmv_ct_make_coarse_depth fed with the host fold of the IN residuals, built without leaving the device.  *kernels = the
+// kernels it launches itself (the radix sort's own launches are not counted); returns the first error of the sort or a launch.
+static cudaError_t cd_launch_from_ba(dmv_ct* c, const CDFromBA& B, int* kernels) {
+  const CDScratch& S = *c->cd;
+  const cudaStream_t s = c->stream;
+  const unsigned npx = (unsigned)(c->w[0] * c->h[0]);
   int end_bit = 1;
   while (end_bit < 32 && (npx >> end_bit) != 0) end_bit++;   // keys are <= npx
   int k = 0;
-  cd_clear(L, s);
+  cd_clear(c);
   cudaMemsetAsync(S.bad, 0x7f, sizeof(int), s);   // 0x7f7f7f7f: above any point index
   if (B.npts > 0) {
     const int g = (B.npts + 255) / 256;
-    cd_key_kernel<<<g, 256, 0, s>>>(B.npts, B.st, B.cu, B.cv, L.w[0], L.h[0], S.key[0], S.ord[0], S.bad);
+    cd_key_kernel<<<g, 256, 0, s>>>(B.npts, B.st, B.cu, B.cv, c->w[0], c->h[0], S.key[0], S.ord[0], S.bad);
     k++;
     if (B.n_moves > 0) {
       cd_move_kernel<<<(B.n_moves + 255) / 256, 256, 0, s>>>(B.n_moves, B.moves, npx, S.key[0], S.ord[0]);
@@ -222,12 +252,148 @@ cudaError_t cd_launch_from_ba(const CDLevels& L, const CDFromBA& B, const CDSort
     // LSD radix sort: stable, so the points of one pixel stay in fold order (array position)
     e = cub::DeviceRadixSort::SortPairs(S.temp, tb, S.key[0], S.key[1], S.ord[0], S.ord[1], B.npts, 0, end_bit, s);
     if (e != cudaSuccess) return e;
-    cd_fold_kernel<<<g, 256, 0, s>>>(B.npts, S.key[1], S.ord[1], B.cid, B.hdi, npx, L.idepth[0], L.ws[0]);
+    cd_fold_kernel<<<g, 256, 0, s>>>(B.npts, S.key[1], S.ord[1], B.cid, B.hdi, npx, S.idepth[0], S.ws[0]);
     k++;
   }
-  k += cd_reduce(L, s);
+  k += cd_reduce(c);
   *kernels = k;
   return cudaGetLastError();
 }
 
 }  // namespace dmv
+
+using namespace dmv;
+
+// working planes of the device makeCoarseDepthL0, allocated on first use
+static int ct_cd_allocate(dmv_ct* c) {
+  if (!c->cd) c->cd = new CDScratch();
+  CDScratch& S = *c->cd;
+  if (S.totals) return DMV_OK;
+  for (int l = 0; l < c->cfg.levels; l++) {
+    const size_t npx = (size_t)c->w[l] * c->h[l];
+    CK(cudaMalloc(&S.idepth[l], npx * sizeof(float)));
+    CK(cudaMalloc(&S.ws[l], npx * sizeof(float)));
+    CK(cudaMalloc(&S.ws2[l], npx * sizeof(float)));
+  }
+  CK(cudaMalloc(&S.rowcnt, sizeof(int) * c->h[0]));
+  CK(cudaMalloc(&S.rowoff, sizeof(int) * c->h[0]));
+  CK(cudaMallocHost(&S.totals, sizeof(int) * (DMV_MAX_PYR_LEVELS + 1)));
+  return DMV_OK;
+}
+// pc_n of every level from the compaction's totals (after the stream synchronisation); a level over capacity is an error
+static int ct_cd_take_counts(dmv_ct* c, int32_t* pc_n_out) {
+  const int* totals = c->cd->totals;
+  for (int l = 0; l < c->cfg.levels; l++) {
+    if (totals[l] > c->cfg.max_points) return set_error(DMV_ERR_INVALID, "level %d: %d reference points exceed max_points %d", l, totals[l], c->cfg.max_points);
+    c->n[l] = totals[l];
+    if (pc_n_out) pc_n_out[l] = c->n[l];
+  }
+  return DMV_OK;
+}
+
+// CoarseTracker::setCoarseTrackingRef -> makeCoarseDepthL0 (CoarseTracker.cpp:L138-295) on the device; the reference frame is
+// the one resident in the handle (last dmv_ct_upload_new_image / dmv_ct_upload_new of every level)
+int dmv_ct_make_coarse_depth(dmv_ct* c, int n, const float* Ku, const float* Kv, const float* new_idepth, const float* HdiF, int32_t* pc_n_out) {
+  if (!c || n < 0 || (n > 0 && (!Ku || !Kv || !new_idepth || !HdiF))) return set_error(DMV_ERR_INVALID, "null argument");
+  CK(cudaSetDevice(c->device));
+  const int L = c->cfg.levels, w0 = c->w[0], h0 = c->h[0];
+  int rc = ct_cd_allocate(c);
+  if (rc != DMV_OK) return rc;
+  // ---- the splat's only order-dependent part on the host: points hitting the same pixel are folded in input order (L144-160)
+  CK(ct_reserve_ip(c, n));
+  CK(ct_wait_staging(c));
+  const size_t cap = c->ip_cap;
+  int* h_pix = reinterpret_cast<int*>(c->h_ip);
+  float* h_idw = c->h_ip + cap;
+  float* h_ws = c->h_ip + 2 * cap;
+  int nu = 0;
+  {
+    std::unordered_map<int, int> slot;
+    slot.reserve((size_t)n * 2);
+    for (int i = 0; i < n; i++) {
+      const int u = Ku[i] + 0.5f, v = Kv[i] + 0.5f;
+      if (u < 0 || v < 0 || u >= w0 || v >= h0) return set_error(DMV_ERR_INVALID, "residual %d projects to (%d,%d) outside the image", i, u, v);
+      const float weight = sqrtf(1e-3 / (HdiF[i] + 1e-12));
+      const int pix = u + w0 * v;
+      auto it = slot.find(pix);
+      if (it == slot.end()) { slot.emplace(pix, nu); h_pix[nu] = pix; h_idw[nu] = 0.f + new_idepth[i] * weight; h_ws[nu] = 0.f + weight; nu++; }
+      else { h_idw[it->second] += new_idepth[i] * weight; h_ws[it->second] += weight; }
+    }
+  }
+  CK(cudaMemcpyAsync(c->d_ip, c->h_ip, sizeof(float) * 3 * cap, cudaMemcpyHostToDevice, c->stream));
+  cd_clear(c);
+  if (nu > 0) cd_scatter_kernel<<<(nu + 255) / 256, 256, 0, c->stream>>>(nu, reinterpret_cast<const int*>(c->d_ip), c->d_ip + cap, c->d_ip + 2 * cap, c->cd->idepth[0], c->cd->ws[0]);
+  cd_reduce(c);
+  c->launches += 2 + 4 * L;
+  CK(cudaGetLastError());
+  CK(cudaStreamSynchronize(c->stream));
+  return ct_cd_take_counts(c, pc_n_out);
+}
+
+// CoarseTracker::setCoarseTrackingRef fed straight from a BA handle on the same device (cd_launch_from_ba).  The points' IN
+// residuals into the window's newest frame are folded on the device; the frame's level-0 plane is copied from the BA slot and the coarser levels
+// are built as dmv_ct_upload_new_image builds them.  Ordered behind the BA stream by an event; one synchronisation at the end (pc_n).
+extern "C" __attribute__((visibility("hidden"))) int dmv_ba_ref_source(dmv_ba* b, CDFromBA* out);
+int dmv_ct_set_ref_from_ba(dmv_ct* c, dmv_ba* ba, int32_t* pc_n_out) {
+  if (!c || !ba) return set_error(DMV_ERR_INVALID, "null argument");
+  CDFromBA B;
+  int rc = dmv_ba_ref_source(ba, &B);
+  if (rc != DMV_OK) return rc;
+  if (B.device != c->device) return set_error(DMV_ERR_INVALID, "the BA handle lives on device %d, the tracker handle on %d", B.device, c->device);
+  if (B.w != c->w[0] || B.h != c->h[0]) return set_error(DMV_ERR_INVALID, "image size mismatch (BA %dx%d vs tracker %dx%d)", B.w, B.h, c->w[0], c->h[0]);
+  CK(cudaSetDevice(c->device));
+  if ((rc = ct_cd_allocate(c)) != DMV_OK) return rc;
+  CDScratch& S = *c->cd;
+  if (!S.ev_ba) CK(cudaEventCreateWithFlags(&S.ev_ba, cudaEventDisableTiming));
+  if (B.npts > S.sort_cap) {
+    CK(cudaStreamSynchronize(c->stream));   // kernels in flight may still use the old scratch
+    for (int k = 0; k < 2; k++) { cudaFree(S.key[k]); cudaFree(S.ord[k]); S.key[k] = nullptr; S.ord[k] = nullptr; }
+    cudaFree(S.temp); S.temp = nullptr;
+    cudaFree(S.moves); S.moves = nullptr;
+    cudaFreeHost(S.h_moves); S.h_moves = nullptr;
+    S.sort_cap = 0;
+    const int cap = std::max(B.npts, 2048);
+    for (int k = 0; k < 2; k++) { CK(cudaMalloc(&S.key[k], sizeof(unsigned) * cap)); CK(cudaMalloc(&S.ord[k], sizeof(int) * cap)); }
+    CK(cudaMalloc(&S.moves, sizeof(int) * 2 * cap));
+    CK(cudaMallocHost(&S.h_moves, sizeof(int) * 2 * cap));
+    S.temp_bytes = cd_sort_temp_bytes(cap);
+    CK(cudaMalloc(&S.temp, std::max<size_t>(S.temp_bytes, 16)));
+    if (!S.bad) CK(cudaMalloc(&S.bad, sizeof(int)));
+    S.sort_cap = cap;
+  }
+  CK(cudaEventRecord(S.ev_ba, B.stream));         // the BA's last linearisation / accumulate / frame upload
+  CK(cudaStreamWaitEvent(c->stream, S.ev_ba, 0));
+  CK(cudaMemcpyAsync(c->d_img[0], B.img, sizeof(float4) * (size_t)c->w[0] * c->h[0], cudaMemcpyDeviceToDevice, c->stream));
+  if ((rc = ct_build_pyramid(c, 1)) != DMV_OK) return rc;
+  if (B.n_moves > 0) {   // the previous call ended in a synchronisation: the pinned staging is free
+    std::memcpy(S.h_moves, B.moves_host, sizeof(int) * 2 * (size_t)B.n_moves);
+    CK(cudaMemcpyAsync(S.moves, S.h_moves, sizeof(int) * 2 * (size_t)B.n_moves, cudaMemcpyHostToDevice, c->stream));
+    B.moves = S.moves;
+  }
+  int kernels = 0;
+  CK(cd_launch_from_ba(c, B, &kernels));
+  c->launches += kernels;   // the pyramid counted itself; the radix sort's own launches are not counted
+  CK(cudaMemcpyAsync(S.totals + DMV_MAX_PYR_LEVELS, S.bad, sizeof(int), cudaMemcpyDeviceToHost, c->stream));
+  CK(cudaGetLastError());
+  CK(cudaStreamSynchronize(c->stream));
+  const int bad = S.totals[DMV_MAX_PYR_LEVELS];
+  if (bad < B.npts) {  // the lists were rebuilt from an inconsistent window: leave no reference to track against
+    for (int l = 0; l < c->cfg.levels; l++) c->n[l] = 0;
+    return set_error(DMV_ERR_INVALID, "point %d: its IN residual into the newest frame projects outside the image", bad);
+  }
+  return ct_cd_take_counts(c, pc_n_out);
+}
+
+// pc_u / pc_v / pc_idepth / pc_color of a level as they sit on the device (tests; any pointer may be NULL); returns pc_n[level] in *n
+int dmv_ct_get_ref(dmv_ct* c, int l, int* n, float* pc_u, float* pc_v, float* pc_idepth, float* pc_color) {
+  if (!c || !n || l < 0 || l >= c->cfg.levels) return set_error(DMV_ERR_INVALID, "bad argument");
+  CK(cudaSetDevice(c->device));
+  CK(cudaStreamSynchronize(c->stream));
+  *n = c->n[l];
+  const size_t bytes = sizeof(float) * c->n[l];
+  if (pc_u) CK(cudaMemcpy(pc_u, c->d_u[l], bytes, cudaMemcpyDeviceToHost));
+  if (pc_v) CK(cudaMemcpy(pc_v, c->d_v[l], bytes, cudaMemcpyDeviceToHost));
+  if (pc_idepth) CK(cudaMemcpy(pc_idepth, c->d_id[l], bytes, cudaMemcpyDeviceToHost));
+  if (pc_color) CK(cudaMemcpy(pc_color, c->d_col[l], bytes, cudaMemcpyDeviceToHost));
+  return DMV_OK;
+}

@@ -6,19 +6,14 @@
 //                      outer product.  Block reduction (ct_block_sum), per-block fp64 partials, and the last
 //                      block to finish (threadfence + ticket) folds the partials in a fixed order -> deterministic, one launch.
 //                      The buf_warped_* lists of the reference are never materialised.
-//   pyr_down_kernel / grad_kernel   FrameHessian::makeImages (HessianBlocks.cpp:L128-191) on the device.
-#include "../../include/dmvio_b200.h"
-#include "common_host.h"
+//   ct_track_cluster_kernel   CoarseTracker::trackNewestCoarse in one launch (below).
+// The entry points of the features built on the handle's resident frame live beside their kernels: ct_ingest.cu (raw frames), ct_depth.cu
+// (makeCoarseDepthL0), ip_trace.cu (immature points) and ps_select.cu (pixel selection); the handle's layout is ct_handle.h.
+#include "ct_handle.h"
 #include "inv3.h"
-#include "ip_trace.h"
-#include "ct_depth.h"
-#include "ct_ingest.h"
-#include "ps_select.h"
 #include <cuda.h>
-#include <unordered_map>
 #include <algorithm>
 #include <cstring>
-#include <vector>
 
 namespace dmv {
 
@@ -636,92 +631,26 @@ __global__ void __launch_bounds__(CTC_THREADS, 1) ct_track_cluster_kernel(const 
   }
 }
 
-__global__ void ct_repack_kernel(const float* __restrict__ src, float4* __restrict__ dst, int n) {
-  const int i = blockIdx.x * blockDim.x + threadIdx.x;
-  if (i < n) dst[i] = make_float4(src[3 * i], src[3 * i + 1], src[3 * i + 2], 0.f);
-}
-// level l+1 intensity = 2x2 box mean of level l (HessianBlocks.cpp:L159-166)
-__global__ void pyr_down_kernel(const float4* __restrict__ src, float* __restrict__ dst, int wl, int hl, int wlm1) {
-  const int x = blockIdx.x * blockDim.x + threadIdx.x, y = blockIdx.y;
-  if (x >= wl || y >= hl) return;
-  const float4* p = src + (size_t)2 * y * wlm1 + 2 * x;
-  dst[(size_t)y * wl + x] = 0.25f * (p[0].x + p[1].x + p[wlm1].x + p[wlm1 + 1].x);
-}
-__global__ void grad_kernel(const float* __restrict__ img, float4* __restrict__ dst, int w, int h) {
-  const int idx = blockIdx.x * blockDim.x + threadIdx.x;
-  if (idx >= w * h) return;
-  float dx = 0.f, dy = 0.f;
-  if (idx >= w && idx < w * (h - 1)) {
-    dx = 0.5f * (img[idx + 1] - img[idx - 1]);
-    dy = 0.5f * (img[idx + w] - img[idx - w]);
-    if (!isfinite(dx)) dx = 0.f;
-    if (!isfinite(dy)) dy = 0.f;
-  }
-  dst[idx] = make_float4(img[idx], dx, dy, 0.f);
-}
-
 }  // namespace dmv
 
 using namespace dmv;
 
-struct dmv_ct {
-  dmv_ct_config cfg;
-  int device = 0;
-  cudaStream_t stream = nullptr;
-  cudaEvent_t ev[2] = {nullptr, nullptr};
-  bool staging_busy = false;  // an asynchronous upload from h_scratch may be in flight
-  bool timing = false;  // CUDA-event timing of every evaluation (dmv_ct_set_timing); off by default: two event records per launch
-  int w[DMV_MAX_PYR_LEVELS], h[DMV_MAX_PYR_LEVELS];
-  float fx[DMV_MAX_PYR_LEVELS], fy[DMV_MAX_PYR_LEVELS], cx[DMV_MAX_PYR_LEVELS], cy[DMV_MAX_PYR_LEVELS];
-  bool haveK[DMV_MAX_PYR_LEVELS];
-  float4* d_img[DMV_MAX_PYR_LEVELS] = {nullptr};
-  float* d_gray[DMV_MAX_PYR_LEVELS] = {nullptr};
-  float* d_stage = nullptr;
-  float *d_u[DMV_MAX_PYR_LEVELS] = {nullptr}, *d_v[DMV_MAX_PYR_LEVELS] = {nullptr}, *d_id[DMV_MAX_PYR_LEVELS] = {nullptr},
-        *d_col[DMV_MAX_PYR_LEVELS] = {nullptr};
-  int n[DMV_MAX_PYR_LEVELS];
-  double* d_partial = nullptr;
-  unsigned int* d_ticket = nullptr;
-  double* d_out = nullptr;
-  double* h_out = nullptr;
-  float* h_scratch = nullptr;
-  // device-side makeCoarseDepthL0 (ct_depth.cu)
-  float *cd_idepth[DMV_MAX_PYR_LEVELS] = {nullptr}, *cd_ws[DMV_MAX_PYR_LEVELS] = {nullptr}, *cd_ws2[DMV_MAX_PYR_LEVELS] = {nullptr};
-  int *cd_rowcnt = nullptr, *cd_rowoff = nullptr, *cd_totals = nullptr;  // cd_totals: pinned host, device-visible; [DMV_MAX_PYR_LEVELS] = bad point
-  // the device fold of dmv_ct_set_ref_from_ba: sort scratch for up to rb_cap points, and the event that orders this stream behind the BA's
-  CDSortScratch rb = {{nullptr, nullptr}, {nullptr, nullptr}, nullptr, 0, nullptr, nullptr, nullptr};
-  int rb_cap = 0;
-  cudaEvent_t ev_ba = nullptr;
-  float* d_ip = nullptr;   // immature-point arrays (dmv_ct_trace_points)
-  float* h_ip = nullptr;
-  int ip_cap = 0;
-  float huber = 9.f;
-  int cluster_size = 0;        // CTAs of ct_track_cluster_kernel's cluster (0 = not probed yet, -1 = none schedulable: dmv_ct_track fails)
-  CTMaps* maps = nullptr;      // TMA descriptors of the level planes (host copy; passed as a kernel parameter)
-  int staged[DMV_MAX_PYR_LEVELS] = {0};   // levels whose map ct_make_tensor_maps encoded: the only ones the cluster kernel stages
-  long long launches = 0;
-  float last_ms[4] = {0, 0, 0, 0};
-  size_t scratch_bytes = 0;    // capacity of h_scratch
-  // raw-frame ingest (dmv_ct_set_undistort / dmv_ct_upload_raw_image)
-  bool have_undistort = false;
-  int wOrg = 0, hOrg = 0, nG = 0, pmode = 0;
-  float2* d_remap = nullptr;
-  float *d_G = nullptr, *d_vigInv = nullptr;
-  void* d_raw = nullptr;
-  // dmv_ct_make_new_traces (ps_select.cu): allocated on first use
-  PSScratch ps;
-};
-
-#define CK(call)                                                                                   \
-  do {                                                                                             \
-    cudaError_t _e = (call);                                                                       \
-    if (_e != cudaSuccess) return dmv::set_error(DMV_ERR_CUDA, "%s failed: %s", #call, cudaGetErrorString(_e)); \
-  } while (0)
+int dmv::ct_build_pyramid(dmv_ct* c, int first_level) {
+  for (int l = first_level; l < c->cfg.levels; l++) {
+    if (l > 0) {
+      launch_pyr_down(c->d_img[l - 1], c->d_gray[l], c->w[l], c->h[l], c->w[l - 1], c->stream);
+      c->launches++;
+    }
+    launch_make_dI(c->d_gray[l], c->d_img[l], c->w[l], c->h[l], c->stream);
+    c->launches++;
+  }
+  CK(cudaGetLastError());
+  return DMV_OK;
+}
 
 extern "C" {
 
 static int ct_allocate(dmv_ct* c, const dmv_ct_config* cfg);
-static int ct_build_pyramid(dmv_ct* c, int first_level);
 
 int dmv_ct_create(const dmv_ct_config* cfg, dmv_ct** out) {
   if (!cfg || !out) return set_error(DMV_ERR_INVALID, "null argument");
@@ -782,11 +711,7 @@ int dmv_ct_destroy(dmv_ct* c) {
   }
   cudaFree(c->d_stage); cudaFree(c->d_partial); cudaFree(c->d_ticket); cudaFree(c->d_out);
   cudaFreeHost(c->h_out); cudaFreeHost(c->h_scratch); cudaFree(c->d_ip); cudaFreeHost(c->h_ip);
-  for (int l = 0; l < DMV_MAX_PYR_LEVELS; l++) { cudaFree(c->cd_idepth[l]); cudaFree(c->cd_ws[l]); cudaFree(c->cd_ws2[l]); }
-  cudaFree(c->cd_rowcnt); cudaFree(c->cd_rowoff); cudaFreeHost(c->cd_totals);
-  for (int k = 0; k < 2; k++) { cudaFree(c->rb.key[k]); cudaFree(c->rb.ord[k]); }
-  cudaFree(c->rb.temp); cudaFree(c->rb.bad); cudaFree(c->rb.moves); cudaFreeHost(c->rb.h_moves);
-  if (c->ev_ba) cudaEventDestroy(c->ev_ba);
+  cd_free(c->cd);
   cudaFree(c->d_remap); cudaFree(c->d_G); cudaFree(c->d_vigInv); cudaFree(c->d_raw);
   ps_free(c->ps);
   if (c->ev[0]) cudaEventDestroy(c->ev[0]);
@@ -814,7 +739,7 @@ int dmv_ct_set_ref(dmv_ct* c, int l, int n, const float* u, const float* v, cons
   CK(cudaSetDevice(c->device));
   c->n[l] = n;
   if (n > 0) {
-    if (c->staging_busy) { CK(cudaStreamSynchronize(c->stream)); c->staging_busy = false; }
+    CK(ct_wait_staging(c));
     float* s = c->h_scratch;
     std::memcpy(s, u, 4 * (size_t)n); std::memcpy(s + n, v, 4 * (size_t)n); std::memcpy(s + 2 * (size_t)n, id, 4 * (size_t)n);
     std::memcpy(s + 3 * (size_t)n, col, 4 * (size_t)n);
@@ -831,10 +756,10 @@ int dmv_ct_upload_new(dmv_ct* c, int l, const float* dIp) {
   if (!c || !dIp || l < 0 || l >= c->cfg.levels) return set_error(DMV_ERR_INVALID, "bad level / pointer");
   CK(cudaSetDevice(c->device));
   const size_t npx = (size_t)c->w[l] * c->h[l];
-  if (c->staging_busy) { CK(cudaStreamSynchronize(c->stream)); c->staging_busy = false; }
+  CK(ct_wait_staging(c));
   std::memcpy(c->h_scratch, dIp, npx * 3 * sizeof(float));
   CK(cudaMemcpyAsync(c->d_stage, c->h_scratch, npx * 3 * sizeof(float), cudaMemcpyHostToDevice, c->stream));
-  ct_repack_kernel<<<(unsigned)((npx + 255) / 256), 256, 0, c->stream>>>(c->d_stage, c->d_img[l], (int)npx);
+  launch_repack(c->d_stage, c->d_img[l], (int)npx, c->stream);
   c->launches++;
   CK(cudaGetLastError());
   CK(cudaStreamSynchronize(c->stream));
@@ -845,7 +770,7 @@ int dmv_ct_upload_new_image(dmv_ct* c, const float* image) {
   if (!c || !image) return set_error(DMV_ERR_INVALID, "null argument");
   CK(cudaSetDevice(c->device));
   const size_t npx = (size_t)c->w[0] * c->h[0];
-  if (c->staging_busy) { CK(cudaStreamSynchronize(c->stream)); c->staging_busy = false; }  // a previous upload may still read the staging buffer
+  CK(ct_wait_staging(c));
   std::memcpy(c->h_scratch, image, npx * sizeof(float));
   CK(cudaMemcpyAsync(c->d_gray[0], c->h_scratch, npx * sizeof(float), cudaMemcpyHostToDevice, c->stream));
   const int rc = ct_build_pyramid(c, 0);
@@ -856,102 +781,11 @@ int dmv_ct_upload_new_image(dmv_ct* c, const float* image) {
   return DMV_OK;
 }
 
-// the pyramid of the frame whose level-0 intensities are in d_gray[0] (first_level 0), or whose level-0 plane d_img[0] is already in place
-// (first_level 1: dmv_ct_set_ref_from_ba copies it from the BA handle)
-static int ct_build_pyramid(dmv_ct* c, int first_level) {
-  for (int l = first_level; l < c->cfg.levels; l++) {
-    const int wl = c->w[l], hl = c->h[l];
-    if (l > 0) {
-      dim3 grid((wl + 127) / 128, hl);
-      pyr_down_kernel<<<grid, 128, 0, c->stream>>>(c->d_img[l - 1], c->d_gray[l], wl, hl, c->w[l - 1]);
-      c->launches++;
-    }
-    grad_kernel<<<(wl * hl + 255) / 256, 256, 0, c->stream>>>(c->d_gray[l], c->d_img[l], wl, hl);
-    c->launches++;
-  }
-  CK(cudaGetLastError());
-  return DMV_OK;
-}
-
-int dmv_ct_set_undistort(dmv_ct* c, const dmv_undistort_config* u) {
-  if (!c || !u) return set_error(DMV_ERR_INVALID, "null argument");
-  const int w = c->w[0], h = c->h[0];
-  if (u->wOrg < 2 || u->hOrg < 2 || (size_t)u->wOrg * u->hOrg > ((size_t)1 << 28)) return set_error(DMV_ERR_INVALID, "bad raw size %d x %d", u->wOrg, u->hOrg);
-  if (!u->remapX != !u->remapY) return set_error(DMV_ERR_INVALID, "remapX and remapY must both be given or both be NULL");
-  if (!u->remapX && (u->wOrg != w || u->hOrg != h)) return set_error(DMV_ERR_INVALID, "passthrough needs the raw size to equal level 0 (%d x %d)", w, h);
-  if (u->photometric_mode < 0 || u->photometric_mode > 2) return set_error(DMV_ERR_INVALID, "photometric_mode must be 0, 1 or 2");
-  if (u->G && (u->nG < 256 || u->nG > 65536)) return set_error(DMV_ERR_INVALID, "nG = %d: the response map has 256 to 65536 entries", u->nG);
-  if (u->G && u->photometric_mode == 2 && !u->vignetteInv) return set_error(DMV_ERR_INVALID, "photometric_mode 2 needs vignetteInv");
-  const size_t npx = (size_t)w * h, nraw = (size_t)u->wOrg * u->hOrg;
-  std::vector<float2> remap;
-  if (u->remapX) {  // every sample the kernel reads must lie inside the raw image (the reference's constructor guarantees it, L920-941)
-    remap.resize(npx);
-    const float xmax = (float)(u->wOrg - 1), ymax = (float)(u->hOrg - 1);
-    for (size_t i = 0; i < npx; i++) {
-      const float x = u->remapX[i], y = u->remapY[i];
-      if (!(x < 0) && !(x >= 0 && x < xmax && y >= 0 && y < ymax))
-        return set_error(DMV_ERR_INVALID, "remap entry %zu = (%g, %g) lies outside [0, %d) x [0, %d)", i, x, y, u->wOrg - 1, u->hOrg - 1);
-      remap[i] = make_float2(x, y);
-    }
-  }
-  CK(cudaSetDevice(c->device));
-  CK(cudaStreamSynchronize(c->stream));  // kernels in flight may read the old tables or the staging buffer
-  c->staging_busy = false;
-  c->have_undistort = false;
-  cudaFree(c->d_remap); cudaFree(c->d_G); cudaFree(c->d_vigInv); cudaFree(c->d_raw);
-  c->d_remap = nullptr; c->d_G = nullptr; c->d_vigInv = nullptr; c->d_raw = nullptr;
-  if (nraw * 2 > c->scratch_bytes) {
-    cudaFreeHost(c->h_scratch);
-    c->h_scratch = nullptr;
-    c->scratch_bytes = 0;
-    CK(cudaMallocHost(&c->h_scratch, nraw * 2));
-    c->scratch_bytes = nraw * 2;
-  }
-  CK(cudaMalloc(&c->d_raw, nraw * 2));
-  if (u->remapX) {
-    CK(cudaMalloc(&c->d_remap, npx * sizeof(float2)));
-    CK(cudaMemcpy(c->d_remap, remap.data(), npx * sizeof(float2), cudaMemcpyHostToDevice));
-  }
-  if (u->G) {
-    CK(cudaMalloc(&c->d_G, (size_t)u->nG * sizeof(float)));
-    CK(cudaMemcpy(c->d_G, u->G, (size_t)u->nG * sizeof(float), cudaMemcpyHostToDevice));
-  }
-  if (u->G && u->vignetteInv) {
-    CK(cudaMalloc(&c->d_vigInv, nraw * sizeof(float)));
-    CK(cudaMemcpy(c->d_vigInv, u->vignetteInv, nraw * sizeof(float), cudaMemcpyHostToDevice));
-  }
-  c->wOrg = u->wOrg; c->hOrg = u->hOrg; c->nG = u->G ? u->nG : 0; c->pmode = u->photometric_mode;
-  c->have_undistort = true;
-  return DMV_OK;
-}
-
-int dmv_ct_upload_raw_image(dmv_ct* c, const void* raw, int bpp, float exposure, float factor) {
-  if (!c || !raw) return set_error(DMV_ERR_INVALID, "null argument");
-  if (bpp != 1 && bpp != 2) return set_error(DMV_ERR_INVALID, "bytes_per_px must be 1 or 2");
-  if (!c->have_undistort) return set_error(DMV_ERR_INVALID, "dmv_ct_set_undistort first");
-  // PhotometricUndistorter::processFrame L222: the calibrated branch needs a valid calibration, exposure_time > 0 and mode != 0
-  const bool use_G = c->d_G && exposure > 0 && c->pmode != 0;
-  if (use_G && c->nG < (bpp == 1 ? 256 : 65536)) return set_error(DMV_ERR_INVALID, "a %d-entry response map does not cover %d-bit pixels", c->nG, 8 * bpp);
-  CK(cudaSetDevice(c->device));
-  const size_t bytes = (size_t)c->wOrg * c->hOrg * bpp;
-  if (c->staging_busy) { CK(cudaStreamSynchronize(c->stream)); c->staging_busy = false; }
-  std::memcpy(c->h_scratch, raw, bytes);
-  CK(cudaMemcpyAsync(c->d_raw, c->h_scratch, bytes, cudaMemcpyHostToDevice, c->stream));
-  IngestTables t;
-  t.npx = c->w[0] * c->h[0]; t.wOrg = c->wOrg; t.remap = c->d_remap; t.G = c->d_G; t.vigInv = c->d_vigInv; t.mode = c->pmode;
-  ingest_launch(t, c->d_raw, bpp, use_G, factor, c->d_gray[0], c->stream);
-  c->launches++;
-  const int rc = ct_build_pyramid(c, 0);
-  if (rc != DMV_OK) return rc;
-  c->staging_busy = true;  // asynchronous like dmv_ct_upload_new_image
-  return DMV_OK;
-}
-
 int dmv_ct_download_frame(dmv_ct* c, int l, float* dIp) {
   if (!c || !dIp || l < 0 || l >= c->cfg.levels) return set_error(DMV_ERR_INVALID, "bad level / pointer");
   CK(cudaSetDevice(c->device));
   const size_t npx = (size_t)c->w[l] * c->h[l];
-  if (c->staging_busy) { CK(cudaStreamSynchronize(c->stream)); c->staging_busy = false; }
+  CK(ct_wait_staging(c));
   // float4 (I, dx, dy, 0) -> 3 floats per pixel into the pinned staging buffer (it holds w*h*3 floats of level 0)
   CK(cudaMemcpy2DAsync(c->h_scratch, 3 * sizeof(float), c->d_img[l], sizeof(float4), 3 * sizeof(float), npx, cudaMemcpyDeviceToHost, c->stream));
   CK(cudaStreamSynchronize(c->stream));
@@ -1119,331 +953,6 @@ int dmv_ct_track(dmv_ct* c, const dmv_ct_track_args* in, dmv_ct_track_result* ou
   for (int i = 0; i < 5; i++) out->lastResiduals[i] = o[14 + i];
   for (int i = 0; i < 3; i++) out->flowIndicators[i] = o[19 + i];
   out->trackingGood = (int)o[22]; out->iterations = (int)o[23]; out->evaluations = (int)o[24]; out->status = (int)o[25];
-  return DMV_OK;
-}
-
-void dmv_ip_default_settings(dmv_ip_settings* s) {
-  s->maxPixSearch = 0.027f; s->trace_stepsize = 1.0f; s->trace_GNThreshold = 0.1f; s->trace_extraSlackOnTH = 1.2f; s->trace_slackInterval = 1.5f;
-  s->trace_minImprovementFactor = 2.f; s->huberTH = 9.f; s->trace_GNIterations = 3; s->minTraceTestRadius = 2;
-}
-
-// working planes of the device makeCoarseDepthL0, allocated on first use
-static int ct_cd_allocate(dmv_ct* c) {
-  if (c->cd_totals) return DMV_OK;
-  for (int l = 0; l < c->cfg.levels; l++) {
-    const size_t npx = (size_t)c->w[l] * c->h[l];
-    CK(cudaMalloc(&c->cd_idepth[l], npx * sizeof(float)));
-    CK(cudaMalloc(&c->cd_ws[l], npx * sizeof(float)));
-    CK(cudaMalloc(&c->cd_ws2[l], npx * sizeof(float)));
-  }
-  CK(cudaMalloc(&c->cd_rowcnt, sizeof(int) * c->h[0]));
-  CK(cudaMalloc(&c->cd_rowoff, sizeof(int) * c->h[0]));
-  CK(cudaMallocHost(&c->cd_totals, sizeof(int) * (DMV_MAX_PYR_LEVELS + 1)));
-  return DMV_OK;
-}
-static CDLevels ct_cd_levels(const dmv_ct* c) {
-  CDLevels Lv;
-  Lv.levels = c->cfg.levels; Lv.cap = c->cfg.max_points;
-  for (int l = 0; l < c->cfg.levels; l++) {
-    Lv.w[l] = c->w[l]; Lv.h[l] = c->h[l];
-    Lv.idepth[l] = c->cd_idepth[l]; Lv.ws[l] = c->cd_ws[l]; Lv.ws2[l] = c->cd_ws2[l]; Lv.img[l] = c->d_img[l];
-    Lv.pc_u[l] = c->d_u[l]; Lv.pc_v[l] = c->d_v[l]; Lv.pc_id[l] = c->d_id[l]; Lv.pc_col[l] = c->d_col[l];
-  }
-  Lv.rowcnt = c->cd_rowcnt; Lv.rowoff = c->cd_rowoff; Lv.totals = c->cd_totals;
-  return Lv;
-}
-// pc_n of every level from the compaction's totals (after the stream synchronisation); a level over capacity is an error
-static int ct_cd_take_counts(dmv_ct* c, int32_t* pc_n_out) {
-  for (int l = 0; l < c->cfg.levels; l++) {
-    if (c->cd_totals[l] > c->cfg.max_points) return set_error(DMV_ERR_INVALID, "level %d: %d reference points exceed max_points %d", l, c->cd_totals[l], c->cfg.max_points);
-    c->n[l] = c->cd_totals[l];
-    if (pc_n_out) pc_n_out[l] = c->n[l];
-  }
-  return DMV_OK;
-}
-
-// CoarseTracker::setCoarseTrackingRef -> makeCoarseDepthL0 (CoarseTracker.cpp:L138-295) on the device (ct_depth.cu); the reference frame is
-// the one resident in the handle (last dmv_ct_upload_new_image / dmv_ct_upload_new of every level)
-int dmv_ct_make_coarse_depth(dmv_ct* c, int n, const float* Ku, const float* Kv, const float* new_idepth, const float* HdiF, int32_t* pc_n_out) {
-  if (!c || n < 0 || (n > 0 && (!Ku || !Kv || !new_idepth || !HdiF))) return set_error(DMV_ERR_INVALID, "null argument");
-  CK(cudaSetDevice(c->device));
-  const int L = c->cfg.levels, w0 = c->w[0], h0 = c->h[0];
-  int rc = ct_cd_allocate(c);
-  if (rc != DMV_OK) return rc;
-  // ---- the splat's only order-dependent part on the host: points hitting the same pixel are folded in input order (L144-160)
-  if (n > c->ip_cap) {
-    if (c->d_ip) cudaFree(c->d_ip);
-    if (c->h_ip) cudaFreeHost(c->h_ip);
-    c->ip_cap = std::max(n, 2048);
-    CK(cudaMalloc(&c->d_ip, sizeof(float) * ((size_t)31 * c->ip_cap + 14 * 64)));
-    CK(cudaMallocHost(&c->h_ip, sizeof(float) * ((size_t)31 * c->ip_cap + 14 * 64)));
-  }
-  if (c->staging_busy) { CK(cudaStreamSynchronize(c->stream)); c->staging_busy = false; }
-  const size_t cap = c->ip_cap;
-  int* h_pix = reinterpret_cast<int*>(c->h_ip);
-  float* h_idw = c->h_ip + cap;
-  float* h_ws = c->h_ip + 2 * cap;
-  int nu = 0;
-  {
-    std::unordered_map<int, int> slot;
-    slot.reserve((size_t)n * 2);
-    for (int i = 0; i < n; i++) {
-      const int u = Ku[i] + 0.5f, v = Kv[i] + 0.5f;
-      if (u < 0 || v < 0 || u >= w0 || v >= h0) return set_error(DMV_ERR_INVALID, "residual %d projects to (%d,%d) outside the image", i, u, v);
-      const float weight = sqrtf(1e-3 / (HdiF[i] + 1e-12));
-      const int pix = u + w0 * v;
-      auto it = slot.find(pix);
-      if (it == slot.end()) { slot.emplace(pix, nu); h_pix[nu] = pix; h_idw[nu] = 0.f + new_idepth[i] * weight; h_ws[nu] = 0.f + weight; nu++; }
-      else { h_idw[it->second] += new_idepth[i] * weight; h_ws[it->second] += weight; }
-    }
-  }
-  CK(cudaMemcpyAsync(c->d_ip, c->h_ip, sizeof(float) * 3 * cap, cudaMemcpyHostToDevice, c->stream));
-  const CDLevels Lv = ct_cd_levels(c);
-  cd_launch(Lv, nu, reinterpret_cast<const int*>(c->d_ip), c->d_ip + cap, c->d_ip + 2 * cap, c->stream);
-  c->launches += 2 + 4 * L;
-  CK(cudaGetLastError());
-  CK(cudaStreamSynchronize(c->stream));
-  return ct_cd_take_counts(c, pc_n_out);
-}
-
-// CoarseTracker::setCoarseTrackingRef fed straight from a BA handle on the same device (ct_depth.cu: cd_launch_from_ba).  The points' IN
-// residuals into the window's newest frame are folded on the device; the frame's level-0 plane is copied from the BA slot and the coarser levels
-// are built as dmv_ct_upload_new_image builds them.  Ordered behind the BA stream by an event; one synchronisation at the end (pc_n).
-extern "C" __attribute__((visibility("hidden"))) int dmv_ba_ref_source(dmv_ba* b, CDFromBA* out);
-int dmv_ct_set_ref_from_ba(dmv_ct* c, dmv_ba* ba, int32_t* pc_n_out) {
-  if (!c || !ba) return set_error(DMV_ERR_INVALID, "null argument");
-  CDFromBA B;
-  int rc = dmv_ba_ref_source(ba, &B);
-  if (rc != DMV_OK) return rc;
-  if (B.device != c->device) return set_error(DMV_ERR_INVALID, "the BA handle lives on device %d, the tracker handle on %d", B.device, c->device);
-  if (B.w != c->w[0] || B.h != c->h[0]) return set_error(DMV_ERR_INVALID, "image size mismatch (BA %dx%d vs tracker %dx%d)", B.w, B.h, c->w[0], c->h[0]);
-  CK(cudaSetDevice(c->device));
-  if ((rc = ct_cd_allocate(c)) != DMV_OK) return rc;
-  if (!c->ev_ba) CK(cudaEventCreateWithFlags(&c->ev_ba, cudaEventDisableTiming));
-  if (B.npts > c->rb_cap) {
-    CK(cudaStreamSynchronize(c->stream));   // kernels in flight may still use the old scratch
-    for (int k = 0; k < 2; k++) { cudaFree(c->rb.key[k]); cudaFree(c->rb.ord[k]); c->rb.key[k] = nullptr; c->rb.ord[k] = nullptr; }
-    cudaFree(c->rb.temp); c->rb.temp = nullptr;
-    cudaFree(c->rb.moves); c->rb.moves = nullptr;
-    cudaFreeHost(c->rb.h_moves); c->rb.h_moves = nullptr;
-    c->rb_cap = 0;
-    const int cap = std::max(B.npts, 2048);
-    for (int k = 0; k < 2; k++) { CK(cudaMalloc(&c->rb.key[k], sizeof(unsigned) * cap)); CK(cudaMalloc(&c->rb.ord[k], sizeof(int) * cap)); }
-    CK(cudaMalloc(&c->rb.moves, sizeof(int) * 2 * cap));
-    CK(cudaMallocHost(&c->rb.h_moves, sizeof(int) * 2 * cap));
-    c->rb.temp_bytes = cd_sort_temp_bytes(cap);
-    CK(cudaMalloc(&c->rb.temp, std::max<size_t>(c->rb.temp_bytes, 16)));
-    if (!c->rb.bad) CK(cudaMalloc(&c->rb.bad, sizeof(int)));
-    c->rb_cap = cap;
-  }
-  CK(cudaEventRecord(c->ev_ba, B.stream));         // the BA's last linearisation / accumulate / frame upload
-  CK(cudaStreamWaitEvent(c->stream, c->ev_ba, 0));
-  CK(cudaMemcpyAsync(c->d_img[0], B.img, sizeof(float4) * (size_t)c->w[0] * c->h[0], cudaMemcpyDeviceToDevice, c->stream));
-  if ((rc = ct_build_pyramid(c, 1)) != DMV_OK) return rc;
-  if (B.n_moves > 0) {   // the previous call ended in a synchronisation: the pinned staging is free
-    std::memcpy(c->rb.h_moves, B.moves_host, sizeof(int) * 2 * (size_t)B.n_moves);
-    CK(cudaMemcpyAsync(c->rb.moves, c->rb.h_moves, sizeof(int) * 2 * (size_t)B.n_moves, cudaMemcpyHostToDevice, c->stream));
-    B.moves = c->rb.moves;
-  }
-  int kernels = 0;
-  CK(cd_launch_from_ba(ct_cd_levels(c), B, c->rb, c->stream, &kernels));
-  c->launches += kernels;   // the pyramid counted itself; the radix sort's own launches are not counted
-  CK(cudaMemcpyAsync(c->cd_totals + DMV_MAX_PYR_LEVELS, c->rb.bad, sizeof(int), cudaMemcpyDeviceToHost, c->stream));
-  CK(cudaGetLastError());
-  CK(cudaStreamSynchronize(c->stream));
-  const int bad = c->cd_totals[DMV_MAX_PYR_LEVELS];
-  if (bad < B.npts) {  // the lists were rebuilt from an inconsistent window: leave no reference to track against
-    for (int l = 0; l < c->cfg.levels; l++) c->n[l] = 0;
-    return set_error(DMV_ERR_INVALID, "point %d: its IN residual into the newest frame projects outside the image", bad);
-  }
-  return ct_cd_take_counts(c, pc_n_out);
-}
-
-// pc_u / pc_v / pc_idepth / pc_color of a level as they sit on the device (tests; any pointer may be NULL); returns pc_n[level] in *n
-int dmv_ct_get_ref(dmv_ct* c, int l, int* n, float* pc_u, float* pc_v, float* pc_idepth, float* pc_color) {
-  if (!c || !n || l < 0 || l >= c->cfg.levels) return set_error(DMV_ERR_INVALID, "bad argument");
-  CK(cudaSetDevice(c->device));
-  CK(cudaStreamSynchronize(c->stream));
-  *n = c->n[l];
-  const size_t bytes = sizeof(float) * c->n[l];
-  if (pc_u) CK(cudaMemcpy(pc_u, c->d_u[l], bytes, cudaMemcpyDeviceToHost));
-  if (pc_v) CK(cudaMemcpy(pc_v, c->d_v[l], bytes, cudaMemcpyDeviceToHost));
-  if (pc_idepth) CK(cudaMemcpy(pc_idepth, c->d_id[l], bytes, cudaMemcpyDeviceToHost));
-  if (pc_color) CK(cudaMemcpy(pc_color, c->d_col[l], bytes, cudaMemcpyDeviceToHost));
-  return DMV_OK;
-}
-
-// ImmaturePoint constructor on the resident frame (ip_trace.cu)
-int dmv_ct_init_points(dmv_ct* c, int n, const int32_t* u, const int32_t* v, float* color8, float* weights8, float* gradH4, float* energyTH, int32_t* ok) {
-  if (!c || n < 0 || (n > 0 && (!u || !v || !color8 || !weights8 || !gradH4 || !energyTH || !ok))) return set_error(DMV_ERR_INVALID, "null argument");
-  if (n == 0) return DMV_OK;
-  for (int i = 0; i < n; i++)
-    if (u[i] < 2 || v[i] < 2 || u[i] >= c->w[0] - 3 || v[i] >= c->h[0] - 3) return set_error(DMV_ERR_INVALID, "point %d (%d,%d): the pattern leaves the image", i, u[i], v[i]);
-  CK(cudaSetDevice(c->device));
-  if (n > c->ip_cap) {
-    if (c->d_ip) cudaFree(c->d_ip);
-    if (c->h_ip) cudaFreeHost(c->h_ip);
-    c->ip_cap = std::max(n, 2048);
-    CK(cudaMalloc(&c->d_ip, sizeof(float) * ((size_t)31 * c->ip_cap + 14 * 64)));
-    CK(cudaMallocHost(&c->h_ip, sizeof(float) * ((size_t)31 * c->ip_cap + 14 * 64)));
-  }
-  if (c->staging_busy) { CK(cudaStreamSynchronize(c->stream)); c->staging_busy = false; }
-  const size_t cap = c->ip_cap;
-  float* hb = c->h_ip;
-  float* d = c->d_ip;
-  // layout (words): u | v | color*8 | weights*8 | gradH*4 | energyTH | ok
-  std::memcpy(hb, u, 4 * (size_t)n); std::memcpy(hb + cap, v, 4 * (size_t)n);
-  CK(cudaMemcpyAsync(d, hb, sizeof(float) * 2 * cap, cudaMemcpyHostToDevice, c->stream));
-  IPInitArgs A;
-  A.n = n; A.w = c->w[0]; A.n_dev = nullptr;
-  A.outlierTHSumComponent = 50.f * 50.f; A.outlierTH = 12.f * 12.f; A.overallEnergyTHWeight = 1.f;  // util/settings.cpp:L111-114, L159
-  A.u = reinterpret_cast<const int*>(d); A.v = reinterpret_cast<const int*>(d + cap);
-  A.color = d + 2 * cap; A.weights = d + 10 * cap; A.gradH = d + 18 * cap; A.energyTH = d + 22 * cap; A.ok = reinterpret_cast<int*>(d + 23 * cap);
-  A.img = c->d_img[0];
-  launch_ip_init(A, c->stream);
-  c->launches++;
-  CK(cudaGetLastError());
-  CK(cudaMemcpyAsync(hb + 2 * cap, d + 2 * cap, sizeof(float) * 22 * cap, cudaMemcpyDeviceToHost, c->stream));
-  CK(cudaStreamSynchronize(c->stream));
-  std::memcpy(color8, hb + 2 * cap, 32 * (size_t)n); std::memcpy(weights8, hb + 10 * cap, 32 * (size_t)n); std::memcpy(gradH4, hb + 18 * cap, 16 * (size_t)n);
-  std::memcpy(energyTH, hb + 22 * cap, 4 * (size_t)n); std::memcpy(ok, hb + 23 * cap, 4 * (size_t)n);
-  return DMV_OK;
-}
-
-// immature points of SEVERAL host frames traced against the resident newest frame in ONE launch (ip_trace.cu): FullSystem::traceNewCoarse's
-// loop over the window's keyframes (FullSystem.cpp:L554-575) collapsed into one upload, one kernel, one download
-int dmv_ct_trace_points_multi(dmv_ct* c, int nsets, const dmv_ip_points* sets, const float* tables14, const dmv_ip_settings* settings) {
-  if (!c || nsets < 0 || (nsets > 0 && (!sets || !tables14))) return set_error(DMV_ERR_INVALID, "null argument");
-  int n = 0;
-  for (int k = 0; k < nsets; k++) {
-    const dmv_ip_points* p = &sets[k];
-    if (p->n < 0 || (p->n > 0 && (!p->u || !p->v || !p->color8 || !p->weights8 || !p->gradH4 || !p->energyTH || !p->idepth_min || !p->idepth_max || !p->quality ||
-                                  !p->lastTraceStatus || !p->lastTraceUV2 || !p->lastTracePixelInterval)))
-      return set_error(DMV_ERR_INVALID, "incomplete dmv_ip_points (set %d)", k);
-    n += p->n;
-  }
-  if (n == 0) return DMV_OK;
-  CK(cudaSetDevice(c->device));
-  const int words = 31;   // 23 read-only floats, 7 in/out words and the set index per point
-  if (n > c->ip_cap) {
-    if (c->d_ip) cudaFree(c->d_ip);
-    if (c->h_ip) cudaFreeHost(c->h_ip);
-    c->ip_cap = std::max(n, 2048);
-    CK(cudaMalloc(&c->d_ip, sizeof(float) * ((size_t)words * c->ip_cap + 14 * 64)));
-    CK(cudaMallocHost(&c->h_ip, sizeof(float) * ((size_t)words * c->ip_cap + 14 * 64)));
-  }
-  if (nsets > 64) return set_error(DMV_ERR_INVALID, "at most 64 host frames per call");
-  if (c->staging_busy) { CK(cudaStreamSynchronize(c->stream)); c->staging_busy = false; }
-  const size_t cap = c->ip_cap;
-  float* hb = c->h_ip;
-  // layout (floats): u | v | color*8 | weights*8 | gradH*4 | energyTH | idmin | idmax | quality | status(int) | uv*2 | interval | set(int) | tables
-  const size_t o_u = 0, o_v = cap, o_col = 2 * cap, o_wgt = 10 * cap, o_g = 18 * cap, o_eth = 22 * cap, o_min = 23 * cap, o_max = 24 * cap, o_q = 25 * cap,
-               o_st = 26 * cap, o_uv = 27 * cap, o_iv = 29 * cap, o_set = 30 * cap, o_tab = 31 * cap;
-  size_t at = 0;
-  for (int k = 0; k < nsets; k++) {
-    const dmv_ip_points* p = &sets[k];
-    const size_t m = (size_t)p->n;
-    if (m == 0) continue;
-    std::memcpy(hb + o_u + at, p->u, 4 * m); std::memcpy(hb + o_v + at, p->v, 4 * m);
-    std::memcpy(hb + o_col + 8 * at, p->color8, 32 * m); std::memcpy(hb + o_wgt + 8 * at, p->weights8, 32 * m);
-    std::memcpy(hb + o_g + 4 * at, p->gradH4, 16 * m); std::memcpy(hb + o_eth + at, p->energyTH, 4 * m);
-    std::memcpy(hb + o_min + at, p->idepth_min, 4 * m); std::memcpy(hb + o_max + at, p->idepth_max, 4 * m); std::memcpy(hb + o_q + at, p->quality, 4 * m);
-    std::memcpy(hb + o_st + at, p->lastTraceStatus, 4 * m); std::memcpy(hb + o_uv + 2 * at, p->lastTraceUV2, 8 * m); std::memcpy(hb + o_iv + at, p->lastTracePixelInterval, 4 * m);
-    int* setp = reinterpret_cast<int*>(hb + o_set + at);
-    for (size_t q = 0; q < m; q++) setp[q] = k;
-    at += m;
-  }
-  std::memcpy(hb + o_tab, tables14, sizeof(float) * 14 * (size_t)nsets);
-  CK(cudaMemcpyAsync(c->d_ip, hb, sizeof(float) * ((size_t)words * cap + 14 * (size_t)nsets), cudaMemcpyHostToDevice, c->stream));
-  IPTraceArgs A;
-  std::memset(&A, 0, sizeof(A));
-  A.n = n; A.w = c->w[0]; A.h = c->h[0];
-  if (settings) A.s = *settings; else dmv_ip_default_settings(&A.s);
-  float* d = c->d_ip;
-  A.tab = d + o_tab; A.set_of = reinterpret_cast<const int*>(d + o_set);
-  A.u = d + o_u; A.v = d + o_v; A.color = d + o_col; A.weights = d + o_wgt; A.gradH = d + o_g; A.energyTH = d + o_eth;
-  A.idepth_min = d + o_min; A.idepth_max = d + o_max; A.quality = d + o_q; A.status = reinterpret_cast<int*>(d + o_st); A.uv = d + o_uv; A.interval = d + o_iv;
-  A.img = c->d_img[0];
-  launch_ip_trace(A, c->stream);
-  c->launches++;
-  CK(cudaGetLastError());
-  CK(cudaMemcpyAsync(hb + o_min, d + o_min, sizeof(float) * 7 * cap, cudaMemcpyDeviceToHost, c->stream));  // the 7 in/out words per point
-  CK(cudaStreamSynchronize(c->stream));
-  at = 0;
-  for (int k = 0; k < nsets; k++) {
-    const dmv_ip_points* p = &sets[k];
-    const size_t m = (size_t)p->n;
-    if (m == 0) continue;
-    std::memcpy(p->idepth_min, hb + o_min + at, 4 * m); std::memcpy(p->idepth_max, hb + o_max + at, 4 * m); std::memcpy(p->quality, hb + o_q + at, 4 * m);
-    std::memcpy(p->lastTraceStatus, hb + o_st + at, 4 * m); std::memcpy(p->lastTraceUV2, hb + o_uv + 2 * at, 8 * m); std::memcpy(p->lastTracePixelInterval, hb + o_iv + at, 4 * m);
-    at += m;
-  }
-  return DMV_OK;
-}
-
-// one host frame's immature points traced against the resident newest frame
-int dmv_ct_trace_points(dmv_ct* c, const dmv_ip_points* p, const float KRKi[9], const float Kt[3], const float aff[2], const dmv_ip_settings* settings) {
-  if (!c || !p || !KRKi || !Kt || !aff) return set_error(DMV_ERR_INVALID, "null argument");
-  float tab[14];
-  std::memcpy(tab, KRKi, 36); std::memcpy(tab + 9, Kt, 12); std::memcpy(tab + 12, aff, 8);
-  return dmv_ct_trace_points_multi(c, 1, p, tab, settings);
-}
-
-void dmv_ps_default_settings(dmv_ps_settings* s) {
-  if (!s) return;
-  s->minGradHistCut = 0.5f; s->minGradHistAdd = 7.f; s->gradDownweightPerLevel = 0.75f;   // util/settings.cpp:L144, L167-170
-  s->selectDirectionDistribution = 1; s->gammaWeightsPixelSelect = 1;
-}
-
-// FullSystem::makeNewTraces on the resident frame (ps_select.cu)
-int dmv_ct_make_new_traces(dmv_ct* c, const dmv_new_traces_args* a) {
-  if (!c || !a) return set_error(DMV_ERR_INVALID, "null argument");
-  if (c->cfg.levels < 3) return set_error(DMV_ERR_INVALID, "pixel selection reads levels 0-2: the handle has %d", c->cfg.levels);
-  const int w = c->w[0], h = c->h[0];
-  if (w % 16 || h % 16) return set_error(DMV_ERR_INVALID, "pixel selection needs w and h divisible by 16 (%d x %d)", w, h);
-  if (!a->potential || !a->n || !a->numPointsTotal || a->cap < 0 || (a->cap > 0 && (!a->u || !a->v || !a->type || !a->color8 || !a->weights8 || !a->gradH4 || !a->energyTH)))
-    return set_error(DMV_ERR_INVALID, "null argument");
-  if (*a->potential < 1) return set_error(DMV_ERR_INVALID, "potential %d < 1", *a->potential);
-  if (!(a->density > 0.f) || !std::isfinite(a->density)) return set_error(DMV_ERR_INVALID, "density must be finite and > 0");
-  if (!(a->thFactor > 0.f) || !std::isfinite(a->thFactor)) return set_error(DMV_ERR_INVALID, "thFactor must be finite and > 0");
-  if (a->recursionsLeft < 0 || a->recursionsLeft > 8) return set_error(DMV_ERR_INVALID, "recursionsLeft must be in 0..8");
-  dmv_ps_settings st;
-  if (a->settings) st = *a->settings; else dmv_ps_default_settings(&st);
-  if (!(st.minGradHistCut < 0.99f) || !std::isfinite(st.minGradHistCut) || !std::isfinite(st.minGradHistAdd) || !std::isfinite(st.gradDownweightPerLevel))
-    return set_error(DMV_ERR_INVALID, "bad dmv_ps_settings");
-  CK(cudaSetDevice(c->device));
-  if (c->ps.w != w || c->ps.h != h) CK(ps_alloc(c->ps, w, h));
-  const int out_cap = std::min(a->cap, w * h);
-  CK(ps_ensure_out(c->ps, std::max(out_cap, 1)));
-  if (c->staging_busy) { CK(cudaStreamSynchronize(c->stream)); c->staging_busy = false; }
-  float B[256];
-  for (int i = 0; i < 256; i++) B[i] = a->B ? a->B[i] : (float)i;   // CalibHessian's constructor: B[i] = i
-  CK(cudaMemcpyAsync(c->ps.B, B, sizeof(B), cudaMemcpyHostToDevice, c->stream));
-  PSArgs A;
-  A.w = w; A.h = h;
-  for (int l = 0; l < 3; l++) A.img[l] = c->d_img[l];
-  A.s = st; A.density = a->density; A.thFactor = a->thFactor; A.recursionsLeft = a->recursionsLeft; A.potential = *a->potential;
-  A.out_cap = out_cap;
-  int kernels = 0;
-  CK(ps_launch(A, c->ps, c->stream, &kernels));
-  c->launches += kernels;
-  if (a->map) CK(cudaMemcpyAsync(a->map, c->ps.map, sizeof(float) * (size_t)w * h, cudaMemcpyDeviceToHost, c->stream));
-  CK(cudaStreamSynchronize(c->stream));
-  PSState S;
-  std::memcpy(&S, c->ps.h_out, sizeof(S));
-  *a->n = S.n_points;
-  // on overflow the selector's state stays as it was, so a retry with a larger cap continues from the same potential
-  if (S.n_points > a->cap) return set_error(DMV_ERR_INVALID, "%d new points exceed cap %d", S.n_points, a->cap);
-  *a->potential = S.ideal;
-  *a->numPointsTotal = S.numHaveSub;
-  const size_t n = (size_t)S.n_points, O = out_cap;
-  const float* o = c->ps.h_out + sizeof(PSState) / sizeof(float);
-  std::memcpy(a->u, o, 4 * n); std::memcpy(a->v, o + O, 4 * n); std::memcpy(a->type, o + 2 * O, 4 * n);
-  for (size_t i = 0; i < n; i++)
-    for (int k = 0; k < 8; k++) { a->color8[8 * i + k] = o[(3 + k) * O + i]; a->weights8[8 * i + k] = o[(11 + k) * O + i]; }
-  for (size_t i = 0; i < n; i++)
-    for (int k = 0; k < 4; k++) a->gradH4[4 * i + k] = o[(19 + k) * O + i];
-  std::memcpy(a->energyTH, o + 23 * O, 4 * n);
   return DMV_OK;
 }
 

@@ -8,10 +8,11 @@
 // THIS TRANSLATION UNIT IS COMPILED WITH -fmad=false: every expression keeps the reference's operation order and rounding (no FMA
 // contraction; IEEE division and sqrt are nvcc's defaults), so the integer decisions (best step, status, GN accept/reject) and the
 // float outputs are bit-identical to the reference's CPU code — tests/test_gpu_trace.py asserts equality, not a tolerance.
-#include "../../include/dmvio_b200.h"
-#include "common_host.h"
+// The flag affects device code only, so the C-ABI entry points of the three kernels (end of the file) are compiled here too.
+#include "ct_handle.h"
+#include "ba_handle.h"
 #include "ip_trace.h"
-#include <cuda_runtime.h>
+#include <cstring>
 #include <math.h>
 
 namespace dmv {
@@ -35,6 +36,19 @@ __device__ __forceinline__ void ip_interp33(const float4* __restrict__ mat, floa
   out[1] = dxdy * br.y + (dy - dxdy) * bl.y + (dx - dxdy) * tr.y + (1 - dx - dy + dxdy) * tl.y;
   out[2] = dxdy * br.z + (dy - dxdy) * bl.z + (dx - dxdy) * tr.z + (1 - dx - dy + dxdy) * tl.z;
 }
+
+struct IPTraceArgs {
+  int n, w, h;
+  float KRKi[9], Kt[3], aff[2];   // one host frame (tab == nullptr)
+  const float* tab;               // several host frames in one launch: [set][14] = KRKi 9 | Kt 3 | aff 2, and set_of[point]
+  const int* set_of;
+  dmv_ip_settings s;
+  const float *u, *v, *color, *weights, *gradH, *energyTH;
+  float *idepth_min, *idepth_max, *quality;
+  int* status;
+  float *uv, *interval;
+  const float4* img;
+};
 
 // One WARP per immature point.  The reference walks the epipolar segment step by step (<= 99 positions x 8 bilinear samples) and keeps the
 // best and second-best energies; here the positions are dealt to the 32 lanes (lane L takes steps L, L+32, L+64, L+96: at most 4 rounds
@@ -298,6 +312,18 @@ __global__ void __launch_bounds__(128) ip_init_kernel(const __grid_constant__ IP
 // behaviour on an out-of-bounds sample: the residual becomes OOB but the sums keep the terms of the samples BEFORE the first bad one.
 // Same -fmad=false rule as the tracing kernel: bit-identical to the CPU code (float/double promotions of the reference kept explicitly).
 // ---------------------------------------------------------------------------------------------------------------------
+struct IPActArgs {
+  int n, nf, w, h, minObs, GNIts;
+  float fxl, fyl, cxl, cyl, fxli, fyli, huberTH, minIdepthH_act;
+  const float4* img[DMV_MAX_FRAMES];
+  const float* RT;    // [h*nf+t][12]
+  const float* aff;   // [h*nf+t][2]
+  const int* host;
+  const float *u, *v, *color, *weights, *energyTH, *idepth_min, *idepth_max;
+  int* status;
+  float* idepth;
+  int* res_state;     // [n][nf]
+};
 struct IPResState { int state, newState; double energy, newEnergy; };
 
 // linearizeResidual for (point, target f) by the point's 8 lanes; every lane returns the same value and updates its copy of (Hdd, bd, rs).
@@ -433,10 +459,167 @@ __global__ void __launch_bounds__(128) ip_activate_kernel(const __grid_constant_
   if (writer) { A.idepth[i] = idepth_out; A.status[i] = status_out; }
 }
 
-void launch_ip_activate(const IPActArgs& A, cudaStream_t s) { ip_activate_kernel<<<(A.n + 15) / 16, 128, 0, s>>>(A); }  // 8 lanes per point
-
 void launch_ip_init(const IPInitArgs& A, cudaStream_t s) { ip_init_kernel<<<(A.n + 127) / 128, 128, 0, s>>>(A); }
 
-void launch_ip_trace(const IPTraceArgs& A, cudaStream_t s) { ip_trace_kernel<<<(A.n + 3) / 4, 128, 0, s>>>(A); }  // 4 warps = 4 points per CTA
-
 }  // namespace dmv
+
+using namespace dmv;
+
+void dmv_ip_default_settings(dmv_ip_settings* s) {
+  s->maxPixSearch = 0.027f; s->trace_stepsize = 1.0f; s->trace_GNThreshold = 0.1f; s->trace_extraSlackOnTH = 1.2f; s->trace_slackInterval = 1.5f;
+  s->trace_minImprovementFactor = 2.f; s->huberTH = 9.f; s->trace_GNIterations = 3; s->minTraceTestRadius = 2;
+}
+
+// ImmaturePoint constructor on the resident frame (ip_init_kernel)
+int dmv_ct_init_points(dmv_ct* c, int n, const int32_t* u, const int32_t* v, float* color8, float* weights8, float* gradH4, float* energyTH, int32_t* ok) {
+  if (!c || n < 0 || (n > 0 && (!u || !v || !color8 || !weights8 || !gradH4 || !energyTH || !ok))) return set_error(DMV_ERR_INVALID, "null argument");
+  if (n == 0) return DMV_OK;
+  for (int i = 0; i < n; i++)
+    if (u[i] < 2 || v[i] < 2 || u[i] >= c->w[0] - 3 || v[i] >= c->h[0] - 3) return set_error(DMV_ERR_INVALID, "point %d (%d,%d): the pattern leaves the image", i, u[i], v[i]);
+  CK(cudaSetDevice(c->device));
+  CK(ct_reserve_ip(c, n));
+  CK(ct_wait_staging(c));
+  const size_t cap = c->ip_cap;
+  float* hb = c->h_ip;
+  float* d = c->d_ip;
+  // layout (words): u | v | color*8 | weights*8 | gradH*4 | energyTH | ok
+  std::memcpy(hb, u, 4 * (size_t)n); std::memcpy(hb + cap, v, 4 * (size_t)n);
+  CK(cudaMemcpyAsync(d, hb, sizeof(float) * 2 * cap, cudaMemcpyHostToDevice, c->stream));
+  IPInitArgs A;
+  A.n = n; A.w = c->w[0]; A.n_dev = nullptr;
+  A.outlierTHSumComponent = 50.f * 50.f; A.outlierTH = 12.f * 12.f; A.overallEnergyTHWeight = 1.f;  // util/settings.cpp:L111-114, L159
+  A.u = reinterpret_cast<const int*>(d); A.v = reinterpret_cast<const int*>(d + cap);
+  A.color = d + 2 * cap; A.weights = d + 10 * cap; A.gradH = d + 18 * cap; A.energyTH = d + 22 * cap; A.ok = reinterpret_cast<int*>(d + 23 * cap);
+  A.img = c->d_img[0];
+  launch_ip_init(A, c->stream);
+  c->launches++;
+  CK(cudaGetLastError());
+  CK(cudaMemcpyAsync(hb + 2 * cap, d + 2 * cap, sizeof(float) * 22 * cap, cudaMemcpyDeviceToHost, c->stream));
+  CK(cudaStreamSynchronize(c->stream));
+  std::memcpy(color8, hb + 2 * cap, 32 * (size_t)n); std::memcpy(weights8, hb + 10 * cap, 32 * (size_t)n); std::memcpy(gradH4, hb + 18 * cap, 16 * (size_t)n);
+  std::memcpy(energyTH, hb + 22 * cap, 4 * (size_t)n); std::memcpy(ok, hb + 23 * cap, 4 * (size_t)n);
+  return DMV_OK;
+}
+
+// immature points of SEVERAL host frames traced against the resident newest frame in ONE launch (ip_trace_kernel): FullSystem::traceNewCoarse's
+// loop over the window's keyframes (FullSystem.cpp:L554-575) collapsed into one upload, one kernel, one download
+int dmv_ct_trace_points_multi(dmv_ct* c, int nsets, const dmv_ip_points* sets, const float* tables14, const dmv_ip_settings* settings) {
+  if (!c || nsets < 0 || (nsets > 0 && (!sets || !tables14))) return set_error(DMV_ERR_INVALID, "null argument");
+  int n = 0;
+  for (int k = 0; k < nsets; k++) {
+    const dmv_ip_points* p = &sets[k];
+    if (p->n < 0 || (p->n > 0 && (!p->u || !p->v || !p->color8 || !p->weights8 || !p->gradH4 || !p->energyTH || !p->idepth_min || !p->idepth_max || !p->quality ||
+                                  !p->lastTraceStatus || !p->lastTraceUV2 || !p->lastTracePixelInterval)))
+      return set_error(DMV_ERR_INVALID, "incomplete dmv_ip_points (set %d)", k);
+    n += p->n;
+  }
+  if (n == 0) return DMV_OK;
+  CK(cudaSetDevice(c->device));
+  const int words = 31;   // 23 read-only floats, 7 in/out words and the set index per point
+  CK(ct_reserve_ip(c, n));
+  if (nsets > 64) return set_error(DMV_ERR_INVALID, "at most 64 host frames per call");
+  CK(ct_wait_staging(c));
+  const size_t cap = c->ip_cap;
+  float* hb = c->h_ip;
+  // layout (floats): u | v | color*8 | weights*8 | gradH*4 | energyTH | idmin | idmax | quality | status(int) | uv*2 | interval | set(int) | tables
+  const size_t o_u = 0, o_v = cap, o_col = 2 * cap, o_wgt = 10 * cap, o_g = 18 * cap, o_eth = 22 * cap, o_min = 23 * cap, o_max = 24 * cap, o_q = 25 * cap,
+               o_st = 26 * cap, o_uv = 27 * cap, o_iv = 29 * cap, o_set = 30 * cap, o_tab = 31 * cap;
+  size_t at = 0;
+  for (int k = 0; k < nsets; k++) {
+    const dmv_ip_points* p = &sets[k];
+    const size_t m = (size_t)p->n;
+    if (m == 0) continue;
+    std::memcpy(hb + o_u + at, p->u, 4 * m); std::memcpy(hb + o_v + at, p->v, 4 * m);
+    std::memcpy(hb + o_col + 8 * at, p->color8, 32 * m); std::memcpy(hb + o_wgt + 8 * at, p->weights8, 32 * m);
+    std::memcpy(hb + o_g + 4 * at, p->gradH4, 16 * m); std::memcpy(hb + o_eth + at, p->energyTH, 4 * m);
+    std::memcpy(hb + o_min + at, p->idepth_min, 4 * m); std::memcpy(hb + o_max + at, p->idepth_max, 4 * m); std::memcpy(hb + o_q + at, p->quality, 4 * m);
+    std::memcpy(hb + o_st + at, p->lastTraceStatus, 4 * m); std::memcpy(hb + o_uv + 2 * at, p->lastTraceUV2, 8 * m); std::memcpy(hb + o_iv + at, p->lastTracePixelInterval, 4 * m);
+    int* setp = reinterpret_cast<int*>(hb + o_set + at);
+    for (size_t q = 0; q < m; q++) setp[q] = k;
+    at += m;
+  }
+  std::memcpy(hb + o_tab, tables14, sizeof(float) * 14 * (size_t)nsets);
+  CK(cudaMemcpyAsync(c->d_ip, hb, sizeof(float) * ((size_t)words * cap + 14 * (size_t)nsets), cudaMemcpyHostToDevice, c->stream));
+  IPTraceArgs A;
+  std::memset(&A, 0, sizeof(A));
+  A.n = n; A.w = c->w[0]; A.h = c->h[0];
+  if (settings) A.s = *settings; else dmv_ip_default_settings(&A.s);
+  float* d = c->d_ip;
+  A.tab = d + o_tab; A.set_of = reinterpret_cast<const int*>(d + o_set);
+  A.u = d + o_u; A.v = d + o_v; A.color = d + o_col; A.weights = d + o_wgt; A.gradH = d + o_g; A.energyTH = d + o_eth;
+  A.idepth_min = d + o_min; A.idepth_max = d + o_max; A.quality = d + o_q; A.status = reinterpret_cast<int*>(d + o_st); A.uv = d + o_uv; A.interval = d + o_iv;
+  A.img = c->d_img[0];
+  ip_trace_kernel<<<(A.n + 3) / 4, 128, 0, c->stream>>>(A);   // 4 warps = 4 points per CTA
+  c->launches++;
+  CK(cudaGetLastError());
+  CK(cudaMemcpyAsync(hb + o_min, d + o_min, sizeof(float) * 7 * cap, cudaMemcpyDeviceToHost, c->stream));  // the 7 in/out words per point
+  CK(cudaStreamSynchronize(c->stream));
+  at = 0;
+  for (int k = 0; k < nsets; k++) {
+    const dmv_ip_points* p = &sets[k];
+    const size_t m = (size_t)p->n;
+    if (m == 0) continue;
+    std::memcpy(p->idepth_min, hb + o_min + at, 4 * m); std::memcpy(p->idepth_max, hb + o_max + at, 4 * m); std::memcpy(p->quality, hb + o_q + at, 4 * m);
+    std::memcpy(p->lastTraceStatus, hb + o_st + at, 4 * m); std::memcpy(p->lastTraceUV2, hb + o_uv + 2 * at, 8 * m); std::memcpy(p->lastTracePixelInterval, hb + o_iv + at, 4 * m);
+    at += m;
+  }
+  return DMV_OK;
+}
+
+// one host frame's immature points traced against the resident newest frame
+int dmv_ct_trace_points(dmv_ct* c, const dmv_ip_points* p, const float KRKi[9], const float Kt[3], const float aff[2], const dmv_ip_settings* settings) {
+  if (!c || !p || !KRKi || !Kt || !aff) return set_error(DMV_ERR_INVALID, "null argument");
+  float tab[14];
+  std::memcpy(tab, KRKi, 36); std::memcpy(tab + 9, Kt, 12); std::memcpy(tab + 12, aff, 8);
+  return dmv_ct_trace_points_multi(c, 1, p, tab, settings);
+}
+
+// FullSystem::optimizeImmaturePoint for a batch of immature points (ip_activate_kernel) on the BA handle's window
+int dmv_ba_activate_points(dmv_ba* b, const dmv_ba_activate_args* a) {
+  if (!b || !a) return set_error(DMV_ERR_INVALID, "null argument");
+  if (b->nf < 2 || !b->have_state) return set_error(DMV_ERR_STATE, "dmv_ba_set_window + dmv_ba_set_state first");
+  if (a->n < 0 || (a->n > 0 && (!a->host || !a->u || !a->v || !a->color8 || !a->weights8 || !a->energyTH || !a->idepth_min || !a->idepth_max || !a->RT ||
+                                !a->status || !a->idepth || !a->res_state)))
+    return set_error(DMV_ERR_INVALID, "incomplete dmv_ba_activate_args");
+  if (a->n == 0) return DMV_OK;
+  const int n = a->n, nf = b->nf;
+  for (int i = 0; i < n; i++)
+    if (a->host[i] < 0 || a->host[i] >= nf) return set_error(DMV_ERR_INVALID, "point %d: host %d out of range", i, a->host[i]);
+  CK(cudaSetDevice(b->device));
+  if (n > b->act_cap) {
+    cudaFree(b->d_act); cudaFreeHost(b->h_act);
+    b->act_cap = std::max(n, 2048);
+    const size_t words = (size_t)MAXF * MAXF * 14 + (size_t)(24 + MAXF) * b->act_cap;
+    CK(cudaMalloc(&b->d_act, sizeof(float) * words));
+    CK(cudaMallocHost(&b->h_act, sizeof(float) * words));
+  }
+  const size_t cap = b->act_cap;
+  float* hb = b->h_act;
+  float* d = b->d_act;
+  // layout (words): RT[64*12] | aff[64*2] | host | u | v | color*8 | weights*8 | energyTH | idmin | idmax | status | idepth | res_state*MAXF
+  const size_t o_rt = 0, o_aff = (size_t)MAXF * MAXF * 12, o_host = (size_t)MAXF * MAXF * 14, o_u = o_host + cap, o_v = o_u + cap, o_col = o_v + cap,
+               o_wgt = o_col + 8 * cap, o_eth = o_wgt + 8 * cap, o_min = o_eth + cap, o_max = o_min + cap, o_st = o_max + cap, o_id = o_st + cap, o_rs = o_id + cap;
+  std::memcpy(hb + o_rt, a->RT, sizeof(float) * 12 * nf * nf);
+  const BAIter& it = b->h_up->it;
+  for (int k = 0; k < nf * nf; k++) { hb[o_aff + 2 * k] = it.precalc[k][24]; hb[o_aff + 2 * k + 1] = it.precalc[k][25]; }  // PRE_aff_mode
+  std::memcpy(hb + o_host, a->host, 4 * (size_t)n); std::memcpy(hb + o_u, a->u, 4 * (size_t)n); std::memcpy(hb + o_v, a->v, 4 * (size_t)n);
+  std::memcpy(hb + o_col, a->color8, 32 * (size_t)n); std::memcpy(hb + o_wgt, a->weights8, 32 * (size_t)n); std::memcpy(hb + o_eth, a->energyTH, 4 * (size_t)n);
+  std::memcpy(hb + o_min, a->idepth_min, 4 * (size_t)n); std::memcpy(hb + o_max, a->idepth_max, 4 * (size_t)n);
+  CK(cudaMemcpyAsync(d, hb, sizeof(float) * o_st, cudaMemcpyHostToDevice, b->stream));
+  IPActArgs A;
+  A.n = n; A.nf = nf; A.w = b->cfg.w; A.h = b->cfg.h; A.minObs = a->minObs; A.GNIts = 3;  // setting_GNItsOnPointActivation
+  A.fxl = it.calib[0]; A.fyl = it.calib[1]; A.cxl = it.calib[2]; A.cyl = it.calib[3]; A.fxli = it.calib[4]; A.fyli = it.calib[5];
+  A.huberTH = b->prm.huberTH; A.minIdepthH_act = 100.f;                                      // setting_minIdepthH_act
+  for (int f = 0; f < MAXF; f++) A.img[f] = f < nf ? b->d_img[b->slots[f]] : nullptr;
+  A.RT = d + o_rt; A.aff = d + o_aff; A.host = reinterpret_cast<const int*>(d + o_host);
+  A.u = d + o_u; A.v = d + o_v; A.color = d + o_col; A.weights = d + o_wgt; A.energyTH = d + o_eth; A.idepth_min = d + o_min; A.idepth_max = d + o_max;
+  A.status = reinterpret_cast<int*>(d + o_st); A.idepth = d + o_id; A.res_state = reinterpret_cast<int*>(d + o_rs);
+  ip_activate_kernel<<<(A.n + 15) / 16, 128, 0, b->stream>>>(A);   // 8 lanes per point
+  b->launches++;
+  CK(cudaGetLastError());
+  CK(cudaMemcpyAsync(hb + o_st, d + o_st, sizeof(float) * (2 * cap + (size_t)nf * n), cudaMemcpyDeviceToHost, b->stream));
+  CK(cudaStreamSynchronize(b->stream));
+  std::memcpy(a->status, hb + o_st, 4 * (size_t)n); std::memcpy(a->idepth, hb + o_id, 4 * (size_t)n);
+  std::memcpy(a->res_state, hb + o_rs, 4 * (size_t)n * nf);
+  return DMV_OK;
+}

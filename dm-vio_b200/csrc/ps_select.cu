@@ -29,13 +29,64 @@
 // the decision to return are no-ops, so the host waits once.  Sub-selection (L248-265): the k-th nonzero map entry in raster order is cleared
 // when randomPattern[k] > (unsigned char)(255*quotia), a prefix count over the map.  makeNewTraces' loop: a raster compaction of the nonzero
 // entries in [3, w-4) x [3, h-4), the existing ip_init_kernel, and a compaction of the finite energyTH into the caller's pinned output.
-#include "ps_select.h"
+#include "ct_handle.h"
 #include "ip_trace.h"
 #include <cub/device/device_scan.cuh>
 #include <climits>
+#include <cmath>
+#include <cstring>
 #include <vector>
 
 namespace dmv {
+
+// makeMaps' running state on the device: the recursion is decided there, so the host learns it only at the end
+struct PSState {
+  int pot;          // potential of the current select pass
+  int recLeft;      // recursions left
+  int done;         // makeMaps has returned: later passes are no-ops
+  int n3, n4;       // level-1 / level-2 picks of the current pass (level 0: the n2 prefix)
+  int numHaveSub;   // makeMaps' return value
+  int ideal;        // idealPotential = the potential makeMaps leaves behind
+  float quotia;
+  int n_cand;       // nonzero map entries inside makeNewTraces' raster window
+  int n_points;     // of those, points with a finite energyTH
+  int n_mixed;      // mixed pot-blocks met, summed over the select passes (the serial chain's length)
+  int pad;
+};
+// per-handle scratch, allocated on first use for the handle's level-0 size
+struct PSScratch {
+  int w = 0, h = 0;
+  uint8_t* pat = nullptr;         // PixelSelector::randomPattern (w*h)
+  uint8_t* nib = nullptr;         // its low nibbles, two per byte (w*h/2): the directions the serial chain reads
+  float* ths = nullptr;           // thsSmoothed (nbW*nbH) and ths (nbW*nbH)
+  float* B = nullptr;             // CalibHessian::B (256)
+  uint32_t* mask = nullptr;       // per pot-block / 2pot-block / 4pot-block: directions with a candidate (w*h + w*h/4 + w*h/16)
+  unsigned long long* best = nullptr;  // per pot-block / 2pot / 4pot: (value bits << 32) | ~position of the first maximum
+  unsigned long long* scan_in = nullptr;  // (w*h+1): constant pick | mixed block << 32 per pot-block key
+  unsigned long long* scan = nullptr;  // (w*h+1): its exclusive prefix of (constant picks | mixed blocks << 32) in nested order
+  int2* mixed = nullptr;          // (w*h): per mixed block in order: (constant-pick prefix, direction mask)
+  int* delta = nullptr;           // (w*h): mixed picks up to and including mixed block j
+  int* n2b = nullptr;             // (w*h+1): level-0 picks before each pot-block in nested order
+  float* map = nullptr;           // selectionMap (w*h)
+  int* flag = nullptr;            // (w*h): scan input
+  int* rank = nullptr;            // (w*h): scan output
+  float* cand = nullptr;          // candidates of makeNewTraces' loop: u | v | type | color*8 | weights*8 | gradH*4 | energyTH | ok  (25 * w*h words)
+  PSState* st = nullptr;
+  void* temp = nullptr;           // CUB scan storage
+  size_t temp_bytes = 0;
+  float* h_out = nullptr;         // pinned, device-visible: PSState then per point u | v | type | color*8 | weights*8 | gradH*4 | energyTH
+  int h_cap = 0;
+  bool smem_chain = false;        // the chain stages the nibbles in shared memory (w*h/2 <= 200 KB); larger frames read them from global memory
+};
+struct PSArgs {
+  int w, h;
+  const float4* img[3];           // the resident frame's levels 0-2 (I, dx, dy, 0)
+  dmv_ps_settings s;
+  float density, thFactor;
+  int recursionsLeft, potential;
+  int out_cap;                    // points written to h_out (min(cap, w*h))
+};
+
 
 // PixelSelector2.cpp:L328-344 (double literals converted to float, as Vec2f's constructor does)
 __constant__ float c_ps_dir[16][2] = {{0, 1.0000},      {0.3827, 0.9239},  {0.1951, 0.9808},  {0.9239, 0.3827},  {0.7071, 0.7071},  {0.3827, -0.9239},
@@ -395,7 +446,8 @@ __global__ void ps_init_state_kernel(PSState* S, int pot, int recLeft) {
 }
 
 // ---- host side
-void ps_random_pattern(uint8_t* out, size_t n, unsigned seed) {
+// glibc's random(3) TYPE_3 generator restated (srand(seed); rand() & 0xFF per entry), without touching the process's rand() state
+static void ps_random_pattern(uint8_t* out, size_t n, unsigned seed) {
   // glibc random_r.c, TYPE_3 (degree 31, separation 3): the state is seeded by the Park-Miller recurrence, 310 outputs are discarded, and
   // each rand() returns (r[i-31] + r[i-3]) >> 1 in 32-bit arithmetic
   std::vector<int32_t> r(344 + n);
@@ -412,7 +464,7 @@ void ps_random_pattern(uint8_t* out, size_t n, unsigned seed) {
   for (size_t k = 0; k < n; k++) out[k] = (uint8_t)(((uint32_t)r[344 + k] >> 1) & 0xFF);
 }
 
-void ps_free(PSScratch& S) {
+static void ps_release(PSScratch& S) {
   cudaFree(S.pat); cudaFree(S.ths); cudaFree(S.B); cudaFree(S.mask); cudaFree(S.best); cudaFree(S.scan); cudaFree(S.scan_in); cudaFree(S.mixed); cudaFree(S.delta);
   cudaFree(S.n2b); cudaFree(S.map); cudaFree(S.flag); cudaFree(S.rank); cudaFree(S.cand); cudaFree(S.st); cudaFree(S.temp);
   cudaFreeHost(S.h_out);
@@ -422,11 +474,18 @@ void ps_free(PSScratch& S) {
 // dynamic shared memory of ps_chain_kernel: one value for the process (the attribute belongs to the kernel, not to a handle)
 static const int PS_SMEM_MAX = 200 * 1024;
 
-cudaError_t ps_alloc(PSScratch& S, int w, int h) {
-  ps_free(S);
+void ps_free(PSScratch* S) {
+  if (!S) return;
+  ps_release(*S);
+  delete S;
+}
+
+// allocates S for a w x h frame and builds the random pattern; returns the first CUDA error
+static cudaError_t ps_alloc(PSScratch& S, int w, int h) {
+  ps_release(S);
   const size_t n = (size_t)w * h;
   cudaError_t e;
-#define PS_TRY(x) do { if ((e = (x)) != cudaSuccess) { ps_free(S); return e; } } while (0)
+#define PS_TRY(x) do { if ((e = (x)) != cudaSuccess) { ps_release(S); return e; } } while (0)
   PS_TRY(cudaMalloc(&S.pat, n + n / 2));
   S.nib = S.pat + n;
   PS_TRY(cudaMalloc(&S.ths, sizeof(float) * 2 * (n / 256)));
@@ -459,7 +518,7 @@ cudaError_t ps_alloc(PSScratch& S, int w, int h) {
   return cudaSuccess;
 }
 
-cudaError_t ps_ensure_out(PSScratch& S, int cap) {
+static cudaError_t ps_ensure_out(PSScratch& S, int cap) {
   if (S.h_out && cap <= S.h_cap) return cudaSuccess;
   if (S.h_out) cudaFreeHost(S.h_out);
   S.h_out = nullptr; S.h_cap = 0;
@@ -468,7 +527,9 @@ cudaError_t ps_ensure_out(PSScratch& S, int cap) {
   return e;
 }
 
-cudaError_t ps_launch(const PSArgs& A, PSScratch& S, cudaStream_t s, int* kernels) {
+// every launch of the call: the points and the final PSState land in S.h_out, which the host reads after one stream synchronisation;
+// the selection map stays in S.map.  *kernels = kernels launched (CUB's own launches not counted)
+static cudaError_t ps_launch(const PSArgs& A, PSScratch& S, cudaStream_t s, int* kernels) {
   const int w = A.w, h = A.h, n = w * h;
   PSDev D;
   D.w = w; D.h = h; D.w1 = w >> 1; D.h1 = h >> 1; D.w2 = w >> 2; D.h2 = h >> 2; D.nbW = w / 16; D.nbH = h / 16;
@@ -527,3 +588,65 @@ cudaError_t ps_launch(const PSArgs& A, PSScratch& S, cudaStream_t s, int* kernel
 }
 
 }  // namespace dmv
+
+using namespace dmv;
+
+void dmv_ps_default_settings(dmv_ps_settings* s) {
+  if (!s) return;
+  s->minGradHistCut = 0.5f; s->minGradHistAdd = 7.f; s->gradDownweightPerLevel = 0.75f;   // util/settings.cpp:L144, L167-170
+  s->selectDirectionDistribution = 1; s->gammaWeightsPixelSelect = 1;
+}
+
+// FullSystem::makeNewTraces on the resident frame
+int dmv_ct_make_new_traces(dmv_ct* c, const dmv_new_traces_args* a) {
+  if (!c || !a) return set_error(DMV_ERR_INVALID, "null argument");
+  if (c->cfg.levels < 3) return set_error(DMV_ERR_INVALID, "pixel selection reads levels 0-2: the handle has %d", c->cfg.levels);
+  const int w = c->w[0], h = c->h[0];
+  if (w % 16 || h % 16) return set_error(DMV_ERR_INVALID, "pixel selection needs w and h divisible by 16 (%d x %d)", w, h);
+  if (!a->potential || !a->n || !a->numPointsTotal || a->cap < 0 || (a->cap > 0 && (!a->u || !a->v || !a->type || !a->color8 || !a->weights8 || !a->gradH4 || !a->energyTH)))
+    return set_error(DMV_ERR_INVALID, "null argument");
+  if (*a->potential < 1) return set_error(DMV_ERR_INVALID, "potential %d < 1", *a->potential);
+  if (!(a->density > 0.f) || !std::isfinite(a->density)) return set_error(DMV_ERR_INVALID, "density must be finite and > 0");
+  if (!(a->thFactor > 0.f) || !std::isfinite(a->thFactor)) return set_error(DMV_ERR_INVALID, "thFactor must be finite and > 0");
+  if (a->recursionsLeft < 0 || a->recursionsLeft > 8) return set_error(DMV_ERR_INVALID, "recursionsLeft must be in 0..8");
+  dmv_ps_settings st;
+  if (a->settings) st = *a->settings; else dmv_ps_default_settings(&st);
+  if (!(st.minGradHistCut < 0.99f) || !std::isfinite(st.minGradHistCut) || !std::isfinite(st.minGradHistAdd) || !std::isfinite(st.gradDownweightPerLevel))
+    return set_error(DMV_ERR_INVALID, "bad dmv_ps_settings");
+  CK(cudaSetDevice(c->device));
+  if (!c->ps) c->ps = new PSScratch();
+  PSScratch& P = *c->ps;
+  if (P.w != w || P.h != h) CK(ps_alloc(P, w, h));
+  const int out_cap = std::min(a->cap, w * h);
+  CK(ps_ensure_out(P, std::max(out_cap, 1)));
+  CK(ct_wait_staging(c));
+  float B[256];
+  for (int i = 0; i < 256; i++) B[i] = a->B ? a->B[i] : (float)i;   // CalibHessian's constructor: B[i] = i
+  CK(cudaMemcpyAsync(P.B, B, sizeof(B), cudaMemcpyHostToDevice, c->stream));
+  PSArgs A;
+  A.w = w; A.h = h;
+  for (int l = 0; l < 3; l++) A.img[l] = c->d_img[l];
+  A.s = st; A.density = a->density; A.thFactor = a->thFactor; A.recursionsLeft = a->recursionsLeft; A.potential = *a->potential;
+  A.out_cap = out_cap;
+  int kernels = 0;
+  CK(ps_launch(A, P, c->stream, &kernels));
+  c->launches += kernels;
+  if (a->map) CK(cudaMemcpyAsync(a->map, P.map, sizeof(float) * (size_t)w * h, cudaMemcpyDeviceToHost, c->stream));
+  CK(cudaStreamSynchronize(c->stream));
+  PSState S;
+  std::memcpy(&S, P.h_out, sizeof(S));
+  *a->n = S.n_points;
+  // on overflow the selector's state stays as it was, so a retry with a larger cap continues from the same potential
+  if (S.n_points > a->cap) return set_error(DMV_ERR_INVALID, "%d new points exceed cap %d", S.n_points, a->cap);
+  *a->potential = S.ideal;
+  *a->numPointsTotal = S.numHaveSub;
+  const size_t n = (size_t)S.n_points, O = out_cap;
+  const float* o = P.h_out + sizeof(PSState) / sizeof(float);
+  std::memcpy(a->u, o, 4 * n); std::memcpy(a->v, o + O, 4 * n); std::memcpy(a->type, o + 2 * O, 4 * n);
+  for (size_t i = 0; i < n; i++)
+    for (int k = 0; k < 8; k++) { a->color8[8 * i + k] = o[(3 + k) * O + i]; a->weights8[8 * i + k] = o[(11 + k) * O + i]; }
+  for (size_t i = 0; i < n; i++)
+    for (int k = 0; k < 4; k++) a->gradH4[4 * i + k] = o[(19 + k) * O + i];
+  std::memcpy(a->energyTH, o + 23 * O, 4 * n);
+  return DMV_OK;
+}
