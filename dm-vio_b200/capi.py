@@ -176,7 +176,7 @@ SYMBOLS = [
     "dmv_ba_batch_create", "dmv_ba_batch_destroy", "dmv_ba_batch_gn_step", "dmv_ba_batch_set_timing", "dmv_ba_batch_last_kernel_ms", "dmv_ba_batch_bench",
     "dmv_ct_create", "dmv_ct_destroy", "dmv_ct_set_K", "dmv_ct_set_ref", "dmv_ct_make_coarse_depth", "dmv_ct_set_ref_from_ba", "dmv_ct_get_ref", "dmv_ct_upload_new", "dmv_ct_upload_new_image", "dmv_ct_set_huber",
     "dmv_ci_create", "dmv_ci_destroy", "dmv_ci_set_K", "dmv_ci_upload_first", "dmv_ci_upload_new", "dmv_ci_set_points", "dmv_ci_calc_res_and_gs", "dmv_ci_kernel_launch_count",
-    "dmv_ct_calc_res_gs", "dmv_ct_track", "dmv_ip_default_settings", "dmv_ct_init_points", "dmv_ct_trace_points", "dmv_ct_trace_points_multi", "dmv_ct_set_timing", "dmv_ct_last_timing", "dmv_ct_kernel_launch_count", "dmv_ct_last_point_evaluations",
+    "dmv_ct_calc_res_gs", "dmv_ct_track", "dmv_ct_track_many", "dmv_ip_default_settings", "dmv_ct_init_points", "dmv_ct_trace_points", "dmv_ct_trace_points_multi", "dmv_ct_set_timing", "dmv_ct_last_timing", "dmv_ct_kernel_launch_count", "dmv_ct_last_point_evaluations",
     "dmv_ct_set_undistort", "dmv_ct_upload_raw_image", "dmv_ct_download_frame", "dmv_ps_default_settings", "dmv_ct_make_new_traces",
 ]
 
@@ -247,6 +247,7 @@ def lib():
         L.dmv_ct_set_huber.argtypes = [vp, C.c_float]
         L.dmv_ct_calc_res_gs.argtypes = [vp, C.c_int, f32p, f32p, f32p, C.c_float, C.c_float, C.c_int, f64p, f64p, f64p, C.POINTER(C.c_int)]
         L.dmv_ct_track.argtypes = [vp, C.POINTER(CTTrackArgs), C.POINTER(CTTrackResult)]
+        L.dmv_ct_track_many.argtypes = [C.POINTER(vp), C.c_int, C.POINTER(CTTrackArgs), C.POINTER(CTTrackResult)]
         L.dmv_ct_init_points.argtypes = [vp, C.c_int, i32p, i32p, f32p, f32p, f32p, f32p, i32p]
         L.dmv_ct_trace_points.argtypes = [vp, C.POINTER(IPPoints), f32p, f32p, f32p, vp]
         L.dmv_ct_trace_points_multi.argtypes = [vp, C.c_int, vp, f32p, vp]
@@ -550,6 +551,37 @@ def nccl_unique_id():
     return bytes(buf.raw)
 
 
+def _track_args(levels, R, t, a, b, ref_a=0.0, ref_b=0.0, ref_exposure=1.0, new_exposure=1.0, cutoff=20.0, affA=1e12, affB=1e8, coarsest=None,
+                minRes=None):
+    """the dmv_ct_track_args of CT.track's arguments for a handle of `levels` levels"""
+    A = CTTrackArgs()
+    A.R[:] = [float(x) for x in np.asarray(R, np.float64).reshape(-1)]
+    A.t[:] = [float(x) for x in np.asarray(t, np.float64).reshape(-1)]
+    A.a, A.b, A.ref_a, A.ref_b = float(a), float(b), float(ref_a), float(ref_b)
+    A.ref_exposure, A.new_exposure, A.coarseCutoffTH, A.affineOptModeA, A.affineOptModeB = ref_exposure, new_exposure, cutoff, affA, affB
+    A.coarsestLvl = levels - 1 if coarsest is None else int(coarsest)
+    A.minResForAbort[:] = [float(x) for x in (np.full(5, np.nan) if minRes is None else np.asarray(minRes, np.float64))]
+    return A
+
+
+def _track_result(r):
+    return dict(R=np.array(r.R).reshape(3, 3), t=np.array(r.t), a=r.a, b=r.b, lastResiduals=np.array(r.lastResiduals), flow=np.array(r.flowIndicators),
+                good=r.trackingGood, iterations=r.iterations, evaluations=r.evaluations, status=r.status)
+
+
+def ct_track_many(handles, args):
+    """dmv_ct_track_many: handles[i] (a CT) tracked with args[i] (a dict of CT.track's keywords), all in one launch.  Returns the list of
+    CT.track's result dicts, each bit-identical to handles[i].track(**args[i])."""
+    if len(handles) != len(args):
+        raise ValueError(f"{len(handles)} handles but {len(args)} argument sets")
+    n = len(handles)
+    H = (vp * n)(*[g.h.value for g in handles])
+    A = (CTTrackArgs * n)(*[_track_args(g.levels, **a) for g, a in zip(handles, args)])
+    r = (CTTrackResult * n)()
+    check(lib().dmv_ct_track_many(H, n, A, r))
+    return [_track_result(x) for x in r]
+
+
 class CT:
     def __init__(self, w, h, levels, max_points=65536, device=0):
         self.L = lib()
@@ -617,17 +649,10 @@ class CT:
               minRes=None):
         """dmv_ct_track (trackNewestCoarse in one launch): every field of dmv_ct_track_result as a dict, status and evaluations included.
         minRes = minResForAbort (None: NaN, never abort); coarsest defaults to the handle's top level."""
-        A = CTTrackArgs()
-        A.R[:] = [float(x) for x in np.asarray(R, np.float64).reshape(-1)]
-        A.t[:] = [float(x) for x in np.asarray(t, np.float64).reshape(-1)]
-        A.a, A.b, A.ref_a, A.ref_b = float(a), float(b), float(ref_a), float(ref_b)
-        A.ref_exposure, A.new_exposure, A.coarseCutoffTH, A.affineOptModeA, A.affineOptModeB = ref_exposure, new_exposure, cutoff, affA, affB
-        A.coarsestLvl = self.levels - 1 if coarsest is None else int(coarsest)
-        A.minResForAbort[:] = [float(x) for x in (np.full(5, np.nan) if minRes is None else np.asarray(minRes, np.float64))]
+        A = _track_args(self.levels, R, t, a, b, ref_a, ref_b, ref_exposure, new_exposure, cutoff, affA, affB, coarsest, minRes)
         r = CTTrackResult()
         check(self.L.dmv_ct_track(self.h, C.byref(A), C.byref(r)))
-        return dict(R=np.array(r.R).reshape(3, 3), t=np.array(r.t), a=r.a, b=r.b, lastResiduals=np.array(r.lastResiduals), flow=np.array(r.flowIndicators),
-                    good=r.trackingGood, iterations=r.iterations, evaluations=r.evaluations, status=r.status)
+        return _track_result(r)
 
     def point_evaluations(self):
         """reference points evaluated by the last track, summed over its evaluations (dmv_ct_last_point_evaluations)"""

@@ -18,6 +18,7 @@ struct dmv_ct {
   int device = 0;
   cudaStream_t stream = nullptr;
   cudaEvent_t ev[2] = {nullptr, nullptr};
+  cudaEvent_t ev_order = nullptr;   // orders a dmv_ct_track_many launch on another member's stream behind this handle's queued work
   bool staging_busy = false;  // an asynchronous upload from h_scratch may be in flight
   bool timing = false;  // CUDA-event timing of every evaluation (dmv_ct_set_timing); off by default: two event records per launch
   int w[DMV_MAX_PYR_LEVELS], h[DMV_MAX_PYR_LEVELS];

@@ -408,6 +408,18 @@ typedef struct dmv_ct_track_result {
   int trackingGood, iterations, evaluations, status;
 } dmv_ct_track_result;
 int dmv_ct_track(dmv_ct* ct, const dmv_ct_track_args* in, dmv_ct_track_result* out);
+/* dmv_ct_track for n independent handles (several cameras or robots served by one host thread) in ONE launch: one thread-block cluster per
+ * handle, so up to n frames are tracked side by side instead of one after the other on 16 SMs each.  Stateless: the handles' descriptors
+ * travel as kernel parameters; pass whichever handles have a frame ready, in any order.
+ * out[i] is bit-identical to what dmv_ct_track(handles[i], &in[i], &out[i]) returns (aborts included), and afterwards
+ * dmv_ct_last_point_evaluations and dmv_ct_kernel_launch_count (+1) of every handle read as after that call.  The launch is ordered behind
+ * the work queued on every handle's stream (asynchronous uploads included); the call returns after one synchronisation, with every
+ * handle's staging buffer free.  dmv_ct_set_timing / dmv_ct_last_timing are not involved.
+ * Errors, all before anything is launched or any out[i] is written: DMV_ERR_INVALID for n outside 1..DMV_CT_TRACK_MANY_MAX, a NULL pointer,
+ * a handle passed twice, handles on different devices, or handles whose probed cluster sizes differ (a handle probes on its first track;
+ * the message names two such handles); and dmv_ct_track's own errors for any member, with the member's index in the message. */
+#define DMV_CT_TRACK_MANY_MAX 16
+int dmv_ct_track_many(dmv_ct* const* handles, int n, const dmv_ct_track_args* in, dmv_ct_track_result* out);
 
 /* ------------------------------------------------------------------------------------------------
  * Immature-point tracing  ==  ImmaturePoint::traceOn (FullSystem/ImmaturePoint.cpp:L77-437) for all immature points of ONE host
