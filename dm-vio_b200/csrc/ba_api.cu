@@ -766,7 +766,10 @@ int dmv_ba_marginalize_points(dmv_ba* b, const dmv_ba_marg_args* a) {
     CK(cudaMemcpyAsync(rtz.data(), b->d_marg_rtz, sizeof(float) * 8 * nslots, cudaMemcpyDeviceToHost, b->stream));
   }
   CK(cudaStreamSynchronize(b->stream));
-  b->have_tentative = false;  // the tentative buffers now hold the flagged points' re-linearisation only
+  // the tentative buffers now hold the flagged points' re-linearisation only.  The getters fall back to the committed linearisation, and so must
+  // dmv_ba_get_target_energies for the newest frame: h_en_newest came from the discarded tentative launch, if there was one
+  if (b->have_tentative) b->en_newest_valid = false;
+  b->have_tentative = false;
   if (b->h_marg_result[nres_d - 1] != 0.0)
     return set_error(DMV_ERR_TIMEOUT, "grid barrier / peer exchange timed out inside ba_fused_kernel (marginalisation launch)");
   unpack_system(b, b->h_marg_result, a->M, a->Mb, a->Msc, a->Mbsc, nullptr);

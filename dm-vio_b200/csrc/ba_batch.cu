@@ -33,6 +33,8 @@ int dmv_ba_batch_create(dmv_ba* const* handles, int n, dmv_ba_batch** out) {
   if (!handles || !out || n < 1 || n > BATCH_MAX) return set_error(DMV_ERR_INVALID, "1..%d handles", BATCH_MAX);
   for (int i = 0; i < n; i++) {
     if (!handles[i]) return set_error(DMV_ERR_INVALID, "handle %d is null", i);
+    for (int j = 0; j < i; j++)  // one launch would run both members on the same buffers
+      if (handles[j] == handles[i]) return set_error(DMV_ERR_INVALID, "handles[%d] and handles[%d] are the same handle", j, i);
     if (handles[i]->device != handles[0]->device || handles[i]->P != handles[0]->P) return set_error(DMV_ERR_INVALID, "all handles of a batch must share the device and chunk_points");
     if (handles[i]->nranks > 1) return set_error(DMV_ERR_INVALID, "sharded handles cannot be batched");
   }
@@ -69,20 +71,25 @@ int dmv_ba_batch_gn_step(dmv_ba_batch* B, const double* const* x, const dmv_ba_s
   if (!B || !st) return set_error(DMV_ERR_INVALID, "null argument");
   CK(cudaSetDevice(B->device));
   const int n = (int)B->h.size();
+  B->P = B->h[0]->P;   // with chunk_points = 0 a handle picks its shape per window: the batch needs ONE shape
+  // every check precedes the first upload: a refused call leaves every member as it was
+  for (int i = 0; i < n; i++) {
+    const dmv_ba* b = B->h[i];
+    if (b->P != B->P) return set_error(DMV_ERR_STATE, "window %d uses %d-point chunks, window 0 %d: create the handles of a batch with an explicit chunk_points", i, b->P, B->P);
+    if (!st[i]) return set_error(DMV_ERR_INVALID, "state %d is null", i);
+    if (!st[i]->precalc || !st[i]->frameEnergyTH) return set_error(DMV_ERR_INVALID, "state %d: precalc / frameEnergyTH required", i);
+    if (b->xchg_on) return set_error(DMV_ERR_STATE, "window %d is sharded with the in-kernel peer exchange: the batched kernel has none", i);
+    if (b->npts < 1) return set_error(DMV_ERR_STATE, "window %d: points not set", i);
+    if (!b->have_adj) return set_error(DMV_ERR_STATE, "window %d: dmv_ba_set_adjoints first", i);
+    if (x && x[i] && !b->have_committed) return set_error(DMV_ERR_STATE, "window %d: no committed linearisation to resubstitute", i);
+  }
   BABatchHdr hdr;
   std::memset(&hdr, 0, sizeof(hdr));
   hdr.B = n;
   B->max_nf = 2;
-  B->P = B->h[0]->P;   // with chunk_points = 0 a handle picks its shape per window: the batch needs ONE shape
   for (int i = 0; i < n; i++) {
     dmv_ba* b = B->h[i];
-    if (b->P != B->P) return set_error(DMV_ERR_STATE, "window %d uses %d-point chunks, window 0 %d: create the handles of a batch with an explicit chunk_points", i, b->P, B->P);
-    if (!st[i]) return set_error(DMV_ERR_INVALID, "state %d is null", i);
-    if (b->xchg_on) return set_error(DMV_ERR_STATE, "window %d is sharded with the in-kernel peer exchange: the batched kernel has none", i);
-    if (b->npts < 1) return set_error(DMV_ERR_STATE, "window %d: points not set", i);
-    if (!b->have_adj) return set_error(DMV_ERR_STATE, "window %d: dmv_ba_set_adjoints first", i);
     const double* xi = x ? x[i] : nullptr;
-    if (xi && !b->have_committed) return set_error(DMV_ERR_STATE, "window %d: no committed linearisation to resubstitute", i);
     if (b->stream != B->stream) CK(cudaStreamSynchronize(b->stream));  // uploads issued on the handle's own stream
     int rc = dmv_ba_stage_state(b, st[i]);   // (idepth uploads, if any, go to the handle's stream: synchronised below)
     if (rc != DMV_OK) return rc;

@@ -70,7 +70,7 @@ struct dmv_ba {
   double* h_result[2] = {nullptr, nullptr};
   float* h_scratch = nullptr;  // max(mp*8, w*h*3) floats
   float* h_en_newest = nullptr; // [mp] en_wo of the residuals targeting the newest frame, written by the kernel itself (zero-copy)
-  bool en_newest_valid = false; // h_en_newest belongs to the most recent linearisation
+  bool en_newest_valid = false; // h_en_newest belongs to the linearisation the getters read (tentative if any, else committed)
   size_t scratch_floats = 0;
   // host bookkeeping
   int host_start[MAXF + 1];

@@ -128,7 +128,9 @@ int dmv_ba_get_residual_outputs(dmv_ba* ba, int32_t* newState, float* newEnergy,
                                 float* JpJdF8);
 
 /* state_NewEnergyWithOutlier of the residuals whose target is frame `target` (input of FullSystem::setNewFrameEnergyTH,
- * FullSystemOptimize.cpp:L96-149): writes at most cap floats, returns the count in *n. Entries < 0 (not evaluated) are skipped. */
+ * FullSystemOptimize.cpp:L96-149): writes at most cap floats, returns the count in *n. Entries < 0 (not evaluated) are skipped.
+ * Every target, the newest frame included, reports the linearisation dmv_ba_get_residual_outputs reports: the tentative one if there is one,
+ * else the committed one (after dmv_ba_marginalize_points: the committed one), in point order. */
 int dmv_ba_get_target_energies(dmv_ba* ba, int target, float* out, int cap, int* n);
 
 /* PointFrameResidual::applyRes(true) + EFResidual::takeDataF for all active residuals (FullSystemOptimize.cpp:L90-94):
@@ -278,9 +280,11 @@ int dmv_ba_p2p_import(dmv_ba* ba, int nranks, int rank, const void* ipc_handles 
  * results are bit-identical to dmv_ba_gn_step on that handle. */
 typedef struct dmv_ba_batch dmv_ba_batch;
 int dmv_ba_batch_create(dmv_ba* const* handles, int n, dmv_ba_batch** out);   /* n <= 64; the handles stay owned by the caller */
+/* A handle may appear only once in a batch: a duplicate is refused with DMV_ERR_INVALID, naming both positions. */
 int dmv_ba_batch_destroy(dmv_ba_batch* batch);
 /* dmv_ba_gn_step on every handle: x[i] may be NULL (x itself may be NULL), st[i] as for dmv_ba_gn_step; out (n entries) and sums3 (3 n doubles)
- * may be NULL.  Afterwards: dmv_ba_apply_res / dmv_ba_accumulate / ... per handle as usual. */
+ * may be NULL.  Afterwards: dmv_ba_apply_res / dmv_ba_accumulate / ... per handle as usual.  Every member is checked before any is staged:
+ * a refused call uploads nothing and leaves every handle as it was. */
 int dmv_ba_batch_gn_step(dmv_ba_batch* batch, const double* const* x, const dmv_ba_state* const* st, dmv_ba_lin_result* out, double* sums3);
 int dmv_ba_batch_set_timing(dmv_ba_batch* batch, int enable);
 int dmv_ba_batch_last_kernel_ms(dmv_ba_batch* batch, float* ms);   /* CUDA-event time of the last batched launch (after set_timing(1)) */
