@@ -63,6 +63,11 @@ class IPPoints(C.Structure):
                                                               "lastTraceStatus", "lastTraceUV2", "lastTracePixelInterval")]
 
 
+class TraceJob(C.Structure):
+    """dmv_ct_trace_job: one handle's arguments of dmv_ct_trace_many"""
+    _fields_ = [("nsets", C.c_int), ("sets", vp), ("tables14", vp)]
+
+
 class IPSettings(C.Structure):
     """dmv_ip_settings (include/dmvio_b200.h); ip_default_settings() fills it as dmv_ip_default_settings does"""
     _fields_ = [(k, C.c_float) for k in ("maxPixSearch", "trace_stepsize", "trace_GNThreshold", "trace_extraSlackOnTH", "trace_slackInterval",
@@ -176,7 +181,7 @@ SYMBOLS = [
     "dmv_ba_batch_create", "dmv_ba_batch_destroy", "dmv_ba_batch_gn_step", "dmv_ba_batch_set_timing", "dmv_ba_batch_last_kernel_ms", "dmv_ba_batch_bench",
     "dmv_ct_create", "dmv_ct_destroy", "dmv_ct_set_K", "dmv_ct_set_ref", "dmv_ct_make_coarse_depth", "dmv_ct_set_ref_from_ba", "dmv_ct_get_ref", "dmv_ct_upload_new", "dmv_ct_upload_new_image", "dmv_ct_set_huber",
     "dmv_ci_create", "dmv_ci_destroy", "dmv_ci_set_K", "dmv_ci_upload_first", "dmv_ci_upload_new", "dmv_ci_set_points", "dmv_ci_calc_res_and_gs", "dmv_ci_kernel_launch_count",
-    "dmv_ct_calc_res_gs", "dmv_ct_track", "dmv_ct_track_many", "dmv_ip_default_settings", "dmv_ct_init_points", "dmv_ct_trace_points", "dmv_ct_trace_points_multi", "dmv_ct_set_timing", "dmv_ct_last_timing", "dmv_ct_kernel_launch_count", "dmv_ct_last_point_evaluations",
+    "dmv_ct_calc_res_gs", "dmv_ct_track", "dmv_ct_track_many", "dmv_ip_default_settings", "dmv_ct_init_points", "dmv_ct_trace_points", "dmv_ct_trace_points_multi", "dmv_ct_trace_many", "dmv_ct_set_timing", "dmv_ct_last_timing", "dmv_ct_kernel_launch_count", "dmv_ct_last_point_evaluations",
     "dmv_ct_set_undistort", "dmv_ct_upload_raw_image", "dmv_ct_download_frame", "dmv_ps_default_settings", "dmv_ct_make_new_traces",
 ]
 
@@ -250,7 +255,8 @@ def lib():
         L.dmv_ct_track_many.argtypes = [C.POINTER(vp), C.c_int, C.POINTER(CTTrackArgs), C.POINTER(CTTrackResult)]
         L.dmv_ct_init_points.argtypes = [vp, C.c_int, i32p, i32p, f32p, f32p, f32p, f32p, i32p]
         L.dmv_ct_trace_points.argtypes = [vp, C.POINTER(IPPoints), f32p, f32p, f32p, vp]
-        L.dmv_ct_trace_points_multi.argtypes = [vp, C.c_int, vp, f32p, vp]
+        L.dmv_ct_trace_points_multi.argtypes = [vp, C.c_int, vp, vp, vp]
+        L.dmv_ct_trace_many.argtypes = [C.POINTER(vp), C.c_int, C.POINTER(TraceJob), vp]
         L.dmv_ct_set_timing.argtypes = [vp, C.c_int]
         L.dmv_ct_last_timing.argtypes = [vp, f32p]
         L.dmv_ct_kernel_launch_count.argtypes = [vp, C.POINTER(C.c_longlong)]
@@ -582,6 +588,50 @@ def ct_track_many(handles, args):
     return [_track_result(x) for x in r]
 
 
+class _TraceSets:
+    """the marshalling shared by CT.trace_points_multi and ct_trace_many: sets = [(P, KRKi, Kt, aff), ...] (P a dict of arrays as
+    oracle.orc.ip_init returns) as one dmv_ct_trace_job.  The in/out fields are copies (P itself is not modified); results() returns the
+    updated dicts."""
+
+    def __init__(self, sets):
+        self.sets = list(sets)
+        ns = len(self.sets)
+        self.arr = (IPPoints * max(ns, 1))()
+        self.tab = np.zeros((max(ns, 1), 14), np.float32)
+        self.keeps, self.outs = [], []
+        for k, (P, KRKi, Kt, aff) in enumerate(self.sets):
+            keep = {q: _c(P[q], np.float32) for q in ("u", "v", "color", "weights", "gradH", "energyTH")}
+            out = {"idepth_min": np.array(P["idepth_min"], np.float32, copy=True), "idepth_max": np.array(P["idepth_max"], np.float32, copy=True),
+                   "quality": np.array(P["quality"], np.float32, copy=True), "status": np.array(P["status"], np.int32, copy=True),
+                   "lastTraceUV": np.array(P["lastTraceUV"], np.float32, copy=True), "lastTracePixelInterval": np.array(P["lastTracePixelInterval"], np.float32, copy=True)}
+            self.arr[k] = IPPoints(len(P["u"]), *[x.ctypes.data for x in (keep["u"], keep["v"], keep["color"], keep["weights"], keep["gradH"], keep["energyTH"],
+                                                                           out["idepth_min"], out["idepth_max"], out["quality"], out["status"], out["lastTraceUV"],
+                                                                           out["lastTracePixelInterval"])])
+            self.tab[k, :9] = np.asarray(KRKi, np.float32).reshape(-1); self.tab[k, 9:12] = Kt; self.tab[k, 12:14] = aff
+            self.keeps.append(keep); self.outs.append(out)
+        self.job = TraceJob(ns, C.addressof(self.arr), self.tab.ctypes.data)
+
+    def results(self):
+        res = []
+        for (P, _, _, _), out in zip(self.sets, self.outs):
+            Q = dict(P); Q.update(out); res.append(Q)
+        return res
+
+
+def ct_trace_many(handles, jobs, settings=None):
+    """dmv_ct_trace_many: jobs[i] (the sets list CT.trace_points_multi takes) traced on handles[i] (a CT), all in one launch.  Returns the
+    list of per-member lists of updated dicts, each bit-identical to handles[i].trace_points_multi(jobs[i], settings).  settings: an
+    IPSettings, or None (NULL: defaults)."""
+    if len(handles) != len(jobs):
+        raise ValueError(f"{len(handles)} handles but {len(jobs)} jobs")
+    n = len(handles)
+    T = [_TraceSets(j) for j in jobs]
+    H = (vp * max(n, 1))(*[g.h.value for g in handles])
+    J = (TraceJob * max(n, 1))(*[t.job for t in T])
+    check(lib().dmv_ct_trace_many(H, n, J, None if settings is None else C.byref(settings)))
+    return [t.results() for t in T]
+
+
 class CT:
     def __init__(self, w, h, levels, max_points=65536, device=0):
         self.L = lib()
@@ -742,24 +792,9 @@ class CT:
     def trace_points_multi(self, sets, settings=None):
         """sets = [(P, KRKi, Kt, aff), ...]: the immature points of several host keyframes in ONE launch (dmv_ct_trace_points_multi);
         returns the list of updated dicts.  settings: an IPSettings, or None (NULL: defaults)."""
-        ns = len(sets)
-        arr = (IPPoints * ns)()
-        keeps, outs = [], []
-        tab = np.zeros((ns, 14), np.float32)
-        for k, (P, KRKi, Kt, aff) in enumerate(sets):
-            keep = {q: _c(P[q], np.float32) for q in ("u", "v", "color", "weights", "gradH", "energyTH")}
-            out = {"idepth_min": np.array(P["idepth_min"], np.float32, copy=True), "idepth_max": np.array(P["idepth_max"], np.float32, copy=True),
-                   "quality": np.array(P["quality"], np.float32, copy=True), "status": np.array(P["status"], np.int32, copy=True),
-                   "lastTraceUV": np.array(P["lastTraceUV"], np.float32, copy=True), "lastTracePixelInterval": np.array(P["lastTracePixelInterval"], np.float32, copy=True)}
-            arr[k] = IPPoints(len(P["u"]), *[a.ctypes.data for a in (keep["u"], keep["v"], keep["color"], keep["weights"], keep["gradH"], keep["energyTH"], out["idepth_min"],
-                                                                      out["idepth_max"], out["quality"], out["status"], out["lastTraceUV"], out["lastTracePixelInterval"])])
-            tab[k, :9] = np.asarray(KRKi, np.float32).reshape(-1); tab[k, 9:12] = Kt; tab[k, 12:14] = aff
-            keeps.append(keep); outs.append(out)
-        check(self.L.dmv_ct_trace_points_multi(self.h, ns, C.addressof(arr), tab.reshape(-1), None if settings is None else C.byref(settings)))
-        res = []
-        for (P, _, _, _), out in zip(sets, outs):
-            Q = dict(P); Q.update(out); res.append(Q)
-        return res
+        T = _TraceSets(sets)
+        check(self.L.dmv_ct_trace_points_multi(self.h, T.job.nsets, T.job.sets, T.job.tables14, None if settings is None else C.byref(settings)))
+        return T.results()
 
     def set_timing(self, enable=True):
         check(self.L.dmv_ct_set_timing(self.h, int(enable)))

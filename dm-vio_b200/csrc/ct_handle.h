@@ -18,7 +18,7 @@ struct dmv_ct {
   int device = 0;
   cudaStream_t stream = nullptr;
   cudaEvent_t ev[2] = {nullptr, nullptr};
-  cudaEvent_t ev_order = nullptr;   // orders a dmv_ct_track_many launch on another member's stream behind this handle's queued work
+  cudaEvent_t ev_order = nullptr;   // orders a dmv_ct_track_many / dmv_ct_trace_many launch on another member's stream behind this handle's queued work
   bool staging_busy = false;  // an asynchronous upload from h_scratch may be in flight
   bool timing = false;  // CUDA-event timing of every evaluation (dmv_ct_set_timing); off by default: two event records per launch
   int w[DMV_MAX_PYR_LEVELS], h[DMV_MAX_PYR_LEVELS];
@@ -67,6 +67,13 @@ inline cudaError_t ct_wait_staging(dmv_ct* c) {
   const cudaError_t e = cudaStreamSynchronize(c->stream);
   if (e == cudaSuccess) c->staging_busy = false;
   return e;
+}
+
+// the error a check of member i of a call over several handles just set, prefixed with the member's index
+inline int ct_member_error(int rc, int i) {
+  char msg[512];
+  snprintf(msg, sizeof(msg), "%s", dmv_last_error());
+  return set_error(rc, "handles[%d]: %s", i, msg);
 }
 
 // d_ip / h_ip hold at least n points: 31 words per point (dmv_ct_trace_points' layout, the widest) and 14 words of tables for each of up

@@ -1006,13 +1006,6 @@ int dmv_ct_track(dmv_ct* c, const dmv_ct_track_args* in, dmv_ct_track_result* ou
   return DMV_OK;
 }
 
-// the error a check of member i just set, prefixed with the member's index
-static int ct_member_error(int rc, int i) {
-  char msg[512];
-  snprintf(msg, sizeof(msg), "%s", dmv_last_error());
-  return set_error(rc, "handles[%d]: %s", i, msg);
-}
-
 // dmv_ct_track for n handles in one launch, one cluster per handle.  Every check precedes the launch.
 int dmv_ct_track_many(dmv_ct* const* handles, int n, const dmv_ct_track_args* in, dmv_ct_track_result* out) {
   if (!handles || !in || !out) return set_error(DMV_ERR_INVALID, "null argument");

@@ -37,18 +37,30 @@ __device__ __forceinline__ void ip_interp33(const float4* __restrict__ mat, floa
   out[2] = dxdy * br.z + (dy - dxdy) * bl.z + (dx - dxdy) * tr.z + (1 - dx - dy + dxdy) * tl.z;
 }
 
-struct IPTraceArgs {
-  int n, w, h;
-  float KRKi[9], Kt[3], aff[2];   // one host frame (tab == nullptr)
-  const float* tab;               // several host frames in one launch: [set][14] = KRKi 9 | Kt 3 | aff 2, and set_of[point]
-  const int* set_of;
-  dmv_ip_settings s;
-  const float *u, *v, *color, *weights, *gradH, *energyTH;
-  float *idepth_min, *idepth_max, *quality;
-  int* status;
-  float *uv, *interval;
+// The tracing staging area d_ip of one handle: ip_cap points per array, the array of word w at d_ip + w * ip_cap (uv and the 8 / 4 per-point
+// vectors interleaved per point), then 14 floats per host frame (KRKi 9 | Kt 3 | aff 2).  The host staging and ip_trace_kernel both read
+// these offsets.  set is the host frame of each point (an int), status an int too.
+namespace ipw {
+constexpr int u = 0, v = 1, color = 2, weights = 10, gradH = 18, energyTH = 22;          // read only
+constexpr int idepth_min = 23, idepth_max = 24, quality = 25, status = 26, uv = 27, interval = 29;   // in/out: the 7 words from idepth_min on
+constexpr int set = 30, tables = 31;
+constexpr int inout = 7;
+}  // namespace ipw
+
+// One member of a trace launch: a coarse-tracker handle's resident level-0 plane and its staging area
+struct IPTraceMember {
   const float4* img;
+  float* ip;          // d_ip (ipw layout)
+  int cap, w, h;
+  int n;              // points
 };
+struct IPTraceArgs {
+  int n;                                     // members
+  int first[DMV_CT_TRACE_MANY_MAX + 1];      // member k's points are the warps first[k] .. first[k] + m[k].n - 1; first[k] % 4 == 0
+  dmv_ip_settings s;
+  IPTraceMember m[DMV_CT_TRACE_MANY_MAX];
+};
+static_assert(sizeof(IPTraceArgs) == 624, "ip_trace_kernel's parameter block");
 
 // One WARP per immature point.  The reference walks the epipolar segment step by step (<= 99 positions x 8 bilinear samples) and keeps the
 // best and second-best energies; here the positions are dealt to the 32 lanes (lane L takes steps L, L+32, L+64, L+96: at most 4 rounds
@@ -70,27 +82,41 @@ __device__ __forceinline__ float ip_step_energy(const IPTraceArgs& A, const floa
   return energy;
 }
 
-__global__ void __launch_bounds__(128) ip_trace_kernel(const __grid_constant__ IPTraceArgs A) {
-  const int i = (blockIdx.x * blockDim.x + threadIdx.x) >> 5;   // warp = point
+// One launch serves up to DMV_CT_TRACE_MANY_MAX handles.  Each member's points start at a CTA (first[k] is a multiple of 4 warps), so the
+// member lookup depends on blockIdx alone: the scan and the member's descriptor live in uniform registers, and the kernel keeps the
+// 72 registers of its one-handle form (7 CTAs per SM).  Warps past a member's last point return at once; the kernel has no block-level
+// synchronisation and returns per warp.
+__global__ void __launch_bounds__(128, 7) ip_trace_kernel(const __grid_constant__ IPTraceArgs A) {
   const int lane = threadIdx.x & 31;
-  if (i >= A.n) return;
+  const int cta_warp = 4 * blockIdx.x;
+  int mem = 0;
+  while (cta_warp >= A.first[mem + 1]) mem++;   // the grid covers first[n] warps; skips empty members (first[mem] == first[mem + 1])
+  const IPTraceMember& M = A.m[mem];
+  const int i = cta_warp + (threadIdx.x >> 5) - A.first[mem];   // warp = point
+  if (i >= M.n) return;
+  float* const ip = M.ip;
+  const size_t cap = M.cap;
+  int* const st_out = reinterpret_cast<int*>(ip + ipw::status * cap);
+  float* const uv_out = ip + ipw::uv * cap;
+  float* const iv_out = ip + ipw::interval * cap;
   const dmv_ip_settings& s = A.s;
-  const int w = A.w, h = A.h;
-  const float4* __restrict__ dI = A.img;
-  const float* tabp = A.tab ? A.tab + 14 * A.set_of[i] : A.KRKi;   // KRKi | Kt | aff are contiguous in both cases
+  const int w = M.w, h = M.h;
+  const float4* __restrict__ dI = M.img;
+  const float* tabp = ip + ipw::tables * cap + 14 * reinterpret_cast<const int*>(ip)[ipw::set * cap + i];
   const float* KRKi = tabp;
   const float* Kt = tabp + 9;
   const float aff0 = tabp[12], aff1 = tabp[13];
-  const int status = A.status[i];
+  const int status = st_out[i];
   if (status == 1) return;  // IPS_OOB stays OOB (ImmaturePoint.cpp:L79)
-  const float u = A.u[i], v = A.v[i];
-  float idepth_min = A.idepth_min[i], idepth_max = A.idepth_max[i];
+  const float u = ip[ipw::u * cap + i], v = ip[ipw::v * cap + i];
+  float idepth_min = ip[ipw::idepth_min * cap + i], idepth_max = ip[ipw::idepth_max * cap + i];
   float color[8];
 #pragma unroll
-  for (int k = 0; k < 8; k++) color[k] = A.color[8 * i + k];
-  const float g0 = A.gradH[4 * i], g1 = A.gradH[4 * i + 1], g2 = A.gradH[4 * i + 2], g3 = A.gradH[4 * i + 3];
-  const float energyTH = A.energyTH[i];
-#define IP_RETURN(st, ux, uy, itv) do { if (lane == 0) { A.status[i] = (st); A.uv[2 * i] = (ux); A.uv[2 * i + 1] = (uy); A.interval[i] = (itv); } return; } while (0)
+  for (int k = 0; k < 8; k++) color[k] = ip[ipw::color * cap + 8 * i + k];
+  const float* gH = ip + ipw::gradH * cap + 4 * i;
+  const float g0 = gH[0], g1 = gH[1], g2 = gH[2], g3 = gH[3];
+  const float energyTH = ip[ipw::energyTH * cap + i];
+#define IP_RETURN(st, ux, uy, itv) do { if (lane == 0) { st_out[i] = (st); uv_out[2 * i] = (ux); uv_out[2 * i + 1] = (uy); iv_out[i] = (itv); } return; } while (0)
   const float maxPixSearch = (w + h) * s.maxPixSearch;
   // ---- the segment [idepth_min, idepth_max] in the new frame (L98-185)
   float pr[3], ptpMin[3];
@@ -200,16 +226,16 @@ __global__ void __launch_bounds__(128) ip_trace_kernel(const __grid_constant__ I
     if (o < secondBest) secondBest = o;
   }
   const float newQuality = secondBest / bestEnergy;
-  float quality = A.quality[i];
+  float quality = ip[ipw::quality * cap + i];
   if (newQuality < quality || numSteps > 10) quality = newQuality;
   __syncwarp();
-  if (lane == 0) A.quality[i] = quality;
+  if (lane == 0) ip[ipw::quality * cap + i] = quality;
   // ---- Gauss-Newton refinement along the line (L280-353): lane idx < 8 samples pattern pixel idx, the sums fold in pattern order
   float uBak = bestU, vBak = bestV, stepBack = 0;
   const float gnstepsize = 1;
   if (s.trace_GNIterations > 0) bestEnergy = 1e5f;
   const int idx8 = lane & 7;
-  const float wgt = A.weights[8 * i + idx8];
+  const float wgt = ip[ipw::weights * cap + 8 * i + idx8];
   float colL = 0.f, rx = 0.f, ry = 0.f;
 #pragma unroll
   for (int k = 0; k < 8; k++) if (k == idx8) { colL = color[k]; rx = rot[k][0]; ry = rot[k][1]; }
@@ -260,7 +286,7 @@ __global__ void __launch_bounds__(128) ip_trace_kernel(const __grid_constant__ I
     idepth_max = (pr[2] * (bestV + errorInPixel * dy) - pr[1]) / (Kt[1] - Kt[2] * (bestV + errorInPixel * dy));
   }
   if (idepth_min > idepth_max) { const float tmp = idepth_min; idepth_min = idepth_max; idepth_max = tmp; }
-  if (lane == 0) { A.idepth_min[i] = idepth_min; A.idepth_max[i] = idepth_max; }   // the reference assigns the members before the final validity test
+  if (lane == 0) { ip[ipw::idepth_min * cap + i] = idepth_min; ip[ipw::idepth_max * cap + i] = idepth_max; }   // the reference assigns the members before the final validity test
   if (!isfinite(idepth_min) || !isfinite(idepth_max) || (idepth_max < 0)) IP_RETURN(2, -1.f, -1.f, 0.f);
   IP_RETURN(0, bestU, bestV, 2 * errorInPixel);
 #undef IP_RETURN
@@ -501,69 +527,125 @@ int dmv_ct_init_points(dmv_ct* c, int n, const int32_t* u, const int32_t* v, flo
   return DMV_OK;
 }
 
-// immature points of SEVERAL host frames traced against the resident newest frame in ONE launch (ip_trace_kernel): FullSystem::traceNewCoarse's
-// loop over the window's keyframes (FullSystem.cpp:L554-575) collapsed into one upload, one kernel, one download
-int dmv_ct_trace_points_multi(dmv_ct* c, int nsets, const dmv_ip_points* sets, const float* tables14, const dmv_ip_settings* settings) {
-  if (!c || nsets < 0 || (nsets > 0 && (!sets || !tables14))) return set_error(DMV_ERR_INVALID, "null argument");
-  int n = 0;
-  for (int k = 0; k < nsets; k++) {
-    const dmv_ip_points* p = &sets[k];
+// dmv_ct_trace_points_multi's checks of one handle's job, in its order; *n = the job's point count.  No CUDA call.
+static int ip_trace_check(const dmv_ct_trace_job& j, int* n) {
+  if (j.nsets < 0 || (j.nsets > 0 && (!j.sets || !j.tables14))) return set_error(DMV_ERR_INVALID, "null argument");
+  *n = 0;
+  for (int k = 0; k < j.nsets; k++) {
+    const dmv_ip_points* p = &j.sets[k];
     if (p->n < 0 || (p->n > 0 && (!p->u || !p->v || !p->color8 || !p->weights8 || !p->gradH4 || !p->energyTH || !p->idepth_min || !p->idepth_max || !p->quality ||
                                   !p->lastTraceStatus || !p->lastTraceUV2 || !p->lastTracePixelInterval)))
       return set_error(DMV_ERR_INVALID, "incomplete dmv_ip_points (set %d)", k);
-    n += p->n;
+    *n += p->n;
   }
-  if (n == 0) return DMV_OK;
-  CK(cudaSetDevice(c->device));
-  const int words = 31;   // 23 read-only floats, 7 in/out words and the set index per point
-  CK(ct_reserve_ip(c, n));
-  if (nsets > 64) return set_error(DMV_ERR_INVALID, "at most 64 host frames per call");
-  CK(ct_wait_staging(c));
-  const size_t cap = c->ip_cap;
-  float* hb = c->h_ip;
-  // layout (floats): u | v | color*8 | weights*8 | gradH*4 | energyTH | idmin | idmax | quality | status(int) | uv*2 | interval | set(int) | tables
-  const size_t o_u = 0, o_v = cap, o_col = 2 * cap, o_wgt = 10 * cap, o_g = 18 * cap, o_eth = 22 * cap, o_min = 23 * cap, o_max = 24 * cap, o_q = 25 * cap,
-               o_st = 26 * cap, o_uv = 27 * cap, o_iv = 29 * cap, o_set = 30 * cap, o_tab = 31 * cap;
-  size_t at = 0;
-  for (int k = 0; k < nsets; k++) {
-    const dmv_ip_points* p = &sets[k];
-    const size_t m = (size_t)p->n;
-    if (m == 0) continue;
-    std::memcpy(hb + o_u + at, p->u, 4 * m); std::memcpy(hb + o_v + at, p->v, 4 * m);
-    std::memcpy(hb + o_col + 8 * at, p->color8, 32 * m); std::memcpy(hb + o_wgt + 8 * at, p->weights8, 32 * m);
-    std::memcpy(hb + o_g + 4 * at, p->gradH4, 16 * m); std::memcpy(hb + o_eth + at, p->energyTH, 4 * m);
-    std::memcpy(hb + o_min + at, p->idepth_min, 4 * m); std::memcpy(hb + o_max + at, p->idepth_max, 4 * m); std::memcpy(hb + o_q + at, p->quality, 4 * m);
-    std::memcpy(hb + o_st + at, p->lastTraceStatus, 4 * m); std::memcpy(hb + o_uv + 2 * at, p->lastTraceUV2, 8 * m); std::memcpy(hb + o_iv + at, p->lastTracePixelInterval, 4 * m);
-    int* setp = reinterpret_cast<int*>(hb + o_set + at);
-    for (size_t q = 0; q < m; q++) setp[q] = k;
-    at += m;
+  if (*n > 0 && j.nsets > 64) return set_error(DMV_ERR_INVALID, "at most 64 host frames per call");
+  return DMV_OK;
+}
+
+// The immature points of n handles (n = 1: dmv_ct_trace_points_multi) traced in ONE launch of ip_trace_kernel.  Every job is checked before
+// anything is allocated, copied or launched (`many`: a job's error names its member).  Member i's points go through its own staging area
+// d_ip / h_ip, uploaded on its own stream; the launch goes on handles[0]'s stream behind every member's queued work, the downloads follow it
+// there, and one synchronisation ends the call.
+// h_ip is written without ct_wait_staging: an upload still in flight reads h_scratch, never h_ip, and every call that fills h_ip synchronises
+// its stream before it returns, so nothing can be reading h_ip here.
+static int ip_trace_run(dmv_ct* const* hs, int n, const dmv_ct_trace_job* jobs, const dmv_ip_settings* settings, bool many) {
+  int np[DMV_CT_TRACE_MANY_MAX];
+  int total = 0;
+  for (int i = 0; i < n; i++) {
+    const int rc = ip_trace_check(jobs[i], &np[i]);
+    if (rc != DMV_OK) return many ? ct_member_error(rc, i) : rc;
+    total += np[i];
   }
-  std::memcpy(hb + o_tab, tables14, sizeof(float) * 14 * (size_t)nsets);
-  CK(cudaMemcpyAsync(c->d_ip, hb, sizeof(float) * ((size_t)words * cap + 14 * (size_t)nsets), cudaMemcpyHostToDevice, c->stream));
+  if (total == 0) return DMV_OK;
+  CK(cudaSetDevice(hs[0]->device));
+  for (int i = 0; i < n; i++)
+    if (np[i] > 0) CK(ct_reserve_ip(hs[i], np[i]));
   IPTraceArgs A;
   std::memset(&A, 0, sizeof(A));
-  A.n = n; A.w = c->w[0]; A.h = c->h[0];
+  A.n = n;
   if (settings) A.s = *settings; else dmv_ip_default_settings(&A.s);
-  float* d = c->d_ip;
-  A.tab = d + o_tab; A.set_of = reinterpret_cast<const int*>(d + o_set);
-  A.u = d + o_u; A.v = d + o_v; A.color = d + o_col; A.weights = d + o_wgt; A.gradH = d + o_g; A.energyTH = d + o_eth;
-  A.idepth_min = d + o_min; A.idepth_max = d + o_max; A.quality = d + o_q; A.status = reinterpret_cast<int*>(d + o_st); A.uv = d + o_uv; A.interval = d + o_iv;
-  A.img = c->d_img[0];
-  ip_trace_kernel<<<(A.n + 3) / 4, 128, 0, c->stream>>>(A);   // 4 warps = 4 points per CTA
-  c->launches++;
+  const cudaStream_t s = hs[0]->stream;
+  for (int i = 0; i < n; i++) {
+    dmv_ct* c = hs[i];
+    const dmv_ct_trace_job& j = jobs[i];
+    A.first[i + 1] = A.first[i] + (np[i] + 3) / 4 * 4;   // whole CTAs per member
+    if (np[i] > 0) {
+      const size_t cap = c->ip_cap;
+      float* hb = c->h_ip;
+      size_t at = 0;
+      for (int k = 0; k < j.nsets; k++) {
+        const dmv_ip_points* p = &j.sets[k];
+        const size_t m = (size_t)p->n;
+        if (m == 0) continue;
+        std::memcpy(hb + ipw::u * cap + at, p->u, 4 * m); std::memcpy(hb + ipw::v * cap + at, p->v, 4 * m);
+        std::memcpy(hb + ipw::color * cap + 8 * at, p->color8, 32 * m); std::memcpy(hb + ipw::weights * cap + 8 * at, p->weights8, 32 * m);
+        std::memcpy(hb + ipw::gradH * cap + 4 * at, p->gradH4, 16 * m); std::memcpy(hb + ipw::energyTH * cap + at, p->energyTH, 4 * m);
+        std::memcpy(hb + ipw::idepth_min * cap + at, p->idepth_min, 4 * m); std::memcpy(hb + ipw::idepth_max * cap + at, p->idepth_max, 4 * m);
+        std::memcpy(hb + ipw::quality * cap + at, p->quality, 4 * m); std::memcpy(hb + ipw::status * cap + at, p->lastTraceStatus, 4 * m);
+        std::memcpy(hb + ipw::uv * cap + 2 * at, p->lastTraceUV2, 8 * m); std::memcpy(hb + ipw::interval * cap + at, p->lastTracePixelInterval, 4 * m);
+        int* setp = reinterpret_cast<int*>(hb + ipw::set * cap + at);
+        for (size_t q = 0; q < m; q++) setp[q] = k;
+        at += m;
+      }
+      std::memcpy(hb + ipw::tables * cap, j.tables14, sizeof(float) * 14 * (size_t)j.nsets);
+      CK(cudaMemcpyAsync(c->d_ip, hb, sizeof(float) * (ipw::tables * cap + 14 * (size_t)j.nsets), cudaMemcpyHostToDevice, c->stream));
+      A.m[i].img = c->d_img[0]; A.m[i].ip = c->d_ip; A.m[i].cap = c->ip_cap; A.m[i].w = c->w[0]; A.m[i].h = c->h[0]; A.m[i].n = np[i];
+    }
+    if (i > 0) {   // the launch goes behind this member's queued work: its frame uploads (dmv_ct_upload_new_image does not synchronise) and the copy above
+      CK(cudaEventRecord(c->ev_order, c->stream));
+      CK(cudaStreamWaitEvent(s, c->ev_order, 0));
+    }
+  }
+  ip_trace_kernel<<<A.first[n] / 4, 128, 0, s>>>(A);   // 4 warps = 4 points per CTA
+  for (int i = 0; i < n; i++)
+    if (np[i] > 0) hs[i]->launches++;
   CK(cudaGetLastError());
-  CK(cudaMemcpyAsync(hb + o_min, d + o_min, sizeof(float) * 7 * cap, cudaMemcpyDeviceToHost, c->stream));  // the 7 in/out words per point
-  CK(cudaStreamSynchronize(c->stream));
-  at = 0;
-  for (int k = 0; k < nsets; k++) {
-    const dmv_ip_points* p = &sets[k];
-    const size_t m = (size_t)p->n;
-    if (m == 0) continue;
-    std::memcpy(p->idepth_min, hb + o_min + at, 4 * m); std::memcpy(p->idepth_max, hb + o_max + at, 4 * m); std::memcpy(p->quality, hb + o_q + at, 4 * m);
-    std::memcpy(p->lastTraceStatus, hb + o_st + at, 4 * m); std::memcpy(p->lastTraceUV2, hb + o_uv + 2 * at, 8 * m); std::memcpy(p->lastTracePixelInterval, hb + o_iv + at, 4 * m);
-    at += m;
+  for (int i = 0; i < n; i++) {   // the 7 in/out words per point
+    if (np[i] == 0) continue;
+    const size_t cap = hs[i]->ip_cap;
+    CK(cudaMemcpyAsync(hs[i]->h_ip + ipw::idepth_min * cap, hs[i]->d_ip + ipw::idepth_min * cap, sizeof(float) * ipw::inout * cap, cudaMemcpyDeviceToHost, s));
+  }
+  CK(cudaStreamSynchronize(s));
+  for (int i = 0; i < n; i++) {
+    hs[i]->staging_busy = false;   // every member's queued work completed before the kernel started
+    const size_t cap = hs[i]->ip_cap;
+    const float* hb = hs[i]->h_ip;
+    size_t at = 0;
+    for (int k = 0; k < jobs[i].nsets; k++) {
+      const dmv_ip_points* p = &jobs[i].sets[k];
+      const size_t m = (size_t)p->n;
+      if (m == 0) continue;
+      std::memcpy(p->idepth_min, hb + ipw::idepth_min * cap + at, 4 * m); std::memcpy(p->idepth_max, hb + ipw::idepth_max * cap + at, 4 * m);
+      std::memcpy(p->quality, hb + ipw::quality * cap + at, 4 * m); std::memcpy(p->lastTraceStatus, hb + ipw::status * cap + at, 4 * m);
+      std::memcpy(p->lastTraceUV2, hb + ipw::uv * cap + 2 * at, 8 * m); std::memcpy(p->lastTracePixelInterval, hb + ipw::interval * cap + at, 4 * m);
+      at += m;
+    }
   }
   return DMV_OK;
+}
+
+// immature points of SEVERAL host frames traced against the resident newest frame in ONE launch (ip_trace_kernel): FullSystem::traceNewCoarse's
+// loop over the window's keyframes (FullSystem.cpp:L554-575) collapsed into one upload, one kernel, one download
+int dmv_ct_trace_points_multi(dmv_ct* c, int nsets, const dmv_ip_points* sets, const float* tables14, const dmv_ip_settings* settings) {
+  if (!c) return set_error(DMV_ERR_INVALID, "null argument");
+  dmv_ct_trace_job j;
+  j.nsets = nsets; j.sets = sets; j.tables14 = tables14;
+  return ip_trace_run(&c, 1, &j, settings, false);
+}
+
+// dmv_ct_trace_points_multi for n handles in one launch.  Every check precedes the first allocation, copy or launch.
+int dmv_ct_trace_many(dmv_ct* const* handles, int n, const dmv_ct_trace_job* jobs, const dmv_ip_settings* settings) {
+  if (!handles || !jobs) return set_error(DMV_ERR_INVALID, "null argument");
+  if (n < 1 || n > DMV_CT_TRACE_MANY_MAX) return set_error(DMV_ERR_INVALID, "n = %d: expected 1 to %d handles", n, DMV_CT_TRACE_MANY_MAX);
+  for (int i = 0; i < n; i++) {
+    if (!handles[i]) return set_error(DMV_ERR_INVALID, "handles[%d] is NULL", i);
+    for (int j = 0; j < i; j++)
+      if (handles[j] == handles[i]) return set_error(DMV_ERR_INVALID, "handles[%d] and handles[%d] are the same handle", j, i);
+    if (handles[i]->device != handles[0]->device)
+      return set_error(DMV_ERR_INVALID, "handles[%d] is on device %d, handles[0] on device %d: one launch runs on one device", i, handles[i]->device,
+                       handles[0]->device);
+  }
+  return ip_trace_run(handles, n, jobs, settings, true);
 }
 
 // one host frame's immature points traced against the resident newest frame

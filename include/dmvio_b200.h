@@ -465,6 +465,26 @@ int dmv_ct_trace_points(dmv_ct* ct, const dmv_ip_points* pts, const float KRKi[9
 /* The same for the immature points of SEVERAL host keyframes at once (the whole loop of FullSystem::traceNewCoarse, FullSystem.cpp:L554-575):
  * sets[k] = the points hosted by keyframe k, tables14 = per host [KRKi 9 | Kt 3 | aff 2]; one upload, one launch, one download. */
 int dmv_ct_trace_points_multi(dmv_ct* ct, int nsets, const dmv_ip_points* sets, const float* tables14, const dmv_ip_settings* settings);
+/* dmv_ct_trace_points_multi for n independent handles (several cameras or robots served by one host thread, each after its tracked frame)
+ * in ONE launch.  jobs[i] holds exactly the arguments dmv_ct_trace_points_multi takes for handles[i].
+ * Result: for every i, jobs[i]'s in/out arrays end bit-identical to what dmv_ct_trace_points_multi(handles[i], jobs[i].nsets, jobs[i].sets,
+ * jobs[i].tables14, settings) leaves; each member traces against its own resident level-0 frame, at its own image size.
+ * Launch count: each member's dmv_ct_kernel_launch_count reads as after that call (+1 if the member has at least one point, +0 otherwise);
+ * a call in which no member has a point launches nothing.
+ * Settings: one for the call, as DSO's settings are process-global; NULL means defaults.
+ * Ordering: the launch is ordered behind the work queued on every member's stream (asynchronous dmv_ct_upload_new_image /
+ * dmv_ct_upload_raw_image included); the call returns after one synchronisation, with every member's staging buffer free.
+ * Errors, all before any allocation, copy or launch and before any output is written: DMV_ERR_INVALID for n outside
+ * 1..DMV_CT_TRACE_MANY_MAX, a NULL handles / jobs, a NULL member, a handle passed twice (the message names both positions) or handles on
+ * different devices; and, for each member, the errors dmv_ct_trace_points_multi reports for its arguments, prefixed "handles[i]: ".  A
+ * member is accepted exactly when dmv_ct_trace_points_multi would accept it. */
+#define DMV_CT_TRACE_MANY_MAX 16
+typedef struct dmv_ct_trace_job {
+  int nsets;                   /* host keyframes of this handle's window, as dmv_ct_trace_points_multi */
+  const dmv_ip_points* sets;   /* in/out exactly as dmv_ct_trace_points_multi */
+  const float* tables14;       /* nsets * 14: KRKi 9 | Kt 3 | aff 2 per host */
+} dmv_ct_trace_job;
+int dmv_ct_trace_many(dmv_ct* const* handles, int n, const dmv_ct_trace_job* jobs, const dmv_ip_settings* settings);
 
 /* ------------------------------------------------------------------------------------------------
  * New immature points of a keyframe  ==  FullSystem::makeNewTraces (FullSystem.cpp:L1640-1667): PixelSelector::makeMaps
