@@ -151,6 +151,18 @@ class CTTrackResult(C.Structure):
                 ("flowIndicators", C.c_double * 3), ("trackingGood", C.c_int), ("iterations", C.c_int), ("evaluations", C.c_int), ("status", C.c_int)]
 
 
+class CTTriesArgs(C.Structure):
+    _fields_ = [("n", C.c_int), ("R", vp), ("t", vp), ("a", C.c_double), ("b", C.c_double), ("ref_a", C.c_double), ("ref_b", C.c_double),
+                ("ref_exposure", C.c_float), ("new_exposure", C.c_float), ("coarseCutoffTH", C.c_float), ("affineOptModeA", C.c_float),
+                ("affineOptModeB", C.c_float), ("coarsestLvl", C.c_int), ("lastCoarseRMSE0", C.c_double), ("reTrackThreshold", C.c_float)]
+
+
+class CTTriesResult(C.Structure):
+    _fields_ = [("R", C.c_double * 9), ("t", C.c_double * 3), ("a", C.c_double), ("b", C.c_double), ("achievedRes", C.c_double * 5),
+                ("flowVecs", C.c_double * 3), ("lastResiduals", C.c_double * 5), ("flowIndicators", C.c_double * 3), ("trackingGood", C.c_int),
+                ("haveOneGood", C.c_int), ("winner", C.c_int), ("tries", C.c_int), ("tries_started", C.c_int)]
+
+
 class UndistortConfig(C.Structure):
     _fields_ = [("wOrg", C.c_int), ("hOrg", C.c_int), ("remapX", vp), ("remapY", vp), ("G", vp), ("nG", C.c_int), ("vignetteInv", vp),
                 ("photometric_mode", C.c_int)]
@@ -181,7 +193,7 @@ SYMBOLS = [
     "dmv_ba_batch_create", "dmv_ba_batch_destroy", "dmv_ba_batch_gn_step", "dmv_ba_batch_set_timing", "dmv_ba_batch_last_kernel_ms", "dmv_ba_batch_bench",
     "dmv_ct_create", "dmv_ct_destroy", "dmv_ct_set_K", "dmv_ct_set_ref", "dmv_ct_make_coarse_depth", "dmv_ct_set_ref_from_ba", "dmv_ct_get_ref", "dmv_ct_upload_new", "dmv_ct_upload_new_image", "dmv_ct_set_huber",
     "dmv_ci_create", "dmv_ci_destroy", "dmv_ci_set_K", "dmv_ci_upload_first", "dmv_ci_upload_new", "dmv_ci_set_points", "dmv_ci_calc_res_and_gs", "dmv_ci_kernel_launch_count",
-    "dmv_ct_calc_res_gs", "dmv_ct_track", "dmv_ct_track_many", "dmv_ip_default_settings", "dmv_ct_init_points", "dmv_ct_trace_points", "dmv_ct_trace_points_multi", "dmv_ct_trace_many", "dmv_ct_set_timing", "dmv_ct_last_timing", "dmv_ct_kernel_launch_count", "dmv_ct_last_point_evaluations",
+    "dmv_ct_calc_res_gs", "dmv_ct_track", "dmv_ct_track_many", "dmv_ct_track_tries", "dmv_ip_default_settings", "dmv_ct_init_points", "dmv_ct_trace_points", "dmv_ct_trace_points_multi", "dmv_ct_trace_many", "dmv_ct_set_timing", "dmv_ct_last_timing", "dmv_ct_kernel_launch_count", "dmv_ct_last_point_evaluations",
     "dmv_ct_set_undistort", "dmv_ct_upload_raw_image", "dmv_ct_download_frame", "dmv_ps_default_settings", "dmv_ct_make_new_traces",
 ]
 
@@ -253,6 +265,7 @@ def lib():
         L.dmv_ct_calc_res_gs.argtypes = [vp, C.c_int, f32p, f32p, f32p, C.c_float, C.c_float, C.c_int, f64p, f64p, f64p, C.POINTER(C.c_int)]
         L.dmv_ct_track.argtypes = [vp, C.POINTER(CTTrackArgs), C.POINTER(CTTrackResult)]
         L.dmv_ct_track_many.argtypes = [C.POINTER(vp), C.c_int, C.POINTER(CTTrackArgs), C.POINTER(CTTrackResult)]
+        L.dmv_ct_track_tries.argtypes = [vp, C.POINTER(CTTriesArgs), C.POINTER(CTTriesResult)]
         L.dmv_ct_init_points.argtypes = [vp, C.c_int, i32p, i32p, f32p, f32p, f32p, f32p, i32p]
         L.dmv_ct_trace_points.argtypes = [vp, C.POINTER(IPPoints), f32p, f32p, f32p, vp]
         L.dmv_ct_trace_points_multi.argtypes = [vp, C.c_int, vp, vp, vp]
@@ -575,6 +588,27 @@ def _track_result(r):
                 good=r.trackingGood, iterations=r.iterations, evaluations=r.evaluations, status=r.status)
 
 
+def _tries_args(levels, R, t, a, b, ref_a=0.0, ref_b=0.0, ref_exposure=1.0, new_exposure=1.0, cutoff=20.0, affA=1e12, affB=1e8, coarsest=None,
+                lastCoarseRMSE0=100.0, reTrackThreshold=1.5):
+    """the dmv_ct_tries_args of CT.track_tries's arguments (R: n 3x3 matrices, t: n 3-vectors) and the arrays it points to; the fields it
+    shares with dmv_ct_track_args go through _track_args"""
+    Rs = np.ascontiguousarray(np.asarray(R, np.float64).reshape(-1, 9))
+    ts = np.ascontiguousarray(np.asarray(t, np.float64).reshape(-1, 3))
+    if len(Rs) != len(ts):
+        raise ValueError(f"{len(Rs)} rotations but {len(ts)} translations")
+    T = _track_args(levels, Rs[0] if len(Rs) else np.eye(3), ts[0] if len(ts) else np.zeros(3), a, b, ref_a, ref_b, ref_exposure, new_exposure,
+                    cutoff, affA, affB, coarsest)
+    A = CTTriesArgs(len(Rs), Rs.ctypes.data, ts.ctypes.data, T.a, T.b, T.ref_a, T.ref_b, T.ref_exposure, T.new_exposure, T.coarseCutoffTH,
+                    T.affineOptModeA, T.affineOptModeB, T.coarsestLvl, float(lastCoarseRMSE0), float(reTrackThreshold))
+    return A, (Rs, ts)
+
+
+def _tries_result(r):
+    return dict(R=np.array(r.R).reshape(3, 3), t=np.array(r.t), a=r.a, b=r.b, achievedRes=np.array(r.achievedRes), flowVecs=np.array(r.flowVecs),
+                lastResiduals=np.array(r.lastResiduals), flow=np.array(r.flowIndicators), good=r.trackingGood, haveOneGood=r.haveOneGood,
+                winner=r.winner, tries=r.tries, tries_started=r.tries_started)
+
+
 def ct_track_many(handles, args):
     """dmv_ct_track_many: handles[i] (a CT) tracked with args[i] (a dict of CT.track's keywords), all in one launch.  Returns the list of
     CT.track's result dicts, each bit-identical to handles[i].track(**args[i])."""
@@ -703,6 +737,16 @@ class CT:
         r = CTTrackResult()
         check(self.L.dmv_ct_track(self.h, C.byref(A), C.byref(r)))
         return _track_result(r)
+
+    def track_tries(self, R, t, a, b, ref_a=0.0, ref_b=0.0, ref_exposure=1.0, new_exposure=1.0, cutoff=20.0, affA=1e12, affB=1e8, coarsest=None,
+                    lastCoarseRMSE0=100.0, reTrackThreshold=1.5):
+        """dmv_ct_track_tries (FullSystem::trackNewCoarse's loop over the tries R[i], t[i] in one launch): every field of
+        dmv_ct_tries_result as a dict (flowIndicators as "flow" and trackingGood as "good", as CT.track names them).  a, b = aff_last_2_l."""
+        A, keep = _tries_args(self.levels, R, t, a, b, ref_a, ref_b, ref_exposure, new_exposure, cutoff, affA, affB, coarsest, lastCoarseRMSE0,
+                              reTrackThreshold)
+        r = CTTriesResult()
+        check(self.L.dmv_ct_track_tries(self.h, C.byref(A), C.byref(r)))
+        return _tries_result(r)
 
     def point_evaluations(self):
         """reference points evaluated by the last track, summed over its evaluations (dmv_ct_last_point_evaluations)"""

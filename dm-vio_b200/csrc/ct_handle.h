@@ -43,6 +43,7 @@ struct dmv_ct {
   int cluster_size = 0;        // CTAs of ct_track_cluster_kernel's cluster (0 = not probed yet, -1 = none schedulable: dmv_ct_track fails)
   dmv::CTMaps* maps = nullptr; // TMA descriptors of the level planes (host copy; passed as a kernel parameter)
   int staged[DMV_MAX_PYR_LEVELS] = {0};   // levels whose map ct_make_tensor_maps encoded: the only ones the cluster kernel stages
+  dmv_ct_tries_result* h_tries = nullptr;   // dmv_ct_track_tries's pinned result, allocated on first use
   long long launches = 0;
   float last_ms[4] = {0, 0, 0, 0};
   size_t scratch_bytes = 0;    // capacity of h_scratch

@@ -8,12 +8,14 @@
 //                      The buf_warped_* lists of the reference are never materialised.
 //   ct_track_cluster_kernel   CoarseTracker::trackNewestCoarse in one launch (below).
 //   ct_track_many_kernel      the same for up to DMV_CT_TRACK_MANY_MAX handles in one launch, one cluster per handle.
+//   ct_track_tries_kernel     FullSystem::trackNewCoarse's loop over up to DMV_CT_MAX_TRIES initial poses in one launch.
 // The entry points of the features built on the handle's resident frame live beside their kernels: ct_ingest.cu (raw frames), ct_depth.cu
 // (makeCoarseDepthL0), ip_trace.cu (immature points) and ps_select.cu (pixel selection); the handle's layout is ct_handle.h.
 #include "ct_handle.h"
 #include "inv3.h"
 #include <cuda.h>
 #include <algorithm>
+#include <cmath>
 #include <cstring>
 #include <memory>
 
@@ -222,6 +224,7 @@ struct CTLM {  // the scalar state of trackNewestCoarse, one copy per CTA (share
   double A[64], rhs[8], Lf[64], Df[8], incs[8], EV[18];   // the damped 8x8 system of the pending LM step, its LDL^T factors, its solution
   double pevals;                  // sum over the evaluations of the level's reference-point count (measurement: algorithmic bytes = 64 B each)
   int need_solve, need_request;   // need_request: 1 = evaluate at (R, t, a, b), 2 = at the candidate (Rn, tn, an, bn) = exp(incs) * (R, t)
+  double minRes[5];               // minResForAbort: T.minRes, or in ct_track_tries_kernel the loop's achievedRes (CTLoop)
 };
 enum { CT_PH_INIT = 0, CT_PH_LM = 1 };
 
@@ -410,7 +413,7 @@ __device__ void ct_end_level(const CTTrack& T, CTLM& S) {  // L722-745
   const double* resOld = S.res[S.cur];
   S.lastResiduals[lvl] = sqrtf((float)(resOld[0] / resOld[1]));
   S.flow[0] = resOld[2]; S.flow[1] = resOld[3]; S.flow[2] = resOld[4];
-  if (isnan(S.lastResiduals[lvl]) || S.lastResiduals[lvl] > 1.5 * T.minRes[lvl]) { S.done = 1; S.good = 0; S.status = 2; return; }
+  if (isnan(S.lastResiduals[lvl]) || S.lastResiduals[lvl] > 1.5 * S.minRes[lvl]) { S.done = 1; S.good = 0; S.status = 2; return; }
   if (S.rep > 1 && !S.haveRepeated) { S.haveRepeated = 1; ct_begin_level(T, S); return; }  // lvl++ ; continue  => the same level again
   S.lvl = lvl - 1;
   if (S.lvl < 0) {  // L747-769
@@ -496,12 +499,20 @@ constexpr int CTC_MAXC = 16;                 // CTAs per cluster (8 portable, 16
 constexpr int CTC_PLANE_BYTES = 80 * 1024;   // largest level plane staged in shared memory
 struct alignas(64) CTMaps { CUtensorMap lvl[CT_L]; };   // level planes as 2-D tensors of 16-byte texels (encoded as pairs of fp64)
 
+struct CTLoop {   // the variables of trackNewCoarse's try loop (FullSystem.cpp:L406-413), one copy per CTA, advanced by thread 0 after each try
+  double achieved[5];              // achievedRes: the next try's minResForAbort
+  double R[9], t[3], a, b, flowVecs[3];   // the winner's lastF_2_fh, aff_g2l, lastFlowIndicators
+  double pevals;                   // point evaluations of the tries so far
+  int haveOneGood, winner, trackingGood, tries, stop;
+};
+
 struct alignas(128) CTCSmem {
   unsigned char plane[CTC_PLANE_BYTES];      // TMA destination: the staged level, row-major float4
   double xch[2][CTC_MAXC][CT_NRED + 3];      // [parity][source CTA][sum]: written by every CTA of the cluster through DSMEM
   float red[CTC_THREADS / 32][64];           // per-warp sums (transposed butterfly output)
   double s_sum[CT_NRED + 3];
   CTLM S;
+  CTLoop loop;                               // ct_track_tries_kernel: trackNewCoarse's loop variables
   unsigned long long mbar;                   // TMA completion barrier
 };
 
@@ -513,9 +524,47 @@ __device__ __forceinline__ void ctc_cluster_sync() {
 __device__ __forceinline__ unsigned ctc_smem_u32(const void* p) { return (unsigned)__cvta_generic_to_shared(p); }
 __device__ __forceinline__ unsigned ctc_cluster_id() { unsigned r; asm volatile("mov.u32 %0, %%clusterid.x;" : "=r"(r)); return r; }
 
-// one frame tracked by the calling cluster.  T and maps are __grid_constant__ kernel parameters (the tensor map must stay in parameter
-// space: its address is the operand of the TMA copy).
-__device__ __forceinline__ void ct_track_cluster(const CTTrack& T, const CTMaps& maps) {
+// ---------------------------------------------------------------------------------------------------------------------
+// ct_track_tries_kernel — the try loop of FullSystem::trackNewCoarse (FullSystem.cpp:L412-506, visual-only) in one launch on one cluster:
+// the tries run one after the other through the trackNewestCoarse body below, each with the loop's achievedRes as its minResForAbort, and
+// after each try thread 0 of every CTA applies the loop's bookkeeping to its own copy of the loop variables (CTLoop).  Every CTA holds the
+// same LM state after a try, so every CTA takes the same decisions, the break included, without any exchange.
+// ---------------------------------------------------------------------------------------------------------------------
+struct CTTries {                   // ct_track_tries_kernel's __grid_constant__ parameter block
+  CTTrack T;                       // the handle's descriptors; T.a0, T.b0 = aff_last_2_l
+  CTMaps maps;
+  double pose[DMV_CT_MAX_TRIES][12];   // lastF_2_fh_tries: R row-major, t
+  int n;
+  float reTrackThreshold;
+  double lastCoarseRMSE0;
+  dmv_ct_tries_result* out;        // pinned host
+};
+static_assert(sizeof(CTTries) <= 32764, "CTTries exceeds the 32,764-byte kernel-parameter limit (CUDA >= 12.1, sm_70+)");
+
+// the loop's bookkeeping after try k (L427-488) from the tracker's state S after it; sets the break (L486)
+__device__ void ct_tries_step(const CTTries& Q, CTLoop& W, const CTLM& S, int k) {
+  const bool good = S.status == 0 && S.good;   // trackingIsGood: false after an abort
+  W.tries = k + 1;
+  W.pevals += S.pevals;
+  if (good) W.trackingGood = 1;
+  const double* lastRes = S.lastResiduals;   // reset to NaN at the start of the try (CoarseTracker.cpp:L551), set up to its last level end
+  if (good && isfinite((float)lastRes[0]) && !(lastRes[0] >= W.achieved[0])) {   // a new winner (L467-473)
+    for (int i = 0; i < 3; i++) W.flowVecs[i] = S.flow[i];
+    for (int i = 0; i < 9; i++) W.R[i] = S.R[i];
+    for (int i = 0; i < 3; i++) W.t[i] = S.t[i];
+    W.a = S.a; W.b = S.b;
+    W.haveOneGood = 1; W.winner = k;
+  }
+  if (W.haveOneGood)   // take over achieved res (L476-483)
+    for (int i = 0; i < 5; i++)
+      if (!isfinite((float)W.achieved[i]) || W.achieved[i] > lastRes[i]) W.achieved[i] = lastRes[i];
+  W.stop = W.haveOneGood && W.achieved[0] < Q.lastCoarseRMSE0 * (double)Q.reTrackThreshold;
+}
+
+// one frame tracked by the calling cluster (TRIES: the tries of ct_track_tries_kernel one after the other).  T and maps are
+// __grid_constant__ kernel parameters (the tensor map must stay in parameter space: its address is the operand of the TMA copy).
+template <bool TRIES>
+__device__ __forceinline__ void ct_track_cluster(const CTTrack& T, const CTMaps& maps, const CTTries* Q) {
   extern __shared__ __align__(128) unsigned char ctc_raw[];
   CTCSmem& M = *reinterpret_cast<CTCSmem*>(ctc_raw);
   CTLM& S = M.S;
@@ -525,119 +574,153 @@ __device__ __forceinline__ void ct_track_cluster(const CTTrack& T, const CTMaps&
   unsigned mphase = 0;
   float4 pts[CTC_SLOTS];
   if (tid == 0) {
-    for (int i = 0; i < 9; i++) S.R[i] = T.R0[i];
-    for (int i = 0; i < 3; i++) S.t[i] = T.t0[i];
-    S.a = T.a0; S.b = T.b0;
-    for (int i = 0; i < 5; i++) S.lastResiduals[i] = __longlong_as_double(0x7ff8000000000000ll);  // NAN
-    for (int i = 0; i < 3; i++) S.flow[i] = 1000;
-    S.haveRepeated = 0; S.iterations = 0; S.evaluations = 0; S.done = 0; S.good = 0; S.status = 0; S.cur = 0; S.need_solve = 0; S.pevals = 0;
-    S.lvl = T.coarsest;
-    ct_begin_level(T, S);
     asm volatile("mbarrier.init.shared::cta.b64 [%0], 1;" ::"r"(ctc_smem_u32(&M.mbar)) : "memory");
     asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
-  }
-  __syncthreads();
-  if (tid < 32) ct_pose_request_warp(T, S, false);
-  __syncthreads();
-  ctc_cluster_sync();  // every CTA's mbarrier exists before the first multicast copy can signal it
-  while (!S.done) {
-    const int l = S.lvl;
-    // ---- level change: stage the plane with TMA if the host encoded its map (one multicast copy issued by CTA 0 lands in every CTA's
-    // shared memory); the host decides, so the kernel never issues a copy on a zeroed descriptor
-    const bool fits = T.staged[l] != 0;
-    if (fits && staged_lvl != l) {
-      const unsigned bytes = (unsigned)(T.w[l] * T.h[l] * sizeof(float4));
-      if (tid == 0) asm volatile("mbarrier.arrive.expect_tx.shared::cta.b64 _, [%0], %1;" ::"r"(ctc_smem_u32(&M.mbar)), "r"(bytes) : "memory");
-      ctc_cluster_sync();  // all barriers armed (and nobody still reads the previous level's plane)
-      if (rank == 0 && tid == 0) {
-        const unsigned short mask = (unsigned short)((1u << NC) - 1u);
-        asm volatile(
-            "cp.async.bulk.tensor.2d.shared::cluster.global.mbarrier::complete_tx::bytes.multicast::cluster [%0], [%1, {%3, %4}], [%2], %5;" ::"r"(
-                ctc_smem_u32(M.plane)),
-            "l"(&maps.lvl[l]), "r"(ctc_smem_u32(&M.mbar)), "r"(0), "r"(0), "h"(mask)
-            : "memory");
-      }
-      {  // wait for the bytes (try_wait suspends the thread between probes)
-        const unsigned mb = ctc_smem_u32(&M.mbar);
-        unsigned done = 0;
-        while (!done)
-          asm volatile("{\n\t.reg .pred p;\n\tmbarrier.try_wait.parity.shared::cta.b64 p, [%1], %2;\n\tselp.b32 %0, 1, 0, p;\n\t}" : "=r"(done) : "r"(mb), "r"(mphase) : "memory");
-      }
-      mphase ^= 1u;
-      staged_lvl = l;
+    if constexpr (TRIES) {   // Vec5::Constant(NAN), haveOneGood = false, trackingGoodRet = false (L406-413)
+      CTLoop& W = M.loop;
+      for (int i = 0; i < 5; i++) W.achieved[i] = __longlong_as_double(0x7ff8000000000000ll);
+      W.pevals = 0; W.haveOneGood = 0; W.winner = -1; W.trackingGood = 0; W.tries = 0; W.stop = 0;
     }
-    // ---- one evaluation: calcRes + calcGSSSE at the requested pose
-    CTParams P;
+  }
+  // the staged plane, its mbarrier phase and the cached reference points stay valid from one try to the next: the frame is the same
+  for (int kt = 0;; kt++) {   // one track per pass; the plain kernels make one pass
+    if (tid == 0) {
+      const double* R0 = TRIES ? Q->pose[kt] : T.R0;
+      const double* t0 = TRIES ? Q->pose[kt] + 9 : T.t0;
+      for (int i = 0; i < 9; i++) S.R[i] = R0[i];
+      for (int i = 0; i < 3; i++) S.t[i] = t0[i];
+      S.a = T.a0; S.b = T.b0;
+      for (int i = 0; i < 5; i++) S.lastResiduals[i] = __longlong_as_double(0x7ff8000000000000ll);  // NAN
+      for (int i = 0; i < 3; i++) S.flow[i] = 1000;
+      for (int i = 0; i < 5; i++) S.minRes[i] = TRIES ? M.loop.achieved[i] : T.minRes[i];
+      S.haveRepeated = 0; S.iterations = 0; S.evaluations = 0; S.done = 0; S.good = 0; S.status = 0; S.cur = 0; S.need_solve = 0; S.pevals = 0;
+      S.lvl = T.coarsest;
+      ct_begin_level(T, S);
+    }
+    __syncthreads();
+    if (tid < 32) ct_pose_request_warp(T, S, false);
+    __syncthreads();
+    if (kt == 0) ctc_cluster_sync();  // every CTA's mbarrier exists before the first multicast copy can signal it
+    while (!S.done) {
+      const int l = S.lvl;
+      // ---- level change: stage the plane with TMA if the host encoded its map (one multicast copy issued by CTA 0 lands in every CTA's
+      // shared memory); the host decides, so the kernel never issues a copy on a zeroed descriptor
+      const bool fits = T.staged[l] != 0;
+      if (fits && staged_lvl != l) {
+        const unsigned bytes = (unsigned)(T.w[l] * T.h[l] * sizeof(float4));
+        if (tid == 0) asm volatile("mbarrier.arrive.expect_tx.shared::cta.b64 _, [%0], %1;" ::"r"(ctc_smem_u32(&M.mbar)), "r"(bytes) : "memory");
+        ctc_cluster_sync();  // all barriers armed (and nobody still reads the previous level's plane)
+        if (rank == 0 && tid == 0) {
+          const unsigned short mask = (unsigned short)((1u << NC) - 1u);
+          asm volatile(
+              "cp.async.bulk.tensor.2d.shared::cluster.global.mbarrier::complete_tx::bytes.multicast::cluster [%0], [%1, {%3, %4}], [%2], %5;" ::"r"(
+                  ctc_smem_u32(M.plane)),
+              "l"(&maps.lvl[l]), "r"(ctc_smem_u32(&M.mbar)), "r"(0), "r"(0), "h"(mask)
+              : "memory");
+        }
+        {  // wait for the bytes (try_wait suspends the thread between probes)
+          const unsigned mb = ctc_smem_u32(&M.mbar);
+          unsigned done = 0;
+          while (!done)
+            asm volatile("{\n\t.reg .pred p;\n\tmbarrier.try_wait.parity.shared::cta.b64 p, [%1], %2;\n\tselp.b32 %0, 1, 0, p;\n\t}" : "=r"(done) : "r"(mb), "r"(mphase) : "memory");
+        }
+        mphase ^= 1u;
+        staged_lvl = l;
+      }
+      // ---- one evaluation: calcRes + calcGSSSE at the requested pose
+      CTParams P;
 #pragma unroll
-    for (int i = 0; i < 9; i++) { P.RKi[i] = S.RKi[i]; P.Ki[i] = T.Ki[l][i]; }
+      for (int i = 0; i < 9; i++) { P.RKi[i] = S.RKi[i]; P.Ki[i] = T.Ki[l][i]; }
 #pragma unroll
-    for (int i = 0; i < 3; i++) P.t[i] = S.tf[i];
-    P.fx = T.fx[l]; P.fy = T.fy[l]; P.cx = T.cx[l]; P.cy = T.cy[l];
-    P.affa = S.affLL[0]; P.affb = S.affLL[1]; P.a_gs = S.affLL[0]; P.b0 = (float)T.ref_b;
-    P.cutoff = S.cutoff; P.huber = T.huber; P.maxEnergy = 2 * T.huber * S.cutoff - T.huber * T.huber;
-    P.w = T.w[l]; P.h = T.h[l]; P.n = T.n[l]; P.lvl = l; P.want_gs = 1;
-    float v[64];
+      for (int i = 0; i < 3; i++) P.t[i] = S.tf[i];
+      P.fx = T.fx[l]; P.fy = T.fy[l]; P.cx = T.cx[l]; P.cy = T.cy[l];
+      P.affa = S.affLL[0]; P.affb = S.affLL[1]; P.a_gs = S.affLL[0]; P.b0 = (float)T.ref_b;
+      P.cutoff = S.cutoff; P.huber = T.huber; P.maxEnergy = 2 * T.huber * S.cutoff - T.huber * T.huber;
+      P.w = T.w[l]; P.h = T.h[l]; P.n = T.n[l]; P.lvl = l; P.want_gs = 1;
+      float v[64];
 #pragma unroll
-    for (int k = 0; k < 64; k++) v[k] = 0.f;
-    const int stride = (int)NC * CTC_THREADS, first = (int)rank * CTC_THREADS + tid;
-    if (cached_lvl != l) {  // the level's reference points of this thread stay in registers for all evaluations of the level
+      for (int k = 0; k < 64; k++) v[k] = 0.f;
+      const int stride = (int)NC * CTC_THREADS, first = (int)rank * CTC_THREADS + tid;
+      if (cached_lvl != l) {  // the level's reference points of this thread stay in registers for all evaluations of the level
+#pragma unroll
+        for (int k = 0; k < CTC_SLOTS; k++) {
+          const int i = first + k * stride;
+          if (i < P.n) { pts[k] = make_float4(__ldg(T.u[l] + i), __ldg(T.v[l] + i), __ldg(T.id[l] + i), __ldg(T.col[l] + i)); }
+        }
+        cached_lvl = l;
+      }
 #pragma unroll
       for (int k = 0; k < CTC_SLOTS; k++) {
         const int i = first + k * stride;
-        if (i < P.n) { pts[k] = make_float4(__ldg(T.u[l] + i), __ldg(T.v[l] + i), __ldg(T.id[l] + i), __ldg(T.col[l] + i)); }
+        if (i < P.n) {
+          if (fits) ct_eval_accumulate<true>(P, i, pts[k].x, pts[k].y, pts[k].z, pts[k].w, T.img[l], reinterpret_cast<const float4*>(M.plane), v);
+          else ct_eval_accumulate<false>(P, i, pts[k].x, pts[k].y, pts[k].z, pts[k].w, T.img[l], nullptr, v);
+        }
       }
-      cached_lvl = l;
-    }
-#pragma unroll
-    for (int k = 0; k < CTC_SLOTS; k++) {
-      const int i = first + k * stride;
-      if (i < P.n) {
-        if (fits) ct_eval_accumulate<true>(P, i, pts[k].x, pts[k].y, pts[k].z, pts[k].w, T.img[l], reinterpret_cast<const float4*>(M.plane), v);
-        else ct_eval_accumulate<false>(P, i, pts[k].x, pts[k].y, pts[k].z, pts[k].w, T.img[l], nullptr, v);
+      for (int i = first + CTC_SLOTS * stride; i < P.n; i += stride) {  // more points than register slots: stream the rest
+        if (fits) ct_eval_accumulate<true>(P, i, __ldg(T.u[l] + i), __ldg(T.v[l] + i), __ldg(T.id[l] + i), __ldg(T.col[l] + i), T.img[l], reinterpret_cast<const float4*>(M.plane), v);
+        else ct_eval_accumulate<false>(P, i, __ldg(T.u[l] + i), __ldg(T.v[l] + i), __ldg(T.id[l] + i), __ldg(T.col[l] + i), T.img[l], nullptr, v);
       }
-    }
-    for (int i = first + CTC_SLOTS * stride; i < P.n; i += stride) {  // more points than register slots: stream the rest
-      if (fits) ct_eval_accumulate<true>(P, i, __ldg(T.u[l] + i), __ldg(T.v[l] + i), __ldg(T.id[l] + i), __ldg(T.col[l] + i), T.img[l], reinterpret_cast<const float4*>(M.plane), v);
-      else ct_eval_accumulate<false>(P, i, __ldg(T.u[l] + i), __ldg(T.v[l] + i), __ldg(T.id[l] + i), __ldg(T.col[l] + i), T.img[l], nullptr, v);
-    }
-    // ---- CTA: fp64 sum over the warps, pushed into EVERY CTA's exchange slot through distributed shared memory
-    const double bs = ct_block_sum<CTC_THREADS / 32>(v, M.red);
-    if (tid < CT_NRED) {
-      const unsigned local = ctc_smem_u32(&M.xch[par][rank][tid]);
-      for (unsigned c = 0; c < NC; c++) {
-        unsigned remote;
-        asm volatile("mapa.shared::cluster.u32 %0, %1, %2;" : "=r"(remote) : "r"(local), "r"(c));
-        asm volatile("st.shared::cluster.f64 [%0], %1;" ::"r"(remote), "d"(bs) : "memory");
+      // ---- CTA: fp64 sum over the warps, pushed into EVERY CTA's exchange slot through distributed shared memory
+      const double bs = ct_block_sum<CTC_THREADS / 32>(v, M.red);
+      if (tid < CT_NRED) {
+        const unsigned local = ctc_smem_u32(&M.xch[par][rank][tid]);
+        for (unsigned c = 0; c < NC; c++) {
+          unsigned remote;
+          asm volatile("mapa.shared::cluster.u32 %0, %1, %2;" : "=r"(remote) : "r"(local), "r"(c));
+          asm volatile("st.shared::cluster.f64 [%0], %1;" ::"r"(remote), "d"(bs) : "memory");
+        }
       }
+      ctc_cluster_sync();  // release / acquire at cluster scope: every CTA's partials are visible in every CTA's shared memory
+      if (tid < CT_NRED) {
+        double sm = 0.0;
+        for (unsigned c = 0; c < NC; c++) sm += M.xch[par][c][tid];  // rank order: bit-identical in every CTA
+        M.s_sum[tid] = sm;
+      }
+      par ^= 1;
+      __syncthreads();
+      ct_finish_parallel(M.s_sum, S.res[S.cur ^ 1], S.H[S.cur ^ 1], S.bb[S.cur ^ 1], tid);
+      __syncthreads();
+      if (tid < 32) ct_advance_warp(T, S);
+      __syncthreads();
     }
-    ctc_cluster_sync();  // release / acquire at cluster scope: every CTA's partials are visible in every CTA's shared memory
-    if (tid < CT_NRED) {
-      double sm = 0.0;
-      for (unsigned c = 0; c < NC; c++) sm += M.xch[par][c][tid];  // rank order: bit-identical in every CTA
-      M.s_sum[tid] = sm;
+    if constexpr (!TRIES) {
+      break;
+    } else {
+      if (tid == 0) ct_tries_step(*Q, M.loop, S, kt);
+      __syncthreads();
+      if (M.loop.stop || kt + 1 == Q->n) break;   // the same in every CTA of the cluster
     }
-    par ^= 1;
-    __syncthreads();
-    ct_finish_parallel(M.s_sum, S.res[S.cur ^ 1], S.H[S.cur ^ 1], S.bb[S.cur ^ 1], tid);
-    __syncthreads();
-    if (tid < 32) ct_advance_warp(T, S);
-    __syncthreads();
   }
   ctc_cluster_sync();  // nobody leaves while a peer may still write into its shared memory
   if (rank == 0 && tid == 0) {
-    double* o = T.out;
-    const bool ok = (S.status == 0);   // an aborted track returns the input pose, like the reference's early return
-    for (int i = 0; i < 9; i++) o[i] = ok ? S.R[i] : T.R0[i];
-    for (int i = 0; i < 3; i++) o[9 + i] = ok ? S.t[i] : T.t0[i];
-    o[12] = ok ? S.a : T.a0; o[13] = ok ? S.b : T.b0;
-    for (int i = 0; i < 5; i++) o[14 + i] = S.lastResiduals[i];
-    for (int i = 0; i < 3; i++) o[19 + i] = S.flow[i];
-    o[22] = S.good; o[23] = S.iterations; o[24] = S.evaluations; o[25] = S.status; o[26] = S.pevals;
+    if constexpr (TRIES) {   // L491-497 when no try was good: try 0's pose, aff_last_2_l, zero flow
+      const CTLoop& W = M.loop;
+      dmv_ct_tries_result* o = Q->out;
+      const bool one = W.haveOneGood != 0;
+      for (int i = 0; i < 9; i++) o->R[i] = one ? W.R[i] : Q->pose[0][i];
+      for (int i = 0; i < 3; i++) o->t[i] = one ? W.t[i] : Q->pose[0][9 + i];
+      o->a = one ? W.a : T.a0; o->b = one ? W.b : T.b0;
+      for (int i = 0; i < 5; i++) { o->achievedRes[i] = W.achieved[i]; o->lastResiduals[i] = S.lastResiduals[i]; }
+      for (int i = 0; i < 3; i++) { o->flowVecs[i] = one ? W.flowVecs[i] : 0.0; o->flowIndicators[i] = S.flow[i]; }
+      o->trackingGood = W.trackingGood; o->haveOneGood = W.haveOneGood; o->winner = one ? W.winner : -1;
+      o->tries = W.tries; o->tries_started = W.tries;
+      T.out[26] = W.pevals;   // dmv_ct_last_point_evaluations
+    } else {
+      double* o = T.out;
+      const bool ok = (S.status == 0);   // an aborted track returns the input pose, like the reference's early return
+      for (int i = 0; i < 9; i++) o[i] = ok ? S.R[i] : T.R0[i];
+      for (int i = 0; i < 3; i++) o[9 + i] = ok ? S.t[i] : T.t0[i];
+      o[12] = ok ? S.a : T.a0; o[13] = ok ? S.b : T.b0;
+      for (int i = 0; i < 5; i++) o[14 + i] = S.lastResiduals[i];
+      for (int i = 0; i < 3; i++) o[19 + i] = S.flow[i];
+      o[22] = S.good; o[23] = S.iterations; o[24] = S.evaluations; o[25] = S.status; o[26] = S.pevals;
+    }
   }
 }
 
 __global__ void __launch_bounds__(CTC_THREADS, 1) ct_track_cluster_kernel(const __grid_constant__ CTTrack T, const __grid_constant__ CTMaps maps) {
-  ct_track_cluster(T, maps);
+  ct_track_cluster<false>(T, maps, nullptr);
 }
 
 // dmv_ct_track_many: cluster i tracks member i, independently of every other cluster (no inter-cluster synchronisation, so clusters beyond
@@ -650,7 +733,11 @@ static_assert(sizeof(CTTrackMany) <= 32764, "CTTrackMany exceeds the 32,764-byte
 
 __global__ void __launch_bounds__(CTC_THREADS, 1) ct_track_many_kernel(const __grid_constant__ CTTrackMany B) {
   const unsigned i = ctc_cluster_id();
-  ct_track_cluster(B.T[i], B.maps[i]);
+  ct_track_cluster<false>(B.T[i], B.maps[i], nullptr);
+}
+
+__global__ void __launch_bounds__(CTC_THREADS, 1) ct_track_tries_kernel(const __grid_constant__ CTTries Q) {
+  ct_track_cluster<true>(Q.T, Q.maps, &Q);
 }
 
 }  // namespace dmv
@@ -732,7 +819,7 @@ int dmv_ct_destroy(dmv_ct* c) {
   for (int l = 0; l < DMV_MAX_PYR_LEVELS; l++) {
     cudaFree(c->d_img[l]); cudaFree(c->d_gray[l]); cudaFree(c->d_u[l]); cudaFree(c->d_v[l]); cudaFree(c->d_id[l]); cudaFree(c->d_col[l]);
   }
-  cudaFree(c->d_stage); cudaFree(c->d_partial); cudaFree(c->d_ticket); cudaFree(c->d_out);
+  cudaFree(c->d_stage); cudaFree(c->d_partial); cudaFree(c->d_ticket); cudaFree(c->d_out); cudaFreeHost(c->h_tries);
   cudaFreeHost(c->h_out); cudaFreeHost(c->h_scratch); cudaFree(c->d_ip); cudaFreeHost(c->h_ip);
   cd_free(c->cd);
   cudaFree(c->d_remap); cudaFree(c->d_G); cudaFree(c->d_vigInv); cudaFree(c->d_raw);
@@ -939,8 +1026,8 @@ static int ct_track_params(dmv_ct* c, const dmv_ct_track_args* in, CTTrack& T) {
 }
 
 // the handle's cluster size, probed on its first track (on the handle's device): the largest cluster the device schedules for
-// ct_track_cluster_kernel (16 needs the non-portable opt-in).  ct_track_many_kernel has the same block, shared memory and launch bounds, so
-// the probed size holds for it too; the probe opts both kernels in.
+// ct_track_cluster_kernel (16 needs the non-portable opt-in).  ct_track_many_kernel and ct_track_tries_kernel have the same block, shared
+// memory and launch bounds, so the probed size holds for them too; the probe opts all three kernels in.
 static int ct_probe_cluster(dmv_ct* c) {
   if (c->cluster_size == 0) {
     c->cluster_size = -1;
@@ -954,8 +1041,10 @@ static int ct_probe_cluster(dmv_ct* c) {
     if (ct_make_tensor_maps(c) == DMV_OK) {
       CK(cudaFuncSetAttribute(ct_track_cluster_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)sizeof(CTCSmem)));
       CK(cudaFuncSetAttribute(ct_track_many_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)sizeof(CTCSmem)));
+      CK(cudaFuncSetAttribute(ct_track_tries_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)sizeof(CTCSmem)));
       cudaFuncSetAttribute(ct_track_cluster_kernel, cudaFuncAttributeNonPortableClusterSizeAllowed, 1);
       cudaFuncSetAttribute(ct_track_many_kernel, cudaFuncAttributeNonPortableClusterSizeAllowed, 1);
+      cudaFuncSetAttribute(ct_track_tries_kernel, cudaFuncAttributeNonPortableClusterSizeAllowed, 1);
       cudaGetLastError();
       for (int nc : {16, 8, 4}) {
         if (want_nc && nc != want_nc) continue;
@@ -1054,6 +1143,45 @@ int dmv_ct_track_many(dmv_ct* const* handles, int n, const dmv_ct_track_args* in
     handles[i]->staging_busy = false;   // each member's uploads completed before the kernel started
     ct_read_result(handles[i], &out[i]);
   }
+  return DMV_OK;
+}
+
+// FullSystem::trackNewCoarse's try loop (FullSystem.cpp:L412-506, visual-only) in one launch: see ct_track_tries_kernel
+int dmv_ct_track_tries(dmv_ct* c, const dmv_ct_tries_args* in, dmv_ct_tries_result* out) {
+  if (!c || !in || !out) return set_error(DMV_ERR_INVALID, "null argument");
+  if (in->n < 1 || in->n > DMV_CT_MAX_TRIES) return set_error(DMV_ERR_INVALID, "n = %d: expected 1 to %d tries", in->n, DMV_CT_MAX_TRIES);
+  if (!in->R || !in->t) return set_error(DMV_ERR_INVALID, "null R / t");
+  dmv_ct_track_args a;   // try 0 with minResForAbort NaN: dmv_ct_track's checks and descriptors
+  std::memcpy(a.R, in->R, sizeof(a.R));
+  std::memcpy(a.t, in->t, sizeof(a.t));
+  a.a = in->a; a.b = in->b; a.ref_a = in->ref_a; a.ref_b = in->ref_b;
+  a.ref_exposure = in->ref_exposure; a.new_exposure = in->new_exposure;
+  a.coarseCutoffTH = in->coarseCutoffTH; a.affineOptModeA = in->affineOptModeA; a.affineOptModeB = in->affineOptModeB;
+  a.coarsestLvl = in->coarsestLvl;
+  for (int i = 0; i < 5; i++) a.minResForAbort[i] = NAN;   // unused: each try aborts against the loop's achievedRes
+  std::unique_ptr<CTTries> Q(new CTTries());
+  int rc = ct_track_params(c, &a, Q->T);
+  if (rc != DMV_OK) return rc;
+  CK(cudaSetDevice(c->device));
+  rc = ct_probe_cluster(c);
+  if (rc != DMV_OK) return rc;
+  if (!c->h_tries) CK(cudaMallocHost(&c->h_tries, sizeof(dmv_ct_tries_result)));
+  for (int l = 0; l < DMV_MAX_PYR_LEVELS; l++) Q->T.staged[l] = c->staged[l];
+  Q->maps = *c->maps;
+  for (int k = 0; k < in->n; k++) {
+    for (int i = 0; i < 9; i++) Q->pose[k][i] = in->R[9 * k + i];
+    for (int i = 0; i < 3; i++) Q->pose[k][9 + i] = in->t[3 * k + i];
+  }
+  Q->n = in->n;
+  Q->reTrackThreshold = in->reTrackThreshold;
+  Q->lastCoarseRMSE0 = in->lastCoarseRMSE0;
+  Q->out = c->h_tries;
+  CTClusterLaunch q(c->cluster_size, 1, c->stream);
+  CK(cudaLaunchKernelEx(&q.cfg, ct_track_tries_kernel, *Q));
+  c->launches++;
+  CK(cudaStreamSynchronize(c->stream));
+  c->staging_busy = false;
+  *out = *c->h_tries;
   return DMV_OK;
 }
 

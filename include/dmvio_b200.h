@@ -424,6 +424,43 @@ int dmv_ct_track(dmv_ct* ct, const dmv_ct_track_args* in, dmv_ct_track_result* o
  * the message names two such handles); and dmv_ct_track's own errors for any member, with the member's index in the message. */
 #define DMV_CT_TRACK_MANY_MAX 16
 int dmv_ct_track_many(dmv_ct* const* handles, int n, const dmv_ct_track_args* in, dmv_ct_track_result* out);
+/* The motion-hypothesis loop of FullSystem::trackNewCoarse (FullSystem.cpp:L412-506, visual-only: setting_useIMU false) in ONE launch: the
+ * tries lastF_2_fh_tries (built by the caller, L364-402) tracked with trackNewestCoarse one after the other, each with the best residuals
+ * so far (achievedRes) as its minResForAbort, until the first try whose achievedRes[0] < lastCoarseRMSE0 * reTrackThreshold.
+ * Every field of out is bit-identical to that loop run with one dmv_ct_track per try on this handle: the winner test
+ * (L467), the take-over of achievedRes with its NaN rules (L476-483), the break (L486), the fallback when no try is good (L491-497: try 0's
+ * pose, (a, b) and zero flow) and CoarseTracker's lastResiduals / lastFlowIndicators after the last try the loop ran (lastResiduals is
+ * reset to NaN at the start of every try, CoarseTracker.cpp:L551).
+ * The tries run one after the other on one thread-block cluster of the handle's probed size, with the loop's bookkeeping on the device
+ * between them; tries_started equals tries, and dmv_ct_last_point_evaluations afterwards reports the sum over the tries the loop ran.
+ * Ordered on the handle's stream behind queued uploads; one synchronisation; dmv_ct_kernel_launch_count + 1.  The handle's frame,
+ * reference and probed cluster size are unchanged, and a later dmv_ct_track behaves as before.  One pinned result (264 bytes) is allocated
+ * on first use.
+ * Errors, all before anything is launched and with out untouched: DMV_ERR_INVALID for n outside 1..DMV_CT_MAX_TRIES, a NULL pointer, and
+ * dmv_ct_track's own errors (coarsestLvl out of range, missing intrinsics, a cluster size the device cannot schedule). */
+#define DMV_CT_MAX_TRIES 32
+typedef struct dmv_ct_tries_args {
+  int n;                         /* 1..DMV_CT_MAX_TRIES, in lastF_2_fh_tries order */
+  const double* R;               /* n*9 row-major refToNew per try */
+  const double* t;               /* n*3 */
+  double a, b;                   /* aff_last_2_l: initial aff_g2l of every try */
+  double ref_a, ref_b;           /* lastRef_aff_g2l */
+  float ref_exposure, new_exposure, coarseCutoffTH, affineOptModeA, affineOptModeB;   /* as dmv_ct_track_args */
+  int coarsestLvl;               /* pyrLevelsUsed-1 in the reference */
+  double lastCoarseRMSE0;        /* FullSystem::lastCoarseRMSE[0] (100 at construction) */
+  float reTrackThreshold;        /* setting_reTrackThreshold = 1.5 */
+} dmv_ct_tries_args;
+typedef struct dmv_ct_tries_result {
+  double R[9], t[3], a, b;       /* lastF_2_fh, aff_g2l: the winner's, else try 0's input pose and (a, b) */
+  double achievedRes[5];         /* becomes lastCoarseRMSE */
+  double flowVecs[3];            /* the winner's lastFlowIndicators, else 0 0 0 */
+  double lastResiduals[5], flowIndicators[3];  /* CoarseTracker state after the last try the loop ran */
+  int trackingGood;              /* trackingGoodRet */
+  int haveOneGood, winner;       /* winner = index of the try taken, -1 if none */
+  int tries;                     /* tryIterations: tries the sequential loop runs */
+  int tries_started;             /* tries the device began (= tries: they run in order) */
+} dmv_ct_tries_result;
+int dmv_ct_track_tries(dmv_ct* ct, const dmv_ct_tries_args* in, dmv_ct_tries_result* out);
 
 /* ------------------------------------------------------------------------------------------------
  * Immature-point tracing  ==  ImmaturePoint::traceOn (FullSystem/ImmaturePoint.cpp:L77-437) for all immature points of ONE host
@@ -529,7 +566,8 @@ int dmv_ct_make_new_traces(dmv_ct* ct, const dmv_new_traces_args* a);
 int dmv_ct_set_timing(dmv_ct* ct, int enable);
 int dmv_ct_last_timing(dmv_ct* ct, float ms[4]);
 int dmv_ct_kernel_launch_count(dmv_ct* ct, long long* n);
-int dmv_ct_last_point_evaluations(dmv_ct* ct, double* n);   /* sum over the last dmv_ct_track's evaluations of the level's reference-point count */
+int dmv_ct_last_point_evaluations(dmv_ct* ct, double* n);   /* sum over the last dmv_ct_track's evaluations of the level's reference-point count
+                                                               (after dmv_ct_track_tries: over its tries) */
 
 /* ------------------------------------------------------------------------------------------------
  * Coarse-initialiser handle  ==  the GPU side of CoarseInitializer::calcResAndGS (FullSystem/CoarseInitializer.{h,cpp})
