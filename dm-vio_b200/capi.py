@@ -19,6 +19,8 @@ vp = C.c_void_p
 
 MAX_FRAMES = 8
 PRECALC_FLOATS = 32
+# dmv_status (include/dmvio_b200.h)
+DMV_OK, DMV_ERR_INVALID, DMV_ERR_NO_DEVICE, DMV_ERR_CUDA, DMV_ERR_STATE, DMV_ERR_NCCL, DMV_ERR_TIMEOUT = 0, -1, -2, -3, -4, -5, -6
 
 
 class DmvError(RuntimeError):
@@ -203,100 +205,123 @@ def lib():
     if _LIB is None:
         if not os.path.exists(LIB_PATH):
             raise DmvError(f"{LIB_PATH} is missing: build it with `make -C dm-vio_b200` (python -c 'import __graft_entry__ as g; g.build()')")
-        L = C.CDLL(LIB_PATH)
-        L.dmv_last_error.restype = C.c_char_p
-        L.dmv_version.restype = C.c_char_p
-        L.dmv_ba_create.argtypes = [C.POINTER(BAConfig), C.POINTER(vp)]
-        L.dmv_ba_destroy.argtypes = [vp]
-        L.dmv_ba_set_params.argtypes = [vp, C.POINTER(BAParams)]
-        L.dmv_ba_default_params.argtypes = [C.POINTER(BAParams)]
-        L.dmv_ba_upload_frame.argtypes = [vp, C.c_int, f32p]
-        L.dmv_ba_upload_image.argtypes = [vp, C.c_int, f32p]
-        L.dmv_ba_set_window.argtypes = [vp, C.c_int, vp]
-        L.dmv_ba_set_points.argtypes = [vp, C.c_int, i32p, f32p, f32p, f32p, vp, f32p, f32p, vp]
-        L.dmv_ba_set_residuals.argtypes = [vp, C.c_int, i32p, i32p, vp, vp]
-        L.dmv_ba_set_adjoints.argtypes = [vp, f64p, f64p]
-        L.dmv_ba_set_state.argtypes = [vp, C.POINTER(BAState)]
-        L.dmv_ba_linearize.argtypes = [vp, C.POINTER(BALinResult)]
-        L.dmv_ba_get_residual_outputs.argtypes = [vp, vp, vp, vp, vp, vp]
-        L.dmv_ba_get_target_energies.argtypes = [vp, C.c_int, f32p, C.c_int, C.POINTER(C.c_int)]
-        L.dmv_ba_apply_res.argtypes = [vp]
-        L.dmv_ba_accumulate.argtypes = [vp, f64p, f64p, f64p, f64p, C.POINTER(C.c_int)]
-        L.dmv_ba_get_point_outputs.argtypes = [vp, vp, vp, vp, vp, vp]
-        L.dmv_ba_resubstitute.argtypes = [vp, f64p, vp, C.c_int, f64p]
-        L.dmv_ba_backup_points.argtypes = [vp]
-        L.dmv_ba_restore_points.argtypes = [vp]
-        L.dmv_ba_get_idepth.argtypes = [vp, vp, vp]
-        L.dmv_ba_gn_step.argtypes = [vp, vp, C.POINTER(BAState), C.POINTER(BALinResult), f64p]
-        L.dmv_nccl_unique_id.argtypes = [vp]
-        L.dmv_ba_comm_init.argtypes = [vp, C.c_int, C.c_int, vp]
-        L.dmv_ba_activate_points.argtypes = [vp, C.POINTER(BAActivateArgs)]
-        L.dmv_ba_select_activation.argtypes = [vp, C.POINTER(BASelectArgs)]
-        L.dmv_ba_marginalize_points.argtypes = [vp, C.POINTER(BAMargArgs)]
-        L.dmv_ba_drop_residuals.argtypes = [vp, C.c_int, i32p]
-        L.dmv_ba_reset_oob.argtypes = [vp]
-        L.dmv_ba_p2p_export.argtypes = [vp, vp]
-        L.dmv_ba_p2p_import.argtypes = [vp, C.c_int, C.c_int, vp]
-        L.dmv_ba_last_timing.argtypes = [vp, f32p]
-        L.dmv_ba_bench_device.argtypes = [vp, vp, C.c_int, C.c_int, C.POINTER(C.c_float), C.POINTER(C.c_float)]
-        L.dmv_ba_bench_phases.argtypes = [vp, vp, C.c_int, C.c_int, C.c_int, vp, C.POINTER(C.c_int), f32p]
-        L.dmv_ba_kernel_launch_count.argtypes = [vp, C.POINTER(C.c_longlong)]
-        L.dmv_ba_set_timing.argtypes = [vp, C.c_int]
-        L.dmv_ba_bench_e2e.argtypes = [vp, vp, C.POINTER(BAState), C.c_int, C.POINTER(C.c_double)]
-        L.dmv_ba_io_bytes.argtypes = [vp, C.POINTER(C.c_longlong), C.POINTER(C.c_longlong)]
-        L.dmv_ba_get_solve_HdiF.argtypes = [vp, f32p]
-        L.dmv_ba_adopt_frame.argtypes = [vp, C.c_int, vp]
-        L.dmv_ba_batch_create.argtypes = [vp, C.c_int, C.POINTER(vp)]
-        L.dmv_ba_batch_destroy.argtypes = [vp]
-        L.dmv_ba_batch_gn_step.argtypes = [vp, vp, vp, vp, vp]
-        L.dmv_ba_batch_set_timing.argtypes = [vp, C.c_int]
-        L.dmv_ba_batch_last_kernel_ms.argtypes = [vp, C.POINTER(C.c_float)]
-        L.dmv_ba_batch_bench.argtypes = [vp, vp, C.c_int, vp, vp, C.c_int, C.POINTER(C.c_double), C.POINTER(C.c_double)]
-        L.dmv_ct_create.argtypes = [C.POINTER(CTConfig), C.POINTER(vp)]
-        L.dmv_ct_destroy.argtypes = [vp]
-        L.dmv_ct_set_K.argtypes = [vp, C.c_int, C.c_float, C.c_float, C.c_float, C.c_float]
-        L.dmv_ct_set_ref.argtypes = [vp, C.c_int, C.c_int, f32p, f32p, f32p, f32p]
-        L.dmv_ct_make_coarse_depth.argtypes = [vp, C.c_int, f32p, f32p, f32p, f32p, i32p]
-        L.dmv_ct_set_ref_from_ba.argtypes = [vp, vp, i32p]
-        L.dmv_ct_get_ref.argtypes = [vp, C.c_int, C.POINTER(C.c_int), vp, vp, vp, vp]
-        L.dmv_ct_upload_new.argtypes = [vp, C.c_int, f32p]
-        L.dmv_ct_upload_new_image.argtypes = [vp, f32p]
-        L.dmv_ct_set_huber.argtypes = [vp, C.c_float]
-        L.dmv_ct_calc_res_gs.argtypes = [vp, C.c_int, f32p, f32p, f32p, C.c_float, C.c_float, C.c_int, f64p, f64p, f64p, C.POINTER(C.c_int)]
-        L.dmv_ct_track.argtypes = [vp, C.POINTER(CTTrackArgs), C.POINTER(CTTrackResult)]
-        L.dmv_ct_track_many.argtypes = [C.POINTER(vp), C.c_int, C.POINTER(CTTrackArgs), C.POINTER(CTTrackResult)]
-        L.dmv_ct_track_tries.argtypes = [vp, C.POINTER(CTTriesArgs), C.POINTER(CTTriesResult)]
-        L.dmv_ct_init_points.argtypes = [vp, C.c_int, i32p, i32p, f32p, f32p, f32p, f32p, i32p]
-        L.dmv_ct_trace_points.argtypes = [vp, C.POINTER(IPPoints), f32p, f32p, f32p, vp]
-        L.dmv_ct_trace_points_multi.argtypes = [vp, C.c_int, vp, vp, vp]
-        L.dmv_ct_trace_many.argtypes = [C.POINTER(vp), C.c_int, C.POINTER(TraceJob), vp]
-        L.dmv_ct_set_timing.argtypes = [vp, C.c_int]
-        L.dmv_ct_last_timing.argtypes = [vp, f32p]
-        L.dmv_ct_kernel_launch_count.argtypes = [vp, C.POINTER(C.c_longlong)]
-        L.dmv_ct_last_point_evaluations.argtypes = [vp, C.POINTER(C.c_double)]
-        L.dmv_ct_set_undistort.argtypes = [vp, C.POINTER(UndistortConfig)]
-        L.dmv_ct_upload_raw_image.argtypes = [vp, vp, C.c_int, C.c_float, C.c_float]
-        L.dmv_ct_download_frame.argtypes = [vp, C.c_int, f32p]
-        L.dmv_ps_default_settings.restype = None
-        L.dmv_ps_default_settings.argtypes = [C.POINTER(PSSettings)]
-        L.dmv_ip_default_settings.restype = None
-        L.dmv_ip_default_settings.argtypes = [C.POINTER(IPSettings)]
-        L.dmv_ct_make_new_traces.argtypes = [vp, C.POINTER(NewTracesArgs)]
-        L.dmv_ci_create.argtypes = [C.POINTER(CTConfig), C.POINTER(vp)]
-        L.dmv_ci_destroy.argtypes = [vp]
-        L.dmv_ci_set_K.argtypes = [vp, C.c_int, C.c_float, C.c_float, C.c_float, C.c_float]
-        L.dmv_ci_upload_first.argtypes = [vp, C.c_int, vp]
-        L.dmv_ci_upload_new.argtypes = [vp, C.c_int, vp]
-        L.dmv_ci_set_points.argtypes = [vp, C.c_int, C.c_int, vp, vp, vp]
-        L.dmv_ci_calc_res_and_gs.argtypes = [vp, C.POINTER(CIEvalArgs), C.POINTER(CIEvalResult)]
-        L.dmv_ci_kernel_launch_count.argtypes = [vp, C.POINTER(C.c_longlong)]
-        _LIB = L
+        _LIB = _bind(C.CDLL(LIB_PATH))
     return _LIB
 
 
-def check(rc):
+def load(path):
+    """another build of libdmvio_b200.so (e.g. the parent commit's, for an A/B in one process), bound as lib() is"""
+    return _bind(C.CDLL(os.path.abspath(path)))
+
+
+def _bind(L):
+    """declares the signatures of include/dmvio_b200.h on a loaded library.  An entry point that an older build lacks stays undeclared, so
+    calling it raises AttributeError."""
+    for name, t in _RESTYPES.items():
+        if hasattr(L, name):
+            getattr(L, name).restype = t
+    for name, t in _ARGTYPES.items():
+        if hasattr(L, name):
+            getattr(L, name).argtypes = t
+    return L
+
+
+_RESTYPES = {
+    "dmv_last_error": C.c_char_p,
+    "dmv_version": C.c_char_p,
+    "dmv_ps_default_settings": None,
+    "dmv_ip_default_settings": None,
+}
+_ARGTYPES = {
+    "dmv_ba_create": [C.POINTER(BAConfig), C.POINTER(vp)],
+    "dmv_ba_destroy": [vp],
+    "dmv_ba_set_params": [vp, C.POINTER(BAParams)],
+    "dmv_ba_default_params": [C.POINTER(BAParams)],
+    "dmv_ba_upload_frame": [vp, C.c_int, f32p],
+    "dmv_ba_upload_image": [vp, C.c_int, f32p],
+    "dmv_ba_set_window": [vp, C.c_int, vp],
+    "dmv_ba_set_points": [vp, C.c_int, i32p, f32p, f32p, f32p, vp, f32p, f32p, vp],
+    "dmv_ba_set_residuals": [vp, C.c_int, i32p, i32p, vp, vp],
+    "dmv_ba_set_adjoints": [vp, f64p, f64p],
+    "dmv_ba_set_state": [vp, C.POINTER(BAState)],
+    "dmv_ba_linearize": [vp, C.POINTER(BALinResult)],
+    "dmv_ba_get_residual_outputs": [vp, vp, vp, vp, vp, vp],
+    "dmv_ba_get_target_energies": [vp, C.c_int, f32p, C.c_int, C.POINTER(C.c_int)],
+    "dmv_ba_apply_res": [vp],
+    "dmv_ba_accumulate": [vp, f64p, f64p, f64p, f64p, C.POINTER(C.c_int)],
+    "dmv_ba_get_point_outputs": [vp, vp, vp, vp, vp, vp],
+    "dmv_ba_resubstitute": [vp, f64p, vp, C.c_int, f64p],
+    "dmv_ba_backup_points": [vp],
+    "dmv_ba_restore_points": [vp],
+    "dmv_ba_get_idepth": [vp, vp, vp],
+    "dmv_ba_gn_step": [vp, vp, C.POINTER(BAState), C.POINTER(BALinResult), f64p],
+    "dmv_nccl_unique_id": [vp],
+    "dmv_ba_comm_init": [vp, C.c_int, C.c_int, vp],
+    "dmv_ba_activate_points": [vp, C.POINTER(BAActivateArgs)],
+    "dmv_ba_select_activation": [vp, C.POINTER(BASelectArgs)],
+    "dmv_ba_marginalize_points": [vp, C.POINTER(BAMargArgs)],
+    "dmv_ba_drop_residuals": [vp, C.c_int, i32p],
+    "dmv_ba_reset_oob": [vp],
+    "dmv_ba_p2p_export": [vp, vp],
+    "dmv_ba_p2p_import": [vp, C.c_int, C.c_int, vp],
+    "dmv_ba_last_timing": [vp, f32p],
+    "dmv_ba_bench_device": [vp, vp, C.c_int, C.c_int, C.POINTER(C.c_float), C.POINTER(C.c_float)],
+    "dmv_ba_bench_phases": [vp, vp, C.c_int, C.c_int, C.c_int, vp, C.POINTER(C.c_int), f32p],
+    "dmv_ba_kernel_launch_count": [vp, C.POINTER(C.c_longlong)],
+    "dmv_ba_set_timing": [vp, C.c_int],
+    "dmv_ba_bench_e2e": [vp, vp, C.POINTER(BAState), C.c_int, C.POINTER(C.c_double)],
+    "dmv_ba_io_bytes": [vp, C.POINTER(C.c_longlong), C.POINTER(C.c_longlong)],
+    "dmv_ba_get_solve_HdiF": [vp, f32p],
+    "dmv_ba_adopt_frame": [vp, C.c_int, vp],
+    "dmv_ba_batch_create": [vp, C.c_int, C.POINTER(vp)],
+    "dmv_ba_batch_destroy": [vp],
+    "dmv_ba_batch_gn_step": [vp, vp, vp, vp, vp],
+    "dmv_ba_batch_set_timing": [vp, C.c_int],
+    "dmv_ba_batch_last_kernel_ms": [vp, C.POINTER(C.c_float)],
+    "dmv_ba_batch_bench": [vp, vp, C.c_int, vp, vp, C.c_int, C.POINTER(C.c_double), C.POINTER(C.c_double)],
+    "dmv_ct_create": [C.POINTER(CTConfig), C.POINTER(vp)],
+    "dmv_ct_destroy": [vp],
+    "dmv_ct_set_K": [vp, C.c_int, C.c_float, C.c_float, C.c_float, C.c_float],
+    "dmv_ct_set_ref": [vp, C.c_int, C.c_int, f32p, f32p, f32p, f32p],
+    "dmv_ct_make_coarse_depth": [vp, C.c_int, f32p, f32p, f32p, f32p, i32p],
+    "dmv_ct_set_ref_from_ba": [vp, vp, i32p],
+    "dmv_ct_get_ref": [vp, C.c_int, C.POINTER(C.c_int), vp, vp, vp, vp],
+    "dmv_ct_upload_new": [vp, C.c_int, f32p],
+    "dmv_ct_upload_new_image": [vp, f32p],
+    "dmv_ct_set_huber": [vp, C.c_float],
+    "dmv_ct_calc_res_gs": [vp, C.c_int, f32p, f32p, f32p, C.c_float, C.c_float, C.c_int, f64p, f64p, f64p, C.POINTER(C.c_int)],
+    "dmv_ct_track": [vp, C.POINTER(CTTrackArgs), C.POINTER(CTTrackResult)],
+    "dmv_ct_track_many": [C.POINTER(vp), C.c_int, C.POINTER(CTTrackArgs), C.POINTER(CTTrackResult)],
+    "dmv_ct_track_tries": [vp, C.POINTER(CTTriesArgs), C.POINTER(CTTriesResult)],
+    "dmv_ct_init_points": [vp, C.c_int, i32p, i32p, f32p, f32p, f32p, f32p, i32p],
+    "dmv_ct_trace_points": [vp, C.POINTER(IPPoints), f32p, f32p, f32p, vp],
+    "dmv_ct_trace_points_multi": [vp, C.c_int, vp, vp, vp],
+    "dmv_ct_trace_many": [C.POINTER(vp), C.c_int, C.POINTER(TraceJob), vp],
+    "dmv_ct_set_timing": [vp, C.c_int],
+    "dmv_ct_last_timing": [vp, f32p],
+    "dmv_ct_kernel_launch_count": [vp, C.POINTER(C.c_longlong)],
+    "dmv_ct_last_point_evaluations": [vp, C.POINTER(C.c_double)],
+    "dmv_ct_set_undistort": [vp, C.POINTER(UndistortConfig)],
+    "dmv_ct_upload_raw_image": [vp, vp, C.c_int, C.c_float, C.c_float],
+    "dmv_ct_download_frame": [vp, C.c_int, f32p],
+    "dmv_ps_default_settings": [C.POINTER(PSSettings)],
+    "dmv_ip_default_settings": [C.POINTER(IPSettings)],
+    "dmv_ct_make_new_traces": [vp, C.POINTER(NewTracesArgs)],
+    "dmv_ci_create": [C.POINTER(CTConfig), C.POINTER(vp)],
+    "dmv_ci_destroy": [vp],
+    "dmv_ci_set_K": [vp, C.c_int, C.c_float, C.c_float, C.c_float, C.c_float],
+    "dmv_ci_upload_first": [vp, C.c_int, vp],
+    "dmv_ci_upload_new": [vp, C.c_int, vp],
+    "dmv_ci_set_points": [vp, C.c_int, C.c_int, vp, vp, vp],
+    "dmv_ci_calc_res_and_gs": [vp, C.POINTER(CIEvalArgs), C.POINTER(CIEvalResult)],
+    "dmv_ci_kernel_launch_count": [vp, C.POINTER(C.c_longlong)],
+}
+
+
+def check(rc, L=None):
+    """raises DmvError with the message of the library L (default lib()) for a non-zero dmv_status"""
     if rc != 0:
-        raise DmvError(f"dmvio_b200 error {rc}: {lib().dmv_last_error().decode()}")
+        raise DmvError(f"dmvio_b200 error {rc}: {(L or lib()).dmv_last_error().decode()}")
 
 
 def _p(a):
@@ -667,13 +692,18 @@ def ct_trace_many(handles, jobs, settings=None):
 
 
 class CT:
-    def __init__(self, w, h, levels, max_points=65536, device=0):
-        self.L = lib()
+    """a dmv_ct handle.  L: the library it lives in, lib() by default or another build from load()"""
+
+    def __init__(self, w, h, levels, max_points=65536, device=0, L=None):
+        self.L = L or lib()
         cfg = CTConfig(w, h, levels, max_points, device)
         self.h = vp()
-        check(self.L.dmv_ct_create(C.byref(cfg), C.byref(self.h)))
+        self._check(self.L.dmv_ct_create(C.byref(cfg), C.byref(self.h)))
         self.levels = levels
         self.size = (w, h)
+
+    def _check(self, rc):
+        check(rc, self.L)
 
     def close(self):
         if self.h:
@@ -687,26 +717,26 @@ class CT:
             pass
 
     def set_K(self, lvl, fx, fy, cx, cy):
-        check(self.L.dmv_ct_set_K(self.h, lvl, fx, fy, cx, cy))
+        self._check(self.L.dmv_ct_set_K(self.h, lvl, fx, fy, cx, cy))
 
     def set_ref(self, lvl, u, v, idepth, color):
-        check(self.L.dmv_ct_set_ref(self.h, lvl, len(u), _c(u, np.float32), _c(v, np.float32), _c(idepth, np.float32), _c(color, np.float32)))
+        self._check(self.L.dmv_ct_set_ref(self.h, lvl, len(u), _c(u, np.float32), _c(v, np.float32), _c(idepth, np.float32), _c(color, np.float32)))
 
     def upload_new(self, lvl, dIp):
-        check(self.L.dmv_ct_upload_new(self.h, lvl, _c(dIp, np.float32).reshape(-1)))
+        self._check(self.L.dmv_ct_upload_new(self.h, lvl, _c(dIp, np.float32).reshape(-1)))
 
     def upload_new_image(self, img):
-        check(self.L.dmv_ct_upload_new_image(self.h, _c(img, np.float32).reshape(-1)))
+        self._check(self.L.dmv_ct_upload_new_image(self.h, _c(img, np.float32).reshape(-1)))
 
     def set_huber(self, th):
-        check(self.L.dmv_ct_set_huber(self.h, th))
+        self._check(self.L.dmv_ct_set_huber(self.h, th))
 
     def set_undistort(self, wOrg, hOrg, remapX=None, remapY=None, G=None, vignetteInv=None, photometric_mode=0):
         """dmv_ct_set_undistort: the per-sequence tables of Undistort (remapX/remapY None = passthrough, G None = no photometric calibration)"""
         keep = [None if a is None else _c(a, np.float32).reshape(-1) for a in (remapX, remapY, G, vignetteInv)]
         p = [None if a is None else a.ctypes.data for a in keep]
         cfg = UndistortConfig(int(wOrg), int(hOrg), p[0], p[1], p[2], 0 if G is None else len(keep[2]), p[3], int(photometric_mode))
-        check(self.L.dmv_ct_set_undistort(self.h, C.byref(cfg)))
+        self._check(self.L.dmv_ct_set_undistort(self.h, C.byref(cfg)))
 
     def upload_raw_image(self, raw, exposure=1.0, factor=None):
         """dmv_ct_upload_raw_image: a uint8 or uint16 frame of the raw size; factor defaults to the reference's readers' (1, or 1/256 for 16 bit)"""
@@ -715,17 +745,17 @@ class CT:
             raise DmvError("raw frames are uint8 or uint16")
         if factor is None:
             factor = 1.0 if raw.itemsize == 1 else 1.0 / 256
-        check(self.L.dmv_ct_upload_raw_image(self.h, raw.ctypes.data, raw.itemsize, float(exposure), float(factor)))
+        self._check(self.L.dmv_ct_upload_raw_image(self.h, raw.ctypes.data, raw.itemsize, float(exposure), float(factor)))
 
     def download_frame(self, lvl, w, h):
         """dmv_ct_download_frame: dIp[lvl] as an (h_l, w_l, 3) array (w, h = level-0 size)"""
         out = np.zeros(((h >> lvl) * (w >> lvl) * 3), np.float32)
-        check(self.L.dmv_ct_download_frame(self.h, lvl, out))
+        self._check(self.L.dmv_ct_download_frame(self.h, lvl, out))
         return out.reshape(h >> lvl, w >> lvl, 3)
 
     def calc_res_gs(self, lvl, RKi, t, affLL, b0, cutoff, want_gs=True):
         res6 = np.zeros(6); H = np.zeros(64); b = np.zeros(8); n = C.c_int(0)
-        check(self.L.dmv_ct_calc_res_gs(self.h, lvl, _c(RKi, np.float32).reshape(-1), _c(t, np.float32), _c(affLL, np.float32), b0, cutoff,
+        self._check(self.L.dmv_ct_calc_res_gs(self.h, lvl, _c(RKi, np.float32).reshape(-1), _c(t, np.float32), _c(affLL, np.float32), b0, cutoff,
                                         int(want_gs), res6, H, b, C.byref(n)))
         return res6, H.reshape(8, 8), b, n.value
 
@@ -735,7 +765,7 @@ class CT:
         minRes = minResForAbort (None: NaN, never abort); coarsest defaults to the handle's top level."""
         A = _track_args(self.levels, R, t, a, b, ref_a, ref_b, ref_exposure, new_exposure, cutoff, affA, affB, coarsest, minRes)
         r = CTTrackResult()
-        check(self.L.dmv_ct_track(self.h, C.byref(A), C.byref(r)))
+        self._check(self.L.dmv_ct_track(self.h, C.byref(A), C.byref(r)))
         return _track_result(r)
 
     def track_tries(self, R, t, a, b, ref_a=0.0, ref_b=0.0, ref_exposure=1.0, new_exposure=1.0, cutoff=20.0, affA=1e12, affB=1e8, coarsest=None,
@@ -745,33 +775,33 @@ class CT:
         A, keep = _tries_args(self.levels, R, t, a, b, ref_a, ref_b, ref_exposure, new_exposure, cutoff, affA, affB, coarsest, lastCoarseRMSE0,
                               reTrackThreshold)
         r = CTTriesResult()
-        check(self.L.dmv_ct_track_tries(self.h, C.byref(A), C.byref(r)))
+        self._check(self.L.dmv_ct_track_tries(self.h, C.byref(A), C.byref(r)))
         return _tries_result(r)
 
     def point_evaluations(self):
         """reference points evaluated by the last track, summed over its evaluations (dmv_ct_last_point_evaluations)"""
         n = C.c_double(0)
-        check(self.L.dmv_ct_last_point_evaluations(self.h, C.byref(n)))
+        self._check(self.L.dmv_ct_last_point_evaluations(self.h, C.byref(n)))
         return n.value
 
     def make_coarse_depth(self, Ku, Kv, new_idepth, HdiF):
         """makeCoarseDepthL0 on the device with the resident frame as the reference; returns pc_n per level"""
         pc_n = np.zeros(8, np.int32)
-        check(self.L.dmv_ct_make_coarse_depth(self.h, len(Ku), _c(Ku, np.float32), _c(Kv, np.float32), _c(new_idepth, np.float32), _c(HdiF, np.float32), pc_n))
+        self._check(self.L.dmv_ct_make_coarse_depth(self.h, len(Ku), _c(Ku, np.float32), _c(Kv, np.float32), _c(new_idepth, np.float32), _c(HdiF, np.float32), pc_n))
         return pc_n
 
     def set_ref_from_ba(self, ba):
         """setCoarseTrackingRef + makeCoarseDepthL0 from a BA handle on the same device (dmv_ct_set_ref_from_ba): the window's newest frame becomes
         the reference.  ba: a BA, or a raw dmv_ba* (e.g. hostapi.WindowBA.ba_handle()).  Returns pc_n per level."""
         pc_n = np.zeros(8, np.int32)
-        check(self.L.dmv_ct_set_ref_from_ba(self.h, ba.h if isinstance(ba, BA) else ba, pc_n))
+        self._check(self.L.dmv_ct_set_ref_from_ba(self.h, ba.h if isinstance(ba, BA) else ba, pc_n))
         return pc_n
 
     def get_ref(self, lvl):
         n = C.c_int(0)
-        check(self.L.dmv_ct_get_ref(self.h, lvl, C.byref(n), None, None, None, None))
+        self._check(self.L.dmv_ct_get_ref(self.h, lvl, C.byref(n), None, None, None, None))
         a = [np.zeros(n.value, np.float32) for _ in range(4)]
-        check(self.L.dmv_ct_get_ref(self.h, lvl, C.byref(n), *[x.ctypes.data for x in a]))
+        self._check(self.L.dmv_ct_get_ref(self.h, lvl, C.byref(n), *[x.ctypes.data for x in a]))
         return dict(u=a[0], v=a[1], idepth=a[2], color=a[3])
 
     def make_new_traces(self, potential, density=1500.0, recursionsLeft=1, thFactor=1.0, B=None, settings=None, cap=16384, want_map=False):
@@ -798,7 +828,7 @@ class CT:
                           None if m is None else m.ctypes.data)
         rc = self.L.dmv_ct_make_new_traces(self.h, C.byref(a))
         self.last_needed, self.last_potential = n.value, pot.value
-        check(rc)
+        self._check(rc)
         out = dict(points={k: P[k][:n.value] for k in P}, numPointsTotal=npt.value, potential=pot.value)
         if want_map:
             out["map"] = m.reshape(H, W)
@@ -810,7 +840,7 @@ class CT:
         P = dict(u=_c(u, np.float32), v=_c(v, np.float32), color=np.zeros((n, 8), np.float32), weights=np.zeros((n, 8), np.float32),
                  gradH=np.zeros((n, 4), np.float32), energyTH=np.zeros(n, np.float32))
         ok = np.zeros(n, np.int32)
-        check(self.L.dmv_ct_init_points(self.h, n, _c(u, np.int32), _c(v, np.int32), P["color"].reshape(-1), P["weights"].reshape(-1), P["gradH"].reshape(-1),
+        self._check(self.L.dmv_ct_init_points(self.h, n, _c(u, np.int32), _c(v, np.int32), P["color"].reshape(-1), P["weights"].reshape(-1), P["gradH"].reshape(-1),
                                         P["energyTH"], ok))
         P["ok"] = ok.astype(np.uint8)
         P.update(idepth_min=np.zeros(n, np.float32), idepth_max=np.full(n, np.nan, np.float32), quality=np.full(n, 10000, np.float32),
@@ -827,7 +857,7 @@ class CT:
                "lastTraceUV": np.array(P["lastTraceUV"], np.float32, copy=True), "lastTracePixelInterval": np.array(P["lastTracePixelInterval"], np.float32, copy=True)}
         pts = IPPoints(n, *[a.ctypes.data for a in (keep["u"], keep["v"], keep["color"], keep["weights"], keep["gradH"], keep["energyTH"], out["idepth_min"],
                                                      out["idepth_max"], out["quality"], out["status"], out["lastTraceUV"], out["lastTracePixelInterval"])])
-        check(self.L.dmv_ct_trace_points(self.h, C.byref(pts), _c(KRKi, np.float32).reshape(-1), _c(Kt, np.float32), _c(aff, np.float32),
+        self._check(self.L.dmv_ct_trace_points(self.h, C.byref(pts), _c(KRKi, np.float32).reshape(-1), _c(Kt, np.float32), _c(aff, np.float32),
                                               None if settings is None else C.byref(settings)))
         Q = dict(P)
         Q.update(out)
@@ -837,20 +867,20 @@ class CT:
         """sets = [(P, KRKi, Kt, aff), ...]: the immature points of several host keyframes in ONE launch (dmv_ct_trace_points_multi);
         returns the list of updated dicts.  settings: an IPSettings, or None (NULL: defaults)."""
         T = _TraceSets(sets)
-        check(self.L.dmv_ct_trace_points_multi(self.h, T.job.nsets, T.job.sets, T.job.tables14, None if settings is None else C.byref(settings)))
+        self._check(self.L.dmv_ct_trace_points_multi(self.h, T.job.nsets, T.job.sets, T.job.tables14, None if settings is None else C.byref(settings)))
         return T.results()
 
     def set_timing(self, enable=True):
-        check(self.L.dmv_ct_set_timing(self.h, int(enable)))
+        self._check(self.L.dmv_ct_set_timing(self.h, int(enable)))
 
     def last_timing(self):
         ms = np.zeros(4, np.float32)
-        check(self.L.dmv_ct_last_timing(self.h, ms))
+        self._check(self.L.dmv_ct_last_timing(self.h, ms))
         return ms
 
     def launch_count(self):
         n = C.c_longlong(0)
-        check(self.L.dmv_ct_kernel_launch_count(self.h, C.byref(n)))
+        self._check(self.L.dmv_ct_kernel_launch_count(self.h, C.byref(n)))
         return n.value
 
 

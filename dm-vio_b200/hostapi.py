@@ -26,6 +26,7 @@ def _bind(L):
     if True:
         L.dmvh_window_create.restype = vp
         L.dmvh_window_create.argtypes = [C.c_int, C.c_int, C.c_int, C.c_int, C.c_int, f64p]
+        L.dmvh_window_set_setting.argtypes = [vp, C.c_char_p, C.c_double]
         L.dmvh_window_destroy.argtypes = [vp]
         L.dmvh_window_error.restype = C.c_char_p
         L.dmvh_window_error.argtypes = [vp]

@@ -4,7 +4,7 @@ import ctypes as C
 
 import pytest
 
-DMV_OK, DMV_ERR_INVALID, DMV_ERR_NO_DEVICE = 0, -1, -2
+from dmvio_b200.capi import DMV_ERR_INVALID, DMV_ERR_NO_DEVICE, DMV_OK
 
 
 @pytest.fixture(scope="module")

@@ -20,20 +20,13 @@ import pytest
 import torch
 
 import dmvio_b200.hostmath as hm
+from dmvio_b200.capi import DMV_ERR_INVALID, DMV_ERR_STATE
 from helpers import RES_IN, SYSTEM_TAU, check_system, make_case, prior_f, schur_bound, schur_reference
+from gpu_harness import device_capi  # noqa: F401  (the "capi" fixture: every test that takes it needs the device)
 
 pytestmark = pytest.mark.gpu
 
 BATCH_MAX = 64           # ba_device.cuh
-ERR_INVALID, ERR_STATE = -1, -4
-
-
-@pytest.fixture(scope="module")
-def capi():
-    import dmvio_b200.capi as c
-    if c.lib().dmv_device_count() < 1:
-        pytest.fail("no CUDA device visible: GPU tests must run on the H100")
-    return c
 
 
 @pytest.fixture(scope="module")
@@ -392,15 +385,15 @@ def test_refusals_leave_members_untouched(capi, orc, synth, sms):
 
         # ---- dmv_ba_batch_gn_step on the batch of the three members
         st = states(members)
-        _refused(capi, _raw_step(capi, None, xs, st), ERR_INVALID, "null argument")
-        _refused(capi, _raw_step(capi, batch.h, xs, None), ERR_INVALID, "null argument")
+        _refused(capi, _raw_step(capi, None, xs, st), DMV_ERR_INVALID, "null argument")
+        _refused(capi, _raw_step(capi, batch.h, xs, None), DMV_ERR_INVALID, "null argument")
         untouched("null batch / null states")
         st = states(members)
-        _refused(capi, _raw_step(capi, batch.h, xs, st[:2] + [None]), ERR_INVALID, "state 2 is null")
+        _refused(capi, _raw_step(capi, batch.h, xs, st[:2] + [None]), DMV_ERR_INVALID, "state 2 is null")
         untouched("null state of member 2")
         st = states(members)
         st[2].precalc = None
-        _refused(capi, _raw_step(capi, batch.h, xs, st), ERR_INVALID, "state 2: precalc")
+        _refused(capi, _raw_step(capi, batch.h, xs, st), DMV_ERR_INVALID, "state 2: precalc")
         untouched("member 2 without precalc")
 
         # ---- batches with one bad member behind two good ones
@@ -412,11 +405,11 @@ def test_refusals_leave_members_untouched(capi, orc, synth, sms):
             untouched(what)
 
         ba, W, ow = handle(dict(nf=3, npts=200, seed=12), adjoints=False)
-        bad_batch(ba, W, ow, None, ERR_STATE, "window 2: dmv_ba_set_adjoints first", "member without adjoints")
+        bad_batch(ba, W, ow, None, DMV_ERR_STATE, "window 2: dmv_ba_set_adjoints first", "member without adjoints")
         ba, W, ow = handle(dict(nf=3, npts=200, seed=13), points=False)
-        bad_batch(ba, W, ow, None, ERR_STATE, "window 2: points not set", "member without points")
+        bad_batch(ba, W, ow, None, DMV_ERR_STATE, "window 2: points not set", "member without points")
         ba, W, ow = handle(dict(nf=3, npts=200, seed=14))
-        bad_batch(ba, W, ow, np.zeros(8 * 3 + 4), ERR_STATE, "window 2: no committed linearisation", "x without a committed linearisation")
+        bad_batch(ba, W, ow, np.zeros(8 * 3 + 4), DMV_ERR_STATE, "window 2: no committed linearisation", "x without a committed linearisation")
         # chunk_points = 0: 16-point chunks when the batch is made, 32-point chunks once the window no longer fits one wave of them
         n32 = 16 * sms + 64
         ba, W, ow = handle(dict(nf=3, npts=200, seed=15), chunk_points=0, max_points=n32)
@@ -427,7 +420,7 @@ def test_refusals_leave_members_untouched(capi, orc, synth, sms):
         ba.set_residuals(W32["res_point"], W32["res_target"])
         ow32 = orc.Window(W32)
         st = states(members[:2]) + [ba._state(ow32.calib()["k8"], ow32.precalc(), ow32.frame_tables()["frameEnergyTH"])]
-        _refused(capi, _raw_step(capi, b.h, xs[:2] + [None], st), ERR_STATE, "window 2 uses 32-point chunks, window 0 16")
+        _refused(capi, _raw_step(capi, b.h, xs[:2] + [None], st), DMV_ERR_STATE, "window 2 uses 32-point chunks, window 0 16")
         untouched("chunk_points = 0 member that resolved to 32-point chunks")
 
         # ---- dmv_ba_batch_create
@@ -443,8 +436,8 @@ def test_refusals_leave_members_untouched(capi, orc, synth, sms):
         L = capi.lib()
         out = C.c_void_p()
         arr = (C.c_void_p * 2)(members[0].bt.h.value, None)
-        _refused(capi, L.dmv_ba_batch_create(arr, 2, C.byref(out)), ERR_INVALID, "handle 1 is null")
-        _refused(capi, L.dmv_ba_batch_create(None, 1, C.byref(out)), ERR_INVALID, "1..64 handles")
+        _refused(capi, L.dmv_ba_batch_create(arr, 2, C.byref(out)), DMV_ERR_INVALID, "handle 1 is null")
+        _refused(capi, L.dmv_ba_batch_create(None, 1, C.byref(out)), DMV_ERR_INVALID, "1..64 handles")
         assert not out.value
         untouched("refused dmv_ba_batch_create")
 

@@ -16,19 +16,12 @@ import dmvio_b200.hostmath as hm
 from helpers import (RES_IN, check_linearize_parity, check_phase_b, edge_window, points_with_in_residual, prior_f, product_ba_from_oracle,
                      ulp32)
 from test_gpu_ba import CONFIGS
+from gpu_harness import device_capi  # noqa: F401  (the "capi" fixture: every test that takes it needs the device)
 
 pytestmark = pytest.mark.gpu
 
 EPS32 = float(np.finfo(np.float32).eps)
 STEP_CONFIGS = [c for c in CONFIGS if not c.get("edge")]
-
-
-@pytest.fixture(scope="module")
-def capi():
-    import dmvio_b200.capi as c
-    if c.lib().dmv_device_count() < 1:
-        pytest.fail("no CUDA device visible: GPU tests must run on the H100")
-    return c
 
 
 def _window(synth, cfg):

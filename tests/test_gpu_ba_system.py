@@ -17,6 +17,7 @@ import pytest
 from helpers import (EPS32, EPS64, RES_IN, RES_OOB, check_system, energy_bound, make_case, product_ba_from_oracle, schur_bound,
                      schur_reference)
 from test_gpu_ba import CONFIGS, cfg_id
+from gpu_harness import device_capi  # noqa: F401  (the "capi" fixture: every test that takes it needs the device)
 
 pytestmark = pytest.mark.gpu
 
@@ -26,14 +27,6 @@ TPB = {16: 448, 32: 224}                                                    # th
 
 def sys_id(c):
     return cfg_id(c) + (f"_{c['w']}x{c['h']}" if "w" in c else "")
-
-
-@pytest.fixture(scope="module")
-def capi():
-    import dmvio_b200.capi as c
-    if c.lib().dmv_device_count() < 1:
-        pytest.fail("no CUDA device visible: GPU tests must run on the H100")
-    return c
 
 
 def check_bound(got, want, bound, what):

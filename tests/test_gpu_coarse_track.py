@@ -12,34 +12,26 @@ import numpy as np
 import pytest
 
 import helpers as H
+from gpu_harness import CONFIGS, ct_handle, ct_scene, empty_coarsest, require_device, set_cluster, track_kw
 
 pytestmark = pytest.mark.gpu
 
-CONFIGS = ["nc16", "nc8", "nc4", "default"]
 TRAJ = ["bench", "aff_free", "aff_fixA", "aff_fixB", "aff_fixAB", "tma0_80x60", "tma0_160x120", "limit", "odd", "stream", "repeat"]
 LINEAR = TRAJ + ["wide", "counts_1", "counts_31", "counts_513"]
-_SC, _REF = {}, {}
+_REF = {}
 RATIOS = {}
 
 
 @pytest.fixture(scope="module")
 def capi():
-    import dmvio_b200.capi as c
-    if c.lib().dmv_device_count() < 1:
-        pytest.fail("no CUDA device visible: GPU tests must run on the H100")
-    yield c
+    """require_device()'s binding; prints the largest error/bound ratios at teardown"""
+    yield require_device()
     for k in sorted(RATIOS):
         print(f"max |err|/bound {k}: {RATIOS[k]:.3g}")
 
 
 def _note(key, v):
     RATIOS[key] = max(RATIOS.get(key, 0.0), float(v))
-
-
-def scene(orc, synth, name):
-    if name not in _SC:
-        _SC[name] = H.ct_scene(orc, synth, name)
-    return _SC[name]
 
 
 def ref(sc):
@@ -49,24 +41,12 @@ def ref(sc):
 
 
 def handle(capi, sc, cfg, monkeypatch, pts=None):
-    monkeypatch.delenv("DMV_CT_CLUSTER", raising=False)
-    if cfg != "default":
-        monkeypatch.setenv("DMV_CT_CLUSTER", cfg[2:])
-    pts = sc["pts"] if pts is None else pts
-    g = capi.CT(sc["w"], sc["h"], sc["levels"], max_points=max(65536, max(len(p["u"]) for p in pts)))
-    for l in range(sc["levels"]):
-        g.set_K(l, *[float(x) for x in sc["k4"][l]])
-        p = pts[l]
-        g.set_ref(l, p["u"], p["v"], p["idepth"], p["color"])
-        g.upload_new(l, sc["planes"][l])
-    return g
+    set_cluster(monkeypatch, cfg)
+    return ct_handle(capi, sc, pts)
 
 
 def track(g, sc, **kw):
-    a = dict(sc["args"])
-    a.update(kw)
-    return g.track(a["R0"], a["t0"], a["a0"], a["b0"], a["ref_a"], a["ref_b"], a["ref_exposure"], a["new_exposure"], 20.0, a["affA"], a["affB"],
-                   a.get("coarsest"), a.get("minRes"))
+    return g.track(**track_kw(sc, **kw))
 
 
 def check_final_linearisation(sc, r, rep, key):
@@ -101,7 +81,7 @@ def test_track_against_fp64_reference(capi, orc, synth, monkeypatch, name, cfg):
     still moves to first order with the pose, and kernel and reference stop at poses up to ~1e-7 apart (the pose tolerance is 1e-6).  On an
     H100 the coarsest level of the bench scene (935 points) differed by 2.0e-5, while check 1 at the kernel's own pose stays below 0.003 of
     its bound, so the difference is the stopping pose, not the sums."""
-    sc = scene(orc, synth, name)
+    sc = ct_scene(orc, synth, name)
     rr = ref(sc) if not name.startswith("counts_") else None
     g = handle(capi, sc, cfg, monkeypatch)
     r = track(g, sc)
@@ -132,7 +112,7 @@ def test_configurations_agree_with_each_other(capi, orc, synth, monkeypatch, nam
     on the HOST_LOOP scenes: those built from makeCoarseDepthL0 with the adapter's photometric and affine settings (the aff_* scenes
     change them).  The host loop evaluates with ct_res_gs_kernel, which gathers every level
     from L2, so on the tma0, limit and odd scenes this also compares the TMA-staged planes with the unstaged ones."""
-    sc = scene(orc, synth, name)
+    sc = ct_scene(orc, synth, name)
     rs = []
     for cfg in CONFIGS:
         g = handle(capi, sc, cfg, monkeypatch)
@@ -155,7 +135,7 @@ def test_configurations_agree_with_each_other(capi, orc, synth, monkeypatch, nam
 @pytest.mark.parametrize("cfg", CONFIGS)
 def test_handle_reuse_after_another_frame(capi, orc, synth, monkeypatch, cfg):
     """check 4: a handle that tracked a different frame in between gives a bit-identical result"""
-    sc = scene(orc, synth, "bench")
+    sc = ct_scene(orc, synth, "bench")
     g = handle(capi, sc, cfg, monkeypatch)
     r1 = track(g, sc)
     for l in range(sc["levels"]):
@@ -177,16 +157,13 @@ ABORTS = [("aff_free", w) for w in ("minRes_coarsest", "minRes_l1", "minRes_l0",
 @pytest.mark.parametrize("name,where", ABORTS)
 def test_abort_contract(capi, orc, synth, monkeypatch, cfg, name, where):
     """check 5: status 2, good 0, R t a b bit-equal to the inputs, NaN for the unfinished levels, finished levels as the run that does not abort"""
-    sc = scene(orc, synth, name)
+    sc = ct_scene(orc, synth, name)
     L = sc["levels"]
     g = handle(capi, sc, cfg, monkeypatch)
     full = track(g, sc)
     if where == "empty_coarsest":
-        pts = list(sc["pts"])
-        e = np.zeros(0, np.float32)
-        pts[L - 1] = dict(u=e, v=e, idepth=e, color=e)
         g.close()
-        g = handle(capi, sc, cfg, monkeypatch, pts=pts)
+        g = handle(capi, sc, cfg, monkeypatch, pts=empty_coarsest(sc))
         r, lvl = track(g, sc), L - 1
     else:
         lvl = {"minRes_coarsest": L - 1, "minRes_l1": 1, "minRes_l0": 0}[where]
@@ -223,7 +200,7 @@ def test_calc_res_gs_against_fp64_reference(capi, orc, synth, monkeypatch, name)
     """check 7: dmv_ct_calc_res_gs (host-loop / IMU entry point) at every logged pose of the reference, within calc_res_ref's bound.
     The padded warped count is compared exactly wherever no point is ambiguous, and at least one such pose has a count that is not a
     multiple of 4, so a missing padding cannot hide inside the bound of H and b."""
-    sc = scene(orc, synth, name)
+    sc = ct_scene(orc, synth, name)
     rr = ref(sc)
     g = handle(capi, sc, "nc16", monkeypatch)
     a = sc["args"]

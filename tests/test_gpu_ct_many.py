@@ -10,84 +10,24 @@ import numpy as np
 import pytest
 
 import helpers as H
+from dmvio_b200.capi import DMV_ERR_INVALID, DMV_ERR_STATE
+from gpu_harness import CONFIGS, assert_same, capi, close, ct_handle, ct_scene, empty_coarsest, gpu, set_cluster, track_kw  # noqa: F401
 
-DMV_ERR_INVALID, DMV_ERR_STATE = -1, -4
-CONFIGS = ["nc16", "nc8", "nc4", "default"]
 # 15 members: 1-5 levels, five image shapes, all four affine modes, staged and L2-gathered levels, the 80 KiB limit, the box-limit level of
 # wide, stream's more-points-than-register-slots loop and repeat's cutoff doubling.  At nc16 they need more clusters than are co-resident.
 MEMBERS = H.CT_SCENES + ["counts_1", "counts_31", "counts_513"]
 ABORTS = [("aff_free", w) for w in ("minRes_coarsest", "minRes_l1", "minRes_l0", "empty_coarsest")] + \
          [(n, w) for n in ("counts_1", "counts_31", "counts_513") for w in ("minRes_coarsest", "empty_coarsest")]
-_SC = {}
-
-
-@pytest.fixture(scope="module")
-def capi():
-    import dmvio_b200.capi as c
-    return c
-
-
-@pytest.fixture
-def gpu(capi):
-    if capi.lib().dmv_device_count() < 1:
-        pytest.fail("no CUDA device visible: GPU tests must run on the H100")
-
-
-def scene(orc, synth, name):
-    if name not in _SC:
-        _SC[name] = H.ct_scene(orc, synth, name)
-    return _SC[name]
-
-
-def set_cluster(monkeypatch, cfg):
-    monkeypatch.delenv("DMV_CT_CLUSTER", raising=False)
-    if cfg != "default":
-        monkeypatch.setenv("DMV_CT_CLUSTER", cfg[2:])
-
-
-def handle(capi, sc, pts=None, k=True, device=0):
-    pts = sc["pts"] if pts is None else pts
-    g = capi.CT(sc["w"], sc["h"], sc["levels"], max_points=max(65536, max(len(p["u"]) for p in pts)), device=device)
-    for l in range(sc["levels"]):
-        if k:
-            g.set_K(l, *[float(x) for x in sc["k4"][l]])
-        p = pts[l]
-        g.set_ref(l, p["u"], p["v"], p["idepth"], p["color"])
-        g.upload_new(l, sc["planes"][l])
-    return g
-
-
-def kw(sc, **over):
-    """CT.track's keywords for the scene's arguments"""
-    a = dict(sc["args"])
-    a.update(over)
-    return dict(R=a["R0"], t=a["t0"], a=a["a0"], b=a["b0"], ref_a=a["ref_a"], ref_b=a["ref_b"], ref_exposure=a["ref_exposure"],
-                new_exposure=a["new_exposure"], cutoff=20.0, affA=a["affA"], affB=a["affB"], coarsest=a.get("coarsest"), minRes=a.get("minRes"))
-
-
-def bits(x):
-    return np.ascontiguousarray(np.asarray(x, np.float64)).view(np.uint64)
-
-
-def assert_same(r, s, what):
-    assert r.keys() == s.keys()
-    for k in r:
-        assert np.array_equal(bits(r[k]), bits(s[k])), (what, k, r[k], s[k])
-
-
-def close(*hs):
-    for g in hs:
-        g.close()
 
 
 @pytest.mark.gpu
 @pytest.mark.parametrize("cfg", CONFIGS)
 def test_many_is_bit_identical_to_single(capi, gpu, orc, synth, monkeypatch, cfg):
     set_cluster(monkeypatch, cfg)
-    scs = [scene(orc, synth, n) for n in MEMBERS]
-    gs = [handle(capi, sc) for sc in scs]
-    twins = [handle(capi, sc) for sc in scs]
-    args = [kw(sc) for sc in scs]
+    scs = [ct_scene(orc, synth, n) for n in MEMBERS]
+    gs = [ct_handle(capi, sc) for sc in scs]
+    twins = [ct_handle(capi, sc) for sc in scs]
+    args = [track_kw(sc) for sc in scs]
     singles = [t.track(**a) for t, a in zip(twins, args)]
     for rep in range(2):   # the members probe in the first call; the second reuses the handles
         before = [g.launch_count() for g in gs]
@@ -107,25 +47,23 @@ def test_aborts_stay_local(capi, gpu, orc, synth, monkeypatch, cfg):
     cases = [("bench", None)] + ABORTS[:5] + [("stream", None)] + ABORTS[5:] + [("aff_fixA", None)]
     gs, twins, args = [], [], []
     for name, where in cases:
-        sc = scene(orc, synth, name)
+        sc = ct_scene(orc, synth, name)
         L = sc["levels"]
         pts = None
         over = {}
         if where == "empty_coarsest":
-            e = np.zeros(0, np.float32)
-            pts = list(sc["pts"])
-            pts[L - 1] = dict(u=e, v=e, idepth=e, color=e)
-        twin = handle(capi, sc, pts)
+            pts = empty_coarsest(sc)
+        twin = ct_handle(capi, sc, pts)
         if where is not None and where.startswith("minRes"):
             lvl = {"minRes_coarsest": L - 1, "minRes_l1": 1, "minRes_l0": 0}[where]
-            full = twin.track(**kw(sc))
+            full = twin.track(**track_kw(sc))
             assert full["status"] == 0 and full["lastResiduals"][lvl] > 0
             mr = np.full(5, np.nan)
             mr[lvl] = full["lastResiduals"][lvl] / 3
             over["minRes"] = mr
-        gs.append(handle(capi, sc, pts))
+        gs.append(ct_handle(capi, sc, pts))
         twins.append(twin)
-        args.append(kw(sc, **over))
+        args.append(track_kw(sc, **over))
     singles = [t.track(**a) for t, a in zip(twins, args)]
     rs = capi.ct_track_many(gs, args)
     for (name, where), r, s, a in zip(cases, rs, singles, args):
@@ -145,10 +83,10 @@ def test_subsets_and_order(capi, gpu, orc, synth, monkeypatch):
     """the same handles in successive calls: every one alone, reversed, every other one and all of them"""
     set_cluster(monkeypatch, "default")
     names = ["bench", "aff_free", "tma0_80x60", "odd", "wide", "repeat"]
-    scs = [scene(orc, synth, n) for n in names]
-    gs = [handle(capi, sc) for sc in scs]
-    twins = [handle(capi, sc) for sc in scs]
-    args = [kw(sc) for sc in scs]
+    scs = [ct_scene(orc, synth, n) for n in names]
+    gs = [ct_handle(capi, sc) for sc in scs]
+    twins = [ct_handle(capi, sc) for sc in scs]
+    args = [track_kw(sc) for sc in scs]
     singles = [t.track(**a) for t, a in zip(twins, args)]
     calls = [[i] for i in range(len(gs))] + [list(range(len(gs)))[::-1], list(range(0, len(gs), 2)), list(range(1, len(gs), 2)), list(range(len(gs)))]
     for idx in calls:
@@ -166,10 +104,10 @@ def test_ordered_behind_asynchronous_uploads(capi, gpu, orc, synth, monkeypatch)
     """dmv_ct_upload_new_image returns before its copy and pyramid have run; the launch must wait for every member's, then a second frame
     goes through the same handles"""
     set_cluster(monkeypatch, "default")
-    scs = [scene(orc, synth, n) for n in H.CT_SCENES]
-    gs = [handle(capi, sc) for sc in scs]
-    twins = [handle(capi, sc) for sc in scs]
-    args = [kw(sc) for sc in scs]
+    scs = [ct_scene(orc, synth, n) for n in H.CT_SCENES]
+    gs = [ct_handle(capi, sc) for sc in scs]
+    twins = [ct_handle(capi, sc) for sc in scs]
+    args = [track_kw(sc) for sc in scs]
     for frame in ("img_ref", "img_new"):
         for g, sc in zip(gs, scs):
             g.upload_new_image(sc["T"][frame])
@@ -200,9 +138,9 @@ def untouched(out):
 @pytest.mark.gpu
 def test_errors_are_rejected_before_launch(capi, gpu, orc, synth, monkeypatch):
     set_cluster(monkeypatch, "default")
-    sc = scene(orc, synth, "tma0_80x60")
-    gs = [handle(capi, sc) for _ in range(17)]
-    a = kw(sc)
+    sc = ct_scene(orc, synth, "tma0_80x60")
+    gs = [ct_handle(capi, sc) for _ in range(17)]
+    a = track_kw(sc)
     gs[0].track(**a)            # one member has probed already, the others probe inside the call
     counts = [g.launch_count() for g in gs]
 
@@ -219,20 +157,20 @@ def test_errors_are_rejected_before_launch(capi, gpu, orc, synth, monkeypatch):
     rejected(gs, [a] * 17, msg="n = 17")
     rejected([gs[0], None, gs[2]], [a] * 3, msg="handles[1] is NULL")
     rejected([gs[0], gs[1], gs[0]], [a] * 3, msg="handles[0] and handles[2]")
-    noK = handle(capi, sc, k=False)
+    noK = ct_handle(capi, sc, k=False)
     n_noK = noK.launch_count()
     rejected([gs[0], gs[1], noK], [a] * 3, code=DMV_ERR_STATE, msg="handles[2]")
     assert noK.launch_count() == n_noK
-    bad = [a] * 3 + [kw(sc, coarsest=sc["levels"])] + [a]
+    bad = [a] * 3 + [track_kw(sc, coarsest=sc["levels"])] + [a]
     text = rejected(gs[:5], bad, msg="handles[3]")
     assert "coarsestLvl" in text
     close(noK)
     # cluster sizes that differ: one handle probed under DMV_CT_CLUSTER=8, another under 16
     monkeypatch.setenv("DMV_CT_CLUSTER", "8")
-    g8 = handle(capi, sc)
+    g8 = ct_handle(capi, sc)
     g8.track(**a)
     monkeypatch.setenv("DMV_CT_CLUSTER", "16")
-    g16 = handle(capi, sc)
+    g16 = ct_handle(capi, sc)
     g16.track(**a)
     n8, n16 = g8.launch_count(), g16.launch_count()
     text = rejected([g16, g8], [a, a], msg="handles[1]")
@@ -245,9 +183,9 @@ def test_handles_on_two_devices_are_rejected(capi, gpu, orc, synth, monkeypatch)
     if capi.lib().dmv_device_count() < 2:
         pytest.skip("needs two visible GPUs")
     set_cluster(monkeypatch, "default")
-    sc = scene(orc, synth, "tma0_80x60")
-    g0, g1 = handle(capi, sc, device=0), handle(capi, sc, device=1)
-    rc, text, out = raw_call(capi, [g0, g1], [kw(sc)] * 2)
+    sc = ct_scene(orc, synth, "tma0_80x60")
+    g0, g1 = ct_handle(capi, sc, device=0), ct_handle(capi, sc, device=1)
+    rc, text, out = raw_call(capi, [g0, g1], [track_kw(sc)] * 2)
     assert rc == DMV_ERR_INVALID and "device" in text and untouched(out)
     assert g0.launch_count() == g1.launch_count()
     close(g0, g1)

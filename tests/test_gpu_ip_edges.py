@@ -12,16 +12,9 @@ import numpy as np
 import pytest
 
 import helpers as H
+from gpu_harness import device_capi  # noqa: F401  (the "capi" fixture: every test that takes it needs the device)
 
 pytestmark = pytest.mark.gpu
-
-
-@pytest.fixture(scope="module")
-def capi():
-    import dmvio_b200.capi as c
-    if c.lib().dmv_device_count() < 1:
-        pytest.fail("no CUDA device visible: GPU tests must run on the H100")
-    return c
 
 
 def _col(orc, k):

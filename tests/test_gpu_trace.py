@@ -4,15 +4,9 @@ with -fmad=false and keeps the reference's operation order."""
 import numpy as np
 import pytest
 
+from gpu_harness import device_capi  # noqa: F401  (the "capi" fixture: every test that takes it needs the device)
+
 pytestmark = pytest.mark.gpu
-
-
-@pytest.fixture(scope="module")
-def capi():
-    import dmvio_b200.capi as c
-    if c.lib().dmv_device_count() < 1:
-        pytest.fail("no CUDA device visible: GPU tests must run on the H100")
-    return c
 
 
 @pytest.mark.parametrize("cfg", [dict(seed=5, trans=0.05, rot=0.01, n=3000), dict(seed=12, trans=0.12, rot=0.03, n=1500, w=512, h=512)], ids=["640x480", "512x512_fast"])

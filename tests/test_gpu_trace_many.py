@@ -10,22 +10,12 @@ import ctypes as C
 import numpy as np
 import pytest
 
+import gpu_harness as G
 import helpers as H
+from dmvio_b200.capi import DMV_ERR_INVALID
+from gpu_harness import capi, close, gpu  # noqa: F401
 
-DMV_ERR_INVALID = -1
 MANY_MAX = 16
-
-
-@pytest.fixture(scope="module")
-def capi():
-    import dmvio_b200.capi as c
-    return c
-
-
-@pytest.fixture
-def gpu(capi):
-    if capi.lib().dmv_device_count() < 1:
-        pytest.fail("no CUDA device visible: GPU tests must run on the H100")
 
 
 class Member:
@@ -77,11 +67,6 @@ def bits(a):
 
 def handles(capi, synth, ms):
     return [capi.CT(m.w, m.h, synth.pyr_levels(m.w, m.h), max_points=1024) for m in ms]
-
-
-def close(*hs):
-    for g in hs:
-        g.close()
 
 
 def step(capi, orc, ms, gs, twins, t, settings=None, oracle=True, upload=None):
@@ -204,7 +189,7 @@ def test_track_after_trace(capi, gpu, orc, synth):
               new_exposure=a["new_exposure"], affA=a["affA"], affB=a["affB"], coarsest=a.get("coarsest"), minRes=a.get("minRes"))
     r, s_ = gs[0].track(**kw), twins[0].track(**kw)
     for k in r:
-        assert np.array_equal(np.asarray(r[k], np.float64).view(np.uint64), np.asarray(s_[k], np.float64).view(np.uint64)), k
+        assert np.array_equal(G.bits(r[k]), G.bits(s_[k])), k
     assert r["status"] == 0
     close(*gs, *twins)
 

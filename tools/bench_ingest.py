@@ -9,14 +9,11 @@ to --out if given.
 import argparse
 import json
 import os
-import subprocess
-import sys
 import time
 
 import numpy as np
 
-ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
-sys.path.insert(0, ROOT)
+import benchkit as K  # first: it puts the repository root on sys.path
 import dmvio_b200.capi as capi  # noqa: E402
 from oracle import undistort as U  # noqa: E402
 
@@ -24,22 +21,13 @@ SHAPES = [("euroc_radtan_752x480_to_640x480_u8", 752, 480, 640, 480, 1), ("tumvi
 LEVELS = 5
 
 
-def card():
-    try:
-        q = subprocess.run(["nvidia-smi", "--query-gpu=name,power.limit", "--format=csv,noheader"], capture_output=True, text=True, timeout=30).stdout
-        return q.strip().splitlines()[0]
-    except Exception as e:  # noqa: BLE001
-        return f"unknown ({e})"
-
-
 def main():
     ap = argparse.ArgumentParser()
     ap.add_argument("--frames", type=int, default=300)
     ap.add_argument("--out", default=None)
     a = ap.parse_args()
-    if capi.lib().dmv_device_count() < 1:
-        raise SystemExit("bench_ingest needs a CUDA device")
-    res = dict(card=card(), frames=a.frames, levels=LEVELS, photometric_mode=2, shapes=[])
+    K.device_lib("bench_ingest")
+    res = dict(card=K.card(), frames=a.frames, levels=LEVELS, photometric_mode=2, shapes=[])
     for name, wOrg, hOrg, w, h, bpp in SHAPES:
         rx, ry = U.synthetic_remap(w, h, wOrg, hOrg)
         nG = 256 if bpp == 1 else 65536

@@ -11,27 +11,16 @@ import argparse
 import ctypes as C
 import json
 import os
-import subprocess
-import sys
 import time
 
 import numpy as np
 
-ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
-sys.path.insert(0, ROOT)
+import benchkit  # first: it puts the repository root on sys.path
 import dmvio_b200.capi as capi  # noqa: E402
 from oracle import select as S  # noqa: E402
 
 SHAPES = [(640, 480, 4), (640, 480, 5), (512, 512, 4), (512, 512, 5)]
 POINT_BYTES = 4 * (2 + 1 + 8 + 8 + 4 + 1)   # u, v, type, color[8], weights[8], gradH[4], energyTH
-
-
-def card():
-    try:
-        q = subprocess.run(["nvidia-smi", "--query-gpu=name,power.limit", "--format=csv,noheader"], capture_output=True, text=True, timeout=30).stdout
-        return q.strip().splitlines()[0]
-    except Exception as e:  # noqa: BLE001
-        return f"unknown ({e})"
 
 
 def host_path(ct, w, h, pot):
@@ -72,7 +61,7 @@ def profile(outdir):
     ct.close()
     table = prof.key_averages().table(sort_by="cuda_time_total", row_limit=40)
     os.makedirs(outdir, exist_ok=True)
-    open(os.path.join(outdir, "new_traces_kernels.txt"), "w").write(card() + "\n" + table + "\n")
+    open(os.path.join(outdir, "new_traces_kernels.txt"), "w").write(benchkit.card() + "\n" + table + "\n")
     print(table)
 
 
@@ -82,11 +71,10 @@ def main():
     ap.add_argument("--out", default=None)
     ap.add_argument("--profile", default=None)
     a = ap.parse_args()
-    if capi.lib().dmv_device_count() < 1:
-        raise SystemExit("bench_new_traces needs a CUDA device")
+    benchkit.device_lib("bench_new_traces")
     if a.profile:
         return profile(a.profile)
-    res = dict(card=card(), keyframes=a.keyframes, density=1500, shapes=[])
+    res = dict(card=benchkit.card(), keyframes=a.keyframes, density=1500, shapes=[])
     identical = True
     for w, h, lv in SHAPES:
         imgs = [S.image("tex" if k % 3 else "high", w, h, 100 + k) for k in range(a.keyframes)]

@@ -12,14 +12,11 @@ name and power limit read in the same run, and writes it to --out if given.
 import argparse
 import json
 import os
-import subprocess
-import sys
 import time
 
 import numpy as np
 
-ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
-sys.path.insert(0, ROOT)
+import benchkit as K  # first: it puts the repository root on sys.path
 import dmvio_b200.capi as capi  # noqa: E402
 import dmvio_b200.hostmath as hm  # noqa: E402
 import dmvio_b200.synth as synth  # noqa: E402
@@ -27,14 +24,6 @@ import dmvio_b200.synth as synth  # noqa: E402
 WINDOWS = [("baseline_c3_7kf_2000pts_640x480", dict(nf=7, npts=2000, w=640, h=480, seed=1234), 5),
            ("7kf_2000pts_512x512", dict(nf=7, npts=2000, w=512, h=512, seed=1234), 4)]
 MAXF = 8   # DMV_MAX_FRAMES: the residual slots the handle keeps per point
-
-
-def card():
-    try:
-        q = subprocess.run(["nvidia-smi", "--query-gpu=name,power.limit", "--format=csv,noheader"], capture_output=True, text=True, timeout=30).stdout
-        return q.strip().splitlines()[0]
-    except Exception as e:  # noqa: BLE001
-        return f"unknown ({e})"
 
 
 def committed_window(W):
@@ -97,9 +86,8 @@ def main():
     ap.add_argument("--warmup", type=int, default=30)
     ap.add_argument("--out", default=None)
     a = ap.parse_args()
-    if capi.lib().dmv_device_count() < 1:
-        raise SystemExit("bench_ref_handoff needs a CUDA device")
-    out = dict(card=card(), reps=a.reps, warmup=a.warmup, windows=[])
+    K.device_lib("bench_ref_handoff")
+    out = dict(card=K.card(), reps=a.reps, warmup=a.warmup, windows=[])
     for name, cfg, levels in WINDOWS:
         W = synth.make_window(**cfg)
         w, h, nf = W["w"], W["h"], W["nf"]

@@ -6,7 +6,6 @@ pyramid, point / residual upload, adjoints, 10 fused GN steps with the dense sol
 frames stay resident across keyframes (image slots).  The CPU side is the oracle's optimize() with 6 worker threads on the same windows
 (its window construction is not timed).  Prints one JSON line.   python tools/bench_stream.py [--keyframes 40]"""
 import argparse
-import ctypes as C
 import json
 import os
 import sys
@@ -67,7 +66,6 @@ def run_stream(keyframes=40, its=10, cpu_keyframes=6, size=512, device=0):
     L = hostapi.lib()
     c = lambda a, t: np.ascontiguousarray(a, t)
     win = L.dmvh_window_create(S["w"], S["h"], 8, NPTS, device, c(S["K"], np.float64))
-    L.dmvh_window_set_setting.argtypes = [C.c_void_p, C.c_char_p, C.c_double]
     assert L.dmvh_window_set_setting(win, b"minOptIterations", float(args.its)) == 0   # no early break: its iterations per keyframe, as the config says
 
     def add_frame(W, k):

@@ -19,27 +19,14 @@ import argparse
 import ctypes as C
 import json
 import os
-import subprocess
-import sys
 import threading
-import time
 
 import numpy as np
 
-ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
-sys.path.insert(0, ROOT)
+import benchkit as K
 
 BS = [1, 2, 4, 8, 16]
 W, H, HOSTS, PTS = 640, 480, 6, 1500
-
-
-def card():
-    try:
-        q = subprocess.run(["nvidia-smi", "--query-gpu=name,power.limit,clocks.max.sm", "--format=csv,noheader"], capture_output=True, text=True,
-                           timeout=30).stdout
-        return q.strip().splitlines()[0]
-    except Exception as e:  # noqa: BLE001
-        return f"unknown ({e})"
 
 
 def make_scene(synth, hm, orc, i):
@@ -103,57 +90,27 @@ class Threads:
 
 
 def stats(t, points):
-    ms = 1e3 * np.asarray(t)
-    med = float(np.median(ms))
-    return dict(median_ms=med, p10_ms=float(np.percentile(ms, 10)), p90_ms=float(np.percentile(ms, 90)), points_per_s=points / med * 1e3)
-
-
-def timed(arms, resets, warmup, reps, L, what):
-    """alternating, rotating rounds of the arms; each round's reset runs outside its timing"""
-    names = list(arms)
-    t = {k: [] for k in names}
-    for rep in range(warmup + reps):
-        for j in range(len(names)):
-            k = names[(rep + j) % len(names)]
-            resets[k]()
-            t0 = time.perf_counter()
-            rc = arms[k]()
-            dt = time.perf_counter() - t0
-            if rc != 0:
-                raise SystemExit(f"{k} {what}: dmvio_b200 error {rc}: {L[k].dmv_last_error().decode()}")
-            if rep >= warmup:
-                t[k].append(dt)
-    return t
+    d = K.stats(t)
+    return dict(d, points_per_s=points / d["median_ms"] * 1e3)
 
 
 def parent_ab(capi, plane, sets, path, warmup, reps):
     """dmv_ct_trace_points_multi on one handle of this library and one of the library at `path`, alternated call by call"""
-    libs = {"this": capi.lib(), "parent": C.CDLL(os.path.abspath(path))}
-    P = libs["parent"]
-    P.dmv_last_error.restype = C.c_char_p
-    P.dmv_ct_create.argtypes = [C.POINTER(capi.CTConfig), C.POINTER(C.c_void_p)]
-    P.dmv_ct_destroy.argtypes = [C.c_void_p]
-    P.dmv_ct_upload_new.argtypes = [C.c_void_p, C.c_int, capi.f32p]
-    P.dmv_ct_trace_points_multi.argtypes = [C.c_void_p, C.c_int, C.c_void_p, C.c_void_p, C.c_void_p]
-    hs = {}
+    libs = K.this_and_parent(path)
+    gs = {}
     for k, L in libs.items():
-        h = C.c_void_p()
-        rc = L.dmv_ct_create(C.byref(capi.CTConfig(W, H, 5, 1024, 0)), C.byref(h))
-        if rc != 0:
-            raise SystemExit(f"{k}: dmv_ct_create: {L.dmv_last_error().decode()}")
-        if L.dmv_ct_upload_new(h, 0, np.ascontiguousarray(plane, np.float32).reshape(-1)) != 0:
-            raise SystemExit(f"{k}: dmv_ct_upload_new: {L.dmv_last_error().decode()}")
-        hs[k] = h
+        gs[k] = capi.CT(W, H, 5, max_points=1024, L=L)
+        gs[k].upload_new(0, plane)
     A = {k: Arm(capi, [(None, sets)]) for k in libs}
-    arms = {k: (lambda k=k: libs[k].dmv_ct_trace_points_multi(hs[k], A[k].T[0].job.nsets, A[k].T[0].job.sets, A[k].T[0].job.tables14, None))
+    arms = {k: (lambda k=k: libs[k].dmv_ct_trace_points_multi(gs[k].h, A[k].T[0].job.nsets, A[k].T[0].job.sets, A[k].T[0].job.tables14, None))
             for k in libs}
-    t = timed(arms, {k: A[k].reset for k in libs}, warmup, reps, libs, "single-handle A/B")
+    t = K.alternate(arms, warmup, reps, "single-handle A/B", libs, {k: A[k].reset for k in libs})
     for k in libs:
         A[k].reset()
         arms[k]()
     same = A["this"].result_bytes() == A["parent"].result_bytes()
-    for k, L in libs.items():
-        L.dmv_ct_destroy(hs[k])
+    for g in gs.values():
+        g.close()
     return dict(parent_lib=os.path.basename(path), bit_identical=same, **{k: stats(t[k], HOSTS * PTS) for k in libs}), same
 
 
@@ -162,22 +119,20 @@ def main():
     ap.add_argument("--warmup", type=int, default=30)
     ap.add_argument("--reps", type=int, default=300)
     ap.add_argument("--parent-lib", default=None, help="another build of libdmvio_b200.so for the single-handle A/B")
-    ap.add_argument("--out", default=os.path.join(ROOT, "records", "h100_trace_many.json"))
+    ap.add_argument("--out", default=os.path.join(K.ROOT, "records", "h100_trace_many.json"))
     a = ap.parse_args()
     import dmvio_b200.capi as capi
     import dmvio_b200.hostmath as hm
     import dmvio_b200.synth as synth
     from oracle import orc
-    L = capi.lib()
-    if L.dmv_device_count() < 1:
-        raise SystemExit("bench_trace_many needs a CUDA device")
+    L = K.device_lib("bench_trace_many")
     scenes = [make_scene(synth, hm, orc, i) for i in range(max(BS))]
     gs = []
     for plane, _ in scenes:
         g = capi.CT(W, H, 5, max_points=1024)
         g.upload_new(0, plane)
         gs.append(g)
-    res = dict(card=card(), shape=[W, H], hosts=HOSTS, points_per_host=PTS, warmup=a.warmup, reps=a.reps,
+    res = dict(card=K.card(), shape=[W, H], hosts=HOSTS, points_per_host=PTS, warmup=a.warmup, reps=a.reps,
                timing="wall clock per round, each round ending in a synchronisation; in/out arrays reset outside the timed call", B={})
     identical = True
     for B in BS:
@@ -194,7 +149,7 @@ def main():
             return rc
 
         arms = dict(seq=seq, threads=th.run, many=lambda: L.dmv_ct_trace_many(hs, B, J, None))
-        t = timed(arms, {k: A[k].reset for k in arms}, a.warmup, a.reps, {k: L for k in arms}, f"at B={B}")
+        t = K.alternate(arms, a.warmup, a.reps, f"at B={B}", dict.fromkeys(arms, L), {k: A[k].reset for k in arms})
         # identity, outside the timed loops: one more round of each arm from the fresh points, every in/out array compared byte for byte
         for k in arms:
             A[k].reset()

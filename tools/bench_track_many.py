@@ -15,27 +15,14 @@ import argparse
 import ctypes as C
 import json
 import os
-import subprocess
-import sys
 import threading
-import time
 
 import numpy as np
 
-ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
-sys.path.insert(0, ROOT)
+import benchkit as K
 
 BS = [1, 2, 4, 8, 16]
 W, H, LEVELS = 640, 480, 5
-
-
-def card():
-    try:
-        q = subprocess.run(["nvidia-smi", "--query-gpu=name,power.limit,clocks.max.sm", "--format=csv,noheader"], capture_output=True, text=True,
-                           timeout=30).stdout
-        return q.strip().splitlines()[0]
-    except Exception as e:  # noqa: BLE001
-        return f"unknown ({e})"
 
 
 def make_handle(capi, synth, orc, i):
@@ -86,17 +73,15 @@ def main():
     ap.add_argument("--cluster", type=int, default=16, choices=[16, 8, 4], help="DMV_CT_CLUSTER for the run: the cluster size every handle uses")
     ap.add_argument("--warmup", type=int, default=30)
     ap.add_argument("--reps", type=int, default=300)
-    ap.add_argument("--out", default=os.path.join(ROOT, "records", "h100_track_many.json"))
+    ap.add_argument("--out", default=os.path.join(K.ROOT, "records", "h100_track_many.json"))
     a = ap.parse_args()
     os.environ["DMV_CT_CLUSTER"] = str(a.cluster)
     import dmvio_b200.capi as capi
     import dmvio_b200.synth as synth
     from oracle import orc
-    L = capi.lib()
-    if L.dmv_device_count() < 1:
-        raise SystemExit("bench_track_many needs a CUDA device")
+    L = K.device_lib("bench_track_many")
     gs = [make_handle(capi, synth, orc, i) for i in range(max(BS))]
-    res = dict(card=card(), cluster=a.cluster, shape=[W, H], levels=LEVELS, warmup=a.warmup, reps=a.reps,
+    res = dict(card=K.card(), cluster=a.cluster, shape=[W, H], levels=LEVELS, warmup=a.warmup, reps=a.reps,
                timing="wall clock per round, each round ending in a synchronisation; ctypes argument blocks built once", B={})
     identical = True
     for B in BS:
@@ -112,20 +97,9 @@ def main():
             return rc
 
         arms = dict(seq=seq, threads=th.run, many=lambda: L.dmv_ct_track_many(hs, B, A, outs["many"]))
-        names = list(arms)
-        t = {k: [] for k in names}
-        for rep in range(a.warmup + a.reps):
-            for j in range(len(names)):
-                k = names[(rep + j) % len(names)]
-                t0 = time.perf_counter()
-                rc = arms[k]()
-                dt = time.perf_counter() - t0
-                if rc != 0:
-                    raise SystemExit(f"{k} at B={B}: dmvio_b200 error {rc}: {L.dmv_last_error().decode()}")
-                if rep >= a.warmup:
-                    t[k].append(dt)
+        t = K.alternate(arms, a.warmup, a.reps, f"at B={B}", dict.fromkeys(arms, L))
         # identity, outside the timed loops: one more round of each arm, every result struct compared byte for byte
-        for k in names:
+        for k in arms:
             for o in outs[k]:
                 C.memset(C.addressof(o), 0, C.sizeof(o))
             arms[k]()
@@ -134,11 +108,9 @@ def main():
         identical = identical and same
         th.close()
         row = dict(bit_identical=same, point_evaluations_per_round=pe)
-        for k in names:
-            ms = 1e3 * np.asarray(t[k])
-            med = float(np.median(ms))
-            row[k] = dict(median_ms=med, p10_ms=float(np.percentile(ms, 10)), p90_ms=float(np.percentile(ms, 90)), frames_per_s=B / med * 1e3,
-                          point_evals_per_s=pe / med * 1e3)
+        for k in arms:
+            d = K.stats(t[k])
+            row[k] = dict(d, frames_per_s=B / d["median_ms"] * 1e3, point_evals_per_s=pe / d["median_ms"] * 1e3)
         res["B"][str(B)] = row
     res["bit_identical"] = identical
     for g in gs:

@@ -21,29 +21,11 @@ import argparse
 import ctypes as C
 import json
 import os
-import subprocess
-import sys
-import time
 
 import numpy as np
 
-ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
-sys.path.insert(0, ROOT)
-sys.path.insert(0, os.path.join(ROOT, "tests"))
-
-
-def card():
-    try:
-        q = subprocess.run(["nvidia-smi", "--query-gpu=name,power.limit,clocks.max.sm", "--format=csv,noheader"], capture_output=True, text=True,
-                           timeout=30).stdout
-        return q.strip().splitlines()[0]
-    except Exception as e:  # noqa: BLE001
-        return f"unknown ({e})"
-
-
-def f32_finite(x):
-    with np.errstate(over="ignore", invalid="ignore"):
-        return bool(np.isfinite(np.float32(x)))
+import benchkit as K
+import gpu_harness as G
 
 
 class HostLoop:
@@ -75,11 +57,11 @@ class HostLoop:
             good = o.trackingGood != 0
             good_ret |= good
             lr = list(o.lastResiduals)
-            if good and f32_finite(lr[0]) and not (lr[0] >= achieved[0]):
+            if good and G.f32_finite(lr[0]) and not (lr[0] >= achieved[0]):
                 best = (list(o.R), list(o.t), o.a, o.b, list(o.flowIndicators), i)
             if best is not None:
                 for q in range(5):
-                    if not f32_finite(achieved[q]) or achieved[q] > lr[q]:
+                    if not G.f32_finite(achieved[q]) or achieved[q] > lr[q]:
                         achieved[q] = lr[q]
                 if achieved[0] < self.bound:
                     break
@@ -93,71 +75,36 @@ class HostLoop:
         return 0
 
 
-def stats(ts):
-    ms = 1e3 * np.asarray(ts)
-    return dict(median_ms=float(np.median(ms)), p10_ms=float(np.percentile(ms, 10)), p90_ms=float(np.percentile(ms, 90)))
-
-
-def workloads(capi, T, sc, g):
+def workloads(capi, sc, g):
     """(name, Rs, ts, track keywords, lastCoarseRMSE0)"""
-    k = T.kw(sc)
-    Rs, ts = T.near_truth_tries(sc)
+    k = G.tries_kw(sc)
+    Rs, ts = G.near_truth_tries(sc)
     out = [("easy", Rs, ts, k, 100.0)]
-    twin = T.handle(capi, sc)
-    for Rs, ts in [T.far_tries(sc, 0.1), T.near_truth_tries(sc), T.far_tries(sc, 0.05)]:
-        _, _, hist = T.loop_reference(twin, Rs, ts, k, lastCoarseRMSE0=0.0)
-        found = T.later_winner_L(hist)
+    twin = G.ct_handle(capi, sc)
+    for Rs, ts in [G.far_tries(sc, 0.1), G.near_truth_tries(sc), G.far_tries(sc, 0.05)]:
+        _, _, hist = G.loop_reference(twin, Rs, ts, k, lastCoarseRMSE0=0.0)
+        found = G.later_winner_L(hist)
         if found is not None:
             out.append(("recovery", Rs, ts, k, found[0]))
             break
     twin.close()
-    Rs, ts = T.far_tries(sc, 0.1)
-    out.append(("lost", Rs, ts, T.kw(sc, ref_b=250.0, b=252.0), 0.0))
+    Rs, ts = G.far_tries(sc, 0.1)
+    out.append(("lost", Rs, ts, G.tries_kw(sc, ref_b=250.0, b=252.0), 0.0))
     return out
 
 
-def parent_ab(capi, T, sc, path, warmup, reps):
+def parent_ab(capi, sc, path, warmup, reps):
     """dmv_ct_track from try 0 of the easy workload through this library and through `path`, alternated call by call"""
-    libs = {"this": C.CDLL(capi.LIB_PATH), "parent": C.CDLL(os.path.abspath(path))}
-    for P in libs.values():
-        P.dmv_ct_create.argtypes = [C.POINTER(capi.CTConfig), C.POINTER(C.c_void_p)]
-        P.dmv_ct_set_K.argtypes = [C.c_void_p, C.c_int, C.c_float, C.c_float, C.c_float, C.c_float]
-        P.dmv_ct_set_ref.argtypes = [C.c_void_p, C.c_int, C.c_int, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p]
-        P.dmv_ct_upload_new.argtypes = [C.c_void_p, C.c_int, C.c_void_p]
-        P.dmv_ct_track.argtypes = [C.c_void_p, C.POINTER(capi.CTTrackArgs), C.POINTER(capi.CTTrackResult)]
-        P.dmv_ct_destroy.argtypes = [C.c_void_p]
-    hs = {}
-    keep = []
-    for name, L in libs.items():
-        h = C.c_void_p()
-        assert L.dmv_ct_create(C.byref(capi.CTConfig(sc["w"], sc["h"], sc["levels"], 65536, 0)), C.byref(h)) == 0
-        for l in range(sc["levels"]):
-            assert L.dmv_ct_set_K(h, l, *[float(x) for x in sc["k4"][l]]) == 0
-            p = {q: np.ascontiguousarray(sc["pts"][l][q], np.float32) for q in ("u", "v", "idepth", "color")}
-            plane = np.ascontiguousarray(sc["planes"][l], np.float32).reshape(-1)
-            keep += list(p.values()) + [plane]
-            assert L.dmv_ct_set_ref(h, l, len(p["u"]), p["u"].ctypes.data, p["v"].ctypes.data, p["idepth"].ctypes.data, p["color"].ctypes.data) == 0
-            assert L.dmv_ct_upload_new(h, l, plane.ctypes.data) == 0
-        hs[name] = h
-    Rs, ts = T.near_truth_tries(sc)
-    A = capi._track_args(sc["levels"], Rs[0], ts[0], **T.kw(sc))
+    libs = K.this_and_parent(path)
+    gs = {k: G.ct_handle(capi, sc, L=L) for k, L in libs.items()}
+    Rs, ts = G.near_truth_tries(sc)
+    A = capi._track_args(sc["levels"], Rs[0], ts[0], **G.tries_kw(sc))
     outs = {k: capi.CTTrackResult() for k in libs}
-    t = {k: [] for k in libs}
-    names = list(libs)
-    for rep in range(warmup + reps):
-        for j in range(2):
-            k = names[(rep + j) % 2]
-            t0 = time.perf_counter()
-            rc = libs[k].dmv_ct_track(hs[k], C.byref(A), C.byref(outs[k]))
-            dt = time.perf_counter() - t0
-            if rc != 0:
-                raise SystemExit(f"dmv_ct_track through {k}: error {rc}")
-            if rep >= warmup:
-                t[k].append(dt)
+    arms = {k: (lambda k=k: libs[k].dmv_ct_track(gs[k].h, C.byref(A), C.byref(outs[k]))) for k in libs}
+    t = K.alternate(arms, warmup, reps, "dmv_ct_track A/B", libs)
     same = bytes(outs["this"]) == bytes(outs["parent"])
-    for k, L in libs.items():
-        L.dmv_ct_destroy(hs[k])
-    return dict(parent_lib=os.path.basename(path), bit_identical=same, **{k: stats(t[k]) for k in libs}), same
+    G.close(*gs.values())
+    return dict(parent_lib=os.path.basename(path), bit_identical=same, **{k: K.stats(t[k]) for k in libs}), same
 
 
 def main():
@@ -165,23 +112,19 @@ def main():
     ap.add_argument("--warmup", type=int, default=30)
     ap.add_argument("--reps", type=int, default=300)
     ap.add_argument("--parent-lib", default=None, help="another build of libdmvio_b200.so for the dmv_ct_track A/B")
-    ap.add_argument("--out", default=os.path.join(ROOT, "records", "h100_track_tries.json"))
+    ap.add_argument("--out", default=os.path.join(K.ROOT, "records", "h100_track_tries.json"))
     a = ap.parse_args()
     os.environ.pop("DMV_CT_CLUSTER", None)
     import dmvio_b200.capi as capi
     import dmvio_b200.synth as synth
-    import helpers as H
-    import test_gpu_track_tries as T
     from oracle import orc
-    L = capi.lib()
-    if L.dmv_device_count() < 1:
-        raise SystemExit("bench_track_tries needs a CUDA device")
-    sc = H.ct_scene(orc, synth, "bench")
-    gs = {arm: T.handle(capi, sc) for arm in ("host", "device")}
-    res = dict(card=card(), shape=[sc["w"], sc["h"]], levels=sc["levels"], tries=31, warmup=a.warmup, reps=a.reps,
+    L = K.device_lib("bench_track_tries")
+    sc = G.ct_scene(orc, synth, "bench")
+    gs = {arm: G.ct_handle(capi, sc) for arm in ("host", "device")}
+    res = dict(card=K.card(), shape=[sc["w"], sc["h"]], levels=sc["levels"], tries=31, warmup=a.warmup, reps=a.reps,
                timing="wall clock per call, each call ending in a synchronisation; ctypes argument blocks built once", workloads={})
     identical = True
-    for name, Rs, ts, k, Lc in workloads(capi, T, sc, gs["host"]):
+    for name, Rs, ts, k, Lc in workloads(capi, sc, gs["host"]):
         host = HostLoop(capi, L, gs["host"], Rs, ts, k, Lc)
         targs, keep = capi._tries_args(sc["levels"], Rs, ts, lastCoarseRMSE0=Lc, **k)
         out = capi.CTTriesResult()
@@ -189,35 +132,24 @@ def main():
         if name == "easy":
             A0, o0 = capi._track_args(sc["levels"], Rs[0], ts[0], **k), capi.CTTrackResult()
             arms["single"] = lambda: L.dmv_ct_track(gs["host"].h, C.byref(A0), C.byref(o0))
-        names = list(arms)
-        t = {q: [] for q in names}
-        for rep in range(a.warmup + a.reps):
-            for j in range(len(names)):
-                q = names[(rep + j) % len(names)]
-                t0 = time.perf_counter()
-                rc = arms[q]()
-                dt = time.perf_counter() - t0
-                if rc != 0:
-                    raise SystemExit(f"{q} on {name}: dmvio_b200 error {rc}: {L.dmv_last_error().decode()}")
-                if rep >= a.warmup:
-                    t[q].append(dt)
+        t = K.alternate(arms, a.warmup, a.reps, f"on {name}", dict.fromkeys(arms, L))
         # identity and counts, outside the timed loop: one more call of each arm
         row = dict(lastCoarseRMSE0=Lc)
         for q in ("host", "device"):
             arms[q]()
             r = host.res if q == "host" else out
-            row[q] = dict(stats(t[q]), tries=r.tries, point_evaluations=host.pe if q == "host" else gs[q].point_evaluations())
+            row[q] = dict(K.stats(t[q]), tries=r.tries, point_evaluations=host.pe if q == "host" else gs[q].point_evaluations())
         row.update(winner=host.res.winner, haveOneGood=host.res.haveOneGood)
         same = bytes(out) == bytes(host.res) and row["device"]["point_evaluations"] == row["host"]["point_evaluations"]
         row["bit_identical"] = same
         identical = identical and same
         if name == "easy":
-            row["single"] = stats(t["single"])
+            row["single"] = K.stats(t["single"])
             row["device_over_single"] = row["device"]["median_ms"] / row["single"]["median_ms"]
         row["device_over_host"] = row["device"]["median_ms"] / row["host"]["median_ms"]
         res["workloads"][name] = row
     if a.parent_lib:
-        res["track_vs_parent"], same = parent_ab(capi, T, sc, a.parent_lib, a.warmup, a.reps)
+        res["track_vs_parent"], same = parent_ab(capi, sc, a.parent_lib, a.warmup, a.reps)
         identical = identical and same
     res["bit_identical"] = identical
     for g in gs.values():
