@@ -93,8 +93,8 @@ int dmv_ba_create(const dmv_ba_config* cfg, dmv_ba** out) {
   }
   dmv_ba* b = new dmv_ba();
   const int rc = ba_allocate(b, cfg);
-  if (rc != DMV_OK) {  // e.g. out of device memory half-way: release what was allocated (the error message of the failing call is kept)
-    dmv_ba_destroy(b);
+  if (rc != DMV_OK) {  // e.g. out of device memory half-way: the members release what was allocated (the failing call's message is kept)
+    delete b;
     return rc;
   }
   *out = b;
@@ -118,49 +118,48 @@ static int ba_allocate(dmv_ba* b, const dmv_ba_config* cfg) {
   const int MF = MAXF, mp = b->mp;
   b->max_chunks = (mp + (b->P_auto ? 16 : b->P) - 1) / (b->P_auto ? 16 : b->P) + MF;
   const size_t npx = (size_t)cfg->w * cfg->h;
-  CK(cudaStreamCreateWithFlags(&b->stream, cudaStreamNonBlocking));
-  for (int i = 0; i < 4; i++) CK(cudaEventCreate(&b->ev[i]));
-  for (int f = 0; f < cfg->max_frames; f++) CK(cudaMalloc(&b->d_img[f], npx * sizeof(float4)));
-  CK(cudaMalloc(&b->d_stage_img, npx * 3 * sizeof(float)));
-  CK(cudaMalloc(&b->d_adj, sizeof(BAAdj)));
-  CK(cudaMalloc(&b->d_uv, sizeof(float2) * mp));
-  CK(cudaMalloc(&b->d_idepth[0], sizeof(float) * mp));
-  CK(cudaMalloc(&b->d_idepth[1], sizeof(float) * mp));
-  CK(cudaMalloc(&b->d_idepth_zero, sizeof(float) * mp));
-  CK(cudaMalloc(&b->d_color, sizeof(float) * mp * 8));
-  CK(cudaMalloc(&b->d_weights, sizeof(float) * mp * 8));
-  CK(cudaMalloc(&b->d_priorF, sizeof(float) * mp));
-  CK(cudaMalloc(&b->d_st_in, (size_t)MF * mp));
-  CK(cudaMalloc(&b->d_en_in, sizeof(float) * MF * mp));
+  CK(cudaStreamCreateWithFlags(b->stream.put(), cudaStreamNonBlocking));
+  for (int i = 0; i < 4; i++) CK(cudaEventCreate(b->ev[i].put()));
+  for (int f = 0; f < cfg->max_frames; f++) CK(b->d_img[f].alloc(npx));
+  CK(b->d_stage_img.alloc(npx * 3));
+  CK(b->d_adj.alloc(1));
+  CK(b->d_uv.alloc(mp));
+  CK(b->d_idepth[0].alloc(mp));
+  CK(b->d_idepth[1].alloc(mp));
+  CK(b->d_idepth_zero.alloc(mp));
+  CK(b->d_color.alloc((size_t)mp * 8));
+  CK(b->d_weights.alloc((size_t)mp * 8));
+  CK(b->d_priorF.alloc(mp));
+  CK(b->d_st_in.alloc((size_t)MF * mp));
+  CK(b->d_en_in.alloc((size_t)MF * mp));
   const int maxT0 = (8 * MF + 4 + 1 + 3) / 4, maxTiles0 = maxT0 * (maxT0 + 1) / 2;
   for (int k = 0; k < 2; k++) {
-    CK(cudaMalloc(&b->d_st_new[k], (size_t)MF * mp));
+    CK(b->d_st_new[k].alloc((size_t)MF * mp));
     CK(cudaMemset(b->d_st_new[k], 0xff, (size_t)MF * mp));
-    CK(cudaMalloc(&b->d_en_new[k], sizeof(float) * MF * mp));
-    CK(cudaMalloc(&b->d_en_wo[k], sizeof(float) * MF * mp));
-    CK(cudaMalloc(&b->d_cpt[k], sizeof(float) * 3 * MF * mp));
-    CK(cudaMalloc(&b->d_jpjd[k], sizeof(float) * 8 * MF * mp));
-    CK(cudaMalloc(&b->d_pout[k], sizeof(float) * 8 * mp));
+    CK(b->d_en_new[k].alloc((size_t)MF * mp));
+    CK(b->d_en_wo[k].alloc((size_t)MF * mp));
+    CK(b->d_cpt[k].alloc((size_t)3 * MF * mp));
+    CK(b->d_jpjd[k].alloc((size_t)8 * MF * mp));
+    CK(b->d_pout[k].alloc((size_t)8 * mp));
     CK(cudaMemset(b->d_pout[k], 0, sizeof(float) * 8 * mp));
-    CK(cudaMalloc(&b->d_result[k], sizeof(double) * result_doubles(8 * MF + 4, maxTiles0)));
-    CK(cudaMallocHost(&b->h_result[k], sizeof(double) * result_doubles(8 * MF + 4, maxTiles0)));
+    CK(b->d_result[k].alloc(result_doubles(8 * MF + 4, maxTiles0)));
+    CK(b->h_result[k].alloc(result_doubles(8 * MF + 4, maxTiles0)));
   }
-  CK(cudaMalloc(&b->d_step, sizeof(float) * mp));
+  CK(b->d_step.alloc(mp));
   CK(cudaMemset(b->d_step, 0, sizeof(float) * mp));
-  CK(cudaMalloc(&b->d_part, sizeof(double) * PART_STRIDE * (size_t)b->max_chunks));
-  CK(cudaMalloc(&b->d_dtab, sizeof(int4) * 2 * DITEMS_MAX));
-  CK(cudaMalloc(&b->d_wg, sizeof(float4) * (size_t)maxT0 * mp));
-  CK(cudaMalloc(&b->d_hdig, sizeof(float) * mp));
-  CK(cudaMalloc(&b->d_hdi_solve, sizeof(float) * mp));
-  CK(cudaMalloc(&b->d_bar, sizeof(unsigned int)));
+  CK(b->d_part.alloc((size_t)PART_STRIDE * b->max_chunks));
+  CK(b->d_dtab.alloc(2 * DITEMS_MAX));
+  CK(b->d_wg.alloc((size_t)maxT0 * mp));
+  CK(b->d_hdig.alloc(mp));
+  CK(b->d_hdi_solve.alloc(mp));
+  CK(b->d_bar.alloc(1));
   CK(cudaMemset(b->d_bar, 0, sizeof(unsigned int)));
-  CK(cudaMalloc(&b->d_resub_sums, sizeof(double) * 4));
-  CK(cudaMallocHost(&b->h_up, sizeof(HostUpload)));
-  CK(cudaMallocHost(&b->h_adj, sizeof(BAAdj)));
+  CK(b->d_resub_sums.alloc(4));
+  CK(b->h_up.alloc(1));
+  CK(b->h_adj.alloc(1));
   std::memset(b->h_up, 0, sizeof(HostUpload));
-  b->scratch_floats = std::max((size_t)mp * std::max(8 * MF, 21), npx * 3);   // 21 floats per point: the staged upload of dmv_ba_set_points
-  CK(cudaMallocHost(&b->h_scratch, sizeof(float) * b->scratch_floats));
-  CK(cudaMallocHost(&b->h_en_newest, sizeof(float) * mp));
+  CK(b->h_scratch.alloc(std::max((size_t)mp * std::max(8 * MF, 21), npx * 3)));   // 21 floats per point: the staged upload of dmv_ba_set_points
+  CK(b->h_en_newest.alloc(mp));
   for (int f = 0; f < MF; f++) b->slots[f] = f;
   return DMV_OK;
 }
@@ -169,27 +168,9 @@ int dmv_ba_destroy(dmv_ba* b) {
   if (!b) return DMV_OK;
   cudaSetDevice(b->device);
   if (b->stream) cudaStreamSynchronize(b->stream);
-  for (int f = 0; f < MAXF; f++) cudaFree(b->d_img[f]);
-  cudaFree(b->d_stage_img); cudaFree(b->d_adj); cudaFree(b->d_uv); cudaFree(b->d_idepth[0]); cudaFree(b->d_idepth[1]);
-  cudaFree(b->d_idepth_zero); cudaFree(b->d_color); cudaFree(b->d_weights); cudaFree(b->d_priorF);
-  cudaFree(b->d_st_in); cudaFree(b->d_en_in);
-  for (int k = 0; k < 2; k++) {
-    cudaFree(b->d_st_new[k]); cudaFree(b->d_en_new[k]); cudaFree(b->d_en_wo[k]); cudaFree(b->d_cpt[k]); cudaFree(b->d_jpjd[k]);
-    cudaFree(b->d_pout[k]); cudaFree(b->d_result[k]); cudaFreeHost(b->h_result[k]);
-  }
-  cudaFree(b->d_step); cudaFree(b->d_resub_sums); cudaFree(b->d_flush);
-  cudaFree(b->d_part); cudaFree(b->d_dtab); cudaFree(b->d_wg); cudaFree(b->d_hdig); cudaFree(b->d_hdi_solve); cudaFree(b->d_bar);
-  cudaFreeHost(b->h_up); cudaFreeHost(b->h_adj); cudaFreeHost(b->h_scratch); cudaFreeHost(b->h_en_newest);
-  for (int i = 0; i < 4; i++) if (b->ev[i]) cudaEventDestroy(b->ev[i]);
   if (b->nccl_comm) dmv::nccl_destroy(b->nccl_comm);
-  cudaFree(b->d_act); cudaFreeHost(b->h_act);
-  cudaFree(b->d_sel); cudaFreeHost(b->h_sel);
-  cudaFree(b->d_marg); cudaFree(b->d_marg_mask); cudaFree(b->d_marg_rtz); cudaFree(b->d_marg_result);
-  cudaFreeHost(b->h_marg_result);
   for (int r = 0; r < XCHG_MAXR; r++)
-    if (b->xchg_map[r] && b->xchg_map[r] != b->xchg_own) cudaIpcCloseMemHandle(b->xchg_map[r]);
-  cudaFree(b->xchg_own);
-  if (b->stream) cudaStreamDestroy(b->stream);
+    if (b->xchg_map[r] && b->xchg_map[r] != b->xchg_own.get()) cudaIpcCloseMemHandle(b->xchg_map[r]);
   delete b;
   return DMV_OK;
 }
@@ -716,13 +697,13 @@ int dmv_ba_marginalize_points(dmv_ba* b, const dmv_ba_marg_args* a) {
   CK(cudaSetDevice(b->device));
   const int nf = b->nf, N = b->N;
   const size_t nres_d = result_doubles(N, b->ntiles), nslots = (size_t)MAXF * b->mp;
-  if (!b->d_marg) {
-    CK(cudaMalloc(&b->d_marg, sizeof(BAMarg)));
-    CK(cudaMalloc(&b->d_marg_mask, b->mp));
-    CK(cudaMalloc(&b->d_marg_rtz, sizeof(float) * 8 * nslots));
+  if (!b->h_marg_result) {   // the last of the group: set only once all of it is (a failed attempt leaves it empty, alloc replaces the rest)
+    CK(b->d_marg.alloc(1));
+    CK(b->d_marg_mask.alloc(b->mp));
+    CK(b->d_marg_rtz.alloc(8 * nslots));
     const size_t maxres = result_doubles(8 * MAXF + 4, ((2 * MAXF + 2) * (2 * MAXF + 3)) / 2);
-    CK(cudaMalloc(&b->d_marg_result, sizeof(double) * maxres));
-    CK(cudaHostAlloc(&b->h_marg_result, sizeof(double) * maxres, cudaHostAllocDefault));
+    CK(b->d_marg_result.alloc(maxres));
+    CK(b->h_marg_result.alloc(maxres));
   }
   // tables
   BAMarg M;
@@ -789,7 +770,7 @@ int dmv_ba_marginalize_points(dmv_ba* b, const dmv_ba_marg_args* a) {
 }
 
 static int fetch_f(dmv_ba* b, const float* dsrc, size_t n) {
-  if (n > b->scratch_floats) return set_error(DMV_ERR_INVALID, "scratch too small");
+  if (n > b->h_scratch.size()) return set_error(DMV_ERR_INVALID, "scratch too small");
   CK(cudaMemcpyAsync(b->h_scratch, dsrc, n * sizeof(float), cudaMemcpyDeviceToHost, b->stream));
   CK(cudaStreamSynchronize(b->stream));
   return DMV_OK;
@@ -900,7 +881,7 @@ extern "C" int dmv_ba_p2p_export(dmv_ba* b, void* ipc_handle64) {
     const int maxT = (8 * MAXF + 4 + 1 + 3) / 4, maxTiles = maxT * (maxT + 1) / 2;
     b->xchg_pitch = (result_doubles(8 * MAXF + 4, maxTiles) + 7) & ~7;
     const size_t bytes = (size_t)2 * XCHG_MAXR * b->xchg_pitch * sizeof(uint4);
-    CK(cudaMalloc(&b->xchg_own, bytes));
+    CK(b->xchg_own.alloc((size_t)2 * XCHG_MAXR * b->xchg_pitch));
     CK(cudaMemset(b->xchg_own, 0, bytes));
     CK(cudaDeviceSynchronize());
   }

@@ -5,6 +5,7 @@
 // same hot path (offline re-optimisation / several sessions per GPU); per window the results are bit-identical to its own launch.
 #include "ba_handle.h"
 #include <cstring>
+#include <memory>
 
 using namespace dmv;
 
@@ -17,12 +18,12 @@ struct dmv_ba_batch {
   std::vector<dmv_ba*> h;
   int device = 0, P = 16, max_nf = 2;
   cudaStream_t stream = nullptr;   // = the first handle's stream
-  BatchUpload* h_up = nullptr;     // pinned staging
-  BAWinDev* d_win = nullptr;
-  BAIter* d_it = nullptr;
-  unsigned int* d_bar = nullptr;
+  PinnedBuf<BatchUpload> h_up;     // pinned staging
+  DevBuf<BAWinDev> d_win;
+  DevBuf<BAIter> d_it;
+  DevBuf<unsigned int> d_bar;
   unsigned int bar_count = 0;
-  cudaEvent_t ev[2] = {nullptr, nullptr};
+  Event ev[2];
   float last_ms = 0.f;
   bool timing = false;
 };
@@ -38,19 +39,19 @@ int dmv_ba_batch_create(dmv_ba* const* handles, int n, dmv_ba_batch** out) {
     if (handles[i]->device != handles[0]->device || handles[i]->P != handles[0]->P) return set_error(DMV_ERR_INVALID, "all handles of a batch must share the device and chunk_points");
     if (handles[i]->nranks > 1) return set_error(DMV_ERR_INVALID, "sharded handles cannot be batched");
   }
-  dmv_ba_batch* B = new dmv_ba_batch();
+  std::unique_ptr<dmv_ba_batch> B(new dmv_ba_batch());   // a failed call below releases what was allocated
   B->h.assign(handles, handles + n);
   B->device = handles[0]->device;
   B->P = handles[0]->P;
   B->stream = handles[0]->stream;
   CK(cudaSetDevice(B->device));
-  CK(cudaMallocHost(&B->h_up, sizeof(BatchUpload)));
-  CK(cudaMalloc(&B->d_win, sizeof(BAWinDev) * BATCH_MAX));
-  CK(cudaMalloc(&B->d_it, sizeof(BAIter) * BATCH_MAX));
-  CK(cudaMalloc(&B->d_bar, sizeof(unsigned int)));
+  CK(B->h_up.alloc(1));
+  CK(B->d_win.alloc(BATCH_MAX));
+  CK(B->d_it.alloc(BATCH_MAX));
+  CK(B->d_bar.alloc(1));
   CK(cudaMemset(B->d_bar, 0, sizeof(unsigned int)));
-  for (int i = 0; i < 2; i++) CK(cudaEventCreate(&B->ev[i]));
-  *out = B;
+  for (int i = 0; i < 2; i++) CK(cudaEventCreate(B->ev[i].put()));
+  *out = B.release();
   return DMV_OK;
 }
 
@@ -58,8 +59,6 @@ int dmv_ba_batch_destroy(dmv_ba_batch* B) {
   if (!B) return DMV_OK;
   cudaSetDevice(B->device);
   cudaStreamSynchronize(B->stream);
-  cudaFreeHost(B->h_up); cudaFree(B->d_win); cudaFree(B->d_it); cudaFree(B->d_bar);
-  for (int i = 0; i < 2; i++) if (B->ev[i]) cudaEventDestroy(B->ev[i]);
   delete B;
   return DMV_OK;
 }

@@ -20,15 +20,14 @@ static int bench_loop(dmv_ba* b, const double* x, int iters, int flush_l2, std::
   if (x && !b->have_committed) return set_error(DMV_ERR_STATE, "no committed linearisation to resubstitute");
   CK(cudaSetDevice(b->device));
   if (flush_l2 && !b->d_flush) {
-    b->flush_n = (size_t)256 * 1024 * 1024 / sizeof(float4);  // 256 MiB > 50 MB L2
-    CK(cudaMalloc(&b->d_flush, b->flush_n * sizeof(float4)));
-    CK(cudaMemset(b->d_flush, 0, b->flush_n * sizeof(float4)));
+    CK(b->d_flush.alloc((size_t)256 * 1024 * 1024 / sizeof(float4)));  // 256 MiB > 50 MB L2
+    CK(cudaMemset(b->d_flush, 0, b->d_flush.size() * sizeof(float4)));
   }
   if (x) dmv_ba_stage_x(b, x); else b->h_up->it.have_x = 0;
-  std::vector<cudaEvent_t> e(3 * (size_t)iters);
-  for (auto& ev : e) CK(cudaEventCreate(&ev));
+  std::vector<Event> e(3 * (size_t)iters);
+  for (auto& ev : e) CK(cudaEventCreate(ev.put()));
   for (int i = 0; i < iters; i++) {
-    if (flush_l2) launch_l2_flush(b->d_flush, b->flush_n, b->stream);
+    if (flush_l2) launch_l2_flush(b->d_flush, b->d_flush.size(), b->stream);
     dmv_ba_fill_descriptor(b);
     dmv_ba_next_exchange(b);
     HostUpload& U = *b->h_up;
@@ -52,7 +51,6 @@ static int bench_loop(dmv_ba* b, const double* x, int iters, int flush_l2, std::
     if (b->nccl_comm && !b->xchg_on) cudaEventElapsedTime(&ms[i], e[3 * i], e[3 * i + 2]);
     else ms[i] = ms_k[i];  // the step IS the kernel (the peer exchange, if any, happens inside it)
   }
-  for (auto& ev : e) cudaEventDestroy(ev);
   b->h_up->it.have_x = 0;
   b->have_tentative = true;
   return DMV_OK;
@@ -80,16 +78,14 @@ int dmv_ba_bench_phases(dmv_ba* b, const double* x, int iters, int flush_l2, int
   if (b->h_up->win.nchunks > max_ctas) return set_error(DMV_ERR_INVALID, "max_ctas below the window's chunk count");
   const size_t n = (size_t)iters * max_ctas * FUSED_NCLK;
   CK(cudaSetDevice(b->device));
-  unsigned long long* d_clk = nullptr;
-  CK(cudaMalloc(&d_clk, n * sizeof(unsigned long long)));
-  if (cudaMemset(d_clk, 0, n * sizeof(unsigned long long)) != cudaSuccess) rc = set_error(DMV_ERR_CUDA, "cudaMemset failed");
+  DevBuf<unsigned long long> d_clk;
+  CK(d_clk.alloc(n));
+  CK(cudaMemset(d_clk, 0, n * sizeof(unsigned long long)));
   std::vector<float> ms, ms_k;
   int grid = 0;
-  if (rc == DMV_OK) rc = bench_loop(b, x, iters, flush_l2, ms, ms_k, d_clk, max_ctas, &grid);
-  if (rc == DMV_OK && cudaMemcpy(stamps, d_clk, n * sizeof(unsigned long long), cudaMemcpyDeviceToHost) != cudaSuccess)
-    rc = set_error(DMV_ERR_CUDA, "cudaMemcpy failed");
-  cudaFree(d_clk);
+  rc = bench_loop(b, x, iters, flush_l2, ms, ms_k, d_clk, max_ctas, &grid);
   if (rc != DMV_OK) return rc;
+  CK(cudaMemcpy(stamps, d_clk, n * sizeof(unsigned long long), cudaMemcpyDeviceToHost));
   *n_ctas = grid;
   for (int i = 0; i < iters; i++) ms_kernel[i] = ms_k[i];
   return DMV_OK;

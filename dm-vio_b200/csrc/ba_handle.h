@@ -26,8 +26,8 @@ struct dmv_ba {
   dmv_ba_config cfg;
   dmv_ba_params prm;
   int device = 0;
-  cudaStream_t stream = nullptr;
-  cudaEvent_t ev[4] = {nullptr, nullptr, nullptr, nullptr};
+  dmv::Stream stream;
+  dmv::Event ev[4];
   int P = 16;            // points per chunk of the CURRENT window (16 or 32)
   bool P_auto = true;    // dmv_ba_config::chunk_points == 0: chosen per window in dmv_ba_set_points
   int sms = 132;
@@ -36,42 +36,39 @@ struct dmv_ba {
   int N = 0, NW = 0, T = 0, ntiles = 0;
   int slots[MAXF];
   // device buffers
-  float4* d_img[MAXF] = {nullptr};
-  float* d_stage_img = nullptr;
-  BAAdj* d_adj = nullptr;
-  float2* d_uv = nullptr;
-  float* d_idepth[2] = {nullptr, nullptr};  // ping-pong: [cur] current depths, [bak] FullSystem::backupState copy
+  dmv::DevBuf<float4> d_img[MAXF];
+  dmv::DevBuf<float> d_stage_img;
+  dmv::DevBuf<BAAdj> d_adj;
+  dmv::DevBuf<float2> d_uv;
+  dmv::DevBuf<float> d_idepth[2];           // ping-pong: [cur] current depths, [bak] FullSystem::backupState copy
   int id_cur = 0, id_bak = 0;
   bool zero_alias = false;                  // idepth_zero == idepth (true after any step / restore)
-  float *d_idepth_zero = nullptr, *d_color = nullptr, *d_weights = nullptr, *d_priorF = nullptr;
-  uint8_t* d_st_in = nullptr;
-  float* d_en_in = nullptr;
-  uint8_t* d_st_new[2] = {nullptr, nullptr};
-  float *d_en_new[2] = {nullptr, nullptr}, *d_en_wo[2] = {nullptr, nullptr}, *d_cpt[2] = {nullptr, nullptr}, *d_jpjd[2] = {nullptr, nullptr},
-        *d_pout[2] = {nullptr, nullptr};
-  double* d_result[2] = {nullptr, nullptr};
-  float* d_step = nullptr;
-  double* d_part = nullptr;        // [max_chunks][PART_STRIDE] per-chunk partial blobs (scratch of one launch)
-  int4* d_dtab = nullptr;          // phase D items [DITEMS_MAX][2] of the current window shape (dmv_ba_set_points)
+  dmv::DevBuf<float> d_idepth_zero, d_color, d_weights, d_priorF;
+  dmv::DevBuf<uint8_t> d_st_in;
+  dmv::DevBuf<float> d_en_in;
+  dmv::DevBuf<uint8_t> d_st_new[2];
+  dmv::DevBuf<float> d_en_new[2], d_en_wo[2], d_cpt[2], d_jpjd[2], d_pout[2];
+  dmv::DevBuf<double> d_result[2];
+  dmv::DevBuf<float> d_step;
+  dmv::DevBuf<double> d_part;      // [max_chunks][PART_STRIDE] per-chunk partial blobs (scratch of one launch)
+  dmv::DevBuf<int4> d_dtab;        // phase D items [DITEMS_MAX][2] of the current window shape (dmv_ba_set_points)
   std::vector<int4> h_dtab;
   int nditems = 0;
-  float4* d_wg = nullptr;          // [WG_GROUPS][mp] Schur vectors, transposed (scratch)
-  float* d_hdig = nullptr;         // [mp] HdiF (scratch)
-  float* d_hdi_solve = nullptr;    // [mp] HdiF of the linearisation the last dmv_ba_accumulate returned (PointHessian::idepth_hessian)
+  dmv::DevBuf<float4> d_wg;        // [WG_GROUPS][mp] Schur vectors, transposed (scratch)
+  dmv::DevBuf<float> d_hdig;       // [mp] HdiF (scratch)
+  dmv::DevBuf<float> d_hdi_solve;  // [mp] HdiF of the linearisation the last dmv_ba_accumulate returned (PointHessian::idepth_hessian)
   int hdi_solve_n = 0;
-  unsigned int* d_bar = nullptr;   // grid-barrier arrival counter
+  dmv::DevBuf<unsigned int> d_bar; // grid-barrier arrival counter
   unsigned int bar_count = 0;      // arrivals issued so far (monotonic, wraps)
-  double* d_resub_sums = nullptr;
-  float4* d_flush = nullptr;
-  size_t flush_n = 0;
+  dmv::DevBuf<double> d_resub_sums;
+  dmv::DevBuf<float4> d_flush;     // L2 scrub of the benches, allocated on first use
   // pinned host
-  HostUpload* h_up = nullptr;
-  BAAdj* h_adj = nullptr;
-  double* h_result[2] = {nullptr, nullptr};
-  float* h_scratch = nullptr;  // max(mp*8, w*h*3) floats
-  float* h_en_newest = nullptr; // [mp] en_wo of the residuals targeting the newest frame, written by the kernel itself (zero-copy)
+  dmv::PinnedBuf<HostUpload> h_up;
+  dmv::PinnedBuf<BAAdj> h_adj;
+  dmv::PinnedBuf<double> h_result[2];
+  dmv::PinnedBuf<float> h_scratch;  // max(mp*8, w*h*3) floats
+  dmv::PinnedBuf<float> h_en_newest; // [mp] en_wo of the residuals targeting the newest frame, written by the kernel itself (zero-copy)
   bool en_newest_valid = false; // h_en_newest belongs to the linearisation the getters read (tentative if any, else committed)
-  size_t scratch_floats = 0;
   // host bookkeeping
   int host_start[MAXF + 1];
   int chunk_beg[MAXF + 1];
@@ -90,20 +87,19 @@ struct dmv_ba {
   // NCCL
   void* nccl_comm = nullptr;
   int nranks = 1, rank = 0;
-  // marginalisation launch (dmv_ba_marginalize_points): allocated on first use
-  BAMarg* d_marg = nullptr;
-  uint8_t* d_marg_mask = nullptr;
-  float* d_marg_rtz = nullptr;
-  double* d_marg_result = nullptr;
-  double* h_marg_result = nullptr;
-  float* d_act = nullptr;      // point-activation staging (dmv_ba_activate_points)
-  float* h_act = nullptr;
-  int act_cap = 0;
-  float* d_sel = nullptr;      // activation-selection staging and scratch (dmv_ba_select_activation, ip_select.cu)
-  float* h_sel = nullptr;
-  size_t sel_words = 0;
+  // marginalisation launch (dmv_ba_marginalize_points): allocated on first use, as a whole
+  dmv::DevBuf<BAMarg> d_marg;
+  dmv::DevBuf<uint8_t> d_marg_mask;
+  dmv::DevBuf<float> d_marg_rtz;
+  dmv::DevBuf<double> d_marg_result;
+  dmv::PinnedBuf<double> h_marg_result;
+  dmv::DevBuf<float> d_act;    // point-activation staging (dmv_ba_activate_points)
+  dmv::PinnedBuf<float> h_act;
+  int act_cap = 0;             // points the staging layout holds (0 while d_act / h_act may be short of it)
+  dmv::DevBuf<float> d_sel;    // activation-selection staging and scratch (dmv_ba_select_activation, ip_select.cu)
+  dmv::PinnedBuf<float> h_sel;
   // peer-memory exchange (inside ba_fused_kernel)
-  void* xchg_own = nullptr;                 // this rank's inbox (cudaMalloc, exported through CUDA IPC)
+  dmv::DevBuf<uint4> xchg_own;              // this rank's inbox (exported through CUDA IPC)
   void* xchg_map[XCHG_MAXR] = {nullptr};    // every rank's inbox as mapped here ([rank] == xchg_own)
   int xchg_pitch = 0;
   bool xchg_on = false;

@@ -212,19 +212,20 @@ using namespace dmv;
 struct dmv_ci {
   dmv_ci_config cfg;
   int device = 0;
-  cudaStream_t stream = nullptr;
+  Stream stream;
   int w[DMV_MAX_PYR_LEVELS], h[DMV_MAX_PYR_LEVELS], n[DMV_MAX_PYR_LEVELS];
   float fx[DMV_MAX_PYR_LEVELS], fy[DMV_MAX_PYR_LEVELS], cx[DMV_MAX_PYR_LEVELS], cy[DMV_MAX_PYR_LEVELS];
   bool haveK[DMV_MAX_PYR_LEVELS], haveFirst[DMV_MAX_PYR_LEVELS], haveNew[DMV_MAX_PYR_LEVELS];
-  float4 *d_first[DMV_MAX_PYR_LEVELS] = {nullptr}, *d_new[DMV_MAX_PYR_LEVELS] = {nullptr};
-  float* d_stage = nullptr;                 // AoS3 staging of one level-0 plane
-  float* d_static[DMV_MAX_PYR_LEVELS] = {nullptr};   // u | v | outlierTH          (3 * max_points)
-  float* d_in = nullptr;                    // idepth_new | energy(2) | iR           (4 * max_points)
-  unsigned char* d_good = nullptr;          // isGood | isGood_new                   (2 * max_points)
-  float* d_outp = nullptr;                  // energy_new(2) | maxstep | lastHessian_new | Jb(10)   (14 * max_points)
-  float* h_pin = nullptr;                   // pinned staging, 18 * max_points floats + bytes
-  double *d_partial = nullptr, *d_out = nullptr, *h_out = nullptr;
-  unsigned int* d_ticket = nullptr;
+  DevBuf<float4> d_first[DMV_MAX_PYR_LEVELS], d_new[DMV_MAX_PYR_LEVELS];
+  DevBuf<float> d_stage;                    // AoS3 staging of one level-0 plane
+  DevBuf<float> d_static[DMV_MAX_PYR_LEVELS];   // u | v | outlierTH          (3 * max_points)
+  DevBuf<float> d_in;                       // idepth_new | energy(2) | iR           (4 * max_points)
+  DevBuf<unsigned char> d_good;             // isGood | isGood_new                   (2 * max_points)
+  DevBuf<float> d_outp;                     // energy_new(2) | maxstep | lastHessian_new | Jb(10)   (14 * max_points)
+  PinnedBuf<float> h_pin;                   // pinned staging, 18 * max_points floats + bytes
+  DevBuf<double> d_partial, d_out;
+  PinnedBuf<double> h_out;
+  DevBuf<unsigned int> d_ticket;
   int grid_max = 0;
   long long launches = 0;
 };
@@ -243,8 +244,8 @@ int dmv_ci_create(const dmv_ci_config* cfg, dmv_ci** out) {
   CK(cudaSetDevice(cfg->device));
   dmv_ci* c = new dmv_ci();
   const int rc = ci_allocate(c, cfg);
-  if (rc != DMV_OK) {  // allocation failed half-way: release what exists, keep the failing call's error message
-    dmv_ci_destroy(c);
+  if (rc != DMV_OK) {  // allocation failed half-way: the members release what exists, the failing call's error message is kept
+    delete c;
     return rc;
   }
   *out = c;
@@ -254,27 +255,27 @@ int dmv_ci_create(const dmv_ci_config* cfg, dmv_ci** out) {
 static int ci_allocate(dmv_ci* c, const dmv_ci_config* cfg) {
   c->cfg = *cfg;
   c->device = cfg->device;
-  CK(cudaStreamCreateWithFlags(&c->stream, cudaStreamNonBlocking));
+  CK(cudaStreamCreateWithFlags(c->stream.put(), cudaStreamNonBlocking));
   const size_t mp = (size_t)cfg->max_points;
   for (int l = 0; l < cfg->levels; l++) {
     c->w[l] = cfg->w >> l; c->h[l] = cfg->h >> l; c->n[l] = 0;
     c->haveK[l] = c->haveFirst[l] = c->haveNew[l] = false;
-    CK(cudaMalloc(&c->d_first[l], sizeof(float4) * (size_t)c->w[l] * c->h[l]));
-    CK(cudaMalloc(&c->d_new[l], sizeof(float4) * (size_t)c->w[l] * c->h[l]));
-    CK(cudaMalloc(&c->d_static[l], sizeof(float) * 3 * mp));
+    CK(c->d_first[l].alloc((size_t)c->w[l] * c->h[l]));
+    CK(c->d_new[l].alloc((size_t)c->w[l] * c->h[l]));
+    CK(c->d_static[l].alloc(3 * mp));
   }
-  CK(cudaMalloc(&c->d_stage, sizeof(float) * 3 * (size_t)cfg->w * cfg->h));
-  CK(cudaMalloc(&c->d_in, sizeof(float) * 4 * mp));
-  CK(cudaMalloc(&c->d_good, 2 * mp));
-  CK(cudaMalloc(&c->d_outp, sizeof(float) * 14 * mp));
-  CK(cudaMallocHost(&c->h_pin, sizeof(float) * 20 * mp));
+  CK(c->d_stage.alloc(3 * (size_t)cfg->w * cfg->h));
+  CK(c->d_in.alloc(4 * mp));
+  CK(c->d_good.alloc(2 * mp));
+  CK(c->d_outp.alloc(14 * mp));
+  CK(c->h_pin.alloc(20 * mp));
   int sms = 0;
   CK(cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, c->device));
   c->grid_max = 2 * sms;
-  CK(cudaMalloc(&c->d_partial, sizeof(double) * CI_NRED * (size_t)c->grid_max));
-  CK(cudaMalloc(&c->d_out, sizeof(double) * CI_NRED));
-  CK(cudaMallocHost(&c->h_out, sizeof(double) * CI_NRED));
-  CK(cudaMalloc(&c->d_ticket, sizeof(unsigned int)));
+  CK(c->d_partial.alloc((size_t)CI_NRED * c->grid_max));
+  CK(c->d_out.alloc(CI_NRED));
+  CK(c->h_out.alloc(CI_NRED));
+  CK(c->d_ticket.alloc(1));
   CK(cudaMemset(c->d_ticket, 0, sizeof(unsigned int)));
   return DMV_OK;
 }
@@ -283,10 +284,6 @@ int dmv_ci_destroy(dmv_ci* c) {
   if (!c) return DMV_OK;
   cudaSetDevice(c->device);
   if (c->stream) cudaStreamSynchronize(c->stream);
-  for (int l = 0; l < DMV_MAX_PYR_LEVELS; l++) { cudaFree(c->d_first[l]); cudaFree(c->d_new[l]); cudaFree(c->d_static[l]); }
-  cudaFree(c->d_stage); cudaFree(c->d_in); cudaFree(c->d_good); cudaFree(c->d_outp); cudaFreeHost(c->h_pin);
-  cudaFree(c->d_partial); cudaFree(c->d_out); cudaFreeHost(c->h_out); cudaFree(c->d_ticket);
-  if (c->stream) cudaStreamDestroy(c->stream);
   delete c;
   return DMV_OK;
 }

@@ -19,31 +19,23 @@ namespace dmv {
 
 // the handle's share (dmv_ct::cd), allocated on first use
 struct CDScratch {
-  float *idepth[DMV_MAX_PYR_LEVELS] = {nullptr}, *ws[DMV_MAX_PYR_LEVELS] = {nullptr}, *ws2[DMV_MAX_PYR_LEVELS] = {nullptr};
-  int *rowcnt = nullptr, *rowoff = nullptr;   // scratch rows of the compaction
-  int* totals = nullptr;    // pinned host, device-visible: pc_n of every level, then [DMV_MAX_PYR_LEVELS] = bad
+  DevBuf<float> idepth[DMV_MAX_PYR_LEVELS], ws[DMV_MAX_PYR_LEVELS], ws2[DMV_MAX_PYR_LEVELS];
+  DevBuf<int> rowcnt, rowoff;   // scratch rows of the compaction
+  PinnedBuf<int> totals;        // device-visible: pc_n of every level, then [DMV_MAX_PYR_LEVELS] = bad
   // the device fold of dmv_ct_set_ref_from_ba, for up to sort_cap points: radix-sort keys / ordinals (double-buffered) and CUB's temporary
   // storage, the moves, and the event that orders the tracker's stream behind the BA's
-  unsigned* key[2] = {nullptr, nullptr};
-  int* ord[2] = {nullptr, nullptr};
-  void* temp = nullptr;
+  DevBuf<unsigned> key[2];
+  DevBuf<int> ord[2];
+  DevBuf<uint8_t> temp;
   size_t temp_bytes = 0;
-  int* bad = nullptr;       // lowest point index whose projection leaves the image (>= npts: none)
-  int* moves = nullptr;     // device copy of CDFromBA::moves_host (2 * sort_cap ints)
-  int* h_moves = nullptr;   // its pinned staging
+  DevBuf<int> bad;          // lowest point index whose projection leaves the image (>= npts: none)
+  DevBuf<int> moves;        // device copy of CDFromBA::moves_host (2 * sort_cap ints)
+  PinnedBuf<int> h_moves;   // its pinned staging
   int sort_cap = 0;
-  cudaEvent_t ev_ba = nullptr;
+  Event ev_ba;
 };
 
-void cd_free(CDScratch* S) {
-  if (!S) return;
-  for (int l = 0; l < DMV_MAX_PYR_LEVELS; l++) { cudaFree(S->idepth[l]); cudaFree(S->ws[l]); cudaFree(S->ws2[l]); }
-  cudaFree(S->rowcnt); cudaFree(S->rowoff); cudaFreeHost(S->totals);
-  for (int k = 0; k < 2; k++) { cudaFree(S->key[k]); cudaFree(S->ord[k]); }
-  cudaFree(S->temp); cudaFree(S->bad); cudaFree(S->moves); cudaFreeHost(S->h_moves);
-  if (S->ev_ba) cudaEventDestroy(S->ev_ba);
-  delete S;
-}
+void CTPartDelete::operator()(CDScratch* p) const { delete p; }
 
 __global__ void cd_scatter_kernel(int n, const int* __restrict__ pix, const float* __restrict__ idw, const float* __restrict__ wsum, float* idepth0, float* ws0) {
   const int i = blockIdx.x * blockDim.x + threadIdx.x;
@@ -250,7 +242,7 @@ static cudaError_t cd_launch_from_ba(dmv_ct* c, const CDFromBA& B, int* kernels)
     if (e != cudaSuccess) return e;
     size_t tb = S.temp_bytes;
     // LSD radix sort: stable, so the points of one pixel stay in fold order (array position)
-    e = cub::DeviceRadixSort::SortPairs(S.temp, tb, S.key[0], S.key[1], S.ord[0], S.ord[1], B.npts, 0, end_bit, s);
+    e = cub::DeviceRadixSort::SortPairs(S.temp, tb, S.key[0].get(), S.key[1].get(), S.ord[0].get(), S.ord[1].get(), B.npts, 0, end_bit, s);
     if (e != cudaSuccess) return e;
     cd_fold_kernel<<<g, 256, 0, s>>>(B.npts, S.key[1], S.ord[1], B.cid, B.hdi, npx, S.idepth[0], S.ws[0]);
     k++;
@@ -264,20 +256,20 @@ static cudaError_t cd_launch_from_ba(dmv_ct* c, const CDFromBA& B, int* kernels)
 
 using namespace dmv;
 
-// working planes of the device makeCoarseDepthL0, allocated on first use
+// working planes of the device makeCoarseDepthL0, allocated on first use; totals, the last of them, is set only once all of them are
 static int ct_cd_allocate(dmv_ct* c) {
-  if (!c->cd) c->cd = new CDScratch();
+  if (!c->cd) c->cd.reset(new CDScratch());
   CDScratch& S = *c->cd;
   if (S.totals) return DMV_OK;
   for (int l = 0; l < c->cfg.levels; l++) {
     const size_t npx = (size_t)c->w[l] * c->h[l];
-    CK(cudaMalloc(&S.idepth[l], npx * sizeof(float)));
-    CK(cudaMalloc(&S.ws[l], npx * sizeof(float)));
-    CK(cudaMalloc(&S.ws2[l], npx * sizeof(float)));
+    CK(S.idepth[l].alloc(npx));
+    CK(S.ws[l].alloc(npx));
+    CK(S.ws2[l].alloc(npx));
   }
-  CK(cudaMalloc(&S.rowcnt, sizeof(int) * c->h[0]));
-  CK(cudaMalloc(&S.rowoff, sizeof(int) * c->h[0]));
-  CK(cudaMallocHost(&S.totals, sizeof(int) * (DMV_MAX_PYR_LEVELS + 1)));
+  CK(S.rowcnt.alloc(c->h[0]));
+  CK(S.rowoff.alloc(c->h[0]));
+  CK(S.totals.alloc(DMV_MAX_PYR_LEVELS + 1));
   return DMV_OK;
 }
 // pc_n of every level from the compaction's totals (after the stream synchronisation); a level over capacity is an error
@@ -303,7 +295,7 @@ int dmv_ct_make_coarse_depth(dmv_ct* c, int n, const float* Ku, const float* Kv,
   CK(ct_reserve_ip(c, n));
   CK(ct_wait_staging(c));
   const size_t cap = c->ip_cap;
-  int* h_pix = reinterpret_cast<int*>(c->h_ip);
+  int* h_pix = reinterpret_cast<int*>(c->h_ip.get());
   float* h_idw = c->h_ip + cap;
   float* h_ws = c->h_ip + 2 * cap;
   int nu = 0;
@@ -322,7 +314,7 @@ int dmv_ct_make_coarse_depth(dmv_ct* c, int n, const float* Ku, const float* Kv,
   }
   CK(cudaMemcpyAsync(c->d_ip, c->h_ip, sizeof(float) * 3 * cap, cudaMemcpyHostToDevice, c->stream));
   cd_clear(c);
-  if (nu > 0) cd_scatter_kernel<<<(nu + 255) / 256, 256, 0, c->stream>>>(nu, reinterpret_cast<const int*>(c->d_ip), c->d_ip + cap, c->d_ip + 2 * cap, c->cd->idepth[0], c->cd->ws[0]);
+  if (nu > 0) cd_scatter_kernel<<<(nu + 255) / 256, 256, 0, c->stream>>>(nu, reinterpret_cast<const int*>(c->d_ip.get()), c->d_ip + cap, c->d_ip + 2 * cap, c->cd->idepth[0], c->cd->ws[0]);
   cd_reduce(c);
   c->launches += 2 + 4 * L;
   CK(cudaGetLastError());
@@ -344,21 +336,17 @@ int dmv_ct_set_ref_from_ba(dmv_ct* c, dmv_ba* ba, int32_t* pc_n_out) {
   CK(cudaSetDevice(c->device));
   if ((rc = ct_cd_allocate(c)) != DMV_OK) return rc;
   CDScratch& S = *c->cd;
-  if (!S.ev_ba) CK(cudaEventCreateWithFlags(&S.ev_ba, cudaEventDisableTiming));
+  if (!S.ev_ba) CK(cudaEventCreateWithFlags(S.ev_ba.put(), cudaEventDisableTiming));
   if (B.npts > S.sort_cap) {
     CK(cudaStreamSynchronize(c->stream));   // kernels in flight may still use the old scratch
-    for (int k = 0; k < 2; k++) { cudaFree(S.key[k]); cudaFree(S.ord[k]); S.key[k] = nullptr; S.ord[k] = nullptr; }
-    cudaFree(S.temp); S.temp = nullptr;
-    cudaFree(S.moves); S.moves = nullptr;
-    cudaFreeHost(S.h_moves); S.h_moves = nullptr;
     S.sort_cap = 0;
     const int cap = std::max(B.npts, 2048);
-    for (int k = 0; k < 2; k++) { CK(cudaMalloc(&S.key[k], sizeof(unsigned) * cap)); CK(cudaMalloc(&S.ord[k], sizeof(int) * cap)); }
-    CK(cudaMalloc(&S.moves, sizeof(int) * 2 * cap));
-    CK(cudaMallocHost(&S.h_moves, sizeof(int) * 2 * cap));
+    for (int k = 0; k < 2; k++) { CK(S.key[k].reserve(cap)); CK(S.ord[k].reserve(cap)); }
+    CK(S.moves.reserve((size_t)2 * cap));
+    CK(S.h_moves.reserve((size_t)2 * cap));
     S.temp_bytes = cd_sort_temp_bytes(cap);
-    CK(cudaMalloc(&S.temp, std::max<size_t>(S.temp_bytes, 16)));
-    if (!S.bad) CK(cudaMalloc(&S.bad, sizeof(int)));
+    CK(S.temp.reserve(std::max<size_t>(S.temp_bytes, 16)));
+    CK(S.bad.reserve(1));
     S.sort_cap = cap;
   }
   CK(cudaEventRecord(S.ev_ba, B.stream));         // the BA's last linearisation / accumulate / frame upload

@@ -4,56 +4,59 @@
 #include "../../include/dmvio_b200.h"
 #include "common_host.h"
 #include <algorithm>
+#include <memory>
 
 namespace dmv {
 struct CTMaps;      // TMA descriptors of the level planes (ct_kernels.cu)
 struct CDScratch;   // makeCoarseDepthL0's working planes and sort scratch (ct_depth.cu), allocated on first use
 struct PSScratch;   // pixel selection's scratch (ps_select.cu), allocated on first use
-void cd_free(CDScratch* s);
-void ps_free(PSScratch* s);
+// deletes the handle's share of a feature: each operator() is defined in the feature's file, where the type is complete
+struct CTPartDelete {
+  void operator()(CTMaps* p) const;
+  void operator()(CDScratch* p) const;
+  void operator()(PSScratch* p) const;
+};
+template <typename T> using CTPart = std::unique_ptr<T, CTPartDelete>;
 }  // namespace dmv
 
 struct dmv_ct {
   dmv_ct_config cfg;
   int device = 0;
-  cudaStream_t stream = nullptr;
-  cudaEvent_t ev[2] = {nullptr, nullptr};
-  cudaEvent_t ev_order = nullptr;   // orders a dmv_ct_track_many / dmv_ct_trace_many launch on another member's stream behind this handle's queued work
+  dmv::Stream stream;
+  dmv::Event ev[2];
+  dmv::Event ev_order;              // orders a dmv_ct_track_many / dmv_ct_trace_many launch on another member's stream behind this handle's queued work
   bool staging_busy = false;  // an asynchronous upload from h_scratch may be in flight
   bool timing = false;  // CUDA-event timing of every evaluation (dmv_ct_set_timing); off by default: two event records per launch
   int w[DMV_MAX_PYR_LEVELS], h[DMV_MAX_PYR_LEVELS];
   float fx[DMV_MAX_PYR_LEVELS], fy[DMV_MAX_PYR_LEVELS], cx[DMV_MAX_PYR_LEVELS], cy[DMV_MAX_PYR_LEVELS];
   bool haveK[DMV_MAX_PYR_LEVELS];
-  float4* d_img[DMV_MAX_PYR_LEVELS] = {nullptr};
-  float* d_gray[DMV_MAX_PYR_LEVELS] = {nullptr};
-  float* d_stage = nullptr;
-  float *d_u[DMV_MAX_PYR_LEVELS] = {nullptr}, *d_v[DMV_MAX_PYR_LEVELS] = {nullptr}, *d_id[DMV_MAX_PYR_LEVELS] = {nullptr},
-        *d_col[DMV_MAX_PYR_LEVELS] = {nullptr};
+  dmv::DevBuf<float4> d_img[DMV_MAX_PYR_LEVELS];
+  dmv::DevBuf<float> d_gray[DMV_MAX_PYR_LEVELS];
+  dmv::DevBuf<float> d_stage;
+  dmv::DevBuf<float> d_u[DMV_MAX_PYR_LEVELS], d_v[DMV_MAX_PYR_LEVELS], d_id[DMV_MAX_PYR_LEVELS], d_col[DMV_MAX_PYR_LEVELS];
   int n[DMV_MAX_PYR_LEVELS];
-  double* d_partial = nullptr;
-  unsigned int* d_ticket = nullptr;
-  double* d_out = nullptr;
-  double* h_out = nullptr;
-  float* h_scratch = nullptr;
-  dmv::CDScratch* cd = nullptr;   // dmv_ct_make_coarse_depth / dmv_ct_set_ref_from_ba
-  float* d_ip = nullptr;   // per-point staging of dmv_ct_make_coarse_depth, dmv_ct_init_points and dmv_ct_trace_points (ct_reserve_ip)
-  float* h_ip = nullptr;
-  int ip_cap = 0;
+  dmv::DevBuf<double> d_partial;
+  dmv::DevBuf<unsigned int> d_ticket;
+  dmv::PinnedBuf<double> h_out;
+  dmv::PinnedBuf<float> h_scratch;
+  dmv::CTPart<dmv::CDScratch> cd;   // dmv_ct_make_coarse_depth / dmv_ct_set_ref_from_ba
+  dmv::DevBuf<float> d_ip;   // per-point staging of dmv_ct_make_coarse_depth, dmv_ct_init_points and dmv_ct_trace_points (ct_reserve_ip)
+  dmv::PinnedBuf<float> h_ip;
+  int ip_cap = 0;            // points the staging layout holds (0 while d_ip / h_ip may be short of it)
   float huber = 9.f;
   int cluster_size = 0;        // CTAs of ct_track_cluster_kernel's cluster (0 = not probed yet, -1 = none schedulable: dmv_ct_track fails)
-  dmv::CTMaps* maps = nullptr; // TMA descriptors of the level planes (host copy; passed as a kernel parameter)
+  dmv::CTPart<dmv::CTMaps> maps;  // TMA descriptors of the level planes (host copy; passed as a kernel parameter)
   int staged[DMV_MAX_PYR_LEVELS] = {0};   // levels whose map ct_make_tensor_maps encoded: the only ones the cluster kernel stages
-  dmv_ct_tries_result* h_tries = nullptr;   // dmv_ct_track_tries's pinned result, allocated on first use
+  dmv::PinnedBuf<dmv_ct_tries_result> h_tries;   // dmv_ct_track_tries's pinned result, allocated on first use
   long long launches = 0;
   float last_ms[4] = {0, 0, 0, 0};
-  size_t scratch_bytes = 0;    // capacity of h_scratch
   // raw-frame ingest (dmv_ct_set_undistort / dmv_ct_upload_raw_image)
   bool have_undistort = false;
   int wOrg = 0, hOrg = 0, nG = 0, pmode = 0;
-  float2* d_remap = nullptr;                   // (remapX, remapY) per level-0 pixel; nullptr = passthrough
-  float *d_G = nullptr, *d_vigInv = nullptr;   // response map; vignetteMapInv (wOrg*hOrg, photometric mode 2)
-  void* d_raw = nullptr;
-  dmv::PSScratch* ps = nullptr;   // dmv_ct_make_new_traces
+  dmv::DevBuf<float2> d_remap;                 // (remapX, remapY) per level-0 pixel; empty = passthrough
+  dmv::DevBuf<float> d_G, d_vigInv;            // response map; vignetteMapInv (wOrg*hOrg, photometric mode 2)
+  dmv::DevBuf<uint8_t> d_raw;
+  dmv::CTPart<dmv::PSScratch> ps;   // dmv_ct_make_new_traces
 };
 
 namespace dmv {
@@ -81,12 +84,11 @@ inline int ct_member_error(int rc, int i) {
 // to 64 host frames
 inline cudaError_t ct_reserve_ip(dmv_ct* c, int n) {
   if (n <= c->ip_cap) return cudaSuccess;
-  cudaFree(c->d_ip); cudaFreeHost(c->h_ip);
-  c->d_ip = nullptr; c->h_ip = nullptr; c->ip_cap = 0;
+  c->ip_cap = 0;
   const int cap = std::max(n, 2048);
   const size_t words = (size_t)31 * cap + 14 * 64;
-  cudaError_t e = cudaMalloc(&c->d_ip, sizeof(float) * words);
-  if (e == cudaSuccess) e = cudaMallocHost(&c->h_ip, sizeof(float) * words);
+  cudaError_t e = c->d_ip.reserve(words);
+  if (e == cudaSuccess) e = c->h_ip.reserve(words);
   if (e == cudaSuccess) c->ip_cap = cap;
   return e;
 }

@@ -94,26 +94,19 @@ int dmv_ct_set_undistort(dmv_ct* c, const dmv_undistort_config* u) {
   CK(cudaStreamSynchronize(c->stream));  // kernels in flight may read the old tables or the staging buffer
   c->staging_busy = false;
   c->have_undistort = false;
-  cudaFree(c->d_remap); cudaFree(c->d_G); cudaFree(c->d_vigInv); cudaFree(c->d_raw);
-  c->d_remap = nullptr; c->d_G = nullptr; c->d_vigInv = nullptr; c->d_raw = nullptr;
-  if (nraw * 2 > c->scratch_bytes) {
-    cudaFreeHost(c->h_scratch);
-    c->h_scratch = nullptr;
-    c->scratch_bytes = 0;
-    CK(cudaMallocHost(&c->h_scratch, nraw * 2));
-    c->scratch_bytes = nraw * 2;
-  }
-  CK(cudaMalloc(&c->d_raw, nraw * 2));
+  c->d_remap = {}; c->d_G = {}; c->d_vigInv = {}; c->d_raw = {};
+  CK(c->h_scratch.reserve((nraw * 2 + sizeof(float) - 1) / sizeof(float)));
+  CK(c->d_raw.alloc(nraw * 2));
   if (u->remapX) {
-    CK(cudaMalloc(&c->d_remap, npx * sizeof(float2)));
+    CK(c->d_remap.alloc(npx));
     CK(cudaMemcpy(c->d_remap, remap.data(), npx * sizeof(float2), cudaMemcpyHostToDevice));
   }
   if (u->G) {
-    CK(cudaMalloc(&c->d_G, (size_t)u->nG * sizeof(float)));
+    CK(c->d_G.alloc(u->nG));
     CK(cudaMemcpy(c->d_G, u->G, (size_t)u->nG * sizeof(float), cudaMemcpyHostToDevice));
   }
   if (u->G && u->vignetteInv) {
-    CK(cudaMalloc(&c->d_vigInv, nraw * sizeof(float)));
+    CK(c->d_vigInv.alloc(nraw));
     CK(cudaMemcpy(c->d_vigInv, u->vignetteInv, nraw * sizeof(float), cudaMemcpyHostToDevice));
   }
   c->wOrg = u->wOrg; c->hOrg = u->hOrg; c->nG = u->G ? u->nG : 0; c->pmode = u->photometric_mode;
@@ -134,8 +127,8 @@ int dmv_ct_upload_raw_image(dmv_ct* c, const void* raw, int bpp, float exposure,
   std::memcpy(c->h_scratch, raw, bytes);
   CK(cudaMemcpyAsync(c->d_raw, c->h_scratch, bytes, cudaMemcpyHostToDevice, c->stream));
   // the level-0 intensity plane d_gray[0] from the raw frame
-  if (bpp == 1) launch_t(c, static_cast<const unsigned char*>(c->d_raw), use_G, factor);
-  else launch_t(c, static_cast<const unsigned short*>(c->d_raw), use_G, factor);
+  if (bpp == 1) launch_t(c, c->d_raw.get(), use_G, factor);
+  else launch_t(c, reinterpret_cast<const unsigned short*>(c->d_raw.get()), use_G, factor);
   c->launches++;
   const int rc = ct_build_pyramid(c, 0);
   if (rc != DMV_OK) return rc;

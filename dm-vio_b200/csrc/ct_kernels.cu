@@ -744,6 +744,8 @@ __global__ void __launch_bounds__(CTC_THREADS, 1) ct_track_tries_kernel(const __
 
 using namespace dmv;
 
+void dmv::CTPartDelete::operator()(CTMaps* p) const { delete p; }
+
 int dmv::ct_build_pyramid(dmv_ct* c, int first_level) {
   for (int l = first_level; l < c->cfg.levels; l++) {
     if (l > 0) {
@@ -774,8 +776,8 @@ int dmv_ct_create(const dmv_ct_config* cfg, dmv_ct** out) {
   CK(cudaSetDevice(cfg->device));
   dmv_ct* c = new dmv_ct();
   const int rc = ct_allocate(c, cfg);
-  if (rc != DMV_OK) {  // allocation failed half-way: release what exists, keep the failing call's error message
-    dmv_ct_destroy(c);
+  if (rc != DMV_OK) {  // allocation failed half-way: the members release what exists, the failing call's error message is kept
+    delete c;
     return rc;
   }
   *out = c;
@@ -785,30 +787,28 @@ int dmv_ct_create(const dmv_ct_config* cfg, dmv_ct** out) {
 static int ct_allocate(dmv_ct* c, const dmv_ct_config* cfg) {
   c->cfg = *cfg;
   c->device = cfg->device;
-  CK(cudaStreamCreateWithFlags(&c->stream, cudaStreamNonBlocking));
-  CK(cudaEventCreate(&c->ev[0]));
-  CK(cudaEventCreate(&c->ev[1]));
-  CK(cudaEventCreateWithFlags(&c->ev_order, cudaEventDisableTiming));
+  CK(cudaStreamCreateWithFlags(c->stream.put(), cudaStreamNonBlocking));
+  CK(cudaEventCreate(c->ev[0].put()));
+  CK(cudaEventCreate(c->ev[1].put()));
+  CK(cudaEventCreateWithFlags(c->ev_order.put(), cudaEventDisableTiming));
   for (int l = 0; l < cfg->levels; l++) {
     c->w[l] = cfg->w >> l; c->h[l] = cfg->h >> l; c->haveK[l] = false; c->n[l] = 0;
     const size_t npx = (size_t)c->w[l] * c->h[l];
-    CK(cudaMalloc(&c->d_img[l], npx * sizeof(float4)));
-    CK(cudaMalloc(&c->d_gray[l], npx * sizeof(float)));
-    CK(cudaMalloc(&c->d_u[l], sizeof(float) * cfg->max_points));
-    CK(cudaMalloc(&c->d_v[l], sizeof(float) * cfg->max_points));
-    CK(cudaMalloc(&c->d_id[l], sizeof(float) * cfg->max_points));
-    CK(cudaMalloc(&c->d_col[l], sizeof(float) * cfg->max_points));
+    CK(c->d_img[l].alloc(npx));
+    CK(c->d_gray[l].alloc(npx));
+    CK(c->d_u[l].alloc(cfg->max_points));
+    CK(c->d_v[l].alloc(cfg->max_points));
+    CK(c->d_id[l].alloc(cfg->max_points));
+    CK(c->d_col[l].alloc(cfg->max_points));
   }
   const size_t npx0 = (size_t)cfg->w * cfg->h;
-  CK(cudaMalloc(&c->d_stage, npx0 * 3 * sizeof(float)));
+  CK(c->d_stage.alloc(npx0 * 3));
   const int maxBlocks = (cfg->max_points + CT_THREADS - 1) / CT_THREADS;
-  CK(cudaMalloc(&c->d_partial, sizeof(double) * CT_NRED * maxBlocks));  // ct_res_gs_kernel's per-block partials
-  CK(cudaMalloc(&c->d_ticket, sizeof(unsigned int)));
+  CK(c->d_partial.alloc((size_t)CT_NRED * maxBlocks));  // ct_res_gs_kernel's per-block partials
+  CK(c->d_ticket.alloc(1));
   CK(cudaMemset(c->d_ticket, 0, sizeof(unsigned int)));
-  CK(cudaMalloc(&c->d_out, sizeof(double) * 64));
-  CK(cudaMallocHost(&c->h_out, sizeof(double) * 64));
-  c->scratch_bytes = sizeof(float) * std::max(npx0 * 3, (size_t)cfg->max_points * 4);
-  CK(cudaMallocHost(&c->h_scratch, c->scratch_bytes));
+  CK(c->h_out.alloc(64));
+  CK(c->h_scratch.alloc(std::max(npx0 * 3, (size_t)cfg->max_points * 4)));
   return DMV_OK;
 }
 
@@ -816,19 +816,6 @@ int dmv_ct_destroy(dmv_ct* c) {
   if (!c) return DMV_OK;
   cudaSetDevice(c->device);
   if (c->stream) cudaStreamSynchronize(c->stream);
-  for (int l = 0; l < DMV_MAX_PYR_LEVELS; l++) {
-    cudaFree(c->d_img[l]); cudaFree(c->d_gray[l]); cudaFree(c->d_u[l]); cudaFree(c->d_v[l]); cudaFree(c->d_id[l]); cudaFree(c->d_col[l]);
-  }
-  cudaFree(c->d_stage); cudaFree(c->d_partial); cudaFree(c->d_ticket); cudaFree(c->d_out); cudaFreeHost(c->h_tries);
-  cudaFreeHost(c->h_out); cudaFreeHost(c->h_scratch); cudaFree(c->d_ip); cudaFreeHost(c->h_ip);
-  cd_free(c->cd);
-  cudaFree(c->d_remap); cudaFree(c->d_G); cudaFree(c->d_vigInv); cudaFree(c->d_raw);
-  ps_free(c->ps);
-  if (c->ev[0]) cudaEventDestroy(c->ev[0]);
-  if (c->ev[1]) cudaEventDestroy(c->ev[1]);
-  if (c->ev_order) cudaEventDestroy(c->ev_order);
-  if (c->stream) cudaStreamDestroy(c->stream);
-  delete c->maps;
   delete c;
   return DMV_OK;
 }
@@ -972,8 +959,8 @@ static int ct_make_tensor_maps(dmv_ct* c) {
     cudaGetLastError();
     return set_error(DMV_ERR_CUDA, "cuTensorMapEncodeTiled is not available");
   }
-  if (!c->maps) c->maps = new CTMaps();
-  std::memset(c->maps, 0, sizeof(CTMaps));
+  if (!c->maps) c->maps.reset(new CTMaps());
+  std::memset(c->maps.get(), 0, sizeof(CTMaps));
   for (int l = 0; l < DMV_MAX_PYR_LEVELS; l++) c->staged[l] = 0;
   for (int l = 0; l < c->cfg.levels; l++) {
     const size_t bytes = (size_t)c->w[l] * c->h[l] * sizeof(float4);
@@ -1165,7 +1152,7 @@ int dmv_ct_track_tries(dmv_ct* c, const dmv_ct_tries_args* in, dmv_ct_tries_resu
   CK(cudaSetDevice(c->device));
   rc = ct_probe_cluster(c);
   if (rc != DMV_OK) return rc;
-  if (!c->h_tries) CK(cudaMallocHost(&c->h_tries, sizeof(dmv_ct_tries_result)));
+  CK(c->h_tries.reserve(1));
   for (int l = 0; l < DMV_MAX_PYR_LEVELS; l++) Q->T.staged[l] = c->staged[l];
   Q->maps = *c->maps;
   for (int k = 0; k < in->n; k++) {

@@ -356,14 +356,8 @@ extern "C" int dmv_ba_select_activation(dmv_ba* b, const dmv_ba_select_args* a) 
                o_ist = o_imax + n, o_iint = o_ist + n, o_iq = o_iint + n, o_ity = o_iq + n, o_act = o_ity + n, o_opt = o_act + n, o_cnt = o_opt + n,
                o_map = o_cnt + 8, o_cell = o_map + ncell, o_frac = o_cell + n, o_rad = o_frac + n, o_stamp = o_rad + n, words = o_stamp + ncell;
   CK(cudaSetDevice(b->device));
-  if (words > b->sel_words) {
-    cudaFree(b->d_sel); cudaFreeHost(b->h_sel);
-    b->d_sel = nullptr; b->h_sel = nullptr; b->sel_words = 0;
-    const size_t cap = words;
-    CK(cudaMalloc(&b->d_sel, 4 * cap));
-    CK(cudaMallocHost(&b->h_sel, 4 * cap));
-    b->sel_words = cap;
-  }
+  CK(b->d_sel.reserve(words));
+  CK(b->h_sel.reserve(words));
   float* hb = b->h_sel;
   float* d = b->d_sel;
   int* hi = reinterpret_cast<int*>(hb);

@@ -669,11 +669,12 @@ int dmv_ba_activate_points(dmv_ba* b, const dmv_ba_activate_args* a) {
     if (a->host[i] < 0 || a->host[i] >= nf) return set_error(DMV_ERR_INVALID, "point %d: host %d out of range", i, a->host[i]);
   CK(cudaSetDevice(b->device));
   if (n > b->act_cap) {
-    cudaFree(b->d_act); cudaFreeHost(b->h_act);
-    b->act_cap = std::max(n, 2048);
-    const size_t words = (size_t)MAXF * MAXF * 14 + (size_t)(24 + MAXF) * b->act_cap;
-    CK(cudaMalloc(&b->d_act, sizeof(float) * words));
-    CK(cudaMallocHost(&b->h_act, sizeof(float) * words));
+    b->act_cap = 0;
+    const int cap = std::max(n, 2048);
+    const size_t words = (size_t)MAXF * MAXF * 14 + (size_t)(24 + MAXF) * cap;
+    CK(b->d_act.reserve(words));
+    CK(b->h_act.reserve(words));
+    b->act_cap = cap;
   }
   const size_t cap = b->act_cap;
   float* hb = b->h_act;
@@ -692,7 +693,7 @@ int dmv_ba_activate_points(dmv_ba* b, const dmv_ba_activate_args* a) {
   A.n = n; A.nf = nf; A.w = b->cfg.w; A.h = b->cfg.h; A.minObs = a->minObs; A.GNIts = 3;  // setting_GNItsOnPointActivation
   A.fxl = it.calib[0]; A.fyl = it.calib[1]; A.cxl = it.calib[2]; A.cyl = it.calib[3]; A.fxli = it.calib[4]; A.fyli = it.calib[5];
   A.huberTH = b->prm.huberTH; A.minIdepthH_act = 100.f;                                      // setting_minIdepthH_act
-  for (int f = 0; f < MAXF; f++) A.img[f] = f < nf ? b->d_img[b->slots[f]] : nullptr;
+  for (int f = 0; f < MAXF; f++) A.img[f] = f < nf ? b->d_img[b->slots[f]].get() : nullptr;
   A.RT = d + o_rt; A.aff = d + o_aff; A.host = reinterpret_cast<const int*>(d + o_host);
   A.u = d + o_u; A.v = d + o_v; A.color = d + o_col; A.weights = d + o_wgt; A.energyTH = d + o_eth; A.idepth_min = d + o_min; A.idepth_max = d + o_max;
   A.status = reinterpret_cast<int*>(d + o_st); A.idepth = d + o_id; A.res_state = reinterpret_cast<int*>(d + o_rs);

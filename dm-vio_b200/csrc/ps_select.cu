@@ -56,26 +56,25 @@ struct PSState {
 // per-handle scratch, allocated on first use for the handle's level-0 size
 struct PSScratch {
   int w = 0, h = 0;
-  uint8_t* pat = nullptr;         // PixelSelector::randomPattern (w*h)
-  uint8_t* nib = nullptr;         // its low nibbles, two per byte (w*h/2): the directions the serial chain reads
-  float* ths = nullptr;           // thsSmoothed (nbW*nbH) and ths (nbW*nbH)
-  float* B = nullptr;             // CalibHessian::B (256)
-  uint32_t* mask = nullptr;       // per pot-block / 2pot-block / 4pot-block: directions with a candidate (w*h + w*h/4 + w*h/16)
-  unsigned long long* best = nullptr;  // per pot-block / 2pot / 4pot: (value bits << 32) | ~position of the first maximum
-  unsigned long long* scan_in = nullptr;  // (w*h+1): constant pick | mixed block << 32 per pot-block key
-  unsigned long long* scan = nullptr;  // (w*h+1): its exclusive prefix of (constant picks | mixed blocks << 32) in nested order
-  int2* mixed = nullptr;          // (w*h): per mixed block in order: (constant-pick prefix, direction mask)
-  int* delta = nullptr;           // (w*h): mixed picks up to and including mixed block j
-  int* n2b = nullptr;             // (w*h+1): level-0 picks before each pot-block in nested order
-  float* map = nullptr;           // selectionMap (w*h)
-  int* flag = nullptr;            // (w*h): scan input
-  int* rank = nullptr;            // (w*h): scan output
-  float* cand = nullptr;          // candidates of makeNewTraces' loop: u | v | type | color*8 | weights*8 | gradH*4 | energyTH | ok  (25 * w*h words)
-  PSState* st = nullptr;
-  void* temp = nullptr;           // CUB scan storage
+  DevBuf<uint8_t> pat;            // PixelSelector::randomPattern (w*h)
+  uint8_t* nib = nullptr;         // its low nibbles, two per byte (w*h/2), at pat + w*h: the directions the serial chain reads
+  DevBuf<float> ths;              // thsSmoothed (nbW*nbH) and ths (nbW*nbH)
+  DevBuf<float> B;                // CalibHessian::B (256)
+  DevBuf<uint32_t> mask;          // per pot-block / 2pot-block / 4pot-block: directions with a candidate (w*h + w*h/4 + w*h/16)
+  DevBuf<unsigned long long> best;     // per pot-block / 2pot / 4pot: (value bits << 32) | ~position of the first maximum
+  DevBuf<unsigned long long> scan_in;  // (w*h+1): constant pick | mixed block << 32 per pot-block key
+  DevBuf<unsigned long long> scan;     // (w*h+1): its exclusive prefix of (constant picks | mixed blocks << 32) in nested order
+  DevBuf<int2> mixed;             // (w*h): per mixed block in order: (constant-pick prefix, direction mask)
+  DevBuf<int> delta;              // (w*h): mixed picks up to and including mixed block j
+  DevBuf<int> n2b;                // (w*h+1): level-0 picks before each pot-block in nested order
+  DevBuf<float> map;              // selectionMap (w*h)
+  DevBuf<int> flag;               // (w*h): scan input
+  DevBuf<int> rank;               // (w*h): scan output
+  DevBuf<float> cand;             // candidates of makeNewTraces' loop: u | v | type | color*8 | weights*8 | gradH*4 | energyTH | ok  (25 * w*h words)
+  DevBuf<PSState> st;
+  DevBuf<uint8_t> temp;           // CUB scan storage
   size_t temp_bytes = 0;
-  float* h_out = nullptr;         // pinned, device-visible: PSState then per point u | v | type | color*8 | weights*8 | gradH*4 | energyTH
-  int h_cap = 0;
+  PinnedBuf<float> h_out;         // device-visible: PSState then per point u | v | type | color*8 | weights*8 | gradH*4 | energyTH
   bool smem_chain = false;        // the chain stages the nibbles in shared memory (w*h/2 <= 200 KB); larger frames read them from global memory
 };
 struct PSArgs {
@@ -464,67 +463,43 @@ static void ps_random_pattern(uint8_t* out, size_t n, unsigned seed) {
   for (size_t k = 0; k < n; k++) out[k] = (uint8_t)(((uint32_t)r[344 + k] >> 1) & 0xFF);
 }
 
-static void ps_release(PSScratch& S) {
-  cudaFree(S.pat); cudaFree(S.ths); cudaFree(S.B); cudaFree(S.mask); cudaFree(S.best); cudaFree(S.scan); cudaFree(S.scan_in); cudaFree(S.mixed); cudaFree(S.delta);
-  cudaFree(S.n2b); cudaFree(S.map); cudaFree(S.flag); cudaFree(S.rank); cudaFree(S.cand); cudaFree(S.st); cudaFree(S.temp);
-  cudaFreeHost(S.h_out);
-  S = PSScratch();
-}
-
 // dynamic shared memory of ps_chain_kernel: one value for the process (the attribute belongs to the kernel, not to a handle)
 static const int PS_SMEM_MAX = 200 * 1024;
 
-void ps_free(PSScratch* S) {
-  if (!S) return;
-  ps_release(*S);
-  delete S;
-}
+void CTPartDelete::operator()(PSScratch* p) const { delete p; }
 
-// allocates S for a w x h frame and builds the random pattern; returns the first CUDA error
-static cudaError_t ps_alloc(PSScratch& S, int w, int h) {
-  ps_release(S);
+// S (empty) for a w x h frame, with the random pattern built; S.w / S.h are set only once all of it is
+static int ps_alloc(PSScratch& S, int w, int h) {
   const size_t n = (size_t)w * h;
-  cudaError_t e;
-#define PS_TRY(x) do { if ((e = (x)) != cudaSuccess) { ps_release(S); return e; } } while (0)
-  PS_TRY(cudaMalloc(&S.pat, n + n / 2));
+  CK(S.pat.alloc(n + n / 2));
   S.nib = S.pat + n;
-  PS_TRY(cudaMalloc(&S.ths, sizeof(float) * 2 * (n / 256)));
-  PS_TRY(cudaMalloc(&S.B, sizeof(float) * 256));
-  PS_TRY(cudaMalloc(&S.mask, sizeof(uint32_t) * (n + n / 4 + n / 16)));
-  PS_TRY(cudaMalloc(&S.best, sizeof(unsigned long long) * (n + n / 4 + n / 16)));
-  PS_TRY(cudaMalloc(&S.scan, sizeof(unsigned long long) * (n + 1)));
-  PS_TRY(cudaMalloc(&S.scan_in, sizeof(unsigned long long) * (n + 1)));
-  PS_TRY(cudaMalloc(&S.mixed, sizeof(int2) * n));
-  PS_TRY(cudaMalloc(&S.delta, sizeof(int) * n));
-  PS_TRY(cudaMalloc(&S.n2b, sizeof(int) * (n + 1)));
-  PS_TRY(cudaMalloc(&S.map, sizeof(float) * n));
-  PS_TRY(cudaMalloc(&S.flag, sizeof(int) * n));
-  PS_TRY(cudaMalloc(&S.rank, sizeof(int) * n));
-  PS_TRY(cudaMalloc(&S.cand, sizeof(float) * 25 * n));
-  PS_TRY(cudaMalloc(&S.st, sizeof(PSState)));
+  CK(S.ths.alloc(2 * (n / 256)));
+  CK(S.B.alloc(256));
+  CK(S.mask.alloc(n + n / 4 + n / 16));
+  CK(S.best.alloc(n + n / 4 + n / 16));
+  CK(S.scan.alloc(n + 1));
+  CK(S.scan_in.alloc(n + 1));
+  CK(S.mixed.alloc(n));
+  CK(S.delta.alloc(n));
+  CK(S.n2b.alloc(n + 1));
+  CK(S.map.alloc(n));
+  CK(S.flag.alloc(n));
+  CK(S.rank.alloc(n));
+  CK(S.cand.alloc(25 * n));
+  CK(S.st.alloc(1));
   size_t t1 = 0, t2 = 0;
-  PS_TRY(cub::DeviceScan::ExclusiveSum(nullptr, t1, (const unsigned long long*)nullptr, (unsigned long long*)nullptr, (int)n + 1));
-  PS_TRY(cub::DeviceScan::ExclusiveSum(nullptr, t2, (const int*)nullptr, (int*)nullptr, (int)n));
+  CK(cub::DeviceScan::ExclusiveSum(nullptr, t1, (const unsigned long long*)nullptr, (unsigned long long*)nullptr, (int)n + 1));
+  CK(cub::DeviceScan::ExclusiveSum(nullptr, t2, (const int*)nullptr, (int*)nullptr, (int)n));
   S.temp_bytes = std::max(t1, t2);
-  PS_TRY(cudaMalloc(&S.temp, S.temp_bytes));
+  CK(S.temp.alloc(S.temp_bytes));
   std::vector<uint8_t> pat(n + n / 2);
   ps_random_pattern(pat.data(), n, 3141592);   // PixelSelector::PixelSelector (L43-47)
   for (size_t i = 0; i < n / 2; i++) pat[n + i] = (uint8_t)((pat[2 * i] & 0xF) | ((pat[2 * i + 1] & 0xF) << 4));
-  PS_TRY(cudaMemcpy(S.pat, pat.data(), n + n / 2, cudaMemcpyHostToDevice));
+  CK(cudaMemcpy(S.pat, pat.data(), n + n / 2, cudaMemcpyHostToDevice));
   S.smem_chain = n / 2 <= (size_t)PS_SMEM_MAX;
-  if (S.smem_chain) PS_TRY(cudaFuncSetAttribute(ps_chain_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, PS_SMEM_MAX));
-#undef PS_TRY
+  if (S.smem_chain) CK(cudaFuncSetAttribute(ps_chain_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, PS_SMEM_MAX));
   S.w = w; S.h = h;
-  return cudaSuccess;
-}
-
-static cudaError_t ps_ensure_out(PSScratch& S, int cap) {
-  if (S.h_out && cap <= S.h_cap) return cudaSuccess;
-  if (S.h_out) cudaFreeHost(S.h_out);
-  S.h_out = nullptr; S.h_cap = 0;
-  const cudaError_t e = cudaMallocHost(&S.h_out, sizeof(PSState) + sizeof(float) * 24 * (size_t)cap);
-  if (e == cudaSuccess) S.h_cap = cap;
-  return e;
+  return DMV_OK;
 }
 
 // every launch of the call: the points and the final PSState land in S.h_out, which the host reads after one stream synchronisation;
@@ -555,7 +530,7 @@ static cudaError_t ps_launch(const PSArgs& A, PSScratch& S, cudaStream_t s, int*
     ps_mask_kernel<<<rows, 128, 0, s>>>(D); k++;
     ps_classify_kernel<<<kb, 256, 0, s>>>(D); k++;
     size_t tb = S.temp_bytes;
-    if ((e = cub::DeviceScan::ExclusiveSum(S.temp, tb, S.scan_in, S.scan, n + 1, s)) != cudaSuccess) return e;
+    if ((e = cub::DeviceScan::ExclusiveSum(S.temp, tb, S.scan_in.get(), S.scan.get(), n + 1, s)) != cudaSuccess) return e;
     ps_scatter_mixed_kernel<<<pb, 256, 0, s>>>(D); k++;
     ps_chain_kernel<<<1, 1024, S.smem_chain ? n / 2 : 0, s>>>(D, S.smem_chain ? 1 : 0); k++;
     ps_resolve_kernel<<<kb, 256, 0, s>>>(D); k++;
@@ -565,22 +540,22 @@ static cudaError_t ps_launch(const PSArgs& A, PSScratch& S, cudaStream_t s, int*
   }
   size_t tb = S.temp_bytes;
   ps_flag_nonzero_kernel<<<pb, 256, 0, s>>>(D); k++;
-  if ((e = cub::DeviceScan::ExclusiveSum(S.temp, tb, S.flag, S.rank, n, s)) != cudaSuccess) return e;
+  if ((e = cub::DeviceScan::ExclusiveSum(S.temp, tb, S.flag.get(), S.rank.get(), n, s)) != cudaSuccess) return e;
   ps_thin_kernel<<<pb, 256, 0, s>>>(D); k++;
   ps_flag_window_kernel<<<pb, 256, 0, s>>>(D); k++;
-  if ((e = cub::DeviceScan::ExclusiveSum(S.temp, tb, S.flag, S.rank, n, s)) != cudaSuccess) return e;
+  if ((e = cub::DeviceScan::ExclusiveSum(S.temp, tb, S.flag.get(), S.rank.get(), n, s)) != cudaSuccess) return e;
   ps_scatter_cand_kernel<<<pb, 256, 0, s>>>(D); k++;
   IPInitArgs I;
   const size_t C = n;
   I.n = n; I.w = w; I.n_dev = &S.st->n_cand;
   I.outlierTHSumComponent = 50.f * 50.f; I.outlierTH = 12.f * 12.f; I.overallEnergyTHWeight = 1.f;  // util/settings.cpp:L111-114, L159
-  I.u = reinterpret_cast<const int*>(S.cand); I.v = reinterpret_cast<const int*>(S.cand + C);
+  I.u = reinterpret_cast<const int*>(S.cand.get()); I.v = reinterpret_cast<const int*>(S.cand + C);
   I.color = S.cand + 3 * C; I.weights = S.cand + 11 * C; I.gradH = S.cand + 19 * C; I.energyTH = S.cand + 23 * C;
   I.ok = reinterpret_cast<int*>(S.cand + 24 * C);
   I.img = A.img[0];
   launch_ip_init(I, s); k++;
   ps_flag_ok_kernel<<<pb, 256, 0, s>>>(D); k++;
-  if ((e = cub::DeviceScan::ExclusiveSum(S.temp, tb, S.flag, S.rank, n, s)) != cudaSuccess) return e;
+  if ((e = cub::DeviceScan::ExclusiveSum(S.temp, tb, S.flag.get(), S.rank.get(), n, s)) != cudaSuccess) return e;
   ps_scatter_out_kernel<<<pb, 256, 0, s>>>(D); k++;
   if ((e = cudaMemcpyAsync(S.h_out, S.st, sizeof(PSState), cudaMemcpyDeviceToHost, s)) != cudaSuccess) return e;
   *kernels = k;
@@ -614,11 +589,15 @@ int dmv_ct_make_new_traces(dmv_ct* c, const dmv_new_traces_args* a) {
   if (!(st.minGradHistCut < 0.99f) || !std::isfinite(st.minGradHistCut) || !std::isfinite(st.minGradHistAdd) || !std::isfinite(st.gradDownweightPerLevel))
     return set_error(DMV_ERR_INVALID, "bad dmv_ps_settings");
   CK(cudaSetDevice(c->device));
-  if (!c->ps) c->ps = new PSScratch();
+  if (!c->ps) c->ps.reset(new PSScratch());
   PSScratch& P = *c->ps;
-  if (P.w != w || P.h != h) CK(ps_alloc(P, w, h));
+  if (P.w != w || P.h != h) {
+    P = PSScratch();
+    const int rc = ps_alloc(P, w, h);
+    if (rc != DMV_OK) { P = PSScratch(); return rc; }
+  }
   const int out_cap = std::min(a->cap, w * h);
-  CK(ps_ensure_out(P, std::max(out_cap, 1)));
+  CK(P.h_out.reserve(sizeof(PSState) / sizeof(float) + 24 * (size_t)std::max(out_cap, 1)));
   CK(ct_wait_staging(c));
   float B[256];
   for (int i = 0; i < 256; i++) B[i] = a->B ? a->B[i] : (float)i;   // CalibHessian's constructor: B[i] = i
