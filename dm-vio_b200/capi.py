@@ -195,7 +195,7 @@ SYMBOLS = [
     "dmv_ba_batch_create", "dmv_ba_batch_destroy", "dmv_ba_batch_gn_step", "dmv_ba_batch_set_timing", "dmv_ba_batch_last_kernel_ms", "dmv_ba_batch_bench",
     "dmv_ct_create", "dmv_ct_destroy", "dmv_ct_set_K", "dmv_ct_set_ref", "dmv_ct_make_coarse_depth", "dmv_ct_set_ref_from_ba", "dmv_ct_get_ref", "dmv_ct_upload_new", "dmv_ct_upload_new_image", "dmv_ct_set_huber",
     "dmv_ci_create", "dmv_ci_destroy", "dmv_ci_set_K", "dmv_ci_upload_first", "dmv_ci_upload_new", "dmv_ci_set_points", "dmv_ci_calc_res_and_gs", "dmv_ci_kernel_launch_count",
-    "dmv_ct_calc_res_gs", "dmv_ct_track", "dmv_ct_track_many", "dmv_ct_track_tries", "dmv_ip_default_settings", "dmv_ct_init_points", "dmv_ct_trace_points", "dmv_ct_trace_points_multi", "dmv_ct_trace_many", "dmv_ct_set_timing", "dmv_ct_last_timing", "dmv_ct_kernel_launch_count", "dmv_ct_last_point_evaluations",
+    "dmv_ct_calc_res_gs", "dmv_ct_track", "dmv_ct_track_many", "dmv_ct_track_tries", "dmv_ct_track_tries_many", "dmv_ip_default_settings", "dmv_ct_init_points", "dmv_ct_trace_points", "dmv_ct_trace_points_multi", "dmv_ct_trace_many", "dmv_ct_set_timing", "dmv_ct_last_timing", "dmv_ct_kernel_launch_count", "dmv_ct_last_point_evaluations",
     "dmv_ct_set_undistort", "dmv_ct_upload_raw_image", "dmv_ct_download_frame", "dmv_ps_default_settings", "dmv_ct_make_new_traces",
 ]
 
@@ -293,6 +293,7 @@ _ARGTYPES = {
     "dmv_ct_track": [vp, C.POINTER(CTTrackArgs), C.POINTER(CTTrackResult)],
     "dmv_ct_track_many": [C.POINTER(vp), C.c_int, C.POINTER(CTTrackArgs), C.POINTER(CTTrackResult)],
     "dmv_ct_track_tries": [vp, C.POINTER(CTTriesArgs), C.POINTER(CTTriesResult)],
+    "dmv_ct_track_tries_many": [C.POINTER(vp), C.c_int, C.POINTER(CTTriesArgs), C.POINTER(CTTriesResult)],
     "dmv_ct_init_points": [vp, C.c_int, i32p, i32p, f32p, f32p, f32p, f32p, i32p],
     "dmv_ct_trace_points": [vp, C.POINTER(IPPoints), f32p, f32p, f32p, vp],
     "dmv_ct_trace_points_multi": [vp, C.c_int, vp, vp, vp],
@@ -645,6 +646,20 @@ def ct_track_many(handles, args):
     r = (CTTrackResult * n)()
     check(lib().dmv_ct_track_many(H, n, A, r))
     return [_track_result(x) for x in r]
+
+
+def ct_track_tries_many(handles, args):
+    """dmv_ct_track_tries_many: handles[i] (a CT) runs trackNewCoarse's try loop with args[i] (a dict of CT.track_tries's keywords, R and t
+    included), all in one launch.  Returns the list of CT.track_tries's result dicts, each bit-identical to handles[i].track_tries(**args[i])."""
+    if len(handles) != len(args):
+        raise ValueError(f"{len(handles)} handles but {len(args)} argument sets")
+    n = len(handles)
+    H = (vp * n)(*[g.h.value for g in handles])
+    made = [_tries_args(g.levels, **a) for g, a in zip(handles, args)]
+    A = (CTTriesArgs * n)(*[m[0] for m in made])
+    r = (CTTriesResult * n)()
+    check(lib().dmv_ct_track_tries_many(H, n, A, r))
+    return [_tries_result(x) for x in r]
 
 
 class _TraceSets:

@@ -24,7 +24,7 @@ struct dmv_ct {
   int device = 0;
   dmv::Stream stream;
   dmv::Event ev[2];
-  dmv::Event ev_order;              // orders a dmv_ct_track_many / dmv_ct_trace_many launch on another member's stream behind this handle's queued work
+  dmv::Event ev_order;              // orders a dmv_ct_track_many / _tries_many / dmv_ct_trace_many launch on another member's stream behind this handle's queued work
   bool staging_busy = false;  // an asynchronous upload from h_scratch may be in flight
   bool timing = false;  // CUDA-event timing of every evaluation (dmv_ct_set_timing); off by default: two event records per launch
   int w[DMV_MAX_PYR_LEVELS], h[DMV_MAX_PYR_LEVELS];
@@ -48,6 +48,7 @@ struct dmv_ct {
   dmv::CTPart<dmv::CTMaps> maps;  // TMA descriptors of the level planes (host copy; passed as a kernel parameter)
   int staged[DMV_MAX_PYR_LEVELS] = {0};   // levels whose map ct_make_tensor_maps encoded: the only ones the cluster kernel stages
   dmv::PinnedBuf<dmv_ct_tries_result> h_tries;   // dmv_ct_track_tries's pinned result, allocated on first use
+  dmv::PinnedBuf<double> h_pose;   // dmv_ct_track_tries_many's try table (DMV_CT_MAX_TRIES x 12: R row-major, t), allocated on first use
   long long launches = 0;
   float last_ms[4] = {0, 0, 0, 0};
   // raw-frame ingest (dmv_ct_set_undistort / dmv_ct_upload_raw_image)

@@ -9,6 +9,7 @@
 //   ct_track_cluster_kernel   CoarseTracker::trackNewestCoarse in one launch (below).
 //   ct_track_many_kernel      the same for up to DMV_CT_TRACK_MANY_MAX handles in one launch, one cluster per handle.
 //   ct_track_tries_kernel     FullSystem::trackNewCoarse's loop over up to DMV_CT_MAX_TRIES initial poses in one launch.
+//   ct_track_tries_many_kernel   the same for up to DMV_CT_TRACK_MANY_MAX handles in one launch, one cluster per handle.
 // The entry points of the features built on the handle's resident frame live beside their kernels: ct_ingest.cu (raw frames), ct_depth.cu
 // (makeCoarseDepthL0), ip_trace.cu (immature points) and ps_select.cu (pixel selection); the handle's layout is ct_handle.h.
 #include "ct_handle.h"
@@ -530,19 +531,23 @@ __device__ __forceinline__ unsigned ctc_cluster_id() { unsigned r; asm volatile(
 // after each try thread 0 of every CTA applies the loop's bookkeeping to its own copy of the loop variables (CTLoop).  Every CTA holds the
 // same LM state after a try, so every CTA takes the same decisions, the break included, without any exchange.
 // ---------------------------------------------------------------------------------------------------------------------
-struct CTTries {                   // ct_track_tries_kernel's __grid_constant__ parameter block
-  CTTrack T;                       // the handle's descriptors; T.a0, T.b0 = aff_last_2_l
-  CTMaps maps;
-  double pose[DMV_CT_MAX_TRIES][12];   // lastF_2_fh_tries: R row-major, t
+typedef double CTPose[12];         // one try of lastF_2_fh_tries: R row-major, t
+struct CTTryLoop {                 // the loop's inputs besides the try table
   int n;
   float reTrackThreshold;
   double lastCoarseRMSE0;
   dmv_ct_tries_result* out;        // pinned host
 };
+struct CTTries {                   // ct_track_tries_kernel's __grid_constant__ parameter block
+  CTTrack T;                       // the handle's descriptors; T.a0, T.b0 = aff_last_2_l
+  CTMaps maps;
+  CTPose pose[DMV_CT_MAX_TRIES];
+  CTTryLoop L;
+};
 static_assert(sizeof(CTTries) <= 32764, "CTTries exceeds the 32,764-byte kernel-parameter limit (CUDA >= 12.1, sm_70+)");
 
 // the loop's bookkeeping after try k (L427-488) from the tracker's state S after it; sets the break (L486)
-__device__ void ct_tries_step(const CTTries& Q, CTLoop& W, const CTLM& S, int k) {
+__device__ void ct_tries_step(const CTTryLoop& Q, CTLoop& W, const CTLM& S, int k) {
   const bool good = S.status == 0 && S.good;   // trackingIsGood: false after an abort
   W.tries = k + 1;
   W.pevals += S.pevals;
@@ -561,10 +566,11 @@ __device__ void ct_tries_step(const CTTries& Q, CTLoop& W, const CTLM& S, int k)
   W.stop = W.haveOneGood && W.achieved[0] < Q.lastCoarseRMSE0 * (double)Q.reTrackThreshold;
 }
 
-// one frame tracked by the calling cluster (TRIES: the tries of ct_track_tries_kernel one after the other).  T and maps are
-// __grid_constant__ kernel parameters (the tensor map must stay in parameter space: its address is the operand of the TMA copy).
+// one frame tracked by the calling cluster (TRIES: the tries pose[0 .. Q->n) one after the other).  T and maps are __grid_constant__
+// kernel parameters (the tensor map must stay in parameter space: its address is the operand of the TMA copy); the try table may lie in
+// parameter space (ct_track_tries_kernel) or in the handle's pinned host memory (ct_track_tries_many_kernel).
 template <bool TRIES>
-__device__ __forceinline__ void ct_track_cluster(const CTTrack& T, const CTMaps& maps, const CTTries* Q) {
+__device__ __forceinline__ void ct_track_cluster(const CTTrack& T, const CTMaps& maps, const CTPose* pose, const CTTryLoop* Q) {
   extern __shared__ __align__(128) unsigned char ctc_raw[];
   CTCSmem& M = *reinterpret_cast<CTCSmem*>(ctc_raw);
   CTLM& S = M.S;
@@ -585,8 +591,8 @@ __device__ __forceinline__ void ct_track_cluster(const CTTrack& T, const CTMaps&
   // the staged plane, its mbarrier phase and the cached reference points stay valid from one try to the next: the frame is the same
   for (int kt = 0;; kt++) {   // one track per pass; the plain kernels make one pass
     if (tid == 0) {
-      const double* R0 = TRIES ? Q->pose[kt] : T.R0;
-      const double* t0 = TRIES ? Q->pose[kt] + 9 : T.t0;
+      const double* R0 = TRIES ? pose[kt] : T.R0;
+      const double* t0 = TRIES ? pose[kt] + 9 : T.t0;
       for (int i = 0; i < 9; i++) S.R[i] = R0[i];
       for (int i = 0; i < 3; i++) S.t[i] = t0[i];
       S.a = T.a0; S.b = T.b0;
@@ -698,8 +704,8 @@ __device__ __forceinline__ void ct_track_cluster(const CTTrack& T, const CTMaps&
       const CTLoop& W = M.loop;
       dmv_ct_tries_result* o = Q->out;
       const bool one = W.haveOneGood != 0;
-      for (int i = 0; i < 9; i++) o->R[i] = one ? W.R[i] : Q->pose[0][i];
-      for (int i = 0; i < 3; i++) o->t[i] = one ? W.t[i] : Q->pose[0][9 + i];
+      for (int i = 0; i < 9; i++) o->R[i] = one ? W.R[i] : pose[0][i];
+      for (int i = 0; i < 3; i++) o->t[i] = one ? W.t[i] : pose[0][9 + i];
       o->a = one ? W.a : T.a0; o->b = one ? W.b : T.b0;
       for (int i = 0; i < 5; i++) { o->achievedRes[i] = W.achieved[i]; o->lastResiduals[i] = S.lastResiduals[i]; }
       for (int i = 0; i < 3; i++) { o->flowVecs[i] = one ? W.flowVecs[i] : 0.0; o->flowIndicators[i] = S.flow[i]; }
@@ -720,7 +726,7 @@ __device__ __forceinline__ void ct_track_cluster(const CTTrack& T, const CTMaps&
 }
 
 __global__ void __launch_bounds__(CTC_THREADS, 1) ct_track_cluster_kernel(const __grid_constant__ CTTrack T, const __grid_constant__ CTMaps maps) {
-  ct_track_cluster<false>(T, maps, nullptr);
+  ct_track_cluster<false>(T, maps, nullptr, nullptr);
 }
 
 // dmv_ct_track_many: cluster i tracks member i, independently of every other cluster (no inter-cluster synchronisation, so clusters beyond
@@ -733,11 +739,27 @@ static_assert(sizeof(CTTrackMany) <= 32764, "CTTrackMany exceeds the 32,764-byte
 
 __global__ void __launch_bounds__(CTC_THREADS, 1) ct_track_many_kernel(const __grid_constant__ CTTrackMany B) {
   const unsigned i = ctc_cluster_id();
-  ct_track_cluster<false>(B.T[i], B.maps[i], nullptr);
+  ct_track_cluster<false>(B.T[i], B.maps[i], nullptr, nullptr);
 }
 
 __global__ void __launch_bounds__(CTC_THREADS, 1) ct_track_tries_kernel(const __grid_constant__ CTTries Q) {
-  ct_track_cluster<true>(Q.T, Q.maps, &Q);
+  ct_track_cluster<true>(Q.T, Q.maps, Q.pose, &Q.L);
+}
+
+// dmv_ct_track_tries_many: cluster i runs member i's try loop, independently of every other cluster, as ct_track_many_kernel tracks.  The
+// 16 try tables (48 KB) do not fit in the parameter block beside the descriptors; each lies in its handle's pinned memory (h_pose), and
+// thread 0 of each CTA reads a try's 12 doubles from there when the try starts.
+struct CTTriesMany {
+  CTTrack T[DMV_CT_TRACK_MANY_MAX];
+  CTMaps maps[DMV_CT_TRACK_MANY_MAX];
+  CTTryLoop L[DMV_CT_TRACK_MANY_MAX];
+  const CTPose* pose[DMV_CT_TRACK_MANY_MAX];   // pinned host, in[i].n tries
+};
+static_assert(sizeof(CTTriesMany) <= 32764, "CTTriesMany exceeds the 32,764-byte kernel-parameter limit (CUDA >= 12.1, sm_70+)");
+
+__global__ void __launch_bounds__(CTC_THREADS, 1) ct_track_tries_many_kernel(const __grid_constant__ CTTriesMany B) {
+  const unsigned i = ctc_cluster_id();
+  ct_track_cluster<true>(B.T[i], B.maps[i], B.pose[i], &B.L[i]);
 }
 
 }  // namespace dmv
@@ -1013,8 +1035,8 @@ static int ct_track_params(dmv_ct* c, const dmv_ct_track_args* in, CTTrack& T) {
 }
 
 // the handle's cluster size, probed on its first track (on the handle's device): the largest cluster the device schedules for
-// ct_track_cluster_kernel (16 needs the non-portable opt-in).  ct_track_many_kernel and ct_track_tries_kernel have the same block, shared
-// memory and launch bounds, so the probed size holds for them too; the probe opts all three kernels in.
+// ct_track_cluster_kernel (16 needs the non-portable opt-in).  ct_track_many_kernel, ct_track_tries_kernel and ct_track_tries_many_kernel
+// have the same block, shared memory and launch bounds, so the probed size holds for them too; the probe opts all four kernels in.
 static int ct_probe_cluster(dmv_ct* c) {
   if (c->cluster_size == 0) {
     c->cluster_size = -1;
@@ -1029,9 +1051,11 @@ static int ct_probe_cluster(dmv_ct* c) {
       CK(cudaFuncSetAttribute(ct_track_cluster_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)sizeof(CTCSmem)));
       CK(cudaFuncSetAttribute(ct_track_many_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)sizeof(CTCSmem)));
       CK(cudaFuncSetAttribute(ct_track_tries_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)sizeof(CTCSmem)));
+      CK(cudaFuncSetAttribute(ct_track_tries_many_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)sizeof(CTCSmem)));
       cudaFuncSetAttribute(ct_track_cluster_kernel, cudaFuncAttributeNonPortableClusterSizeAllowed, 1);
       cudaFuncSetAttribute(ct_track_many_kernel, cudaFuncAttributeNonPortableClusterSizeAllowed, 1);
       cudaFuncSetAttribute(ct_track_tries_kernel, cudaFuncAttributeNonPortableClusterSizeAllowed, 1);
+      cudaFuncSetAttribute(ct_track_tries_many_kernel, cudaFuncAttributeNonPortableClusterSizeAllowed, 1);
       cudaGetLastError();
       for (int nc : {16, 8, 4}) {
         if (want_nc && nc != want_nc) continue;
@@ -1082,9 +1106,8 @@ int dmv_ct_track(dmv_ct* c, const dmv_ct_track_args* in, dmv_ct_track_result* ou
   return DMV_OK;
 }
 
-// dmv_ct_track for n handles in one launch, one cluster per handle.  Every check precedes the launch.
-int dmv_ct_track_many(dmv_ct* const* handles, int n, const dmv_ct_track_args* in, dmv_ct_track_result* out) {
-  if (!handles || !in || !out) return set_error(DMV_ERR_INVALID, "null argument");
+// the membership rules of the calls over several handles: 1..DMV_CT_TRACK_MANY_MAX handles, none NULL, none twice, all on one device
+static int ct_many_members(dmv_ct* const* handles, int n) {
   if (n < 1 || n > DMV_CT_TRACK_MANY_MAX) return set_error(DMV_ERR_INVALID, "n = %d: expected 1 to %d handles", n, DMV_CT_TRACK_MANY_MAX);
   for (int i = 0; i < n; i++) {
     if (!handles[i]) return set_error(DMV_ERR_INVALID, "handles[%d] is NULL", i);
@@ -1094,12 +1117,11 @@ int dmv_ct_track_many(dmv_ct* const* handles, int n, const dmv_ct_track_args* in
       return set_error(DMV_ERR_INVALID, "handles[%d] is on device %d, handles[0] on device %d: one launch runs on one device", i, handles[i]->device,
                        handles[0]->device);
   }
-  std::unique_ptr<CTTrackMany> B(new CTTrackMany());
-  for (int i = 0; i < n; i++) {
-    const int rc = ct_track_params(handles[i], &in[i], B->T[i]);
-    if (rc != DMV_OK) return ct_member_error(rc, i);
-  }
-  CK(cudaSetDevice(handles[0]->device));
+  return DMV_OK;
+}
+
+// every member probed (on handles[0]'s device, which is current) and one cluster size among them
+static int ct_many_cluster(dmv_ct* const* handles, int n) {
   for (int i = 0; i < n; i++) {
     const int rc = ct_probe_cluster(handles[i]);
     if (rc != DMV_OK) return ct_member_error(rc, i);
@@ -1109,16 +1131,39 @@ int dmv_ct_track_many(dmv_ct* const* handles, int n, const dmv_ct_track_args* in
     if (handles[i]->cluster_size != nc)
       return set_error(DMV_ERR_INVALID, "handles[0] tracks with clusters of %d CTAs, handles[%d] with %d: one launch needs one cluster size", nc, i,
                        handles[i]->cluster_size);
+  return DMV_OK;
+}
+
+// the launch on handles[0]'s stream goes behind every member's queued uploads (dmv_ct_upload_new_image does not synchronise)
+static int ct_many_order(dmv_ct* const* handles, int n) {
+  for (int i = 1; i < n; i++) {
+    CK(cudaEventRecord(handles[i]->ev_order, handles[i]->stream));
+    CK(cudaStreamWaitEvent(handles[0]->stream, handles[i]->ev_order, 0));
+  }
+  return DMV_OK;
+}
+
+// dmv_ct_track for n handles in one launch, one cluster per handle.  Every check precedes the launch.
+int dmv_ct_track_many(dmv_ct* const* handles, int n, const dmv_ct_track_args* in, dmv_ct_track_result* out) {
+  if (!handles || !in || !out) return set_error(DMV_ERR_INVALID, "null argument");
+  int rc = ct_many_members(handles, n);
+  if (rc != DMV_OK) return rc;
+  std::unique_ptr<CTTrackMany> B(new CTTrackMany());
+  for (int i = 0; i < n; i++) {
+    rc = ct_track_params(handles[i], &in[i], B->T[i]);
+    if (rc != DMV_OK) return ct_member_error(rc, i);
+  }
+  CK(cudaSetDevice(handles[0]->device));
+  rc = ct_many_cluster(handles, n);
+  if (rc != DMV_OK) return rc;
+  const int nc = handles[0]->cluster_size;
   cudaStream_t s = handles[0]->stream;
   for (int i = 0; i < n; i++) {
-    dmv_ct* c = handles[i];
-    for (int l = 0; l < DMV_MAX_PYR_LEVELS; l++) B->T[i].staged[l] = c->staged[l];
-    B->maps[i] = *c->maps;
-    if (i > 0) {  // the launch goes behind every member's queued uploads (dmv_ct_upload_new_image does not synchronise)
-      CK(cudaEventRecord(c->ev_order, c->stream));
-      CK(cudaStreamWaitEvent(s, c->ev_order, 0));
-    }
+    for (int l = 0; l < DMV_MAX_PYR_LEVELS; l++) B->T[i].staged[l] = handles[i]->staged[l];
+    B->maps[i] = *handles[i]->maps;
   }
+  rc = ct_many_order(handles, n);
+  if (rc != DMV_OK) return rc;
   CTClusterLaunch q(nc, n, s);
   // one member: the single-handle kernel, the same device function with a 1.7 KB instead of a 27 KB parameter block (through
   // ct_track_many_kernel one 640x480, 5-level track took 0.360 ms against dmv_ct_track's 0.336 ms, H100 80GB HBM3 at 700 W)
@@ -1133,9 +1178,9 @@ int dmv_ct_track_many(dmv_ct* const* handles, int n, const dmv_ct_track_args* in
   return DMV_OK;
 }
 
-// FullSystem::trackNewCoarse's try loop (FullSystem.cpp:L412-506, visual-only) in one launch: see ct_track_tries_kernel
-int dmv_ct_track_tries(dmv_ct* c, const dmv_ct_tries_args* in, dmv_ct_tries_result* out) {
-  if (!c || !in || !out) return set_error(DMV_ERR_INVALID, "null argument");
+// dmv_ct_track_tries's argument checks and the launch parameters of one handle's loop, all but staged[] (decided by the probe) and the
+// result pointer (allocated after every check); no CUDA call
+static int ct_tries_params(dmv_ct* c, const dmv_ct_tries_args* in, CTTrack& T, CTTryLoop& L) {
   if (in->n < 1 || in->n > DMV_CT_MAX_TRIES) return set_error(DMV_ERR_INVALID, "n = %d: expected 1 to %d tries", in->n, DMV_CT_MAX_TRIES);
   if (!in->R || !in->t) return set_error(DMV_ERR_INVALID, "null R / t");
   dmv_ct_track_args a;   // try 0 with minResForAbort NaN: dmv_ct_track's checks and descriptors
@@ -1146,8 +1191,28 @@ int dmv_ct_track_tries(dmv_ct* c, const dmv_ct_tries_args* in, dmv_ct_tries_resu
   a.coarseCutoffTH = in->coarseCutoffTH; a.affineOptModeA = in->affineOptModeA; a.affineOptModeB = in->affineOptModeB;
   a.coarsestLvl = in->coarsestLvl;
   for (int i = 0; i < 5; i++) a.minResForAbort[i] = NAN;   // unused: each try aborts against the loop's achievedRes
+  const int rc = ct_track_params(c, &a, T);
+  if (rc != DMV_OK) return rc;
+  L.n = in->n;
+  L.reTrackThreshold = in->reTrackThreshold;
+  L.lastCoarseRMSE0 = in->lastCoarseRMSE0;
+  L.out = nullptr;
+  return DMV_OK;
+}
+
+// lastF_2_fh_tries of in as the kernels' try table
+static void ct_fill_tries(const dmv_ct_tries_args* in, CTPose* pose) {
+  for (int k = 0; k < in->n; k++) {
+    for (int i = 0; i < 9; i++) pose[k][i] = in->R[9 * k + i];
+    for (int i = 0; i < 3; i++) pose[k][9 + i] = in->t[3 * k + i];
+  }
+}
+
+// FullSystem::trackNewCoarse's try loop (FullSystem.cpp:L412-506, visual-only) in one launch: see ct_track_tries_kernel
+int dmv_ct_track_tries(dmv_ct* c, const dmv_ct_tries_args* in, dmv_ct_tries_result* out) {
+  if (!c || !in || !out) return set_error(DMV_ERR_INVALID, "null argument");
   std::unique_ptr<CTTries> Q(new CTTries());
-  int rc = ct_track_params(c, &a, Q->T);
+  int rc = ct_tries_params(c, in, Q->T, Q->L);
   if (rc != DMV_OK) return rc;
   CK(cudaSetDevice(c->device));
   rc = ct_probe_cluster(c);
@@ -1155,20 +1220,61 @@ int dmv_ct_track_tries(dmv_ct* c, const dmv_ct_tries_args* in, dmv_ct_tries_resu
   CK(c->h_tries.reserve(1));
   for (int l = 0; l < DMV_MAX_PYR_LEVELS; l++) Q->T.staged[l] = c->staged[l];
   Q->maps = *c->maps;
-  for (int k = 0; k < in->n; k++) {
-    for (int i = 0; i < 9; i++) Q->pose[k][i] = in->R[9 * k + i];
-    for (int i = 0; i < 3; i++) Q->pose[k][9 + i] = in->t[3 * k + i];
-  }
-  Q->n = in->n;
-  Q->reTrackThreshold = in->reTrackThreshold;
-  Q->lastCoarseRMSE0 = in->lastCoarseRMSE0;
-  Q->out = c->h_tries;
+  ct_fill_tries(in, Q->pose);
+  Q->L.out = c->h_tries;
   CTClusterLaunch q(c->cluster_size, 1, c->stream);
   CK(cudaLaunchKernelEx(&q.cfg, ct_track_tries_kernel, *Q));
   c->launches++;
   CK(cudaStreamSynchronize(c->stream));
   c->staging_busy = false;
   *out = *c->h_tries;
+  return DMV_OK;
+}
+
+// dmv_ct_track_tries for n handles in one launch, one cluster per handle.  Every check precedes the first allocation and the launch.
+int dmv_ct_track_tries_many(dmv_ct* const* handles, int n, const dmv_ct_tries_args* in, dmv_ct_tries_result* out) {
+  if (!handles || !in || !out) return set_error(DMV_ERR_INVALID, "null argument");
+  int rc = ct_many_members(handles, n);
+  if (rc != DMV_OK) return rc;
+  std::unique_ptr<CTTriesMany> B(new CTTriesMany());
+  for (int i = 0; i < n; i++) {
+    rc = ct_tries_params(handles[i], &in[i], B->T[i], B->L[i]);
+    if (rc != DMV_OK) return ct_member_error(rc, i);
+  }
+  CK(cudaSetDevice(handles[0]->device));
+  rc = ct_many_cluster(handles, n);
+  if (rc != DMV_OK) return rc;
+  const int nc = handles[0]->cluster_size;
+  cudaStream_t s = handles[0]->stream;
+  for (int i = 0; i < n; i++) {
+    dmv_ct* c = handles[i];
+    CK(c->h_tries.reserve(1));
+    if (n > 1) CK(c->h_pose.reserve((size_t)DMV_CT_MAX_TRIES * 12));
+    for (int l = 0; l < DMV_MAX_PYR_LEVELS; l++) B->T[i].staged[l] = c->staged[l];
+    B->maps[i] = *c->maps;
+    B->L[i].out = c->h_tries;
+    B->pose[i] = reinterpret_cast<const CTPose*>(c->h_pose.get());
+  }
+  rc = ct_many_order(handles, n);
+  if (rc != DMV_OK) return rc;
+  CTClusterLaunch q(nc, n, s);
+  if (n == 1) {   // one member: the single-handle kernel and its 4.8 KB parameter block, as dmv_ct_track_many launches ct_track_cluster_kernel
+    std::unique_ptr<CTTries> Q(new CTTries());
+    Q->T = B->T[0]; Q->maps = B->maps[0]; Q->L = B->L[0];
+    ct_fill_tries(&in[0], Q->pose);
+    CK(cudaLaunchKernelEx(&q.cfg, ct_track_tries_kernel, *Q));
+  } else {
+    // the try tables are read by the kernel from pinned memory: no previous call reads them any more (every call synchronises before it
+    // returns), and this one does not return before the kernel has finished
+    for (int i = 0; i < n; i++) ct_fill_tries(&in[i], reinterpret_cast<CTPose*>(handles[i]->h_pose.get()));
+    CK(cudaLaunchKernelEx(&q.cfg, ct_track_tries_many_kernel, *B));
+  }
+  for (int i = 0; i < n; i++) handles[i]->launches++;
+  CK(cudaStreamSynchronize(s));
+  for (int i = 0; i < n; i++) {
+    handles[i]->staging_busy = false;   // each member's uploads completed before the kernel started
+    out[i] = *handles[i]->h_tries;
+  }
   return DMV_OK;
 }
 

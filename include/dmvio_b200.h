@@ -461,6 +461,19 @@ typedef struct dmv_ct_tries_result {
   int tries_started;             /* tries the device began (= tries: they run in order) */
 } dmv_ct_tries_result;
 int dmv_ct_track_tries(dmv_ct* ct, const dmv_ct_tries_args* in, dmv_ct_tries_result* out);
+/* dmv_ct_track_tries for n independent handles (several visual-only camera streams served by one host thread) in ONE launch: one
+ * thread-block cluster per handle runs that handle's try loop, and the clusters retire independently, so a frame that needs many tries
+ * delays only its own member.  in[i] may differ from member to member in every field (n, coarsestLvl, lastCoarseRMSE0, exposures, affine
+ * state), and the handles in image size and level count, as long as their probed cluster sizes match.
+ * out[i] is bit-identical to what dmv_ct_track_tries(handles[i], &in[i], &out[i]) returns, and afterwards dmv_ct_last_point_evaluations
+ * and dmv_ct_kernel_launch_count (+1) of every handle read as after that call.  Each handle's frame, reference and probed cluster size are
+ * unchanged.  The launch goes on handles[0]'s stream, ordered behind the work queued on every handle's stream (asynchronous uploads
+ * included); the call returns after one synchronisation, with every handle's staging buffer free.  With n > 1 each handle holds its try
+ * table in a pinned block of 3 KB, allocated on first use beside dmv_ct_track_tries's result.
+ * Errors, all before anything is launched or any out[i] is written, and with every launch count unchanged: those of dmv_ct_track_many
+ * (n outside 1..DMV_CT_TRACK_MANY_MAX, a NULL pointer, a handle passed twice, handles on different devices or with different cluster sizes)
+ * and dmv_ct_track_tries's own errors for any member, with the member's index in the message ("handles[3]: ..."). */
+int dmv_ct_track_tries_many(dmv_ct* const* handles, int n, const dmv_ct_tries_args* in, dmv_ct_tries_result* out);
 
 /* ------------------------------------------------------------------------------------------------
  * Immature-point tracing  ==  ImmaturePoint::traceOn (FullSystem/ImmaturePoint.cpp:L77-437) for all immature points of ONE host
