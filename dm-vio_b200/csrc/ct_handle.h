@@ -81,6 +81,27 @@ inline int ct_member_error(int rc, int i) {
   return set_error(rc, "handles[%d]: %s", i, msg);
 }
 
+// the member list of a call over several handles: 1..max handles, none NULL, none twice, all on one device
+inline int ct_check_members(dmv_ct* const* handles, int n, int max) {
+  if (n < 1 || n > max) return set_error(DMV_ERR_INVALID, "n = %d: expected 1 to %d handles", n, max);
+  for (int i = 0; i < n; i++) {
+    if (!handles[i]) return set_error(DMV_ERR_INVALID, "handles[%d] is NULL", i);
+    for (int j = 0; j < i; j++)
+      if (handles[j] == handles[i]) return set_error(DMV_ERR_INVALID, "handles[%d] and handles[%d] are the same handle", j, i);
+    if (handles[i]->device != handles[0]->device)
+      return set_error(DMV_ERR_INVALID, "handles[%d] is on device %d, handles[0] on device %d: one launch runs on one device", i, handles[i]->device,
+                       handles[0]->device);
+  }
+  return DMV_OK;
+}
+
+// work enqueued on stream s from now on runs behind the work queued on member c's stream so far: a launch over several handles goes on one
+// member's stream, behind every other member's uploads (dmv_ct_upload_new_image does not synchronise)
+inline cudaError_t ct_order_behind(dmv_ct* c, cudaStream_t s) {
+  const cudaError_t e = cudaEventRecord(c->ev_order, c->stream);
+  return e == cudaSuccess ? cudaStreamWaitEvent(s, c->ev_order, 0) : e;
+}
+
 // d_ip / h_ip hold at least n points: 31 words per point (dmv_ct_trace_points' layout, the widest) and 14 words of tables for each of up
 // to 64 host frames
 inline cudaError_t ct_reserve_ip(dmv_ct* c, int n) {

@@ -196,6 +196,13 @@ __global__ void __launch_bounds__(CT_THREADS) ct_res_gs_kernel(CTParams P, const
 // CTA, so no broadcast is needed.
 // ---------------------------------------------------------------------------------------------------------------------
 constexpr int CT_L = DMV_MAX_PYR_LEVELS;
+// a track's result in the handle's pinned block h_out, which also takes ct_res_gs_kernel's 53 sums; written by CTA 0 of the cluster
+struct CTTrackOut {
+  double R[9], t[3], a, b, lastResiduals[5], flow[3];
+  double good, iterations, evaluations, status;
+  double pevals;   // dmv_ct_last_point_evaluations; the tries kernels write only this
+};
+static_assert(sizeof(CTTrackOut) == 27 * sizeof(double), "CTTrackOut must fit the first 27 of h_out's 64 doubles");
 struct CTTrack {
   int levels, coarsest;
   int n[CT_L], w[CT_L], h[CT_L];
@@ -209,7 +216,7 @@ struct CTTrack {
   float huber, cutoffTH, affModeA, affModeB;
   double minRes[5];
   int staged[CT_L];              // level l's plane is TMA-staged (ct_make_tensor_maps encoded its map)
-  double* out;                  // pinned host: R[9] t[3] a b lastResiduals[5] flow[3] good iterations evaluations status
+  CTTrackOut* out;              // pinned host
 };
 
 struct CTLM {  // the scalar state of trackNewestCoarse, one copy per CTA (shared memory), advanced by thread 0
@@ -711,16 +718,16 @@ __device__ __forceinline__ void ct_track_cluster(const CTTrack& T, const CTMaps&
       for (int i = 0; i < 3; i++) { o->flowVecs[i] = one ? W.flowVecs[i] : 0.0; o->flowIndicators[i] = S.flow[i]; }
       o->trackingGood = W.trackingGood; o->haveOneGood = W.haveOneGood; o->winner = one ? W.winner : -1;
       o->tries = W.tries; o->tries_started = W.tries;
-      T.out[26] = W.pevals;   // dmv_ct_last_point_evaluations
+      T.out->pevals = W.pevals;
     } else {
-      double* o = T.out;
+      CTTrackOut* o = T.out;
       const bool ok = (S.status == 0);   // an aborted track returns the input pose, like the reference's early return
-      for (int i = 0; i < 9; i++) o[i] = ok ? S.R[i] : T.R0[i];
-      for (int i = 0; i < 3; i++) o[9 + i] = ok ? S.t[i] : T.t0[i];
-      o[12] = ok ? S.a : T.a0; o[13] = ok ? S.b : T.b0;
-      for (int i = 0; i < 5; i++) o[14 + i] = S.lastResiduals[i];
-      for (int i = 0; i < 3; i++) o[19 + i] = S.flow[i];
-      o[22] = S.good; o[23] = S.iterations; o[24] = S.evaluations; o[25] = S.status; o[26] = S.pevals;
+      for (int i = 0; i < 9; i++) o->R[i] = ok ? S.R[i] : T.R0[i];
+      for (int i = 0; i < 3; i++) o->t[i] = ok ? S.t[i] : T.t0[i];
+      o->a = ok ? S.a : T.a0; o->b = ok ? S.b : T.b0;
+      for (int i = 0; i < 5; i++) o->lastResiduals[i] = S.lastResiduals[i];
+      for (int i = 0; i < 3; i++) o->flow[i] = S.flow[i];
+      o->good = S.good; o->iterations = S.iterations; o->evaluations = S.evaluations; o->status = S.status; o->pevals = S.pevals;
     }
   }
 }
@@ -1011,6 +1018,8 @@ struct CTClusterLaunch {
   }
 };
 
+static CTTrackOut* ct_track_out(const dmv_ct* c) { return reinterpret_cast<CTTrackOut*>(c->h_out.get()); }
+
 // dmv_ct_track's argument checks and the launch parameters of one handle, all but staged[] (decided by the probe); no CUDA call
 static int ct_track_params(dmv_ct* c, const dmv_ct_track_args* in, CTTrack& T) {
   if (in->coarsestLvl < 0 || in->coarsestLvl >= c->cfg.levels || in->coarsestLvl >= 5) return set_error(DMV_ERR_INVALID, "coarsestLvl out of range");
@@ -1030,7 +1039,7 @@ static int ct_track_params(dmv_ct* c, const dmv_ct_track_args* in, CTTrack& T) {
   T.ref_exposure = in->ref_exposure; T.new_exposure = in->new_exposure;
   T.huber = c->huber; T.cutoffTH = in->coarseCutoffTH; T.affModeA = in->affineOptModeA; T.affModeB = in->affineOptModeB;
   for (int i = 0; i < 5; i++) T.minRes[i] = in->minResForAbort[i];
-  T.out = c->h_out;
+  T.out = ct_track_out(c);
   return DMV_OK;
 }
 
@@ -1048,14 +1057,12 @@ static int ct_probe_cluster(dmv_ct* c) {
       return set_error(DMV_ERR_INVALID, "DMV_CT_CLUSTER=%s: expected 16, 8 or 4", env_nc);
     }
     if (ct_make_tensor_maps(c) == DMV_OK) {
-      CK(cudaFuncSetAttribute(ct_track_cluster_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)sizeof(CTCSmem)));
-      CK(cudaFuncSetAttribute(ct_track_many_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)sizeof(CTCSmem)));
-      CK(cudaFuncSetAttribute(ct_track_tries_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)sizeof(CTCSmem)));
-      CK(cudaFuncSetAttribute(ct_track_tries_many_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)sizeof(CTCSmem)));
-      cudaFuncSetAttribute(ct_track_cluster_kernel, cudaFuncAttributeNonPortableClusterSizeAllowed, 1);
-      cudaFuncSetAttribute(ct_track_many_kernel, cudaFuncAttributeNonPortableClusterSizeAllowed, 1);
-      cudaFuncSetAttribute(ct_track_tries_kernel, cudaFuncAttributeNonPortableClusterSizeAllowed, 1);
-      cudaFuncSetAttribute(ct_track_tries_many_kernel, cudaFuncAttributeNonPortableClusterSizeAllowed, 1);
+      const void* const kernels[] = {(const void*)ct_track_cluster_kernel, (const void*)ct_track_many_kernel, (const void*)ct_track_tries_kernel,
+                                     (const void*)ct_track_tries_many_kernel};
+      for (const void* k : kernels) {
+        CK(cudaFuncSetAttribute(k, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)sizeof(CTCSmem)));
+        cudaFuncSetAttribute(k, cudaFuncAttributeNonPortableClusterSizeAllowed, 1);   // without it the probe finds at most 8
+      }
       cudaGetLastError();
       for (int nc : {16, 8, 4}) {
         if (want_nc && nc != want_nc) continue;
@@ -1078,104 +1085,84 @@ static int ct_probe_cluster(dmv_ct* c) {
 
 // the result the kernel wrote into the handle's pinned output block
 static void ct_read_result(const dmv_ct* c, dmv_ct_track_result* out) {
-  const double* o = c->h_out;
-  for (int i = 0; i < 9; i++) out->R[i] = o[i];
-  for (int i = 0; i < 3; i++) out->t[i] = o[9 + i];
-  out->a = o[12]; out->b = o[13];
-  for (int i = 0; i < 5; i++) out->lastResiduals[i] = o[14 + i];
-  for (int i = 0; i < 3; i++) out->flowIndicators[i] = o[19 + i];
-  out->trackingGood = (int)o[22]; out->iterations = (int)o[23]; out->evaluations = (int)o[24]; out->status = (int)o[25];
+  const CTTrackOut* o = ct_track_out(c);
+  for (int i = 0; i < 9; i++) out->R[i] = o->R[i];
+  for (int i = 0; i < 3; i++) out->t[i] = o->t[i];
+  out->a = o->a; out->b = o->b;
+  for (int i = 0; i < 5; i++) out->lastResiduals[i] = o->lastResiduals[i];
+  for (int i = 0; i < 3; i++) out->flowIndicators[i] = o->flow[i];
+  out->trackingGood = (int)o->good; out->iterations = (int)o->iterations; out->evaluations = (int)o->evaluations; out->status = (int)o->status;
 }
 
-// CoarseTracker::trackNewestCoarse (CoarseTracker.cpp:L539-770, visual-only branch) in one persistent launch
+// the last checks of a track over hs[0..n), after every member's own: each member probed on hs[0]'s device, which this makes current
+// (`many`: a member's error names it), and one cluster size among them.  Then each member's staged levels and tensor maps into its launch
+// parameters T[i], maps[i].
+static int ct_cluster_ready(dmv_ct* const* hs, int n, bool many, CTTrack* T, CTMaps* maps) {
+  CK(cudaSetDevice(hs[0]->device));
+  for (int i = 0; i < n; i++) {
+    const int rc = ct_probe_cluster(hs[i]);
+    if (rc != DMV_OK) return many ? ct_member_error(rc, i) : rc;
+  }
+  for (int i = 1; i < n; i++)
+    if (hs[i]->cluster_size != hs[0]->cluster_size)
+      return set_error(DMV_ERR_INVALID, "handles[0] tracks with clusters of %d CTAs, handles[%d] with %d: one launch needs one cluster size",
+                       hs[0]->cluster_size, i, hs[i]->cluster_size);
+  for (int i = 0; i < n; i++) {
+    for (int l = 0; l < DMV_MAX_PYR_LEVELS; l++) T[i].staged[l] = hs[i]->staged[l];
+    maps[i] = *hs[i]->maps;
+  }
+  return DMV_OK;
+}
+
+// kernel (args: pointers to its parameters) on one cluster per member, on hs[0]'s stream behind every other member's queued work; counted
+// on every member and awaited
+static int ct_cluster_launch(dmv_ct* const* hs, int n, const void* kernel, void** args) {
+  const cudaStream_t s = hs[0]->stream;
+  for (int i = 1; i < n; i++) CK(ct_order_behind(hs[i], s));
+  CTClusterLaunch q(hs[0]->cluster_size, n, s);
+  CK(cudaLaunchKernelExC(&q.cfg, kernel, args));
+  for (int i = 0; i < n; i++) hs[i]->launches++;
+  CK(cudaStreamSynchronize(s));
+  for (int i = 0; i < n; i++) hs[i]->staging_busy = false;   // each member's uploads completed before the kernel started
+  return DMV_OK;
+}
+
+// CoarseTracker::trackNewestCoarse (CoarseTracker.cpp:L539-770, visual-only branch) for hs[0..n) in one launch, one cluster per handle.
+// Every check precedes the launch; `many`: a member's error names it.  One handle launches ct_track_cluster_kernel, the same device function
+// with a 1.7 KB instead of a 27 KB parameter block (through ct_track_many_kernel one 640x480, 5-level track took 0.360 ms against 0.336 ms,
+// H100 80GB HBM3 at 700 W).
+static int ct_track_run(dmv_ct* const* hs, int n, const dmv_ct_track_args* in, dmv_ct_track_result* out, bool many) {
+  CTTrack T1;
+  CTMaps M1;
+  std::unique_ptr<CTTrackMany> B(n > 1 ? new CTTrackMany() : nullptr);
+  CTTrack* T = n > 1 ? B->T : &T1;
+  for (int i = 0; i < n; i++) {
+    const int rc = ct_track_params(hs[i], &in[i], T[i]);
+    if (rc != DMV_OK) return many ? ct_member_error(rc, i) : rc;
+  }
+  int rc = ct_cluster_ready(hs, n, many, T, n > 1 ? B->maps : &M1);
+  if (rc != DMV_OK) return rc;
+  if (n == 1) {
+    void* args[] = {&T1, &M1};
+    rc = ct_cluster_launch(hs, 1, (const void*)ct_track_cluster_kernel, args);
+  } else {
+    void* args[] = {B.get()};
+    rc = ct_cluster_launch(hs, n, (const void*)ct_track_many_kernel, args);
+  }
+  if (rc != DMV_OK) return rc;
+  for (int i = 0; i < n; i++) ct_read_result(hs[i], &out[i]);
+  return DMV_OK;
+}
+
 int dmv_ct_track(dmv_ct* c, const dmv_ct_track_args* in, dmv_ct_track_result* out) {
   if (!c || !in || !out) return set_error(DMV_ERR_INVALID, "null argument");
-  CTTrack T;
-  int rc = ct_track_params(c, in, T);
-  if (rc != DMV_OK) return rc;
-  CK(cudaSetDevice(c->device));
-  rc = ct_probe_cluster(c);
-  if (rc != DMV_OK) return rc;
-  for (int l = 0; l < DMV_MAX_PYR_LEVELS; l++) T.staged[l] = c->staged[l];
-  CTClusterLaunch q(c->cluster_size, 1, c->stream);
-  CK(cudaLaunchKernelEx(&q.cfg, ct_track_cluster_kernel, T, *c->maps));
-  c->launches++;
-  CK(cudaStreamSynchronize(c->stream));
-  c->staging_busy = false;
-  ct_read_result(c, out);
-  return DMV_OK;
+  return ct_track_run(&c, 1, in, out, false);
 }
 
-// the membership rules of the calls over several handles: 1..DMV_CT_TRACK_MANY_MAX handles, none NULL, none twice, all on one device
-static int ct_many_members(dmv_ct* const* handles, int n) {
-  if (n < 1 || n > DMV_CT_TRACK_MANY_MAX) return set_error(DMV_ERR_INVALID, "n = %d: expected 1 to %d handles", n, DMV_CT_TRACK_MANY_MAX);
-  for (int i = 0; i < n; i++) {
-    if (!handles[i]) return set_error(DMV_ERR_INVALID, "handles[%d] is NULL", i);
-    for (int j = 0; j < i; j++)
-      if (handles[j] == handles[i]) return set_error(DMV_ERR_INVALID, "handles[%d] and handles[%d] are the same handle", j, i);
-    if (handles[i]->device != handles[0]->device)
-      return set_error(DMV_ERR_INVALID, "handles[%d] is on device %d, handles[0] on device %d: one launch runs on one device", i, handles[i]->device,
-                       handles[0]->device);
-  }
-  return DMV_OK;
-}
-
-// every member probed (on handles[0]'s device, which is current) and one cluster size among them
-static int ct_many_cluster(dmv_ct* const* handles, int n) {
-  for (int i = 0; i < n; i++) {
-    const int rc = ct_probe_cluster(handles[i]);
-    if (rc != DMV_OK) return ct_member_error(rc, i);
-  }
-  const int nc = handles[0]->cluster_size;
-  for (int i = 1; i < n; i++)
-    if (handles[i]->cluster_size != nc)
-      return set_error(DMV_ERR_INVALID, "handles[0] tracks with clusters of %d CTAs, handles[%d] with %d: one launch needs one cluster size", nc, i,
-                       handles[i]->cluster_size);
-  return DMV_OK;
-}
-
-// the launch on handles[0]'s stream goes behind every member's queued uploads (dmv_ct_upload_new_image does not synchronise)
-static int ct_many_order(dmv_ct* const* handles, int n) {
-  for (int i = 1; i < n; i++) {
-    CK(cudaEventRecord(handles[i]->ev_order, handles[i]->stream));
-    CK(cudaStreamWaitEvent(handles[0]->stream, handles[i]->ev_order, 0));
-  }
-  return DMV_OK;
-}
-
-// dmv_ct_track for n handles in one launch, one cluster per handle.  Every check precedes the launch.
 int dmv_ct_track_many(dmv_ct* const* handles, int n, const dmv_ct_track_args* in, dmv_ct_track_result* out) {
   if (!handles || !in || !out) return set_error(DMV_ERR_INVALID, "null argument");
-  int rc = ct_many_members(handles, n);
-  if (rc != DMV_OK) return rc;
-  std::unique_ptr<CTTrackMany> B(new CTTrackMany());
-  for (int i = 0; i < n; i++) {
-    rc = ct_track_params(handles[i], &in[i], B->T[i]);
-    if (rc != DMV_OK) return ct_member_error(rc, i);
-  }
-  CK(cudaSetDevice(handles[0]->device));
-  rc = ct_many_cluster(handles, n);
-  if (rc != DMV_OK) return rc;
-  const int nc = handles[0]->cluster_size;
-  cudaStream_t s = handles[0]->stream;
-  for (int i = 0; i < n; i++) {
-    for (int l = 0; l < DMV_MAX_PYR_LEVELS; l++) B->T[i].staged[l] = handles[i]->staged[l];
-    B->maps[i] = *handles[i]->maps;
-  }
-  rc = ct_many_order(handles, n);
-  if (rc != DMV_OK) return rc;
-  CTClusterLaunch q(nc, n, s);
-  // one member: the single-handle kernel, the same device function with a 1.7 KB instead of a 27 KB parameter block (through
-  // ct_track_many_kernel one 640x480, 5-level track took 0.360 ms against dmv_ct_track's 0.336 ms, H100 80GB HBM3 at 700 W)
-  if (n == 1) CK(cudaLaunchKernelEx(&q.cfg, ct_track_cluster_kernel, B->T[0], B->maps[0]));
-  else CK(cudaLaunchKernelEx(&q.cfg, ct_track_many_kernel, *B));
-  for (int i = 0; i < n; i++) handles[i]->launches++;
-  CK(cudaStreamSynchronize(s));
-  for (int i = 0; i < n; i++) {
-    handles[i]->staging_busy = false;   // each member's uploads completed before the kernel started
-    ct_read_result(handles[i], &out[i]);
-  }
-  return DMV_OK;
+  const int rc = ct_check_members(handles, n, DMV_CT_TRACK_MANY_MAX);
+  return rc != DMV_OK ? rc : ct_track_run(handles, n, in, out, true);
 }
 
 // dmv_ct_track_tries's argument checks and the launch parameters of one handle's loop, all but staged[] (decided by the probe) and the
@@ -1208,74 +1195,52 @@ static void ct_fill_tries(const dmv_ct_tries_args* in, CTPose* pose) {
   }
 }
 
-// FullSystem::trackNewCoarse's try loop (FullSystem.cpp:L412-506, visual-only) in one launch: see ct_track_tries_kernel
-int dmv_ct_track_tries(dmv_ct* c, const dmv_ct_tries_args* in, dmv_ct_tries_result* out) {
-  if (!c || !in || !out) return set_error(DMV_ERR_INVALID, "null argument");
-  std::unique_ptr<CTTries> Q(new CTTries());
-  int rc = ct_tries_params(c, in, Q->T, Q->L);
+// FullSystem::trackNewCoarse's try loop (FullSystem.cpp:L412-506, visual-only) for hs[0..n) in one launch, one cluster per handle: see
+// ct_track_tries_kernel.  Every check precedes the first allocation and the launch; `many`: a member's error names it.  One handle launches
+// ct_track_tries_kernel and its 4.8 KB parameter block, as ct_track_run launches ct_track_cluster_kernel.
+static int ct_tries_run(dmv_ct* const* hs, int n, const dmv_ct_tries_args* in, dmv_ct_tries_result* out, bool many) {
+  std::unique_ptr<CTTries> Q(n == 1 ? new CTTries() : nullptr);
+  std::unique_ptr<CTTriesMany> B(n > 1 ? new CTTriesMany() : nullptr);
+  CTTrack* T = n > 1 ? B->T : &Q->T;
+  CTTryLoop* L = n > 1 ? B->L : &Q->L;
+  for (int i = 0; i < n; i++) {
+    const int rc = ct_tries_params(hs[i], &in[i], T[i], L[i]);
+    if (rc != DMV_OK) return many ? ct_member_error(rc, i) : rc;
+  }
+  int rc = ct_cluster_ready(hs, n, many, T, n > 1 ? B->maps : &Q->maps);
   if (rc != DMV_OK) return rc;
-  CK(cudaSetDevice(c->device));
-  rc = ct_probe_cluster(c);
+  for (int i = 0; i < n; i++) {
+    dmv_ct* c = hs[i];
+    CK(c->h_tries.reserve(1));
+    L[i].out = c->h_tries;
+    if (n > 1) {   // the kernel reads the try table from pinned memory: no earlier call still reads it, every call synchronises before it returns
+      CK(c->h_pose.reserve((size_t)DMV_CT_MAX_TRIES * 12));
+      ct_fill_tries(&in[i], reinterpret_cast<CTPose*>(c->h_pose.get()));
+      B->pose[i] = reinterpret_cast<const CTPose*>(c->h_pose.get());
+    }
+  }
+  if (n == 1) {
+    ct_fill_tries(&in[0], Q->pose);
+    void* args[] = {Q.get()};
+    rc = ct_cluster_launch(hs, 1, (const void*)ct_track_tries_kernel, args);
+  } else {
+    void* args[] = {B.get()};
+    rc = ct_cluster_launch(hs, n, (const void*)ct_track_tries_many_kernel, args);
+  }
   if (rc != DMV_OK) return rc;
-  CK(c->h_tries.reserve(1));
-  for (int l = 0; l < DMV_MAX_PYR_LEVELS; l++) Q->T.staged[l] = c->staged[l];
-  Q->maps = *c->maps;
-  ct_fill_tries(in, Q->pose);
-  Q->L.out = c->h_tries;
-  CTClusterLaunch q(c->cluster_size, 1, c->stream);
-  CK(cudaLaunchKernelEx(&q.cfg, ct_track_tries_kernel, *Q));
-  c->launches++;
-  CK(cudaStreamSynchronize(c->stream));
-  c->staging_busy = false;
-  *out = *c->h_tries;
+  for (int i = 0; i < n; i++) out[i] = *hs[i]->h_tries;
   return DMV_OK;
 }
 
-// dmv_ct_track_tries for n handles in one launch, one cluster per handle.  Every check precedes the first allocation and the launch.
+int dmv_ct_track_tries(dmv_ct* c, const dmv_ct_tries_args* in, dmv_ct_tries_result* out) {
+  if (!c || !in || !out) return set_error(DMV_ERR_INVALID, "null argument");
+  return ct_tries_run(&c, 1, in, out, false);
+}
+
 int dmv_ct_track_tries_many(dmv_ct* const* handles, int n, const dmv_ct_tries_args* in, dmv_ct_tries_result* out) {
   if (!handles || !in || !out) return set_error(DMV_ERR_INVALID, "null argument");
-  int rc = ct_many_members(handles, n);
-  if (rc != DMV_OK) return rc;
-  std::unique_ptr<CTTriesMany> B(new CTTriesMany());
-  for (int i = 0; i < n; i++) {
-    rc = ct_tries_params(handles[i], &in[i], B->T[i], B->L[i]);
-    if (rc != DMV_OK) return ct_member_error(rc, i);
-  }
-  CK(cudaSetDevice(handles[0]->device));
-  rc = ct_many_cluster(handles, n);
-  if (rc != DMV_OK) return rc;
-  const int nc = handles[0]->cluster_size;
-  cudaStream_t s = handles[0]->stream;
-  for (int i = 0; i < n; i++) {
-    dmv_ct* c = handles[i];
-    CK(c->h_tries.reserve(1));
-    if (n > 1) CK(c->h_pose.reserve((size_t)DMV_CT_MAX_TRIES * 12));
-    for (int l = 0; l < DMV_MAX_PYR_LEVELS; l++) B->T[i].staged[l] = c->staged[l];
-    B->maps[i] = *c->maps;
-    B->L[i].out = c->h_tries;
-    B->pose[i] = reinterpret_cast<const CTPose*>(c->h_pose.get());
-  }
-  rc = ct_many_order(handles, n);
-  if (rc != DMV_OK) return rc;
-  CTClusterLaunch q(nc, n, s);
-  if (n == 1) {   // one member: the single-handle kernel and its 4.8 KB parameter block, as dmv_ct_track_many launches ct_track_cluster_kernel
-    std::unique_ptr<CTTries> Q(new CTTries());
-    Q->T = B->T[0]; Q->maps = B->maps[0]; Q->L = B->L[0];
-    ct_fill_tries(&in[0], Q->pose);
-    CK(cudaLaunchKernelEx(&q.cfg, ct_track_tries_kernel, *Q));
-  } else {
-    // the try tables are read by the kernel from pinned memory: no previous call reads them any more (every call synchronises before it
-    // returns), and this one does not return before the kernel has finished
-    for (int i = 0; i < n; i++) ct_fill_tries(&in[i], reinterpret_cast<CTPose*>(handles[i]->h_pose.get()));
-    CK(cudaLaunchKernelEx(&q.cfg, ct_track_tries_many_kernel, *B));
-  }
-  for (int i = 0; i < n; i++) handles[i]->launches++;
-  CK(cudaStreamSynchronize(s));
-  for (int i = 0; i < n; i++) {
-    handles[i]->staging_busy = false;   // each member's uploads completed before the kernel started
-    out[i] = *handles[i]->h_tries;
-  }
-  return DMV_OK;
+  const int rc = ct_check_members(handles, n, DMV_CT_TRACK_MANY_MAX);
+  return rc != DMV_OK ? rc : ct_tries_run(handles, n, in, out, true);
 }
 
 // library-internal: the resident level-0 float4 plane of the coarse-tracker handle (dmv_ba_adopt_frame copies it device-to-device)
@@ -1295,10 +1260,11 @@ int dmv_ct_last_timing(dmv_ct* c, float ms[4]) {
   for (int i = 0; i < 4; i++) ms[i] = c->last_ms[i];
   return DMV_OK;
 }
-// instrumentation: reference points evaluated by the last dmv_ct_track, summed over its calcRes / calcGSSSE evaluations
+// instrumentation: reference points evaluated by the last dmv_ct_track, summed over its calcRes / calcGSSSE evaluations.  After a
+// dmv_ct_calc_res_gs it reads sum 26 of that call's 53, which share the pinned block.
 int dmv_ct_last_point_evaluations(dmv_ct* c, double* n) {
   if (!c || !n) return set_error(DMV_ERR_INVALID, "null argument");
-  *n = c->h_out[26];
+  *n = ct_track_out(c)->pevals;
   return DMV_OK;
 }
 int dmv_ct_kernel_launch_count(dmv_ct* c, long long* n) {

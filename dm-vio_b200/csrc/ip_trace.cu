@@ -591,10 +591,7 @@ static int ip_trace_run(dmv_ct* const* hs, int n, const dmv_ct_trace_job* jobs, 
       CK(cudaMemcpyAsync(c->d_ip, hb, sizeof(float) * (ipw::tables * cap + 14 * (size_t)j.nsets), cudaMemcpyHostToDevice, c->stream));
       A.m[i].img = c->d_img[0]; A.m[i].ip = c->d_ip; A.m[i].cap = c->ip_cap; A.m[i].w = c->w[0]; A.m[i].h = c->h[0]; A.m[i].n = np[i];
     }
-    if (i > 0) {   // the launch goes behind this member's queued work: its frame uploads (dmv_ct_upload_new_image does not synchronise) and the copy above
-      CK(cudaEventRecord(c->ev_order, c->stream));
-      CK(cudaStreamWaitEvent(s, c->ev_order, 0));
-    }
+    if (i > 0) CK(ct_order_behind(c, s));   // behind this member's frame uploads and the copy above
   }
   ip_trace_kernel<<<A.first[n] / 4, 128, 0, s>>>(A);   // 4 warps = 4 points per CTA
   for (int i = 0; i < n; i++)
@@ -636,15 +633,8 @@ int dmv_ct_trace_points_multi(dmv_ct* c, int nsets, const dmv_ip_points* sets, c
 // dmv_ct_trace_points_multi for n handles in one launch.  Every check precedes the first allocation, copy or launch.
 int dmv_ct_trace_many(dmv_ct* const* handles, int n, const dmv_ct_trace_job* jobs, const dmv_ip_settings* settings) {
   if (!handles || !jobs) return set_error(DMV_ERR_INVALID, "null argument");
-  if (n < 1 || n > DMV_CT_TRACE_MANY_MAX) return set_error(DMV_ERR_INVALID, "n = %d: expected 1 to %d handles", n, DMV_CT_TRACE_MANY_MAX);
-  for (int i = 0; i < n; i++) {
-    if (!handles[i]) return set_error(DMV_ERR_INVALID, "handles[%d] is NULL", i);
-    for (int j = 0; j < i; j++)
-      if (handles[j] == handles[i]) return set_error(DMV_ERR_INVALID, "handles[%d] and handles[%d] are the same handle", j, i);
-    if (handles[i]->device != handles[0]->device)
-      return set_error(DMV_ERR_INVALID, "handles[%d] is on device %d, handles[0] on device %d: one launch runs on one device", i, handles[i]->device,
-                       handles[0]->device);
-  }
+  const int rc = ct_check_members(handles, n, DMV_CT_TRACE_MANY_MAX);
+  if (rc != DMV_OK) return rc;
   return ip_trace_run(handles, n, jobs, settings, true);
 }
 

@@ -15,8 +15,9 @@ Every round ends in a synchronisation (each call returns after one).  The arms a
 ctypes argument blocks are built once.  Reported per arm: median / p10 / p90 wall time per round and tracked frames/s.  Outside the timed
 loops the three arms must return bit-identical results and point evaluations, or the run exits non-zero.
 --parent-lib PATH adds an A/B between this library and another build of it, e.g. the parent commit's, loaded side by side and alternated
-call by call: dmv_ct_track (try 0 of the easy workload), dmv_ct_track_many (B = 4, the same) and dmv_ct_track_tries (easy); their results
-must be bit-identical too.  The card's name, power limit and maximum SM clock are read in the same run (read-only nvidia-smi query).
+call by call: dmv_ct_track (try 0 of the easy workload), dmv_ct_track_many (B = 4, the same), dmv_ct_track_tries (easy) and
+dmv_ct_track_tries_many (B = 4, easy); their results must be bit-identical too.  The card's name, power limit and maximum SM clock are read
+in the same run (read-only nvidia-smi query).
 Prints one JSON line and writes it to --out.
     python tools/bench_track_tries_many.py [--warmup 30] [--reps 300] [--parent-lib PATH] [--out records/h100_track_tries_many.json]"""
 import argparse
@@ -132,21 +133,26 @@ def one_workload(capi, L, gs, jobs, B, warmup, reps, what):
 
 
 def parent_ab(capi, synth, orc, path, warmup, reps):
-    """dmv_ct_track, dmv_ct_track_many (B = 4) and dmv_ct_track_tries on the easy workload through this library and through `path`,
-    alternated call by call"""
+    """dmv_ct_track, dmv_ct_track_many (B = 4), dmv_ct_track_tries and dmv_ct_track_tries_many (B = 4) on the easy workload through this
+    library and through `path`, alternated call by call"""
     libs = K.this_and_parent(path)
     res, identical = dict(parent_lib=os.path.basename(path)), True
     made = {k: [make_handle(capi, synth, orc, i, L=L) for i in range(4)] for k, L in libs.items()}
     sc = made["this"][0][1]
     Rs, ts, kw, Lc = easy(sc)
     A1 = capi._track_args(LEVELS, Rs[0], ts[0], **kw)
-    A4 = (capi.CTTrackArgs * 4)(*[capi._track_args(LEVELS, R[0], t[0], **kw) for R, t, _, _ in (easy(s) for _, s in made["this"])])
+    easies = [easy(s) for _, s in made["this"]]
+    A4 = (capi.CTTrackArgs * 4)(*[capi._track_args(LEVELS, R[0], t[0], **kw) for R, t, _, _ in easies])
     At, keep = capi._tries_args(LEVELS, Rs, ts, lastCoarseRMSE0=Lc, **kw)
+    made4 = [capi._tries_args(LEVELS, R, t, lastCoarseRMSE0=L_, **k) for R, t, k, L_ in easies]
+    At4 = (capi.CTTriesArgs * 4)(*[m[0] for m in made4])
     hs = {k: (C.c_void_p * 4)(*[g.h.value for g, _ in made[k]]) for k in libs}
-    outs = {k: dict(track=capi.CTTrackResult(), many=(capi.CTTrackResult * 4)(), tries=capi.CTTriesResult()) for k in libs}
+    outs = {k: dict(track=capi.CTTrackResult(), many=(capi.CTTrackResult * 4)(), tries=capi.CTTriesResult(), tries_many=(capi.CTTriesResult * 4)())
+            for k in libs}
     calls = dict(track=lambda k: libs[k].dmv_ct_track(hs[k][0], C.byref(A1), C.byref(outs[k]["track"])),
                  many=lambda k: libs[k].dmv_ct_track_many(hs[k], 4, A4, outs[k]["many"]),
-                 tries=lambda k: libs[k].dmv_ct_track_tries(hs[k][0], C.byref(At), C.byref(outs[k]["tries"])))
+                 tries=lambda k: libs[k].dmv_ct_track_tries(hs[k][0], C.byref(At), C.byref(outs[k]["tries"])),
+                 tries_many=lambda k: libs[k].dmv_ct_track_tries_many(hs[k], 4, At4, outs[k]["tries_many"]))
     for name, call in calls.items():
         arms = {k: (lambda k=k, call=call: call(k)) for k in libs}
         t = K.alternate(arms, warmup, reps, f"{name} A/B", libs)
