@@ -70,6 +70,11 @@ class TraceJob(C.Structure):
     _fields_ = [("nsets", C.c_int), ("sets", vp), ("tables14", vp)]
 
 
+class TraceStoreJob(C.Structure):
+    """dmv_ct_trace_store_job: one handle's arguments of dmv_ct_trace_store_many"""
+    _fields_ = [("store", vp), ("nslots", C.c_int), ("tables14", vp)]
+
+
 class IPSettings(C.Structure):
     """dmv_ip_settings (include/dmvio_b200.h); ip_default_settings() fills it as dmv_ip_default_settings does"""
     _fields_ = [(k, C.c_float) for k in ("maxPixSearch", "trace_stepsize", "trace_GNThreshold", "trace_extraSlackOnTH", "trace_slackInterval",
@@ -195,7 +200,7 @@ SYMBOLS = [
     "dmv_ba_batch_create", "dmv_ba_batch_destroy", "dmv_ba_batch_gn_step", "dmv_ba_batch_set_timing", "dmv_ba_batch_last_kernel_ms", "dmv_ba_batch_bench",
     "dmv_ct_create", "dmv_ct_destroy", "dmv_ct_set_K", "dmv_ct_set_ref", "dmv_ct_make_coarse_depth", "dmv_ct_set_ref_from_ba", "dmv_ct_get_ref", "dmv_ct_upload_new", "dmv_ct_upload_new_image", "dmv_ct_set_huber",
     "dmv_ci_create", "dmv_ci_destroy", "dmv_ci_set_K", "dmv_ci_upload_first", "dmv_ci_upload_new", "dmv_ci_set_points", "dmv_ci_calc_res_and_gs", "dmv_ci_kernel_launch_count",
-    "dmv_ct_calc_res_gs", "dmv_ct_track", "dmv_ct_track_many", "dmv_ct_track_tries", "dmv_ct_track_tries_many", "dmv_ip_default_settings", "dmv_ct_init_points", "dmv_ct_trace_points", "dmv_ct_trace_points_multi", "dmv_ct_trace_many", "dmv_ct_set_timing", "dmv_ct_last_timing", "dmv_ct_kernel_launch_count", "dmv_ct_last_point_evaluations",
+    "dmv_ct_calc_res_gs", "dmv_ct_track", "dmv_ct_track_many", "dmv_ct_track_tries", "dmv_ct_track_tries_many", "dmv_ip_default_settings", "dmv_ct_init_points", "dmv_ct_trace_points", "dmv_ct_trace_points_multi", "dmv_ct_trace_many", "dmv_ip_store_create", "dmv_ip_store_destroy", "dmv_ip_store_put", "dmv_ip_store_get", "dmv_ip_store_remove", "dmv_ct_trace_store", "dmv_ct_trace_store_many", "dmv_ct_set_timing", "dmv_ct_last_timing", "dmv_ct_kernel_launch_count", "dmv_ct_last_point_evaluations",
     "dmv_ct_set_undistort", "dmv_ct_upload_raw_image", "dmv_ct_download_frame", "dmv_ps_default_settings", "dmv_ct_make_new_traces",
 ]
 
@@ -298,6 +303,13 @@ _ARGTYPES = {
     "dmv_ct_trace_points": [vp, C.POINTER(IPPoints), f32p, f32p, f32p, vp],
     "dmv_ct_trace_points_multi": [vp, C.c_int, vp, vp, vp],
     "dmv_ct_trace_many": [C.POINTER(vp), C.c_int, C.POINTER(TraceJob), vp],
+    "dmv_ip_store_create": [C.c_int, C.POINTER(vp)],
+    "dmv_ip_store_destroy": [vp],
+    "dmv_ip_store_put": [vp, C.c_int, C.POINTER(IPPoints)],
+    "dmv_ip_store_get": [vp, C.c_int, C.POINTER(IPPoints)],
+    "dmv_ip_store_remove": [vp, C.c_int, C.c_int, vp, vp],
+    "dmv_ct_trace_store": [vp, vp, C.c_int, vp, vp],
+    "dmv_ct_trace_store_many": [C.POINTER(vp), C.c_int, C.POINTER(TraceStoreJob), vp],
     "dmv_ct_set_timing": [vp, C.c_int],
     "dmv_ct_last_timing": [vp, f32p],
     "dmv_ct_kernel_launch_count": [vp, C.POINTER(C.c_longlong)],
@@ -706,6 +718,88 @@ def ct_trace_many(handles, jobs, settings=None):
     return [t.results() for t in T]
 
 
+def _tables14(tables):
+    """the tables14 array of a store trace: an (nslots, 14) array as it is, or one row per slot from (KRKi, Kt, aff), None for a slot
+    without points (zeros)"""
+    if isinstance(tables, np.ndarray):
+        return np.ascontiguousarray(tables, np.float32).reshape(-1, 14)
+    tab = np.zeros((len(tables), 14), np.float32)
+    for k, t in enumerate(tables):
+        if t is not None:
+            KRKi, Kt, aff = t
+            tab[k, :9] = np.asarray(KRKi, np.float32).reshape(-1); tab[k, 9:12] = Kt; tab[k, 12:14] = aff
+    return tab
+
+
+IP_OUT_KEYS = ("idepth_min", "idepth_max", "quality", "status", "lastTraceUV", "lastTracePixelInterval")
+
+
+class IPStore:
+    """a dmv_ip_store: the immature points of up to 64 host keyframes (slot k = one keyframe's list) kept on one device between frames.
+    counts mirrors the store's points per slot.  L: the library, as CT takes it."""
+
+    SLOTS = 64
+
+    def __init__(self, device=0, L=None):
+        self.L = L or lib()
+        self.h = vp()
+        check(self.L.dmv_ip_store_create(device, C.byref(self.h)), self.L)
+        self.counts = [0] * self.SLOTS
+
+    def _check(self, rc):
+        check(rc, self.L)
+
+    def close(self):
+        if self.h:
+            self.L.dmv_ip_store_destroy(self.h)
+            self.h = vp()
+
+    def __del__(self):
+        try:
+            self.close()
+        except Exception:
+            pass
+
+    def put(self, slot, P):
+        """the slot's points become P (a dict of arrays as oracle.orc.ip_init returns, in/out fields included); an empty P empties it"""
+        T = _TraceSets([(P, np.zeros(9), np.zeros(3), np.zeros(2))])
+        self._check(self.L.dmv_ip_store_put(self.h, slot, C.byref(T.arr[0])))
+        self.counts[slot] = len(P["u"])
+
+    def get(self, slot, P=None):
+        """the slot's in/out fields (IP_OUT_KEYS): a dict of them, or dict(P) updated with them"""
+        n = self.counts[slot]
+        out = {"idepth_min": np.zeros(n, np.float32), "idepth_max": np.zeros(n, np.float32), "quality": np.zeros(n, np.float32),
+               "status": np.zeros(n, np.int32), "lastTraceUV": np.zeros((n, 2), np.float32), "lastTracePixelInterval": np.zeros(n, np.float32)}
+        pts = IPPoints(n, *([None] * 6), *[out[k].ctypes.data for k in IP_OUT_KEYS])
+        self._check(self.L.dmv_ip_store_get(self.h, slot, C.byref(pts)))
+        Q = dict(P) if P is not None else {}
+        Q.update(out)
+        return Q
+
+    def remove(self, slot, idx):
+        """activatePointsMT's removal of the slot's points idx (FullSystem.cpp:L761-769); returns each survivor's index before the call, in
+        the slot's new order"""
+        idx = np.ascontiguousarray(idx, np.int32)
+        order = np.zeros(max(self.counts[slot] - len(idx), 0), np.int32)
+        self._check(self.L.dmv_ip_store_remove(self.h, slot, len(idx), idx.ctypes.data if len(idx) else None, order.ctypes.data))
+        self.counts[slot] -= len(idx)
+        return order
+
+
+def trace_store_many(handles, jobs, settings=None):
+    """dmv_ct_trace_store_many: jobs[i] = (store, tables) (an IPStore, and tables as CT.trace_store takes them, nslots = len(tables)) traced
+    against handles[i]'s frame, all in one launch"""
+    if len(handles) != len(jobs):
+        raise ValueError(f"{len(handles)} handles but {len(jobs)} jobs")
+    n = len(handles)
+    L = handles[0].L if handles else lib()
+    tabs = [_tables14(t) for _, t in jobs]
+    H = (vp * max(n, 1))(*[g.h.value for g in handles])
+    J = (TraceStoreJob * max(n, 1))(*[TraceStoreJob(st.h.value, len(tb), tb.ctypes.data if len(tb) else None) for (st, _), tb in zip(jobs, tabs)])
+    check(L.dmv_ct_trace_store_many(H, n, J, None if settings is None else C.byref(settings)), L)
+
+
 class CT:
     """a dmv_ct handle.  L: the library it lives in, lib() by default or another build from load()"""
 
@@ -884,6 +978,12 @@ class CT:
         T = _TraceSets(sets)
         self._check(self.L.dmv_ct_trace_points_multi(self.h, T.job.nsets, T.job.sets, T.job.tables14, None if settings is None else C.byref(settings)))
         return T.results()
+
+    def trace_store(self, store, tables, settings=None):
+        """dmv_ct_trace_store: the points of store (an IPStore) traced against the resident newest frame, slot k with tables[k] (an
+        (nslots, 14) array, or (KRKi, Kt, aff) per slot with None for an empty slot; nslots = len(tables))"""
+        tab = _tables14(tables)
+        self._check(self.L.dmv_ct_trace_store(self.h, store.h, len(tab), tab.ctypes.data if len(tab) else None, None if settings is None else C.byref(settings)))
 
     def set_timing(self, enable=True):
         self._check(self.L.dmv_ct_set_timing(self.h, int(enable)))

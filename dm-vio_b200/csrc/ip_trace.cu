@@ -37,31 +37,7 @@ __device__ __forceinline__ void ip_interp33(const float4* __restrict__ mat, floa
   out[2] = dxdy * br.z + (dy - dxdy) * bl.z + (dx - dxdy) * tr.z + (1 - dx - dy + dxdy) * tl.z;
 }
 
-// The tracing staging area d_ip of one handle: ip_cap points per array, the array of word w at d_ip + w * ip_cap (uv and the 8 / 4 per-point
-// vectors interleaved per point), then 14 floats per host frame (KRKi 9 | Kt 3 | aff 2).  The host staging and ip_trace_kernel both read
-// these offsets.  set is the host frame of each point (an int), status an int too.
-namespace ipw {
-constexpr int u = 0, v = 1, color = 2, weights = 10, gradH = 18, energyTH = 22;          // read only
-constexpr int idepth_min = 23, idepth_max = 24, quality = 25, status = 26, uv = 27, interval = 29;   // in/out: the 7 words from idepth_min on
-constexpr int set = 30, tables = 31;
-constexpr int inout = 7;
-}  // namespace ipw
-
-// One member of a trace launch: a coarse-tracker handle's resident level-0 plane and its staging area
-struct IPTraceMember {
-  const float4* img;
-  float* ip;          // d_ip (ipw layout)
-  int cap, w, h;
-  int n;              // points
-};
-struct IPTraceArgs {
-  int n;                                     // members
-  int first[DMV_CT_TRACE_MANY_MAX + 1];      // member k's points are the warps first[k] .. first[k] + m[k].n - 1; first[k] % 4 == 0
-  dmv_ip_settings s;
-  IPTraceMember m[DMV_CT_TRACE_MANY_MAX];
-};
-static_assert(sizeof(IPTraceArgs) == 624, "ip_trace_kernel's parameter block");
-
+// The point arrays (ipw layout), IPTraceMember and IPTraceArgs are declared in ip_trace.h.
 // One WARP per immature point.  The reference walks the epipolar segment step by step (<= 99 positions x 8 bilinear samples) and keeps the
 // best and second-best energies; here the positions are dealt to the 32 lanes (lane L takes steps L, L+32, L+64, L+96: at most 4 rounds
 // instead of 99), the winner is a warp arg-min with the sequential scan's tie rule (lowest step index), the 8 pattern samples of a
@@ -487,6 +463,27 @@ __global__ void __launch_bounds__(128) ip_activate_kernel(const __grid_constant_
 
 void launch_ip_init(const IPInitArgs& A, cudaStream_t s) { ip_init_kernel<<<(A.n + 127) / 128, 128, 0, s>>>(A); }
 
+void ip_trace_args(IPTraceArgs& A, int n, const dmv_ip_settings* settings) {
+  std::memset(&A, 0, sizeof(A));
+  A.n = n;
+  if (settings) A.s = *settings; else dmv_ip_default_settings(&A.s);
+}
+
+void ip_trace_member(IPTraceArgs& A, int i, const dmv_ct* c, float* ip, int cap, int np) {
+  A.first[i + 1] = A.first[i] + (np + 3) / 4 * 4;   // whole CTAs per member
+  if (np > 0) { A.m[i].img = c->d_img[0]; A.m[i].ip = ip; A.m[i].cap = cap; A.m[i].w = c->w[0]; A.m[i].h = c->h[0]; A.m[i].n = np; }
+}
+
+int ip_trace_launch(dmv_ct* const* hs, const IPTraceArgs& A) {
+  const cudaStream_t s = hs[0]->stream;
+  for (int i = 1; i < A.n; i++) CK(ct_order_behind(hs[i], s));   // behind each member's frame uploads and the copies its caller queued there
+  ip_trace_kernel<<<A.first[A.n] / 4, 128, 0, s>>>(A);   // 4 warps = 4 points per CTA
+  for (int i = 0; i < A.n; i++)
+    if (A.m[i].n > 0) hs[i]->launches++;
+  CK(cudaGetLastError());
+  return DMV_OK;
+}
+
 }  // namespace dmv
 
 using namespace dmv;
@@ -561,14 +558,12 @@ static int ip_trace_run(dmv_ct* const* hs, int n, const dmv_ct_trace_job* jobs, 
   for (int i = 0; i < n; i++)
     if (np[i] > 0) CK(ct_reserve_ip(hs[i], np[i]));
   IPTraceArgs A;
-  std::memset(&A, 0, sizeof(A));
-  A.n = n;
-  if (settings) A.s = *settings; else dmv_ip_default_settings(&A.s);
+  ip_trace_args(A, n, settings);
   const cudaStream_t s = hs[0]->stream;
   for (int i = 0; i < n; i++) {
     dmv_ct* c = hs[i];
     const dmv_ct_trace_job& j = jobs[i];
-    A.first[i + 1] = A.first[i] + (np[i] + 3) / 4 * 4;   // whole CTAs per member
+    ip_trace_member(A, i, c, c->d_ip, c->ip_cap, np[i]);
     if (np[i] > 0) {
       const size_t cap = c->ip_cap;
       float* hb = c->h_ip;
@@ -589,14 +584,10 @@ static int ip_trace_run(dmv_ct* const* hs, int n, const dmv_ct_trace_job* jobs, 
       }
       std::memcpy(hb + ipw::tables * cap, j.tables14, sizeof(float) * 14 * (size_t)j.nsets);
       CK(cudaMemcpyAsync(c->d_ip, hb, sizeof(float) * (ipw::tables * cap + 14 * (size_t)j.nsets), cudaMemcpyHostToDevice, c->stream));
-      A.m[i].img = c->d_img[0]; A.m[i].ip = c->d_ip; A.m[i].cap = c->ip_cap; A.m[i].w = c->w[0]; A.m[i].h = c->h[0]; A.m[i].n = np[i];
     }
-    if (i > 0) CK(ct_order_behind(c, s));   // behind this member's frame uploads and the copy above
   }
-  ip_trace_kernel<<<A.first[n] / 4, 128, 0, s>>>(A);   // 4 warps = 4 points per CTA
-  for (int i = 0; i < n; i++)
-    if (np[i] > 0) hs[i]->launches++;
-  CK(cudaGetLastError());
+  const int rc = ip_trace_launch(hs, A);
+  if (rc != DMV_OK) return rc;
   for (int i = 0; i < n; i++) {   // the 7 in/out words per point
     if (np[i] == 0) continue;
     const size_t cap = hs[i]->ip_cap;

@@ -536,6 +536,46 @@ typedef struct dmv_ct_trace_job {
 } dmv_ct_trace_job;
 int dmv_ct_trace_many(dmv_ct* const* handles, int n, const dmv_ct_trace_job* jobs, const dmv_ip_settings* settings);
 
+/* Immature-point store: a window's immature points kept on one device between frames, so that traceNewCoarse after every tracked frame
+ * uploads only the 14-float tables of each host keyframe and downloads nothing.  Slot k holds the points hosted by one keyframe
+ * (FrameHessian::immaturePoints), in that list's order.  A store belongs to no tracker handle: it can be traced against either of
+ * FullSystem's two coarse trackers, which swap roles at every keyframe.
+ * Results: any sequence of dmv_ct_trace_store calls between a put and a get leaves the slot's in/out fields bit-identical to the same
+ * sequence of dmv_ct_trace_points_multi calls on host arrays with sets[k] = slot k, the same tables and the same frames.
+ * Every call checks all its arguments before any allocation, copy or launch (a refused call leaves the store unchanged) and returns after
+ * one synchronisation.  The caller serialises the calls on one store (the reference holds mapMutex over traceNewCoarse and activatePointsMT).
+ * Device memory: 31 words per point in two buffers, grown on demand with their contents kept. */
+typedef struct dmv_ip_store dmv_ip_store;
+#define DMV_IP_STORE_SLOTS 64        /* = the per-call limit of host frames of dmv_ct_trace_points_multi */
+int dmv_ip_store_create(int device, dmv_ip_store** out);
+int dmv_ip_store_destroy(dmv_ip_store* s);
+/* replaces the slot's points by pts (every field, read-only and in/out); pts->n == 0 empties the slot */
+int dmv_ip_store_put(dmv_ip_store* s, int slot, const dmv_ip_points* pts);
+/* downloads the 7 in/out words of the slot's points (idepth_min, idepth_max, quality, lastTraceStatus, lastTraceUV2, lastTracePixelInterval);
+ * the read-only pointers of pts are not used.  pts->n must equal the slot's count (the error message gives it). */
+int dmv_ip_store_get(dmv_ip_store* s, int slot, dmv_ip_points* pts);
+/* removes the slot's points idx[0..n) (indices into the slot's current order, distinct) with activatePointsMT's swap-with-back loop
+ * (FullSystem.cpp:L761-769): the slot's order afterwards is the host's immaturePoints order after that loop.  order_out (optional, one
+ * entry per survivor) = each survivor's index before the call, so the caller can reorder its own copies of the read-only fields. */
+int dmv_ip_store_remove(dmv_ip_store* s, int slot, int n, const int32_t* idx, int32_t* order_out);
+/* traceNewCoarse over the store: the points of slot k traced with tables14[14k .. 14k + 14) (KRKi 9 | Kt 3 | aff 2, as
+ * dmv_ct_trace_points_multi) against ct's resident level-0 frame.  Slots at or above nslots must be empty; tables14 may be NULL when no
+ * slot below nslots holds a point.  One launch on ct's stream (launch count +1) when a point is present, none otherwise; ct's own
+ * staging area (dmv_ct_trace_points_multi's) is not used.  Errors: DMV_ERR_INVALID for a NULL ct / s, nslots outside
+ * 0..DMV_IP_STORE_SLOTS, a point in a slot at or above nslots, a NULL tables14 with points present, or a store on another device than ct. */
+int dmv_ct_trace_store(dmv_ct* ct, dmv_ip_store* s, int nslots, const float* tables14, const dmv_ip_settings* settings);
+/* dmv_ct_trace_store for n handles in ONE launch: member i traces jobs[i].store against handles[i]'s frame, bit-identical to
+ * dmv_ct_trace_store(handles[i], jobs[i].store, jobs[i].nslots, jobs[i].tables14, settings).  Membership, launch counts and ordering as
+ * dmv_ct_trace_many: the launch goes on handles[0]'s stream behind the work queued on every member's stream.  Errors, all before anything
+ * is allocated, copied or launched: those of dmv_ct_trace_many's member list, a NULL handles / jobs, a store passed twice, and each member's
+ * dmv_ct_trace_store errors prefixed "handles[i]: ". */
+typedef struct dmv_ct_trace_store_job {
+  dmv_ip_store* store;
+  int nslots;
+  const float* tables14;       /* nslots * 14 */
+} dmv_ct_trace_store_job;
+int dmv_ct_trace_store_many(dmv_ct* const* handles, int n, const dmv_ct_trace_store_job* jobs, const dmv_ip_settings* settings);
+
 /* ------------------------------------------------------------------------------------------------
  * New immature points of a keyframe  ==  FullSystem::makeNewTraces (FullSystem.cpp:L1640-1667): PixelSelector::makeMaps
  * (FullSystem/PixelSelector2.cpp:L158-307) on the handle's RESIDENT frame (the one last given to dmv_ct_upload_new_image /
