@@ -55,6 +55,13 @@ class BASelectArgs(C.Structure):
                [("currentMinActDist", C.c_float), ("minTraceQuality", C.c_float), ("cap", C.c_int)] + [(k, vp) for k in ("n_opt", "action", "opt_idx", "map", "stats")]
 
 
+class BAActivateStoreArgs(C.Structure):
+    _fields_ = [("nf", C.c_int), ("newest", C.c_int), ("tables12", vp), ("flagged", vp), ("n_active", C.c_int)] + \
+               [(k, vp) for k in ("act_u", "act_v", "act_idepth_scaled", "act_host", "slot", "my_type")] + \
+               [("currentMinActDist", C.c_float), ("minTraceQuality", C.c_float), ("RT", vp), ("minObs", C.c_int), ("cap", C.c_int)] + \
+               [(k, vp) for k in ("n_opt", "opt_frame", "opt_index", "status", "idepth", "res_state", "order_out", "n_kept", "action", "map", "stats")]
+
+
 class BAMargArgs(C.Structure):
     _fields_ = [("n", C.c_int32), ("point", C.c_void_p), ("adHTdeltaF", C.c_void_p), ("cDeltaF", C.c_float * 4), ("idepthFixPriorMargFac", C.c_float)] + \
                [(k, C.c_void_p) for k in ("M", "Mb", "Msc", "Mbsc", "resInM", "ngoodRes", "res_toZeroF", "isLinearized")]
@@ -196,7 +203,7 @@ SYMBOLS = [
     "dmv_ba_set_window", "dmv_ba_set_points", "dmv_ba_set_residuals", "dmv_ba_set_adjoints", "dmv_ba_set_state", "dmv_ba_linearize",
     "dmv_ba_get_residual_outputs", "dmv_ba_get_target_energies", "dmv_ba_apply_res", "dmv_ba_accumulate", "dmv_ba_get_point_outputs", "dmv_ba_get_solve_HdiF",
     "dmv_ba_resubstitute", "dmv_ba_backup_points", "dmv_ba_restore_points", "dmv_ba_get_idepth", "dmv_ba_gn_step", "dmv_nccl_unique_id",
-    "dmv_ba_comm_init", "dmv_ba_activate_points", "dmv_ba_select_activation", "dmv_ba_marginalize_points", "dmv_ba_drop_residuals", "dmv_ba_reset_oob", "dmv_ba_p2p_export", "dmv_ba_p2p_import", "dmv_ba_last_timing", "dmv_ba_bench_device", "dmv_ba_bench_phases", "dmv_ba_kernel_launch_count", "dmv_ba_io_bytes", "dmv_ba_set_timing", "dmv_ba_bench_e2e",
+    "dmv_ba_comm_init", "dmv_ba_activate_points", "dmv_ba_select_activation", "dmv_ba_activate_store", "dmv_ba_marginalize_points", "dmv_ba_drop_residuals", "dmv_ba_reset_oob", "dmv_ba_p2p_export", "dmv_ba_p2p_import", "dmv_ba_last_timing", "dmv_ba_bench_device", "dmv_ba_bench_phases", "dmv_ba_kernel_launch_count", "dmv_ba_io_bytes", "dmv_ba_set_timing", "dmv_ba_bench_e2e",
     "dmv_ba_batch_create", "dmv_ba_batch_destroy", "dmv_ba_batch_gn_step", "dmv_ba_batch_set_timing", "dmv_ba_batch_last_kernel_ms", "dmv_ba_batch_bench",
     "dmv_ct_create", "dmv_ct_destroy", "dmv_ct_set_K", "dmv_ct_set_ref", "dmv_ct_make_coarse_depth", "dmv_ct_set_ref_from_ba", "dmv_ct_get_ref", "dmv_ct_upload_new", "dmv_ct_upload_new_image", "dmv_ct_set_huber",
     "dmv_ci_create", "dmv_ci_destroy", "dmv_ci_set_K", "dmv_ci_upload_first", "dmv_ci_upload_new", "dmv_ci_set_points", "dmv_ci_calc_res_and_gs", "dmv_ci_kernel_launch_count",
@@ -264,6 +271,7 @@ _ARGTYPES = {
     "dmv_ba_comm_init": [vp, C.c_int, C.c_int, vp],
     "dmv_ba_activate_points": [vp, C.POINTER(BAActivateArgs)],
     "dmv_ba_select_activation": [vp, C.POINTER(BASelectArgs)],
+    "dmv_ba_activate_store": [vp, vp, C.POINTER(BAActivateStoreArgs)],
     "dmv_ba_marginalize_points": [vp, C.POINTER(BAMargArgs)],
     "dmv_ba_drop_residuals": [vp, C.c_int, i32p],
     "dmv_ba_reset_oob": [vp],
@@ -554,6 +562,42 @@ class BA:
         if rc != 0:
             raise DmvError(f"dmvio_b200 error {rc}: {lib().dmv_last_error().decode()}", n_opt.value)
         return action[:n], opt[:n_opt.value].copy(), m, dict(undecided=int(stats[0]), floods=int(stats[1]), rounds=int(stats[2]))
+
+    def activate_store(self, store, newest, tables12, flagged, act_u, act_v, act_idepth_scaled, act_host, slot, my_type, min_act_dist, RT,
+                       min_trace_quality=3.0, minObs=1, cap=None, want_map=False):
+        """FullSystem::activatePointsMT on the immature points of an IPStore (dmv_ba_activate_store): frame f's points are slot slot[f]
+        (-1: none), my_type[f] their types (None for a frame without points).  Updates store.counts.  Returns a dict: opt_frame,
+        opt_index (toOptimize as (frame, index in its slot before the call)), status, idepth, res_state (n_opt, nf), order (one segment
+        per frame), n_kept [nf], action, map ((h/2, w/2) or None), stats (undecided, floods, rounds).  On cap overflow DmvError carries
+        the count needed."""
+        nf = self.nf
+        slot = _c(slot, np.int32)
+        counts = [store.counts[k] if k >= 0 else 0 for k in slot]
+        n = int(sum(counts))
+        types = [None if t is None else _c(t, np.float32) for t in my_type]
+        tptr = (vp * max(nf, 1))(*[None if t is None else t.ctypes.data for t in types])
+        keep = [_c(tables12, np.float32), _c(flagged, np.uint8), _c(act_u, np.float32), _c(act_v, np.float32), _c(act_idepth_scaled, np.float32),
+                _c(act_host, np.int32), _c(RT, np.float32)]
+        cap = n if cap is None else int(cap)
+        ofr, oix, st, idp = (np.zeros(max(cap, 1), t) for t in (np.int32, np.int32, np.int32, np.float32))
+        rs = np.zeros((max(cap, 1), nf), np.int32)
+        order, n_kept, action = np.zeros(max(n, 1), np.int32), np.zeros(nf, np.int32), np.zeros(max(n, 1), np.int32)
+        m = np.zeros((self.hh // 2, self.w // 2), np.float32) if want_map else None
+        n_opt, stats = C.c_int(0), np.zeros(3, np.int32)
+        a = BAActivateStoreArgs(nf, int(newest), keep[0].ctypes.data, keep[1].ctypes.data, len(keep[2]), *[k.ctypes.data for k in keep[2:6]],
+                                slot.ctypes.data, C.cast(tptr, vp), float(min_act_dist), float(min_trace_quality), keep[6].ctypes.data, int(minObs), cap,
+                                C.addressof(n_opt), *[x.ctypes.data for x in (ofr, oix, st, idp, rs, order, n_kept, action)],
+                                m.ctypes.data if want_map else None, stats.ctypes.data)
+        rc = self.L.dmv_ba_activate_store(self.h, store.h, C.byref(a))
+        if rc != 0:
+            raise DmvError(f"dmvio_b200 error {rc}: {lib().dmv_last_error().decode()}", n_opt.value)
+        for k, kept in zip(slot, n_kept):
+            if k >= 0:
+                store.counts[k] = int(kept)
+        k = n_opt.value
+        return dict(opt_frame=ofr[:k].copy(), opt_index=oix[:k].copy(), status=st[:k].copy(), idepth=idp[:k].copy(), res_state=rs[:k].copy(),
+                    order=order[:int(n_kept.sum())].copy(), n_kept=n_kept, action=action[:n].copy(), map=m,
+                    stats=dict(undecided=int(stats[0]), floods=int(stats[1]), rounds=int(stats[2])))
 
     def reset_oob(self):
         check(self.L.dmv_ba_reset_oob(self.h))

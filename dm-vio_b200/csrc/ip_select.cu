@@ -41,6 +41,8 @@
 #include "../../include/dmvio_b200.h"
 #include "ba_handle.h"
 #include "common_host.h"
+#include "ip_store.h"
+#include "ip_trace.h"
 #include <algorithm>
 #include <climits>
 #include <cstring>
@@ -327,13 +329,43 @@ __global__ void __launch_bounds__(SEL_T) sel_chain_kernel(const SelArgs A) {
   if (tid == 0) { A.counters[0] = s_total; A.counters[1] = s_fid; A.counters[2] = rounds; }
 }
 
+// Staging layout (4-byte words): tab 96 | flagged 8 | off 9 (header 128) | active u v idepth host | immature u v idmin idmax status interval
+// quality type | action | opt | counters 8 | map | cell | frac | rad | stamp.  [0, act) goes up, [act, map (+ ncell)) comes back.
+struct SelLayout {
+  size_t au, av, aid, ah, iu, iv, imin, imax, ist, iint, iq, ity, act, opt, cnt, map, cell, frac, rad, stamp, words;
+  SelLayout(size_t n, size_t na, size_t ncell) {
+    au = 128; av = au + na; aid = av + na; ah = aid + na; iu = ah + na; iv = iu + n; imin = iv + n; imax = imin + n; ist = imax + n; iint = ist + n;
+    iq = iint + n; ity = iq + n; act = ity + n; opt = act + n; cnt = opt + n; map = cnt + 8; cell = map + ncell; frac = cell + n; rad = frac + n;
+    stamp = rad + n; words = stamp + ncell;
+  }
+};
+
+// The selection's immature-point rows fed from a store: row i of group f = row src[f] + i - off[f] of the store's buffer (capacity scap).
+// Copies the 7 words the selection reads from the store (u, v, idepth_min, idepth_max, status, interval, quality) into the staging arrays.
+struct SelGatherArgs {
+  int n, nf, scap;
+  int off[MAXF + 1], src[MAXF];
+  const unsigned* pts;
+  unsigned* dst;      // the staging's u (the 7 arrays follow it at stride n)
+};
+__global__ void __launch_bounds__(128) sel_gather_kernel(const __grid_constant__ SelGatherArgs G) {
+  const int i = blockIdx.x * blockDim.x + threadIdx.x;
+  if (i >= G.n) return;
+  int f = 0;
+  while (G.off[f + 1] <= i) f++;
+  const size_t r = G.src[f] + (i - G.off[f]), cap = G.scap, n = G.n;
+  G.dst[i] = G.pts[ipw::u * cap + r];
+  G.dst[n + i] = G.pts[ipw::v * cap + r];
+  G.dst[2 * n + i] = G.pts[ipw::idepth_min * cap + r];
+  G.dst[3 * n + i] = G.pts[ipw::idepth_max * cap + r];
+  G.dst[4 * n + i] = G.pts[ipw::status * cap + r];
+  G.dst[5 * n + i] = G.pts[ipw::interval * cap + r];
+  G.dst[6 * n + i] = G.pts[ipw::quality * cap + r];
+}
+
 }  // namespace
-}  // namespace dmv
 
-using namespace dmv;
-
-extern "C" int dmv_ba_select_activation(dmv_ba* b, const dmv_ba_select_args* a) {
-  if (!b || !a) return set_error(DMV_ERR_INVALID, "null argument");
+int sel_check(const dmv_ba* b, const dmv_ba_select_args* a, bool from_store) {
   const int nf = a->nf;
   if (nf < 1 || nf > DMV_MAX_FRAMES || a->newest < 0 || a->newest >= nf) return set_error(DMV_ERR_INVALID, "nf %d / newest %d out of range", nf, a->newest);
   if (!a->tables12 || !a->flagged || !a->imm_offset || !a->n_opt || a->n_active < 0 || a->cap < 0)
@@ -343,52 +375,54 @@ extern "C" int dmv_ba_select_activation(dmv_ba* b, const dmv_ba_select_args* a) 
   for (int f = 0; f < nf; f++)
     if (a->imm_offset[f + 1] < a->imm_offset[f]) return set_error(DMV_ERR_INVALID, "imm_offset decreases at frame %d", f);
   const int n = a->imm_offset[nf], na = a->n_active;
-  if (n > 0 && (!a->u || !a->v || !a->idepth_min || !a->idepth_max || !a->lastTraceStatus || !a->lastTracePixelInterval || !a->quality || !a->my_type ||
-                !a->action || (a->cap > 0 && !a->opt_idx)))
+  if (!from_store && n > 0 && (!a->u || !a->v || !a->idepth_min || !a->idepth_max || !a->lastTraceStatus || !a->lastTracePixelInterval || !a->quality ||
+                               !a->my_type || !a->action || (a->cap > 0 && !a->opt_idx)))
     return set_error(DMV_ERR_INVALID, "incomplete immature points");
   for (int p = 0; p < na; p++)
     if (a->act_host[p] < 0 || a->act_host[p] >= nf) return set_error(DMV_ERR_INVALID, "active point %d: host %d out of range", p, a->act_host[p]);
-  const int w1 = b->cfg.w >> 1, h1 = b->cfg.h >> 1, ncell = w1 * h1;
-  if (w1 < 3 || h1 < 3) return set_error(DMV_ERR_INVALID, "image too small for a level-1 distance map");
-  // staging layout (4-byte words): tab 96 | flagged 8 | off 9 (header 128) | active u v idepth host | immature u v idmin idmax status
-  // interval quality type | action | opt | counters 8 | map | cell | frac | rad | stamp.  [0, o_act) goes up, [o_act, o_map (+ ncell)) comes back.
-  const size_t o_au = 128, o_av = o_au + na, o_aid = o_av + na, o_ah = o_aid + na, o_iu = o_ah + na, o_iv = o_iu + n, o_imin = o_iv + n, o_imax = o_imin + n,
-               o_ist = o_imax + n, o_iint = o_ist + n, o_iq = o_iint + n, o_ity = o_iq + n, o_act = o_ity + n, o_opt = o_act + n, o_cnt = o_opt + n,
-               o_map = o_cnt + 8, o_cell = o_map + ncell, o_frac = o_cell + n, o_rad = o_frac + n, o_stamp = o_rad + n, words = o_stamp + ncell;
+  if ((b->cfg.w >> 1) < 3 || (b->cfg.h >> 1) < 3) return set_error(DMV_ERR_INVALID, "image too small for a level-1 distance map");
+  return DMV_OK;
+}
+
+// the header and the active points into h_sel, d_sel and h_sel grown to the layout
+static int sel_stage(dmv_ba* b, const dmv_ba_select_args* a, const SelLayout& o) {
+  const int nf = a->nf, na = a->n_active;
   CK(cudaSetDevice(b->device));
-  CK(b->d_sel.reserve(words));
-  CK(b->h_sel.reserve(words));
+  CK(b->d_sel.reserve(o.words));
+  CK(b->h_sel.reserve(o.words));
   float* hb = b->h_sel;
-  float* d = b->d_sel;
   int* hi = reinterpret_cast<int*>(hb);
   std::memcpy(hb, a->tables12, sizeof(float) * 12 * nf);
   for (int f = 0; f < nf; f++) hi[96 + f] = a->flagged[f] != 0;
   std::memcpy(hi + 104, a->imm_offset, sizeof(int) * (nf + 1));
   if (na > 0) {
-    std::memcpy(hb + o_au, a->act_u, 4 * (size_t)na); std::memcpy(hb + o_av, a->act_v, 4 * (size_t)na);
-    std::memcpy(hb + o_aid, a->act_idepth_scaled, 4 * (size_t)na); std::memcpy(hi + o_ah, a->act_host, 4 * (size_t)na);
+    std::memcpy(hb + o.au, a->act_u, 4 * (size_t)na); std::memcpy(hb + o.av, a->act_v, 4 * (size_t)na);
+    std::memcpy(hb + o.aid, a->act_idepth_scaled, 4 * (size_t)na); std::memcpy(hi + o.ah, a->act_host, 4 * (size_t)na);
   }
-  if (n > 0) {
-    std::memcpy(hb + o_iu, a->u, 4 * (size_t)n); std::memcpy(hb + o_iv, a->v, 4 * (size_t)n);
-    std::memcpy(hb + o_imin, a->idepth_min, 4 * (size_t)n); std::memcpy(hb + o_imax, a->idepth_max, 4 * (size_t)n);
-    std::memcpy(hi + o_ist, a->lastTraceStatus, 4 * (size_t)n); std::memcpy(hb + o_iint, a->lastTracePixelInterval, 4 * (size_t)n);
-    std::memcpy(hb + o_iq, a->quality, 4 * (size_t)n); std::memcpy(hb + o_ity, a->my_type, 4 * (size_t)n);
-  }
-  CK(cudaMemcpyAsync(d, hb, 4 * o_act, cudaMemcpyHostToDevice, b->stream));
+  return DMV_OK;
+}
+
+// The selection on the staged d_sel (map init, seed, the 39 BFS steps, classify, reach, chain), its read-back and one synchronisation;
+// then a's outputs.  Returns DMV_ERR_INVALID when toOptimize exceeds cap (*n_opt, action, map and stats written).
+static int sel_launch(dmv_ba* b, const dmv_ba_select_args* a, const SelLayout& o) {
+  const int n = a->imm_offset[a->nf], na = a->n_active, w1 = b->cfg.w >> 1, h1 = b->cfg.h >> 1, ncell = w1 * h1;
+  float* hb = b->h_sel;
+  int* hi = reinterpret_cast<int*>(hb);
+  float* d = b->d_sel;
   int* di = reinterpret_cast<int*>(d);
   SelArgs A;
-  A.n = n; A.na = na; A.nf = nf; A.newest = a->newest; A.w1 = w1; A.h1 = h1; A.want_map = a->map != nullptr;
+  A.n = n; A.na = na; A.nf = a->nf; A.newest = a->newest; A.w1 = w1; A.h1 = h1; A.want_map = a->map != nullptr;
   A.tile = 8;
   while (((w1 + A.tile - 1) / A.tile) * ((h1 + A.tile - 1) / A.tile) > SEL_TILES) A.tile *= 2;
   A.minActDist = a->currentMinActDist; A.minTraceQuality = a->minTraceQuality;
   A.tab = d; A.flagged = di + 96; A.off = di + 104;
-  A.au = d + o_au; A.av = d + o_av; A.aid = d + o_aid; A.ah = di + o_ah;
-  A.u = d + o_iu; A.v = d + o_iv; A.idmin = d + o_imin; A.idmax = d + o_imax; A.status = di + o_ist; A.interval = d + o_iint; A.quality = d + o_iq;
-  A.type = d + o_ity; A.action = di + o_act; A.opt = di + o_opt; A.counters = di + o_cnt; A.map = d + o_map; A.cell = di + o_cell; A.frac = d + o_frac;
-  A.last_undecided = di + o_cnt + 3; A.rad = di + o_rad; A.stamp = di + o_stamp;
+  A.au = d + o.au; A.av = d + o.av; A.aid = d + o.aid; A.ah = di + o.ah;
+  A.u = d + o.iu; A.v = d + o.iv; A.idmin = d + o.imin; A.idmax = d + o.imax; A.status = di + o.ist; A.interval = d + o.iint; A.quality = d + o.iq;
+  A.type = d + o.ity; A.action = di + o.act; A.opt = di + o.opt; A.counters = di + o.cnt; A.map = d + o.map; A.cell = di + o.cell; A.frac = d + o.frac;
+  A.last_undecided = di + o.cnt + 3; A.rad = di + o.rad; A.stamp = di + o.stamp;
   const cudaStream_t s = b->stream;
-  CK(cudaMemsetAsync(di + o_cnt, 0, 4 * 8, s));
-  CK(cudaMemsetAsync(di + o_cnt + 3, 0xFF, 4, s));
+  CK(cudaMemsetAsync(di + o.cnt, 0, 4 * 8, s));
+  CK(cudaMemsetAsync(di + o.cnt + 3, 0xFF, 4, s));
   CK(cudaMemsetAsync(A.stamp, 0xFF, 4 * (size_t)ncell, s));
   sel_map_init_kernel<<<(ncell + 255) / 256, 256, 0, s>>>(A.map, ncell);
   if (na > 0) sel_seed_kernel<<<(na + 255) / 256, 256, 0, s>>>(A);
@@ -399,14 +433,66 @@ extern "C" int dmv_ba_select_activation(dmv_ba* b, const dmv_ba_select_args* a) 
   }
   sel_chain_kernel<<<1, SEL_T, 0, s>>>(A);
   CK(cudaGetLastError());
-  CK(cudaMemcpyAsync(hb + o_act, d + o_act, 4 * (o_map - o_act + (a->map ? (size_t)ncell : 0)), cudaMemcpyDeviceToHost, s));
+  CK(cudaMemcpyAsync(hb + o.act, d + o.act, 4 * (o.map - o.act + (a->map ? (size_t)ncell : 0)), cudaMemcpyDeviceToHost, s));
   CK(cudaStreamSynchronize(s));
-  const int nopt = hi[o_cnt];
-  if (n > 0) std::memcpy(a->action, hi + o_act, 4 * (size_t)n);
-  if (a->map) std::memcpy(a->map, hb + o_map, 4 * (size_t)ncell);
-  if (a->stats) { a->stats[0] = hi[o_cnt + 4]; a->stats[1] = hi[o_cnt + 1]; a->stats[2] = hi[o_cnt + 2]; }
+  const int nopt = hi[o.cnt];
+  if (n > 0) std::memcpy(a->action, hi + o.act, 4 * (size_t)n);
+  if (a->map) std::memcpy(a->map, hb + o.map, 4 * (size_t)ncell);
+  if (a->stats) { a->stats[0] = hi[o.cnt + 4]; a->stats[1] = hi[o.cnt + 1]; a->stats[2] = hi[o.cnt + 2]; }
   *a->n_opt = nopt;
   if (nopt > a->cap) return set_error(DMV_ERR_INVALID, "%d points to optimise exceed cap %d", nopt, a->cap);
-  if (nopt > 0) std::memcpy(a->opt_idx, hi + o_opt, 4 * (size_t)nopt);
+  if (nopt > 0) std::memcpy(a->opt_idx, hi + o.opt, 4 * (size_t)nopt);
   return DMV_OK;
+}
+
+int ip_select_from_store(dmv_ba* b, const dmv_ba_select_args* a, const dmv_ip_store* s, const int* slot, const float* const* my_type, const int** d_opt) {
+  const int nf = a->nf, n = a->imm_offset[nf];
+  const SelLayout o(n, a->n_active, (size_t)(b->cfg.w >> 1) * (b->cfg.h >> 1));
+  int rc = sel_stage(b, a, o);
+  if (rc != DMV_OK) return rc;
+  float* hb = b->h_sel;
+  float* d = b->d_sel;
+  SelGatherArgs G;
+  G.n = n; G.nf = nf; G.scap = s->cap[s->cur];
+  for (int f = 0; f < nf; f++) {
+    G.off[f] = a->imm_offset[f];
+    G.src[f] = slot[f] >= 0 ? ip_store_first(s, slot[f]) : 0;
+    const int m = a->imm_offset[f + 1] - a->imm_offset[f];
+    if (m > 0) std::memcpy(hb + o.ity + a->imm_offset[f], my_type[f], 4 * (size_t)m);
+  }
+  G.off[nf] = n;
+  G.pts = reinterpret_cast<const unsigned*>(s->d_pts[s->cur].get());
+  G.dst = reinterpret_cast<unsigned*>(d + o.iu);
+  CK(cudaMemcpyAsync(d, hb, 4 * o.iu, cudaMemcpyHostToDevice, b->stream));
+  if (n > 0) {
+    CK(cudaMemcpyAsync(d + o.ity, hb + o.ity, 4 * (size_t)n, cudaMemcpyHostToDevice, b->stream));
+    sel_gather_kernel<<<(n + 127) / 128, 128, 0, b->stream>>>(G);
+  }
+  rc = sel_launch(b, a, o);
+  *d_opt = reinterpret_cast<const int*>(d + o.opt);
+  return rc;
+}
+
+}  // namespace dmv
+
+using namespace dmv;
+
+extern "C" int dmv_ba_select_activation(dmv_ba* b, const dmv_ba_select_args* a) {
+  if (!b || !a) return set_error(DMV_ERR_INVALID, "null argument");
+  int rc = sel_check(b, a, false);
+  if (rc != DMV_OK) return rc;
+  const int n = a->imm_offset[a->nf];
+  const SelLayout o(n, a->n_active, (size_t)(b->cfg.w >> 1) * (b->cfg.h >> 1));
+  rc = sel_stage(b, a, o);
+  if (rc != DMV_OK) return rc;
+  float* hb = b->h_sel;
+  int* hi = reinterpret_cast<int*>(hb);
+  if (n > 0) {
+    std::memcpy(hb + o.iu, a->u, 4 * (size_t)n); std::memcpy(hb + o.iv, a->v, 4 * (size_t)n);
+    std::memcpy(hb + o.imin, a->idepth_min, 4 * (size_t)n); std::memcpy(hb + o.imax, a->idepth_max, 4 * (size_t)n);
+    std::memcpy(hi + o.ist, a->lastTraceStatus, 4 * (size_t)n); std::memcpy(hb + o.iint, a->lastTracePixelInterval, 4 * (size_t)n);
+    std::memcpy(hb + o.iq, a->quality, 4 * (size_t)n); std::memcpy(hb + o.ity, a->my_type, 4 * (size_t)n);
+  }
+  CK(cudaMemcpyAsync(b->d_sel, hb, 4 * o.act, cudaMemcpyHostToDevice, b->stream));
+  return sel_launch(b, a, o);
 }

@@ -4,23 +4,13 @@
 // uploads 14 floats per slot and downloads nothing.
 // put and remove rebuild the point list by one gather (ip_store_gather_kernel) into the second of two buffers: new row j = old row
 // perm[j], or a row of the slot just uploaded.  The kernel only copies words, so an edit changes no bit of a point that stays.
+#include "ba_handle.h"
 #include "ct_handle.h"
+#include "ip_store.h"
 #include "ip_trace.h"
 #include "remove_outliers.h"
 #include <cstring>
 #include <vector>
-
-struct dmv_ip_store {
-  int device = 0;
-  dmv::Stream stream;                 // put, get and remove; a trace runs on its handle's stream
-  dmv::DevBuf<float> d_pts[2];        // ipw layout of cap[k] points, then 14 x DMV_IP_STORE_SLOTS table floats; d_pts[cur] holds the points
-  int cap[2] = {0, 0};
-  int cur = 0;
-  int count[DMV_IP_STORE_SLOTS] = {0};   // points per slot, in slot order in d_pts[cur]
-  dmv::DevBuf<float> d_edit;          // an edit's uploaded words: put's rows (ipw layout, capacity = their count), then the row map perm
-  dmv::PinnedBuf<float> h_edit;       // its host side; get's downloaded words
-  dmv::PinnedBuf<float> h_tab;        // a trace's tables
-};
 
 namespace dmv {
 
@@ -52,7 +42,7 @@ static int ip_store_total(const dmv_ip_store* s) {
   return n;
 }
 
-static int ip_store_first(const dmv_ip_store* s, int slot) {
+int ip_store_first(const dmv_ip_store* s, int slot) {
   int at = 0;
   for (int k = 0; k < slot; k++) at += s->count[k];
   return at;
@@ -98,6 +88,31 @@ static int ip_store_stage(dmv_ip_store* s, int m, int n) {
   CK(s->h_edit.reserve(words));
   CK(s->d_edit.reserve(words));
   return DMV_OK;
+}
+
+int ip_store_remove_dead(dmv_ip_store* s, const std::vector<char> (&alive)[DMV_IP_STORE_SLOTS], std::vector<int> (&order)[DMV_IP_STORE_SLOTS]) {
+  int count[DMV_IP_STORE_SLOTS], total = 0, removed = 0;
+  for (int k = 0; k < DMV_IP_STORE_SLOTS; k++) {
+    const int m = s->count[k];
+    if (alive[k].empty()) {
+      order[k].resize(m);
+      for (int q = 0; q < m; q++) order[k][q] = q;
+    } else {
+      order[k] = remove_outliers_order(0, m, alive[k]);   // activatePointsMT's loop (FullSystem.cpp:L761-769), on indices
+    }
+    count[k] = (int)order[k].size();
+    total += count[k];
+    removed += m - count[k];
+  }
+  if (removed == 0) return DMV_OK;
+  CK(cudaSetDevice(s->device));
+  const int rc = ip_store_stage(s, 0, total);
+  if (rc != DMV_OK) return rc;
+  std::vector<int> perm;
+  perm.reserve(total);
+  for (int k = 0, first = 0; k < DMV_IP_STORE_SLOTS; first += s->count[k], k++)
+    for (int o : order[k]) perm.push_back(first + o);
+  return ip_store_apply(s, perm, 0, count);
 }
 
 // the checks of one store job (dmv_ct_trace_store's arguments after the NULL checks); *n = the points it traces.  No CUDA call.
@@ -252,28 +267,18 @@ int dmv_ip_store_remove(dmv_ip_store* s, int slot, int n, const int32_t* idx, in
   if (n < 0 || (n > 0 && !idx)) return set_error(DMV_ERR_INVALID, "null argument");
   const int m = s->count[slot];
   if (n > m) return set_error(DMV_ERR_INVALID, "n = %d: slot %d holds %d points", n, slot, m);
-  std::vector<char> alive(m, 1);
+  std::vector<char> alive[DMV_IP_STORE_SLOTS];
+  alive[slot].assign(m, 1);
   for (int q = 0; q < n; q++) {
     if (idx[q] < 0 || idx[q] >= m) return set_error(DMV_ERR_INVALID, "idx[%d] = %d: slot %d holds %d points", q, idx[q], slot, m);
-    if (!alive[idx[q]]) return set_error(DMV_ERR_INVALID, "idx[%d] = %d appears twice", q, idx[q]);
-    alive[idx[q]] = 0;
+    if (!alive[slot][idx[q]]) return set_error(DMV_ERR_INVALID, "idx[%d] = %d appears twice", q, idx[q]);
+    alive[slot][idx[q]] = 0;
   }
-  const std::vector<int> order = remove_outliers_order(0, m, alive);   // activatePointsMT's loop (FullSystem.cpp:L761-769), on indices
-  if (order_out) std::memcpy(order_out, order.data(), sizeof(int32_t) * order.size());
-  if (n == 0) return DMV_OK;
-  const int total = ip_store_total(s) - n, first = ip_store_first(s, slot);
-  CK(cudaSetDevice(s->device));
-  rc = ip_store_stage(s, 0, total);
+  std::vector<int> order[DMV_IP_STORE_SLOTS];
+  rc = ip_store_remove_dead(s, alive, order);
   if (rc != DMV_OK) return rc;
-  std::vector<int> perm;
-  perm.reserve(total);
-  for (int q = 0; q < first; q++) perm.push_back(q);
-  for (int o : order) perm.push_back(first + o);
-  for (int q = first + m; q < total + n; q++) perm.push_back(q);
-  int count[DMV_IP_STORE_SLOTS];
-  std::memcpy(count, s->count, sizeof(count));
-  count[slot] = m - n;
-  return ip_store_apply(s, perm, 0, count);
+  if (order_out) std::memcpy(order_out, order[slot].data(), sizeof(int32_t) * order[slot].size());
+  return DMV_OK;
 }
 
 int dmv_ct_trace_store(dmv_ct* c, dmv_ip_store* s, int nslots, const float* tables14, const dmv_ip_settings* settings) {
@@ -288,4 +293,68 @@ int dmv_ct_trace_store_many(dmv_ct* const* handles, int n, const dmv_ct_trace_st
   const int rc = ct_check_members(handles, n, DMV_CT_TRACE_MANY_MAX);
   if (rc != DMV_OK) return rc;
   return ip_store_trace_run(handles, n, jobs, settings, true);
+}
+
+// dmv_ba_activate_store: the selection and the activation on rows gathered from the store on the device, then the removal as one edit
+int dmv_ba_activate_store(dmv_ba* b, dmv_ip_store* s, const dmv_ba_activate_store_args* a) {
+  if (!b || !s || !a) return set_error(DMV_ERR_INVALID, "null argument");
+  if (b->nf < 2 || !b->have_state) return set_error(DMV_ERR_STATE, "dmv_ba_set_window + dmv_ba_set_state first");
+  const int nf = a->nf;
+  if (nf != b->nf) return set_error(DMV_ERR_INVALID, "nf = %d: the window has %d frames", nf, b->nf);
+  if (s->device != b->device) return set_error(DMV_ERR_INVALID, "the store is on device %d, the handle on device %d", s->device, b->device);
+  if (!a->slot || !a->my_type) return set_error(DMV_ERR_INVALID, "incomplete dmv_ba_activate_store_args");
+  int off[MAXF + 1] = {0};
+  for (int f = 0; f < nf; f++) {
+    const int k = a->slot[f];
+    if (k < -1 || k >= DMV_IP_STORE_SLOTS) return set_error(DMV_ERR_INVALID, "slot[%d] = %d: expected -1 to %d", f, k, DMV_IP_STORE_SLOTS - 1);
+    for (int g = 0; g < f; g++)
+      if (k >= 0 && a->slot[g] == k) return set_error(DMV_ERR_INVALID, "slot[%d] and slot[%d] are both %d", g, f, k);
+    const int m = k >= 0 ? s->count[k] : 0;
+    if (m > 0 && !a->my_type[f]) return set_error(DMV_ERR_INVALID, "my_type[%d] is NULL for %d points", f, m);
+    off[f + 1] = off[f] + m;
+  }
+  const int n = off[nf];
+  std::vector<int32_t> action(a->action ? 0 : n), opt(std::max(a->cap, 0));
+  dmv_ba_select_args sa;
+  std::memset(&sa, 0, sizeof(sa));
+  sa.nf = nf; sa.newest = a->newest; sa.tables12 = a->tables12; sa.flagged = a->flagged; sa.n_active = a->n_active;
+  sa.act_u = a->act_u; sa.act_v = a->act_v; sa.act_idepth_scaled = a->act_idepth_scaled; sa.act_host = a->act_host; sa.imm_offset = off;
+  sa.currentMinActDist = a->currentMinActDist; sa.minTraceQuality = a->minTraceQuality; sa.cap = a->cap; sa.n_opt = a->n_opt;
+  sa.action = a->action ? a->action : action.data(); sa.opt_idx = opt.data(); sa.map = a->map; sa.stats = a->stats;
+  int rc = sel_check(b, &sa, true);
+  if (rc != DMV_OK) return rc;
+  if (a->cap > 0 && (!a->RT || !a->opt_frame || !a->opt_index || !a->status || !a->idepth || !a->res_state))
+    return set_error(DMV_ERR_INVALID, "incomplete dmv_ba_activate_store_args");
+  const int* d_opt = nullptr;
+  rc = ip_select_from_store(b, &sa, s, a->slot, a->my_type, &d_opt);
+  if (rc != DMV_OK) return rc;
+  const int nopt = *a->n_opt;
+  std::vector<int32_t> trace_status(nopt);
+  rc = ip_act_from_store(b, s, off, a->slot, d_opt, nopt, a->RT, a->minObs, a->status, a->idepth, a->res_state, trace_status.data());
+  if (rc != DMV_OK) return rc;
+  // activatePointsMT's removals (FullSystem.cpp:L732-770): deleted by the selection, activated (1), outliers (-1), and not activated but OOB
+  std::vector<char> alive[DMV_IP_STORE_SLOTS];
+  for (int f = 0; f < nf; f++)
+    if (a->slot[f] >= 0 && f != a->newest) alive[a->slot[f]].assign(off[f + 1] - off[f], 1);
+  for (int f = 0; f < nf; f++)
+    for (int i = off[f]; f != a->newest && i < off[f + 1]; i++)
+      if (sa.action[i] == DMV_ACT_DELETE) alive[a->slot[f]][i - off[f]] = 0;
+  for (int j = 0; j < nopt; j++) {
+    const int i = opt[j];
+    int f = 0;
+    while (off[f + 1] <= i) f++;
+    a->opt_frame[j] = f;
+    a->opt_index[j] = i - off[f];
+    if (a->status[j] != 0 || trace_status[j] == 1) alive[a->slot[f]][i - off[f]] = 0;   // IPS_OOB
+  }
+  std::vector<int> order[DMV_IP_STORE_SLOTS];
+  rc = ip_store_remove_dead(s, alive, order);
+  if (rc != DMV_OK) return rc;
+  for (int f = 0, at = 0; f < nf; f++) {
+    const int kept = a->slot[f] >= 0 ? (int)order[a->slot[f]].size() : 0;
+    if (a->order_out && kept > 0) std::memcpy(a->order_out + at, order[a->slot[f]].data(), sizeof(int32_t) * kept);
+    if (a->n_kept) a->n_kept[f] = kept;
+    at += kept;
+  }
+  return DMV_OK;
 }

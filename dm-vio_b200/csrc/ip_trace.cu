@@ -11,6 +11,7 @@
 // The flag affects device code only, so the C-ABI entry points of the three kernels (end of the file) are compiled here too.
 #include "ct_handle.h"
 #include "ba_handle.h"
+#include "ip_store.h"
 #include "ip_trace.h"
 #include <cstring>
 #include <math.h>
@@ -484,6 +485,118 @@ int ip_trace_launch(dmv_ct* const* hs, const IPTraceArgs& A) {
   return DMV_OK;
 }
 
+// dmv_ba_activate_points' staging (words): RT[64*12] | aff[64*2] | host | u | v | color*8 | weights*8 | energyTH | idmin | idmax | status | idepth |
+// res_state*MAXF | lastTraceStatus (dmv_ba_activate_store only), cap points per array.  [0, st) goes up, status .. res_state come back.
+struct ActLayout {
+  size_t rt, aff, host, u, v, col, wgt, eth, min, max, st, id, rs, ts, words;
+};
+static ActLayout act_layout(size_t cap) {
+  ActLayout o;
+  o.rt = 0; o.aff = (size_t)MAXF * MAXF * 12; o.host = (size_t)MAXF * MAXF * 14; o.u = o.host + cap; o.v = o.u + cap; o.col = o.v + cap;
+  o.wgt = o.col + 8 * cap; o.eth = o.wgt + 8 * cap; o.min = o.eth + cap; o.max = o.min + cap; o.st = o.max + cap; o.id = o.st + cap; o.rs = o.id + cap;
+  o.ts = o.rs + MAXF * cap; o.words = o.ts + cap;
+  return o;
+}
+
+// d_act / h_act hold n points; RT and the window's PRE_aff_mode staged in h_act
+static int act_stage(dmv_ba* b, int n, const float* RT) {
+  if (n > b->act_cap) {
+    b->act_cap = 0;
+    const int cap = std::max(n, 2048);
+    const size_t words = act_layout(cap).words;
+    CK(b->d_act.reserve(words));
+    CK(b->h_act.reserve(words));
+    b->act_cap = cap;
+  }
+  const ActLayout o = act_layout(b->act_cap);
+  const int nf = b->nf;
+  float* hb = b->h_act;
+  std::memcpy(hb + o.rt, RT, sizeof(float) * 12 * nf * nf);
+  const BAIter& it = b->h_up->it;
+  for (int k = 0; k < nf * nf; k++) { hb[o.aff + 2 * k] = it.precalc[k][24]; hb[o.aff + 2 * k + 1] = it.precalc[k][25]; }  // PRE_aff_mode
+  return DMV_OK;
+}
+
+// ip_activate_kernel on the n points staged in d_act, the read-back (and the rows' lastTraceStatus when trace_status is not NULL) and one
+// synchronisation
+static int act_launch(dmv_ba* b, int n, int minObs, int32_t* status, float* idepth, int32_t* res_state, int32_t* trace_status) {
+  const int nf = b->nf;
+  const ActLayout o = act_layout(b->act_cap);
+  float* hb = b->h_act;
+  float* d = b->d_act;
+  const BAIter& it = b->h_up->it;
+  IPActArgs A;
+  A.n = n; A.nf = nf; A.w = b->cfg.w; A.h = b->cfg.h; A.minObs = minObs; A.GNIts = 3;  // setting_GNItsOnPointActivation
+  A.fxl = it.calib[0]; A.fyl = it.calib[1]; A.cxl = it.calib[2]; A.cyl = it.calib[3]; A.fxli = it.calib[4]; A.fyli = it.calib[5];
+  A.huberTH = b->prm.huberTH; A.minIdepthH_act = 100.f;                                      // setting_minIdepthH_act
+  for (int f = 0; f < MAXF; f++) A.img[f] = f < nf ? b->d_img[b->slots[f]].get() : nullptr;
+  A.RT = d + o.rt; A.aff = d + o.aff; A.host = reinterpret_cast<const int*>(d + o.host);
+  A.u = d + o.u; A.v = d + o.v; A.color = d + o.col; A.weights = d + o.wgt; A.energyTH = d + o.eth; A.idepth_min = d + o.min; A.idepth_max = d + o.max;
+  A.status = reinterpret_cast<int*>(d + o.st); A.idepth = d + o.id; A.res_state = reinterpret_cast<int*>(d + o.rs);
+  ip_activate_kernel<<<(A.n + 15) / 16, 128, 0, b->stream>>>(A);   // 8 lanes per point
+  b->launches++;
+  CK(cudaGetLastError());
+  CK(cudaMemcpyAsync(hb + o.st, d + o.st, sizeof(float) * (o.rs - o.st + (size_t)nf * n), cudaMemcpyDeviceToHost, b->stream));
+  if (trace_status) CK(cudaMemcpyAsync(hb + o.ts, d + o.ts, 4 * (size_t)n, cudaMemcpyDeviceToHost, b->stream));
+  CK(cudaStreamSynchronize(b->stream));
+  std::memcpy(status, hb + o.st, 4 * (size_t)n); std::memcpy(idepth, hb + o.id, 4 * (size_t)n);
+  std::memcpy(res_state, hb + o.rs, 4 * (size_t)n * nf);
+  if (trace_status) std::memcpy(trace_status, hb + o.ts, 4 * (size_t)n);
+  return DMV_OK;
+}
+
+// The activation's rows fed from a store: row j = toOptimize entry opt[j], an index into the groups' concatenation; group f's row i is the
+// store's row src[f] + i - off[f].  Copies host frame f, u, v, color8, weights8, energyTH, idepth_min, idepth_max and lastTraceStatus
+// into dmv_ba_activate_points' staging.
+struct ActGatherArgs {
+  int n, nf, scap;
+  int off[MAXF + 1], src[MAXF];
+  const int* opt;
+  const unsigned* pts;
+  unsigned* d;        // d_act
+  ActLayout o;
+};
+__global__ void __launch_bounds__(128) ip_act_gather_kernel(const __grid_constant__ ActGatherArgs G) {
+  const int j = blockIdx.x * blockDim.x + threadIdx.x;
+  if (j >= G.n) return;
+  const int i = G.opt[j];
+  int f = 0;
+  while (G.off[f + 1] <= i) f++;
+  const size_t r = G.src[f] + (i - G.off[f]), scap = G.scap;
+  const ActLayout& o = G.o;
+  G.d[o.host + j] = f;
+  G.d[o.u + j] = G.pts[ipw::u * scap + r];
+  G.d[o.v + j] = G.pts[ipw::v * scap + r];
+#pragma unroll
+  for (int k = 0; k < 8; k++) {
+    G.d[o.col + 8 * j + k] = G.pts[ipw::color * scap + 8 * r + k];
+    G.d[o.wgt + 8 * j + k] = G.pts[ipw::weights * scap + 8 * r + k];
+  }
+  G.d[o.eth + j] = G.pts[ipw::energyTH * scap + r];
+  G.d[o.min + j] = G.pts[ipw::idepth_min * scap + r];
+  G.d[o.max + j] = G.pts[ipw::idepth_max * scap + r];
+  G.d[o.ts + j] = G.pts[ipw::status * scap + r];
+}
+
+int ip_act_from_store(dmv_ba* b, const dmv_ip_store* s, const int* imm_offset, const int* slot, const int* d_opt, int n, const float* RT, int minObs,
+                      int32_t* status, float* idepth, int32_t* res_state, int32_t* trace_status) {
+  if (n == 0) return DMV_OK;
+  CK(cudaSetDevice(b->device));
+  const int rc = act_stage(b, n, RT);
+  if (rc != DMV_OK) return rc;
+  ActGatherArgs G;
+  G.n = n; G.nf = b->nf; G.scap = s->cap[s->cur];
+  for (int f = 0; f < b->nf; f++) { G.off[f] = imm_offset[f]; G.src[f] = slot[f] >= 0 ? ip_store_first(s, slot[f]) : 0; }
+  G.off[b->nf] = imm_offset[b->nf];
+  G.opt = d_opt;
+  G.pts = reinterpret_cast<const unsigned*>(s->d_pts[s->cur].get());
+  G.d = reinterpret_cast<unsigned*>(b->d_act.get());
+  G.o = act_layout(b->act_cap);
+  CK(cudaMemcpyAsync(b->d_act, b->h_act, sizeof(float) * G.o.host, cudaMemcpyHostToDevice, b->stream));
+  ip_act_gather_kernel<<<(n + 127) / 128, 128, 0, b->stream>>>(G);
+  return act_launch(b, n, minObs, status, idepth, res_state, trace_status);
+}
+
 }  // namespace dmv
 
 using namespace dmv;
@@ -649,41 +762,13 @@ int dmv_ba_activate_points(dmv_ba* b, const dmv_ba_activate_args* a) {
   for (int i = 0; i < n; i++)
     if (a->host[i] < 0 || a->host[i] >= nf) return set_error(DMV_ERR_INVALID, "point %d: host %d out of range", i, a->host[i]);
   CK(cudaSetDevice(b->device));
-  if (n > b->act_cap) {
-    b->act_cap = 0;
-    const int cap = std::max(n, 2048);
-    const size_t words = (size_t)MAXF * MAXF * 14 + (size_t)(24 + MAXF) * cap;
-    CK(b->d_act.reserve(words));
-    CK(b->h_act.reserve(words));
-    b->act_cap = cap;
-  }
-  const size_t cap = b->act_cap;
+  const int rc = act_stage(b, n, a->RT);
+  if (rc != DMV_OK) return rc;
+  const ActLayout o = act_layout(b->act_cap);
   float* hb = b->h_act;
-  float* d = b->d_act;
-  // layout (words): RT[64*12] | aff[64*2] | host | u | v | color*8 | weights*8 | energyTH | idmin | idmax | status | idepth | res_state*MAXF
-  const size_t o_rt = 0, o_aff = (size_t)MAXF * MAXF * 12, o_host = (size_t)MAXF * MAXF * 14, o_u = o_host + cap, o_v = o_u + cap, o_col = o_v + cap,
-               o_wgt = o_col + 8 * cap, o_eth = o_wgt + 8 * cap, o_min = o_eth + cap, o_max = o_min + cap, o_st = o_max + cap, o_id = o_st + cap, o_rs = o_id + cap;
-  std::memcpy(hb + o_rt, a->RT, sizeof(float) * 12 * nf * nf);
-  const BAIter& it = b->h_up->it;
-  for (int k = 0; k < nf * nf; k++) { hb[o_aff + 2 * k] = it.precalc[k][24]; hb[o_aff + 2 * k + 1] = it.precalc[k][25]; }  // PRE_aff_mode
-  std::memcpy(hb + o_host, a->host, 4 * (size_t)n); std::memcpy(hb + o_u, a->u, 4 * (size_t)n); std::memcpy(hb + o_v, a->v, 4 * (size_t)n);
-  std::memcpy(hb + o_col, a->color8, 32 * (size_t)n); std::memcpy(hb + o_wgt, a->weights8, 32 * (size_t)n); std::memcpy(hb + o_eth, a->energyTH, 4 * (size_t)n);
-  std::memcpy(hb + o_min, a->idepth_min, 4 * (size_t)n); std::memcpy(hb + o_max, a->idepth_max, 4 * (size_t)n);
-  CK(cudaMemcpyAsync(d, hb, sizeof(float) * o_st, cudaMemcpyHostToDevice, b->stream));
-  IPActArgs A;
-  A.n = n; A.nf = nf; A.w = b->cfg.w; A.h = b->cfg.h; A.minObs = a->minObs; A.GNIts = 3;  // setting_GNItsOnPointActivation
-  A.fxl = it.calib[0]; A.fyl = it.calib[1]; A.cxl = it.calib[2]; A.cyl = it.calib[3]; A.fxli = it.calib[4]; A.fyli = it.calib[5];
-  A.huberTH = b->prm.huberTH; A.minIdepthH_act = 100.f;                                      // setting_minIdepthH_act
-  for (int f = 0; f < MAXF; f++) A.img[f] = f < nf ? b->d_img[b->slots[f]].get() : nullptr;
-  A.RT = d + o_rt; A.aff = d + o_aff; A.host = reinterpret_cast<const int*>(d + o_host);
-  A.u = d + o_u; A.v = d + o_v; A.color = d + o_col; A.weights = d + o_wgt; A.energyTH = d + o_eth; A.idepth_min = d + o_min; A.idepth_max = d + o_max;
-  A.status = reinterpret_cast<int*>(d + o_st); A.idepth = d + o_id; A.res_state = reinterpret_cast<int*>(d + o_rs);
-  ip_activate_kernel<<<(A.n + 15) / 16, 128, 0, b->stream>>>(A);   // 8 lanes per point
-  b->launches++;
-  CK(cudaGetLastError());
-  CK(cudaMemcpyAsync(hb + o_st, d + o_st, sizeof(float) * (2 * cap + (size_t)nf * n), cudaMemcpyDeviceToHost, b->stream));
-  CK(cudaStreamSynchronize(b->stream));
-  std::memcpy(a->status, hb + o_st, 4 * (size_t)n); std::memcpy(a->idepth, hb + o_id, 4 * (size_t)n);
-  std::memcpy(a->res_state, hb + o_rs, 4 * (size_t)n * nf);
-  return DMV_OK;
+  std::memcpy(hb + o.host, a->host, 4 * (size_t)n); std::memcpy(hb + o.u, a->u, 4 * (size_t)n); std::memcpy(hb + o.v, a->v, 4 * (size_t)n);
+  std::memcpy(hb + o.col, a->color8, 32 * (size_t)n); std::memcpy(hb + o.wgt, a->weights8, 32 * (size_t)n); std::memcpy(hb + o.eth, a->energyTH, 4 * (size_t)n);
+  std::memcpy(hb + o.min, a->idepth_min, 4 * (size_t)n); std::memcpy(hb + o.max, a->idepth_max, 4 * (size_t)n);
+  CK(cudaMemcpyAsync(b->d_act, hb, sizeof(float) * o.st, cudaMemcpyHostToDevice, b->stream));
+  return act_launch(b, n, a->minObs, a->status, a->idepth, a->res_state, nullptr);
 }

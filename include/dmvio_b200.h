@@ -576,6 +576,47 @@ typedef struct dmv_ct_trace_store_job {
 } dmv_ct_trace_store_job;
 int dmv_ct_trace_store_many(dmv_ct* const* handles, int n, const dmv_ct_trace_store_job* jobs, const dmv_ip_settings* settings);
 
+/* FullSystem::activatePointsMT (FullSystem.cpp:L642-770) from makeDistanceMap through the removal loop, with the window's immature points
+ * read from a store: frame f's host->immaturePoints are slot slot[f] (-1: none; slots need not follow frame order).  Bit-identical to
+ *   1. dmv_ip_store_get of every slot named by a frame, 2. dmv_ba_select_activation on those points (imm_offset from the slots' counts),
+ *   3. dmv_ba_activate_points on its toOptimize, 4. activatePointsMT's choice of the points to drop, 5. dmv_ip_store_remove of every slot:
+ * every output, the store's contents and counts, and every later trace of the store.  Removed: action DMV_ACT_DELETE, and toOptimize entries
+ * with status 1 or -1, or status 0 and lastTraceStatus IPS_OOB (1); each slot keeps L761-769's order.  Slots no frame names and the newest
+ * frame's slot are not touched.  The other arguments are those of dmv_ba_select_activation and dmv_ba_activate_points; my_type[f] is frame
+ * f's ImmaturePoint::my_type in its slot's order (the only field the selection reads that the store does not hold).  Reads no BA state but
+ * what dmv_ba_activate_points reads (images, calibration, PRE_aff_mode); its launch count moves as dmv_ba_activate_points' does (+1 when
+ * toOptimize is not empty).  Three synchronisations.
+ * Errors, all before any allocation, copy or launch, with the store unchanged: DMV_ERR_STATE as dmv_ba_activate_points; DMV_ERR_INVALID for a
+ * NULL ba / s / a, nf other than the window's, a store on another device, a slot outside -1..DMV_IP_STORE_SLOTS-1 or named twice, a NULL
+ * my_type[f] for a frame with points, NULL RT / opt_frame / opt_index / status / idepth / res_state with cap > 0, and every argument
+ * dmv_ba_select_activation refuses.  More than cap entries in toOptimize: DMV_ERR_INVALID after the selection with *n_opt = the count
+ * needed (action, map and stats written) and nothing removed. */
+typedef struct dmv_ba_activate_store_args {
+  int nf, newest;                      /* nf = the window's frames */
+  const float* tables12;               /* as dmv_ba_select_args */
+  const uint8_t* flagged;
+  int n_active;
+  const float *act_u, *act_v, *act_idepth_scaled;
+  const int32_t* act_host;
+  const int32_t* slot;                 /* nf */
+  const float* const* my_type;         /* nf pointers, count of slot[f] floats each (NULL allowed for a frame without points) */
+  float currentMinActDist, minTraceQuality;
+  const float* RT;                     /* as dmv_ba_activate_args */
+  int minObs;
+  int cap;                             /* capacity of opt_frame, opt_index, status, idepth and res_state (nf per entry) */
+  int* n_opt;                          /* out: toOptimize's size (on overflow the count needed) */
+  int32_t *opt_frame, *opt_index;      /* out: toOptimize as (frame, index in its slot before the call) */
+  int32_t* status;                     /* out, per toOptimize entry: as dmv_ba_activate_args */
+  float* idepth;
+  int32_t* res_state;
+  int32_t* order_out;                  /* optional out: each survivor's index before the call, one segment per frame in frame order */
+  int32_t* n_kept;                     /* optional out, nf: points left in frame f's slot (the segment lengths of order_out) */
+  int32_t* action;                     /* optional out: as dmv_ba_select_args, the frames' points concatenated in frame order */
+  float* map;                          /* optional out: as dmv_ba_select_args */
+  int* stats;                          /* optional out [3]: as dmv_ba_select_args */
+} dmv_ba_activate_store_args;
+int dmv_ba_activate_store(dmv_ba* ba, dmv_ip_store* s, const dmv_ba_activate_store_args* a);
+
 /* ------------------------------------------------------------------------------------------------
  * New immature points of a keyframe  ==  FullSystem::makeNewTraces (FullSystem.cpp:L1640-1667): PixelSelector::makeMaps
  * (FullSystem/PixelSelector2.cpp:L158-307) on the handle's RESIDENT frame (the one last given to dmv_ct_upload_new_image /
