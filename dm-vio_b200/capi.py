@@ -62,6 +62,10 @@ class BAActivateStoreArgs(C.Structure):
                [(k, vp) for k in ("n_opt", "opt_frame", "opt_index", "status", "idepth", "res_state", "order_out", "n_kept", "action", "map", "stats")]
 
 
+class BAEditArgs(C.Structure):
+    _fields_ = [("nf", C.c_int), ("slots", vp), ("frame_src", vp), ("npts", C.c_int), ("point_src", vp), ("new_res_target", C.c_int)]
+
+
 class BAMargArgs(C.Structure):
     _fields_ = [("n", C.c_int32), ("point", C.c_void_p), ("adHTdeltaF", C.c_void_p), ("cDeltaF", C.c_float * 4), ("idepthFixPriorMargFac", C.c_float)] + \
                [(k, C.c_void_p) for k in ("M", "Mb", "Msc", "Mbsc", "resInM", "ngoodRes", "res_toZeroF", "isLinearized")]
@@ -203,7 +207,7 @@ SYMBOLS = [
     "dmv_ba_set_window", "dmv_ba_set_points", "dmv_ba_set_residuals", "dmv_ba_set_adjoints", "dmv_ba_set_state", "dmv_ba_linearize",
     "dmv_ba_get_residual_outputs", "dmv_ba_get_target_energies", "dmv_ba_apply_res", "dmv_ba_accumulate", "dmv_ba_get_point_outputs", "dmv_ba_get_solve_HdiF",
     "dmv_ba_resubstitute", "dmv_ba_backup_points", "dmv_ba_restore_points", "dmv_ba_get_idepth", "dmv_ba_gn_step", "dmv_nccl_unique_id",
-    "dmv_ba_comm_init", "dmv_ba_activate_points", "dmv_ba_select_activation", "dmv_ba_activate_store", "dmv_ba_marginalize_points", "dmv_ba_drop_residuals", "dmv_ba_reset_oob", "dmv_ba_p2p_export", "dmv_ba_p2p_import", "dmv_ba_last_timing", "dmv_ba_bench_device", "dmv_ba_bench_phases", "dmv_ba_kernel_launch_count", "dmv_ba_io_bytes", "dmv_ba_set_timing", "dmv_ba_bench_e2e",
+    "dmv_ba_comm_init", "dmv_ba_activate_points", "dmv_ba_select_activation", "dmv_ba_activate_store", "dmv_ba_edit_window", "dmv_ba_marginalize_points", "dmv_ba_drop_residuals", "dmv_ba_reset_oob", "dmv_ba_p2p_export", "dmv_ba_p2p_import", "dmv_ba_last_timing", "dmv_ba_bench_device", "dmv_ba_bench_phases", "dmv_ba_kernel_launch_count", "dmv_ba_io_bytes", "dmv_ba_set_timing", "dmv_ba_bench_e2e",
     "dmv_ba_batch_create", "dmv_ba_batch_destroy", "dmv_ba_batch_gn_step", "dmv_ba_batch_set_timing", "dmv_ba_batch_last_kernel_ms", "dmv_ba_batch_bench",
     "dmv_ct_create", "dmv_ct_destroy", "dmv_ct_set_K", "dmv_ct_set_ref", "dmv_ct_make_coarse_depth", "dmv_ct_set_ref_from_ba", "dmv_ct_get_ref", "dmv_ct_upload_new", "dmv_ct_upload_new_image", "dmv_ct_set_huber",
     "dmv_ci_create", "dmv_ci_destroy", "dmv_ci_set_K", "dmv_ci_upload_first", "dmv_ci_upload_new", "dmv_ci_set_points", "dmv_ci_calc_res_and_gs", "dmv_ci_kernel_launch_count",
@@ -272,6 +276,7 @@ _ARGTYPES = {
     "dmv_ba_activate_points": [vp, C.POINTER(BAActivateArgs)],
     "dmv_ba_select_activation": [vp, C.POINTER(BASelectArgs)],
     "dmv_ba_activate_store": [vp, vp, C.POINTER(BAActivateStoreArgs)],
+    "dmv_ba_edit_window": [vp, C.POINTER(BAEditArgs)],
     "dmv_ba_marginalize_points": [vp, C.POINTER(BAMargArgs)],
     "dmv_ba_drop_residuals": [vp, C.c_int, i32p],
     "dmv_ba_reset_oob": [vp],
@@ -598,6 +603,16 @@ class BA:
         return dict(opt_frame=ofr[:k].copy(), opt_index=oix[:k].copy(), status=st[:k].copy(), idepth=idp[:k].copy(), res_state=rs[:k].copy(),
                     order=order[:int(n_kept.sum())].copy(), n_kept=n_kept, action=action[:n].copy(), map=m,
                     stats=dict(undecided=int(stats[0]), floods=int(stats[1]), rounds=int(stats[2])))
+
+    def edit_window(self, nf, slots, frame_src, point_src, new_res_target=-1, *, nres):
+        """dmv_ba_edit_window: the window becomes nf frames (image slots `slots`, None = 0..nf-1; frame_src[f] = the frame's current index or
+        -1) and the points point_src (a current index, or -1 - k for entry k of the last activation).  nres is the new window's residual count
+        by the header's rules (the caller replays them, as it keeps the lists the per-residual read-backs are ordered by); it sizes
+        residual_outputs and the other per-residual read-backs."""
+        s, fs, ps = _c(slots, np.int32), _c(frame_src, np.int32), _c(point_src, np.int32)
+        a = BAEditArgs(int(nf), None if s is None else s.ctypes.data, fs.ctypes.data, len(ps), ps.ctypes.data, int(new_res_target))
+        check(self.L.dmv_ba_edit_window(self.h, C.byref(a)))
+        self.nf, self.N, self.npts, self.nres = int(nf), 8 * int(nf) + 4, len(ps), int(nres)
 
     def reset_oob(self):
         check(self.L.dmv_ba_reset_oob(self.h))

@@ -63,6 +63,60 @@ void dmv_ba_next_exchange(dmv_ba* b) {
   b->h_up->win.xc.seq = b->xchg_seq;
 }
 
+// The chunk shape of npts points ordered by host frame.  One thread per residual (P = 32, fewest instructions) pays off once the window no
+// longer fits one wave of 16-point chunks (measured at 7 KF / 8000 points: 54 vs 68 us per step); below that the 4-lanes-per-residual
+// shape (P = 16) has the shorter critical path (29.6 vs 37.9 us)
+void dmv_ba_window_shape(const dmv_ba* b, int npts, const int32_t* host, BAShape* s) {
+  s->P = b->P_auto ? ((npts > 16 * b->sms) ? 32 : 16) : b->P;
+  int p = 0, c = 0;
+  for (int h = 0; h < MAXF; h++) {
+    s->host_start[h] = p;
+    s->chunk_beg[h] = c;
+    int cnt = 0;
+    while (p < npts && host[p] == h) { p++; cnt++; }
+    c += (cnt + s->P - 1) / s->P;
+  }
+  s->host_start[MAXF] = npts;
+  s->chunk_beg[MAXF] = c;
+  s->nchunks = c;
+}
+
+// The window takes the shape s, and the phase D items of that shape (ba_fused.cu: fused_reduce) go up on the handle's stream
+int dmv_ba_take_shape(dmv_ba* b, const BAShape* s) {
+  b->P = s->P;
+  for (int h = 0; h <= MAXF; h++) { b->host_start[h] = s->host_start[h]; b->chunk_beg[h] = s->chunk_beg[h]; }
+  b->nchunks = s->nchunks;
+  if (b->nchunks > b->max_chunks) return set_error(DMV_ERR_INVALID, "too many chunks");
+  const int nf = b->nf, N = b->N, nch = b->nchunks;
+  const int* cb = b->chunk_beg;
+  std::vector<int4>& t = b->h_dtab;
+  t.clear();
+  // one offset over [lo, hi): split at DSEG chunks into the two segments of an item (the same partials, summed in the same order)
+  auto one = [&](int off, int d0, int d1, int lo, int hi) {
+    const int mid = std::min(hi, lo + DSEG);
+    t.push_back(make_int4(off, off, d0, d1));
+    t.push_back(make_int4(lo, mid, mid, hi));
+  };
+  for (int a = 0; a < nf; a++)  // off-diagonal blocks H[a, c], a < c: partials of host a's chunks (slot c), then of host c's (slot a)
+    for (int c = a + 1; c < nf; c++)
+      for (int ij = 0; ij < 64; ij++) {
+        const int i = ij >> 3, j = ij & 7;
+        t.push_back(make_int4(c * PART_SLOT + i * 8 + j, a * PART_SLOT + j * 8 + i, (4 + 8 * a + i) * N + 4 + 8 * c + j, (4 + 8 * c + j) * N + 4 + 8 * a + i));
+        t.push_back(make_int4(cb[a], cb[a + 1], cb[c], cb[c + 1]));
+      }
+  for (int a = 0; a < nf; a++)
+    for (int ij = 0; ij < 64; ij++) one(a * PART_SLOT + 64 + ij, (4 + 8 * a + (ij >> 3)) * N + 4 + 8 * a + (ij & 7), -1, 0, nch);
+  for (int a = 0; a < nf; a++)
+    for (int ic = 0; ic < 32; ic++) one(a * PART_SLOT + 128 + ic, (4 + 8 * a + (ic >> 2)) * N + (ic & 3), (ic & 3) * N + 4 + 8 * a + (ic >> 2), 0, nch);
+  for (int e = 0; e < nf * 8; e++) one((e >> 3) * PART_SLOT + 160 + (e & 7), N * N + 4 + e, -1, 0, nch);
+  for (int e = 0; e < 16; e++) one(PART_CC + e, (e >> 2) * N + (e & 3), -1, 0, nch);
+  for (int e = 0; e < 4; e++) one(PART_CC + 16 + e, N * N + e, -1, 0, nch);
+  for (int e = 0; e < ACC_MISC - 1; e++) one(PART_MISC + e, N * N + N + b->ntiles * 16 + e, -1, 0, nch);  // the error-flag slot is written on error only
+  b->nditems = (int)t.size() / 2;
+  CK(cudaMemcpyAsync(b->d_dtab, t.data(), sizeof(int4) * t.size(), cudaMemcpyHostToDevice, b->stream));
+  return DMV_OK;
+}
+
 extern "C" {
 
 static int ba_allocate(dmv_ba* b, const dmv_ba_config* cfg);
@@ -277,6 +331,8 @@ int dmv_ba_set_window(dmv_ba* b, int nf, const int* slots) {
   b->ntiles = b->T * (b->T + 1) / 2;
   b->have_adj = b->have_state = b->have_tentative = b->have_committed = false;
   b->npts = b->nres = b->nchunks = 0;
+  b->act_n = -1;
+  b->res_valid = false;
   return DMV_OK;
 }
 
@@ -292,52 +348,11 @@ int dmv_ba_set_points(dmv_ba* b, int npts, const int32_t* host, const float* u, 
   CK(cudaSetDevice(b->device));
   b->npts = npts;
   b->host_of_point.assign(host, host + npts);
-  // one thread per residual (P = 32, fewest instructions) pays off once the window no longer fits one wave of 16-point chunks (measured at
-  // 7 KF / 8000 points: 54 vs 68 us per step); below that the 4-lanes-per-residual shape (P = 16) has the shorter critical path (29.6 vs 37.9 us)
-  if (b->P_auto) b->P = (npts > 16 * b->sms) ? 32 : 16;
-  {
-    int p = 0, c = 0;
-    for (int h = 0; h < MAXF; h++) {
-      b->host_start[h] = p;
-      b->chunk_beg[h] = c;
-      int cnt = 0;
-      while (p < npts && host[p] == h) { p++; cnt++; }
-      c += (cnt + b->P - 1) / b->P;
-    }
-    b->host_start[MAXF] = npts;
-    b->chunk_beg[MAXF] = c;
-    b->nchunks = c;
-  }
-  if (b->nchunks > b->max_chunks) return set_error(DMV_ERR_INVALID, "too many chunks");
-  {  // phase D items of this window shape (ba_fused.cu: fused_reduce), uploaded ahead of the point data below
-    const int nf = b->nf, N = b->N, nch = b->nchunks;
-    const int* cb = b->chunk_beg;
-    std::vector<int4>& t = b->h_dtab;
-    t.clear();
-    // one offset over [lo, hi): split at DSEG chunks into the two segments of an item (the same partials, summed in the same order)
-    auto one = [&](int off, int d0, int d1, int lo, int hi) {
-      const int mid = std::min(hi, lo + DSEG);
-      t.push_back(make_int4(off, off, d0, d1));
-      t.push_back(make_int4(lo, mid, mid, hi));
-    };
-    for (int a = 0; a < nf; a++)  // off-diagonal blocks H[a, c], a < c: partials of host a's chunks (slot c), then of host c's (slot a)
-      for (int c = a + 1; c < nf; c++)
-        for (int ij = 0; ij < 64; ij++) {
-          const int i = ij >> 3, j = ij & 7;
-          t.push_back(make_int4(c * PART_SLOT + i * 8 + j, a * PART_SLOT + j * 8 + i, (4 + 8 * a + i) * N + 4 + 8 * c + j, (4 + 8 * c + j) * N + 4 + 8 * a + i));
-          t.push_back(make_int4(cb[a], cb[a + 1], cb[c], cb[c + 1]));
-        }
-    for (int a = 0; a < nf; a++)
-      for (int ij = 0; ij < 64; ij++) one(a * PART_SLOT + 64 + ij, (4 + 8 * a + (ij >> 3)) * N + 4 + 8 * a + (ij & 7), -1, 0, nch);
-    for (int a = 0; a < nf; a++)
-      for (int ic = 0; ic < 32; ic++) one(a * PART_SLOT + 128 + ic, (4 + 8 * a + (ic >> 2)) * N + (ic & 3), (ic & 3) * N + 4 + 8 * a + (ic >> 2), 0, nch);
-    for (int e = 0; e < nf * 8; e++) one((e >> 3) * PART_SLOT + 160 + (e & 7), N * N + 4 + e, -1, 0, nch);
-    for (int e = 0; e < 16; e++) one(PART_CC + e, (e >> 2) * N + (e & 3), -1, 0, nch);
-    for (int e = 0; e < 4; e++) one(PART_CC + 16 + e, N * N + e, -1, 0, nch);
-    for (int e = 0; e < ACC_MISC - 1; e++) one(PART_MISC + e, N * N + N + b->ntiles * 16 + e, -1, 0, nch);  // the error-flag slot is written on error only
-    b->nditems = (int)t.size() / 2;
-    CK(cudaMemcpyAsync(b->d_dtab, t.data(), sizeof(int4) * t.size(), cudaMemcpyHostToDevice, b->stream));
-  }
+  b->res_valid = false;
+  BAShape shape;
+  dmv_ba_window_shape(b, npts, host, &shape);
+  const int rc = dmv_ba_take_shape(b, &shape);
+  if (rc != DMV_OK) return rc;
   // one pinned staging block, the copies queued back to back, ONE synchronisation (was: seven blocking copies from pageable memory)
   float* s = b->h_scratch;   // >= 8 * MAXF * mp floats
   const size_t n = (size_t)npts;
@@ -370,6 +385,7 @@ int dmv_ba_set_residuals(dmv_ba* b, int nres, const int32_t* point, const int32_
   if (b->npts < 1) return set_error(DMV_ERR_STATE, "dmv_ba_set_points first");
   CK(cudaSetDevice(b->device));
   const size_t ns = (size_t)MAXF * b->mp;
+  b->res_valid = false;
   b->h_st_in.assign(ns, (uint8_t)RES_NONE);
   b->h_en_in.assign(ns, 0.f);
   b->res_slot.resize(nres);
@@ -386,6 +402,7 @@ int dmv_ba_set_residuals(dmv_ba* b, int nres, const int32_t* point, const int32_
     b->res_slot[i] = (int)slot;
   }
   b->nres = nres;
+  b->res_valid = true;
   b->st_in_clean = true;
   for (int i = 0; i < nres; i++)
     if (b->h_st_in[b->res_slot[i]] != RES_IN || b->h_en_in[b->res_slot[i]] != 0.f) { b->st_in_clean = false; break; }

@@ -96,6 +96,14 @@ struct dmv_ba {
   dmv::DevBuf<float> d_act;    // point-activation staging (dmv_ba_activate_points)
   dmv::PinnedBuf<float> h_act;
   int act_cap = 0;             // points the staging layout holds (0 while d_act / h_act may be short of it)
+  int act_n = -1;              // entries of the last activation on this window, whose host, status and res_state h_act holds (-1: none)
+  // window edit (dmv_ba_edit_window, ba_edit.cu): the gather's destinations, swapped with the point arrays and input grids above; its
+  // per-point upload and the carried residuals' compacted states.  Allocated on first use, as a whole
+  dmv::DevBuf<float2> e_uv;
+  dmv::DevBuf<float> e_idepth_zero, e_color, e_weights, e_priorF, e_en_in, e_cen;
+  dmv::DevBuf<uint8_t> e_st_in, e_cst;
+  dmv::DevBuf<int> e_src;
+  bool res_valid = false;      // h_st_in / h_en_in / res_slot describe the current points (dmv_ba_set_residuals or an edit since set_points)
   dmv::DevBuf<float> d_sel;    // activation-selection staging and scratch (dmv_ba_select_activation, ip_select.cu)
   dmv::PinnedBuf<float> h_sel;
   // peer-memory exchange (inside ba_fused_kernel)
@@ -104,6 +112,25 @@ struct dmv_ba {
   int xchg_pitch = 0;
   bool xchg_on = false;
   unsigned int xchg_seq = 0;
+};
+
+// dmv_ba_activate_points' staging (words): RT[64*12] | aff[64*2] | host | u | v | color*8 | weights*8 | energyTH | idmin | idmax | status | idepth |
+// res_state*MAXF | lastTraceStatus (dmv_ba_activate_store only), cap points per array.  [0, st) goes up, status .. res_state come back.
+struct ActLayout {
+  size_t rt, aff, host, u, v, col, wgt, eth, min, max, st, id, rs, ts, words;
+};
+inline ActLayout act_layout(size_t cap) {
+  ActLayout o;
+  o.rt = 0; o.aff = (size_t)MAXF * MAXF * 12; o.host = (size_t)MAXF * MAXF * 14; o.u = o.host + cap; o.v = o.u + cap; o.col = o.v + cap;
+  o.wgt = o.col + 8 * cap; o.eth = o.wgt + 8 * cap; o.min = o.eth + cap; o.max = o.min + cap; o.st = o.max + cap; o.id = o.st + cap; o.rs = o.id + cap;
+  o.ts = o.rs + MAXF * cap; o.words = o.ts + cap;
+  return o;
+}
+
+// chunk shape of a window of points ordered by host frame: P, each host's first point and first chunk (dmv_ba_set_points, dmv_ba_edit_window)
+struct BAShape {
+  int P, nchunks;
+  int host_start[MAXF + 1], chunk_beg[MAXF + 1];
 };
 
 // shared by the product path and the benches (library-internal: hidden from the dynamic symbol table)
@@ -115,3 +142,5 @@ DMV_INTERNAL void dmv_ba_stage_x(dmv_ba* b, const double* x);
 DMV_INTERNAL int dmv_ba_check_ready(dmv_ba* b);
 DMV_INTERNAL int dmv_ba_stage_state(dmv_ba* b, const dmv_ba_state* st);
 DMV_INTERNAL int dmv_ba_finish_linearize(dmv_ba* b, dmv_ba_lin_result* out, double sums[3]);
+DMV_INTERNAL void dmv_ba_window_shape(const dmv_ba* b, int npts, const int32_t* host, BAShape* s);
+DMV_INTERNAL int dmv_ba_take_shape(dmv_ba* b, const BAShape* s);

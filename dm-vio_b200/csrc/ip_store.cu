@@ -339,15 +339,18 @@ int dmv_ba_activate_store(dmv_ba* b, dmv_ip_store* s, const dmv_ba_activate_stor
   for (int f = 0; f < nf; f++)
     for (int i = off[f]; f != a->newest && i < off[f + 1]; i++)
       if (sa.action[i] == DMV_ACT_DELETE) alive[a->slot[f]][i - off[f]] = 0;
+  int32_t* act_host = nopt > 0 ? reinterpret_cast<int32_t*>(b->h_act.get() + act_layout(b->act_cap).host) : nullptr;   // as the gather wrote d_act
   for (int j = 0; j < nopt; j++) {
     const int i = opt[j];
     int f = 0;
     while (off[f + 1] <= i) f++;
+    act_host[j] = f;
     a->opt_frame[j] = f;
     a->opt_index[j] = i - off[f];
     if (a->status[j] != 0 || trace_status[j] == 1) alive[a->slot[f]][i - off[f]] = 0;   // IPS_OOB
   }
   std::vector<int> order[DMV_IP_STORE_SLOTS];
+  b->act_n = nopt;
   rc = ip_store_remove_dead(s, alive, order);
   if (rc != DMV_OK) return rc;
   for (int f = 0, at = 0; f < nf; f++) {

@@ -485,21 +485,9 @@ int ip_trace_launch(dmv_ct* const* hs, const IPTraceArgs& A) {
   return DMV_OK;
 }
 
-// dmv_ba_activate_points' staging (words): RT[64*12] | aff[64*2] | host | u | v | color*8 | weights*8 | energyTH | idmin | idmax | status | idepth |
-// res_state*MAXF | lastTraceStatus (dmv_ba_activate_store only), cap points per array.  [0, st) goes up, status .. res_state come back.
-struct ActLayout {
-  size_t rt, aff, host, u, v, col, wgt, eth, min, max, st, id, rs, ts, words;
-};
-static ActLayout act_layout(size_t cap) {
-  ActLayout o;
-  o.rt = 0; o.aff = (size_t)MAXF * MAXF * 12; o.host = (size_t)MAXF * MAXF * 14; o.u = o.host + cap; o.v = o.u + cap; o.col = o.v + cap;
-  o.wgt = o.col + 8 * cap; o.eth = o.wgt + 8 * cap; o.min = o.eth + cap; o.max = o.min + cap; o.st = o.max + cap; o.id = o.st + cap; o.rs = o.id + cap;
-  o.ts = o.rs + MAXF * cap; o.words = o.ts + cap;
-  return o;
-}
-
 // d_act / h_act hold n points; RT and the window's PRE_aff_mode staged in h_act
 static int act_stage(dmv_ba* b, int n, const float* RT) {
+  b->act_n = -1;   // the staging no longer holds the last activation's entries
   if (n > b->act_cap) {
     b->act_cap = 0;
     const int cap = std::max(n, 2048);
@@ -757,7 +745,10 @@ int dmv_ba_activate_points(dmv_ba* b, const dmv_ba_activate_args* a) {
   if (a->n < 0 || (a->n > 0 && (!a->host || !a->u || !a->v || !a->color8 || !a->weights8 || !a->energyTH || !a->idepth_min || !a->idepth_max || !a->RT ||
                                 !a->status || !a->idepth || !a->res_state)))
     return set_error(DMV_ERR_INVALID, "incomplete dmv_ba_activate_args");
-  if (a->n == 0) return DMV_OK;
+  if (a->n == 0) {
+    b->act_n = 0;
+    return DMV_OK;
+  }
   const int n = a->n, nf = b->nf;
   for (int i = 0; i < n; i++)
     if (a->host[i] < 0 || a->host[i] >= nf) return set_error(DMV_ERR_INVALID, "point %d: host %d out of range", i, a->host[i]);
@@ -770,5 +761,7 @@ int dmv_ba_activate_points(dmv_ba* b, const dmv_ba_activate_args* a) {
   std::memcpy(hb + o.col, a->color8, 32 * (size_t)n); std::memcpy(hb + o.wgt, a->weights8, 32 * (size_t)n); std::memcpy(hb + o.eth, a->energyTH, 4 * (size_t)n);
   std::memcpy(hb + o.min, a->idepth_min, 4 * (size_t)n); std::memcpy(hb + o.max, a->idepth_max, 4 * (size_t)n);
   CK(cudaMemcpyAsync(b->d_act, hb, sizeof(float) * o.st, cudaMemcpyHostToDevice, b->stream));
-  return act_launch(b, n, a->minObs, a->status, a->idepth, a->res_state, nullptr);
+  const int rc2 = act_launch(b, n, a->minObs, a->status, a->idepth, a->res_state, nullptr);
+  if (rc2 == DMV_OK) b->act_n = n;
+  return rc2;
 }

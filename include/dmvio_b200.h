@@ -617,6 +617,42 @@ typedef struct dmv_ba_activate_store_args {
 } dmv_ba_activate_store_args;
 int dmv_ba_activate_store(dmv_ba* ba, dmv_ip_store* s, const dmv_ba_activate_store_args* a);
 
+/* One change of the window's membership (FullSystem::makeKeyFrame's makeIDX points: a frame joins, activated points are inserted, points
+ * and frames leave) made on the window already on the device.  Bit-identical to downloading the state (dmv_ba_get_idepth,
+ * dmv_ba_get_residual_outputs) and re-uploading the whole window with dmv_ba_set_window + dmv_ba_set_points + dmv_ba_set_residuals from
+ * lists built by these rules:
+ *   - carried point (point_src[j] = i >= 0, point i of the current list): host frame remapped through frame_src; u, v, color8, weights8,
+ *     priorF, and idepth / idepth_zero as dmv_ba_get_idepth reports them, kept.
+ *   - activated point (point_src[j] = -1 - k): entry k of the last dmv_ba_activate_points / dmv_ba_activate_store on this window, whose
+ *     status must be 1.  host, u, v, color8, weights8 from that call; idepth = idepth_zero = its idepth, priorF = 0; one IN / 0 residual per
+ *     frame with res_state 0, remapped through frame_src (optimizeImmaturePoint's setIdepthZero / setIdepth, EFPoint::takeData without prior).
+ *   - carried residual: (p, t) is kept when p is carried and t stays; its state and energy are those the next linearisation would read: the
+ *     committed linearisation's state_NewState / state_NewEnergy if there is one, else the input state.  A tentative linearisation is
+ *     discarded (as by dmv_ba_set_points).  Residuals into a frame that leaves are dropped.
+ *   - new_res_target >= 0: every carried point gets an IN / 0 residual into that (new) frame index (makeKeyFrame's residuals of the old
+ *     points into the new keyframe).
+ *   - residual order (dmv_ba_get_residual_outputs): the carried residuals in their current order, then the new_res_target residuals in new
+ *     point order, then the activated points' residuals in new point order, target ascending.
+ * Afterwards the handle is as the three set calls leave it: no linearisation, adjoints and state must be set again, dmv_ba_get_solve_HdiF
+ * refuses, and the chunk shape, host ranges and phase-D table are the new window's; no activation is available to a later edit.  One launch
+ * (the gather; the handle's launch count moves by 1), about 4 + 4 bytes per point up and, when a committed linearisation exists, 5 bytes per
+ * carried residual down; one synchronisation.
+ * Errors, all before any allocation, copy or launch, with the handle unchanged: DMV_ERR_INVALID for NULL ba / a / frame_src / point_src,
+ * nf or a slot outside dmv_ba_set_window's range, frame_src entries outside -1..nf_current-1 or repeated, npts outside 1..max_points,
+ * point_src entries out of range or repeated, an activation entry without an activation on this window, beyond its size or with a status
+ * other than 1, a point whose host frame leaves, points not ordered by host frame, a new_res_target outside -1..nf-1 or equal to a carried
+ * point's host or to a target it already has a residual into, and too many chunks; DMV_ERR_STATE for a sharded handle or a window without
+ * points and residuals. */
+typedef struct dmv_ba_edit_args {
+  int nf;                    /* frames of the new window, as dmv_ba_set_window */
+  const int* slots;          /* nf image slots, as dmv_ba_set_window (NULL: 0..nf-1) */
+  const int32_t* frame_src;  /* nf: the frame's index in the current window, or -1 for a frame that joins */
+  int npts;                  /* points of the new window (ordered by host frame, as dmv_ba_set_points requires) */
+  const int32_t* point_src;  /* npts: index in the current point list (>= 0), or -1 - k for entry k of the last activation */
+  int new_res_target;        /* new frame index: every carried point gets an IN / 0 residual into it, or -1 */
+} dmv_ba_edit_args;
+int dmv_ba_edit_window(dmv_ba* ba, const dmv_ba_edit_args* a);
+
 /* ------------------------------------------------------------------------------------------------
  * New immature points of a keyframe  ==  FullSystem::makeNewTraces (FullSystem.cpp:L1640-1667): PixelSelector::makeMaps
  * (FullSystem/PixelSelector2.cpp:L158-307) on the handle's RESIDENT frame (the one last given to dmv_ct_upload_new_image /
