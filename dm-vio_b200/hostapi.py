@@ -119,9 +119,10 @@ ALLGATHER_CB = C.CFUNCTYPE(None, C.c_void_p, C.c_void_p, C.c_size_t, C.c_void_p)
 class WindowBA:
     """dmvio_b200::WindowBA loaded from a synth.make_window() dict."""
 
-    def __init__(self, W, device=0, use_device_pyramid=False, shard=None):
+    def __init__(self, W, device=0, use_device_pyramid=False, shard=None, settings=None):
         """shard (multi-GPU, one WindowBA per rank): dict(rank, nranks, allgather=f(bytes) -> bytes of all ranks in rank order,
-        exchange="p2p" | "nccl", uid=NCCL unique id for "nccl").  Every rank passes the SAME window."""
+        exchange="p2p" | "nccl", uid=NCCL unique id for "nccl").  Every rank passes the SAME window.  settings: {name: value} for
+        dmvh_window_set_setting, applied before the window is prepared (its BA parameters reach the device there)."""
         self.L = lib()
         self.nf, self.npts, self.nres = W["nf"], len(W["host"]), len(W["res_point"])
         self.N = 8 * self.nf + 4
@@ -147,6 +148,9 @@ class WindowBA:
             rc = self.L.dmvh_window_comm_init(self.h, shard["uid"]) if shard.get("exchange", "p2p") == "nccl" else self.L.dmvh_window_p2p_setup(self.h)
             if rc != 0:
                 raise capi.DmvError(self.L.dmvh_window_error(self.h).decode())
+        for k, v in (settings or {}).items():
+            if self.L.dmvh_window_set_setting(self.h, k.encode(), float(v)) != 0:
+                raise ValueError(f"unknown WindowBA setting {k}")
         if self.L.dmvh_window_prepare(self.h) != 0:
             raise capi.DmvError(self.L.dmvh_window_error(self.h).decode())
 

@@ -101,7 +101,7 @@ def _declare(L):
     L.orc_ct_calc_gs.argtypes = [vp, C.c_int, C.c_double, C.c_double, C.c_int, f64p, f64p]
     L.orc_ct_track.argtypes = [vp, f64p, f64p, C.POINTER(C.c_double), C.POINTER(C.c_double), C.c_int, f64p, C.c_int, f64p, f64p, C.POINTER(C.c_int)]
     L.orc_ip_activate.argtypes = [C.c_int, C.c_int, C.c_int, C.c_int, f32p, f32p, f32p, f32p, i32p, f32p, f32p, f32p, f32p, f32p, f32p, f32p, C.c_int,
-                                  i32p, f32p, i32p]
+                                  C.c_float, i32p, f32p, i32p]
     L.orc_ip_init.argtypes = [C.c_int, f32p, C.c_int, C.c_int, i32p, i32p, f32p, f32p, f32p, f32p, u8p]
     L.orc_ip_trace.argtypes = [C.c_int, f32p, C.c_int, C.c_int, f32p, f32p, f32p, f32p, f32p, f32p, f32p, f32p, f32p, f32p, f32p, f32p, i32p, f32p, f32p]
     L.orc_ip_trace_diag.argtypes = L.orc_ip_trace.argtypes + [i32p]
@@ -444,9 +444,9 @@ def ip_trace(P, dI, w, h, KRKi, Kt, aff, _fn=None, diag=False):
     return Q
 
 
-def ip_activate(W, RT, aff, calib6, host, P, minObs=1):
+def ip_activate(W, RT, aff, calib6, host, P, minObs=1, huberTH=9.0):
     """FullSystem::optimizeImmaturePoint for the immature points P (dict as ip_init / ip_trace) hosted in frames `host` of the window W.
-    RT: (nf*nf, 12), aff: (nf*nf, 2), calib6 = fxl fyl cxl cyl fxli fyli.  Returns status (1/0/-1), idepth, res_state (n, nf)."""
+    RT: (nf*nf, 12), aff: (nf*nf, 2), calib6 = fxl fyl cxl cyl fxli fyli, huberTH = setting_huberTH.  Returns status (1/0/-1), idepth, res_state (n, nf)."""
     nf, w, h = W["nf"], W["w"], W["h"]
     n = len(P["u"])
     c = lambda a, t: np.ascontiguousarray(a, t)
@@ -454,7 +454,7 @@ def ip_activate(W, RT, aff, calib6, host, P, minObs=1):
     status = np.zeros(n, np.int32); idepth = np.zeros(n, np.float32); rs = np.zeros((n, nf), np.int32)
     lib().orc_ip_activate(n, nf, w, h, c(calib6, np.float32), dI_all.reshape(-1), c(RT, np.float32).reshape(-1), c(aff, np.float32).reshape(-1),
                           c(host, np.int32), P["u"], P["v"], P["color"], P["weights"], P["energyTH"], c(P["idepth_min"], np.float32),
-                          c(P["idepth_max"], np.float32), int(minObs), status, idepth, rs.reshape(-1))
+                          c(P["idepth_max"], np.float32), int(minObs), float(huberTH), status, idepth, rs.reshape(-1))
     return status, idepth, rs
 
 

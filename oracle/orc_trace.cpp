@@ -392,7 +392,8 @@ static int optimizeImmaturePoint(const ActFrameTables& F, int host, float pu, fl
 
 extern "C" void orc_ip_activate(int n, int nf, int w, int h, const float calib6[6], const float* dI_all, const float* RT, const float* aff,
                                 const int32_t* host, const float* u, const float* v, const float* color8, const float* weights8, const float* energyTH,
-                                const float* idepth_min, const float* idepth_max, int minObs, int32_t* status, float* idepth, int32_t* res_state) {
+                                const float* idepth_min, const float* idepth_max, int minObs, float huberTH, int32_t* status, float* idepth,
+                                int32_t* res_state) {
   orc::ActFrameTables F;
   F.nf = nf; F.w = w; F.h = h;
   F.fxl = calib6[0]; F.fyl = calib6[1]; F.cxl = calib6[2]; F.cyl = calib6[3]; F.fxli = calib6[4]; F.fyli = calib6[5];
@@ -400,6 +401,6 @@ extern "C" void orc_ip_activate(int n, int nf, int w, int h, const float calib6[
   for (int f = 0; f < nf; f++) planes[f] = dI_all + (size_t)f * w * h * 3;
   F.dI = planes; F.RT = RT; F.aff = aff;
   for (int i = 0; i < n; i++)
-    status[i] = orc::optimizeImmaturePoint(F, host[i], u[i], v[i], color8 + 8 * i, weights8 + 8 * i, energyTH[i], idepth_min[i], idepth_max[i], minObs, 9.f,
+    status[i] = orc::optimizeImmaturePoint(F, host[i], u[i], v[i], color8 + 8 * i, weights8 + 8 * i, energyTH[i], idepth_min[i], idepth_max[i], minObs, huberTH,
                                            100.f, 3, idepth + i, res_state + (size_t)i * nf);
 }

@@ -78,8 +78,9 @@ void orc_ip_trace_diag(int n, const float* dI, int w, int h, const float* KRKi9,
 extern "C" {
 // FullSystem::optimizeImmaturePoint for n immature points of a window: dI_all = nf planes (w*h*3 each); RT[h*nf+t][12] = PRE_RTll (row-major) | PRE_tTll;
 // aff[h*nf+t][2] = PRE_aff_mode; calib6 = fxl fyl cxl cyl fxli fyli.  status: 1 activated, 0 skipped (not well constrained), -1 outlier;
-// idepth: the optimised inverse depth; res_state[i*nf + f]: 0 IN, 1 OOB, 2 OUTLIER, 255 no residual (f == host or early exit).
+// huberTH: setting_huberTH (9 in DSO's defaults); idepth: the optimised inverse depth; res_state[i*nf + f]: 0 IN, 1 OOB, 2 OUTLIER, 255 no residual
+// (f == host or early exit).
 void orc_ip_activate(int n, int nf, int w, int h, const float calib6[6], const float* dI_all, const float* RT, const float* aff, const int32_t* host,
                      const float* u, const float* v, const float* color8, const float* weights8, const float* energyTH, const float* idepth_min,
-                     const float* idepth_max, int minObs, int32_t* status, float* idepth, int32_t* res_state);
+                     const float* idepth_max, int minObs, float huberTH, int32_t* status, float* idepth, int32_t* res_state);
 }

@@ -623,6 +623,12 @@ def track_ref(sc, R0, t0, a0, b0, ref_a=0.0, ref_b=0.0, ref_exposure=1.0, new_ex
 CT_AFF = dict(R0=None, a0=0.6, b0=4.5, ref_a=0.1, ref_b=3.0, ref_exposure=1.3, new_exposure=0.8)
 CT_MODES = dict(free=(1e12, 1e8), fixA=(-1.0, 1e8), fixB=(1e12, -1.0), fixAB=(-1.0, -1.0))
 CT_SCENES = ["bench", "aff_free", "aff_fixA", "aff_fixB", "aff_fixAB", "tma0_80x60", "tma0_160x120", "limit", "odd", "wide", "stream", "repeat"]
+# scenes whose new frame is lit differently from the keyframe: (gain, offset, arguments).  The new planes are intensity * gain + offset,
+# gradients * gain.  aff_zeroA / aff_zeroB: the exposures (ref_b) predict the change, so a, b stay near 0 and the default modes' tests
+# |a| > 1.2, |b| > 200 pass, while mode 0's |log ra| = log 5 > 1.5 and |rb| = 250 > 200 fail.  aff_bigA: gain 4 the exposures do not
+# predict, so a ends near log 4 = 1.39: the default mode's |a| > 1.2 fails and mode 0's |log ra| < 1.5 passes
+CT_LIGHT = dict(aff_zeroA=(5.0, 0.0, dict(new_exposure=5.0, affA=0.0)), aff_zeroB=(1.0, 250.0, dict(ref_b=-250.0, affB=0.0)),
+                aff_bigA=(4.0, 0.0, dict(a0=float(np.log(4.0)) - 0.05)))
 
 
 def _ct_random_points(T, n, seed):
@@ -655,7 +661,11 @@ def ct_scene(orc, synth, name, npts=None):
     args = dict(R0=np.eye(3), t0=np.zeros(3), a0=0.0, b0=0.0, ref_a=0.0, ref_b=0.0, ref_exposure=1.0, new_exposure=1.0, affA=1e12, affB=1e8)
     geo = dict(bench=(640, 480, 5, 4321), repeat=(640, 480, 5, 4321), tma0_80x60=(80, 60, 1, 11), tma0_160x120=(160, 120, 2, 12),
                limit=(256, 80, 2, 13), odd=(752, 480, 5, 20), wide=(640, 96, 3, 15))
-    if name.startswith("aff_"):
+    if name in CT_LIGHT:
+        w, h, L, seed = 640, 480, 4, 99
+        args["R0"], args["t0"] = synth.se3_exp(np.array([0.005, -0.004, 0.003, 0.002, -0.001, 0.002]))
+        args.update(CT_LIGHT[name][2])
+    elif name.startswith("aff_"):
         w, h, L, seed = 640, 480, 4, 99
         args.update({k: v for k, v in CT_AFF.items() if k != "R0"})
         args["R0"], args["t0"] = synth.se3_exp(np.array([0.005, -0.004, 0.003, 0.002, -0.001, 0.002]))
@@ -676,7 +686,13 @@ def ct_scene(orc, synth, name, npts=None):
     if name == "repeat":
         args["b0"] = -21.0
     k4 = [oc.K(l)[0] for l in range(L)]
-    return dict(name=name, w=w, h=h, levels=L, K=T["K"], pts=pts, planes=T["pyr_new"], k4=k4, Ki=[ct_Ki(k) for k in k4], args=args, T=T)
+    planes = T["pyr_new"]
+    if name in CT_LIGHT:
+        gain, offset, _ = CT_LIGHT[name]
+        planes = [np.asarray(p, np.float32) * np.float32(gain) for p in planes]
+        for p in planes:
+            p[..., 0] += np.float32(offset)
+    return dict(name=name, w=w, h=h, levels=L, K=T["K"], pts=pts, planes=planes, k4=k4, Ki=[ct_Ki(k) for k in k4], args=args, T=T)
 
 
 def ct_oracle(orc, sc):

@@ -151,18 +151,21 @@ def test_batched_windows_identical_to_single_launches_chunk32(capi, orc, synth):
     _batched_vs_single_launches(capi, orc, synth, P=32)
 
 
-def _batched_vs_single_launches(capi, orc, synth, P):
+def _batched_vs_single_launches(capi, orc, synth, P, params=None):
+    """params: one dmv_ba_set_params keyword dict per window (None: every window at the defaults)"""
     import dmvio_b200.hostmath as hm
     cfgs = [dict(nf=7, npts=2000, seed=1234), dict(nf=4, npts=333, seed=5), dict(nf=8, npts=777, seed=99, hosts="all", edge=True),
             dict(nf=2, npts=200, seed=3, hosts="first")]
     Ws = [make_case(synth, c) for c in cfgs]
+    params = params or [{}] * len(Ws)
 
-    def load(W):
+    def load(W, prm):
         ow = orc.Window(W)
         ba = product_ba_from_oracle(capi, W, ow, chunk_points=P)
+        ba.set_params(**prm)
         return ba, (ow.calib()["k8"], ow.precalc(), ow.frame_tables()["frameEnergyTH"])
 
-    singles, batched = [load(W) for W in Ws], [load(W) for W in Ws]
+    singles, batched = [load(W, p) for W, p in zip(Ws, params)], [load(W, p) for W, p in zip(Ws, params)]
     batch = capi.BABatch([b for b, _ in batched])
     keys = ("HA", "bA", "Hsc", "bsc")
     # ---- first linearisation

@@ -45,15 +45,17 @@ class Level:
         g.set_points(lvl, self.u, self.v, self.th)
 
 
-def _eval(L, st, synth, sms, worst, tag, wzp=(0.0, 0.0)):
-    """one launch against ci_calc_ref: every exact check and every bounded one; worst collects the largest |err|/bound per quantity"""
+def _eval(L, st, synth, sms, worst, tag, wzp=(0.0, 0.0), huber=9.0):
+    """one launch against ci_calc_ref at the Huber threshold `huber`: every exact check and every bounded one; worst collects the largest
+    |err|/bound per quantity"""
     R, t, RKi, tlog = ci_operands(synth, L.k4, st)
     aff = (np.float32(np.exp(st["a"])), np.float32(st["b"]))
     n = L.n
-    sg = L.g.calc_res_and_gs(L.lvl, RKi, t, tlog, aff, st["idepth_new"], st["isGood"], st["energy"], st["iR"], wzpx=wzp[0], wzpy=wzp[1])
+    sg = L.g.calc_res_and_gs(L.lvl, RKi, t, tlog, aff, st["idepth_new"], st["isGood"], st["energy"], st["iR"], huberTH=huber, wzpx=wzp[0],
+                             wzpy=wzp[1])
     good = sg["isGood_new"] != 0
     ref = ci_calc_ref(L.first, L.new, L.k4, L.u, L.v, L.th, st["idepth_new"], st["isGood"], st["energy"], st["iR"], RKi, t, tlog, aff,
-                      wzp=wzp, depth=ci_kernel_depth(n, sms), verdict=good)
+                      huber=huber, wzp=wzp, depth=ci_kernel_depth(n, sms), verdict=good)
     sure = ~ref["amb"]
     assert np.array_equal(good[sure], ref["isGood_new"][sure]), (tag, np.nonzero(good[sure] != ref["isGood_new"][sure])[0][:10])
     np.testing.assert_array_equal(sg["energy_new"][~good], st["energy"][~good], err_msg=tag)

@@ -31,9 +31,17 @@ def _case(synth, orc, cfg, frac):
                                         (dict(nf=8, npts=777, seed=99, hosts="all"), 0.1, 32), (dict(nf=3, npts=333, seed=7), 1.0, 16)],
                          ids=["nf7_n2000_third", "nf4_n400_half", "nf8_n777_tenth", "nf3_n333_all"])
 def test_marginalize_points_parity(capi, orc, synth, cfg, frac, P):
+    marginalize_parity(capi, orc, synth, cfg, frac, P)
+
+
+def marginalize_parity(capi, orc, synth, cfg, frac, P, settings=None):
+    """the launch against the oracle on _case(cfg, frac), both at `settings` (dmv_ba_set_params keywords; None: the defaults).  Returns the
+    launch's result."""
     W, pts = _case(synth, orc, cfg, frac)
-    ow = orc.Window(W)
+    ow = orc.Window(W, settings=settings)
     ba = product_ba_from_oracle(capi, W, ow, chunk_points=P)   # carries the points' priorF (hasDepthPrior)
+    if settings:
+        ba.set_params(**settings)
     # a committed linearisation exists in real use (the window has just been optimised): the marginalisation must not disturb it
     ba.linearize(); ba.apply_res()
     before = ba.accumulate()
@@ -68,6 +76,7 @@ def test_marginalize_points_parity(capi, orc, synth, cfg, frac, P):
     print(f"check_system vs oracle: worst |error| / Jacobi scale: M {r[0]:.2e} Mb {r[1]:.2e} Msc {r[2]:.2e} Mbsc {r[3]:.2e}")
     assert np.allclose(g["M"], g["M"].T) and np.allclose(g["Msc"], g["Msc"].T, rtol=1e-12, atol=0)
     ba.close()
+    return g
 
 
 def test_marginalize_empty_and_errors(capi, orc, synth):
