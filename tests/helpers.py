@@ -63,6 +63,228 @@ def edge_window(synth, cfg, seed_offset=101):
     return W
 
 
+HARD_LABELS = ("none", "nan", "flat", "border", "behind")
+HARD_DESIGNED = dict(nan=RES_OOB, flat=RES_OUTLIER, border=RES_OOB, behind=RES_OOB)   # the state each exit of PointFrameResidual::linearize gives
+HARD_MARGIN = 1e-3      # px: no projected coordinate of a labelled residual lies closer than this to a bound or a texel boundary
+
+
+def make_images_level0(img):
+    """FrameHessian::makeImages' level 0 (HessianBlocks.cpp:L169-179) of an intensity image: [I, dx, dy] with central differences on the flat
+    pixel index (row ends wrap into the neighbouring rows), a non-finite gradient set to 0, the first and last rows' gradients 0"""
+    import dmvio_b200.synth as synth
+    with np.errstate(invalid="ignore"):
+        d = synth.make_pyramid(img, 1)[0].copy()
+    d[..., 1:][~np.isfinite(d[..., 1:])] = 0.0
+    return d
+
+
+def _plane_coords(synth, W, k, D=2.0, tex_size=1536):
+    """texture coordinates (s, t) of frame k's pixels on synth.make_window's world plane Z = D, and their depths, at the pose the frame's
+    state gives (exp(state[:6]) * evalPT: within 1e-3 of the pose it was rendered at)"""
+    w, h = W["w"], W["h"]
+    fx, fy, cx, cy = W["K"]
+    R, t = synth.se3_mul(*synth.se3_exp(W["state"][k, :6]), W["R_eval"][k], W["t_eval"][k])
+    ys, xs = np.mgrid[0:h, 0:w].astype(np.float64)
+    rw = np.stack([(xs - cx) / fx, (ys - cy) / fy, np.ones_like(xs)], axis=-1) @ R
+    cw = -R.T @ t
+    lam = (D - cw[2]) / rw[..., 2]
+    tpu = fx / D
+    return (cw[0] + lam * rw[..., 0]) * tpu + tex_size / 2, (cw[1] + lam * rw[..., 1]) * tpu + tex_size / 2, lam
+
+
+def hard_labels(W, pc):
+    """Per residual, in fp64 from the fp32 tables pc (orc.Window.precalc(), pair h * nf + t) and the window's dI, which exit of
+    PointFrameResidual::linearize (Residuals.cpp:L108-273) it takes, in the reference's order:
+      behind  the FEJ centre (idepth_zero) has drescale <= 0;
+      border  the centre or one of the 8 pattern pixels (idepth) projects outside 1.1 < Ku < w - 3, 1.1 < Kv < h - 3;
+      nan     a pattern sample's 2x2 bilinear footprint holds a non-finite intensity;
+      flat    every footprint texel has zero gradient: wJI2_sum = 0 < 2;
+      none    none of these.
+    Returns (labels, tie, foot): tie marks residuals with a deciding coordinate within HARD_MARGIN of its bound, or a sample within
+    HARD_MARGIN of a texel boundary next to a non-finite texel; foot[i, j] is sample j's top-left footprint texel (x, y)."""
+    import dmvio_b200.synth as synth
+    w, h, nf = W["w"], W["h"], W["nf"]
+    fx, fy, cx, cy = (float(np.float32(k)) for k in W["K"])
+    rp, rt = np.asarray(W["res_point"]), np.asarray(W["res_target"])
+    hh = np.asarray(W["host"])[rp]
+    T = np.asarray(pc, np.float32).astype(np.float64)[hh * nf + rt]
+    u, v = (np.asarray(W[k], np.float32).astype(np.float64)[rp] for k in ("u", "v"))
+    idp, idz = (np.asarray(W[k], np.float32).astype(np.float64)[rp] for k in ("idepth", "idepth_zero"))
+    lo, hu, hv = 1.1, w - 3.0, h - 3.0
+    Kl0, Kl1 = (u - cx) / fx, (v - cy) / fy
+    q2 = T[:, 18] * Kl0 + T[:, 19] * Kl1 + T[:, 20] + T[:, 23] * idz
+    with np.errstate(divide="ignore", invalid="ignore"):
+        cKu = (T[:, 12] * Kl0 + T[:, 13] * Kl1 + T[:, 14] + T[:, 21] * idz) / q2 * fx + cx
+        cKv = (T[:, 15] * Kl0 + T[:, 16] * Kl1 + T[:, 17] + T[:, 22] * idz) / q2 * fy + cy
+    pu = u[:, None] + synth.PATTERN[None, :, 0]
+    pv = v[:, None] + synth.PATTERN[None, :, 1]
+    r2 = T[:, 6:7] * pu + T[:, 7:8] * pv + T[:, 8:9] + T[:, 11:12] * idp[:, None]
+    Ku = (T[:, 0:1] * pu + T[:, 1:2] * pv + T[:, 2:3] + T[:, 9:10] * idp[:, None]) / r2
+    Kv = (T[:, 3:4] * pu + T[:, 4:5] * pv + T[:, 5:6] + T[:, 10:11] * idp[:, None]) / r2
+
+    def inside(a, b):
+        return (a > lo) & (b > lo) & (a < hu) & (b < hv)
+
+    def near(a):
+        return (np.abs(a - lo) < HARD_MARGIN) | (np.abs(a - hu) < HARD_MARGIN) | (np.abs(a - hv) < HARD_MARGIN)
+
+    behind = ~(q2 > 0)
+    c_in = inside(cKu, cKv)
+    p_in = inside(Ku, Kv).all(1)
+    border = ~behind & ~(c_in & p_in)
+    tie = np.abs(q2) < 1e-4
+    tie |= ~behind & (near(cKu) | near(cKv) | near(Ku).any(1) | near(Kv).any(1))
+    # footprints of the samples of the residuals that project inside
+    ok = ~behind & ~border
+    ix = np.where(ok[:, None], np.floor(Ku), 2).astype(np.int64)
+    iy = np.where(ok[:, None], np.floor(Kv), 2).astype(np.int64)
+    nan, flat = np.zeros(len(rp), bool), np.ones(len(rp), bool)
+    for t in range(nf):
+        m = rt == t
+        if not m.any():
+            continue
+        dI = np.asarray(W["dI"][t], np.float32).reshape(h, w, 3)
+        bad = ~np.isfinite(dI[..., 0])
+        grad0 = (dI[..., 1] == 0) & (dI[..., 2] == 0)
+        x, y = ix[m], iy[m]
+        taps = [(y, x), (y, x + 1), (y + 1, x), (y + 1, x + 1)]
+        nan[m] = np.any([bad[a, b] for a, b in taps], axis=0).any(1)
+        flat[m] = np.all([grad0[a, b] for a, b in taps], axis=0).all(1)
+        # a sample within HARD_MARGIN of a texel boundary next to a non-finite texel: fp32 may take the neighbouring footprint
+        fu, fv = Ku[m] - x, Kv[m] - y
+        edge = (np.minimum(fu, 1 - fu) < HARD_MARGIN) | (np.minimum(fv, 1 - fv) < HARD_MARGIN)
+        pad = np.pad(bad, 1)
+        near_bad = np.any([pad[y + 1 + a, x + 1 + b] for a in range(-1, 3) for b in range(-1, 3)], axis=0)
+        tie[m] |= ok[m] & (edge & near_bad).any(1)
+    labels = np.full(len(rp), "none", dtype="<U6")
+    labels[ok & flat] = "flat"
+    labels[ok & nan] = "nan"
+    labels[border] = "border"
+    labels[behind] = "behind"
+    return labels, tie, np.stack([ix, iy], -1)
+
+
+def hard_window(synth, orc, cfg, seed_offset=202):
+    """edge_window(cfg) with what real sequences bring and synth.make_window never does (labels of every residual: hard_labels):
+      * lighting: exposures in [0.6, 1.6], affine a in [-0.3, 0.3] and b in [-30, 30]; frame k is rendered as e_k exp(a_k) tex + b_k
+        (AffLight::fromToVecExposure's model) and clipped to [0, 255], so that 3-7 % of the pixels saturate into flat bright areas;
+      * two flat squares of the world plane (tex = 128): zero gradient wherever they are seen, in every frame;
+      * in the targets 1 .. nf-1: a NaN block, a NaN row, a +inf column and single NaN texels, each in the footprint of exactly one pattern
+        sample j of some residual, for every j in 0..7 (the LPR = 4 launch: one lane of the four sees it);
+      * points 2-4 px from each border (half of them with idepth_zero far from idepth, so that the centre and the pattern disagree),
+        points whose idepth_zero puts the FEJ centre behind the camera (inside the image, so only drescale > 0 rejects it) while idepth > 0,
+        points with idepth = 0 and with idepth < 0.
+    Host colours and weights come from the clean relit images; W["images"] holds the intensities (NaN, inf included) and W["dI"] their
+    makeImages level 0.  A residual with a deciding coordinate within HARD_MARGIN px of its bound enters as OOB (none is expected).
+    Adds W["labels"], W["single_nan"] (residual, sample j) pairs and W["hard_points"] (border, reverse, behind, zero, negative)."""
+    W = edge_window(synth, cfg)
+    rng = np.random.default_rng(cfg["seed"] + seed_offset)
+    w, h, nf = W["w"], W["h"], W["nf"]
+    npts = len(W["host"])
+    # ---- lighting
+    e = rng.uniform(0.6, 1.6, nf).astype(np.float32)
+    A, B = rng.uniform(-0.3, 0.3, nf), rng.uniform(-30, 30, nf)
+    dz = W["state_zero"][:, 6:8] - W["state"][:, 6:8]
+    flat = rng.uniform(700, 836, (2, 2))      # texture coordinates of the flat squares' centres: in view of every frame
+    for k in range(nf):
+        a0, b0 = W["state"][k, 6] * synth.SCALE_A, W["state"][k, 7] * synth.SCALE_B
+        T = (W["images"][k].astype(np.float64) - b0) / np.exp(a0)
+        s, t, _ = _plane_coords(synth, W, k)
+        for (sc, tc) in flat:
+            T[(np.abs(s - sc) < 40) & (np.abs(t - tc) < 40)] = 128.0
+        W["images"][k] = np.clip(float(e[k]) * np.exp(A[k]) * T + B[k], 0, 255).astype(np.float32)
+    W["exposure"] = e
+    W["state"][:, 6], W["state"][:, 7] = A / synth.SCALE_A, B / synth.SCALE_B
+    W["state_zero"][:, 6:8] = W["state"][:, 6:8] + dz
+    # ---- geometry: border points (and their depth on the plane), idepth = 0 and < 0
+    host = W["host"]
+    cand = rng.permutation(npts)
+    nb = max(8, npts // 12)
+    border, behind_c, zero, neg = cand[:nb], cand[nb:2 * nb], cand[2 * nb:2 * nb + npts // 100 + 2], cand[2 * nb + npts // 100 + 2:2 * nb + npts // 50 + 4]
+    side = rng.integers(0, 4, nb)
+    dist = rng.integers(2, 5, nb)
+    u, v = W["u"], W["v"]
+    u[border] = np.where(side == 0, dist, np.where(side == 1, np.minimum(w - 1 - dist, w - 4), u[border]))
+    v[border] = np.where(side == 2, dist, np.where(side == 3, np.minimum(h - 1 - dist, h - 4), v[border]))
+    depth = {k: _plane_coords(synth, W, k)[2] for k in np.unique(host[border])}
+    for p in border:
+        W["idepth"][p] = np.float32(1.0 / depth[host[p]][int(v[p]), int(u[p])] * (1 + 1e-2 * rng.standard_normal()))
+    W["idepth_zero"][border] = W["idepth"][border]
+    reverse = border[::2]
+    W["idepth_zero"][reverse] = (W["idepth"][reverse] * rng.uniform(0.3, 1.7, len(reverse))).astype(np.float32)
+    W["idepth"][zero] = 0.0
+    W["idepth_zero"][zero] = 0.0
+    W["idepth"][neg] = -rng.uniform(0.02, 0.2, len(neg)).astype(np.float32)
+    W["idepth_zero"][neg] = W["idepth"][neg]
+    # ---- host colours and weights from the clean relit images (makeImages' level 0: [I, dx, dy])
+    clean = [make_images_level0(img) for img in W["images"]]
+    for k in range(nf):
+        m = host == k
+        for j in range(8):
+            c, gx, gy = synth.interp33_bilin(clean[k], u[m] + synth.PATTERN[j, 0], v[m] + synth.PATTERN[j, 1])
+            W["color"][m, j] = c
+            W["weights"][m, j] = np.sqrt(np.float32(2500.0) / (np.float32(2500.0) + gx * gx + gy * gy))
+    W["dI"] = [d.reshape(-1).copy() for d in clean]
+    pc = orc.Window(W).precalc()       # the tables depend on the frames alone: points and images may change below
+    # ---- FEJ centre behind the camera: idepth_zero on the far side of q2 = 0 for one target, the centre still inside the image
+    fx, fy, cx, cy = (float(k) for k in W["K"])
+
+    def behind_idz(p):
+        Kl = np.array([(u[p] - cx) / fx, (v[p] - cy) / fy, 1.0])
+        for t in rng.permutation(nf):
+            T = pc[host[p] * nf + t].astype(np.float64)
+            a2, b2 = T[18:21] @ Kl, T[23]
+            if t == host[p] or abs(b2) < 1e-3:
+                continue
+            for s in (0.05, 0.1, 0.2, 0.5, 1.0, 2.0, 5.0):
+                z = -(a2 + s) / b2                            # q2 = -s
+                cu = -(T[12:15] @ Kl + T[21] * z) / s * fx + cx
+                cv = -(T[15:18] @ Kl + T[22] * z) / s * fy + cy
+                if 3 < cu < w - 5 and 3 < cv < h - 5:
+                    return z
+        return None
+
+    behind = []
+    for p in behind_c:
+        z = behind_idz(p)
+        if z is not None:
+            W["idepth_zero"][p] = np.float32(z)
+            behind.append(p)
+    behind = np.array(behind, np.int64)
+    # ---- non-finite texels in the targets 1 .. nf-1
+    for k in range(1, nf):
+        img = W["images"][k]
+        y0, x0 = rng.integers(20, h - 80), rng.integers(20, w - 100)
+        img[y0:y0 + 40, x0:x0 + 60] = np.nan
+        img[rng.integers(20, h - 20), :] = np.nan
+        img[:, rng.integers(20, w - 20)] = np.inf
+    W["dI"] = [make_images_level0(img).reshape(-1) for img in W["images"]]
+    labels, tie, foot = hard_labels(W, pc)
+    # single NaN texels: sample j of a residual that has no other exit, at a texel of j's footprint no other sample of it reads
+    st = W["res_state"]
+    single = []
+    free = np.nonzero((labels == "none") & ~tie & (st != RES_OOB) & (W["res_target"] > 0))[0]
+    for j in range(8):
+        for i in rng.permutation(free)[:40]:
+            if sum(1 for (_, jj) in single if jj == j) >= 4:
+                break
+            x, y = foot[i, j]
+            others = {(int(a) + da, int(b) + db) for jj, (a, b) in enumerate(foot[i]) if jj != j for da in (0, 1) for db in (0, 1)}
+            texels = [(int(x) + da, int(y) + db) for da in (0, 1) for db in (0, 1) if (int(x) + da, int(y) + db) not in others]
+            if not texels:
+                continue
+            tx, ty = texels[int(rng.integers(0, len(texels)))]
+            W["images"][W["res_target"][i]][ty, tx] = np.nan
+            single.append((int(i), j))
+            free = free[free != i]
+    W["dI"] = [make_images_level0(img).reshape(-1) for img in W["images"]]
+    labels, tie, foot = hard_labels(W, pc)
+    st[tie] = RES_OOB
+    W["labels"], W["single_nan"] = labels, np.array(single, np.int64)
+    W["hard_points"] = dict(border=np.sort(border), reverse=np.sort(reverse), behind=np.sort(behind), zero=np.sort(zero), negative=np.sort(neg))
+    return W
+
+
 def make_case(synth, cfg):
     """a CONFIGS entry -> window: plain synth.make_window, or edge_window when the entry carries edge=True"""
     cfg = dict(cfg)

@@ -51,7 +51,11 @@ def test_schur_against_fp64(capi, orc, synth, cfg, P):
       * phase E: HdiF * v_i (u), times v_j (u), per-thread fp32 sums over m = ceil(npts / TPB) points (m u), TPB = 448 (P = 16) or 224
         (P = 32), then the 5-step fp32 butterfly (5 u), then fp64 across warps (< u);
     so |error| <= (15 + 15 + 1 + 1 + m + 5 + 1) u Habs = (m + 38) / 2 eps32 Habs (first order)."""
-    W = make_case(synth, cfg)
+    schur_against_fp64(capi, orc, make_case(synth, cfg), P, sys_id(cfg))
+
+
+def schur_against_fp64(capi, orc, W, P, name):
+    """test_schur_against_fp64 on the window W"""
     ow = orc.Window(W)
     ba = product_ba_from_oracle(capi, W, ow, chunk_points=P)
     ba.linearize()
@@ -64,7 +68,7 @@ def test_schur_against_fp64(capi, orc, synth, cfg, P):
     rH = check_bound(a["Hsc"], Hsc, gamma * EPS32 * Habs, "H_sc")
     rb = check_bound(a["bsc"], bsc, gamma * EPS32 * babs, "b_sc")
     jH, jb = check_system(a["Hsc"], a["bsc"], Hsc, bsc, schur_bound(po["HdiF"], po["bdSumF"]), 1.0, "Schur system vs fp64")  # reported only
-    print(f"P={P} {sys_id(cfg)}: H_sc |err|/bound {rH:.3f}  b_sc {rb:.3f}  (gamma {gamma}); Jacobi-scaled H {jH:.2e} b {jb:.2e}")
+    print(f"P={P} {name}: H_sc |err|/bound {rH:.3f}  b_sc {rb:.3f}  (gamma {gamma}); Jacobi-scaled H {jH:.2e} b {jb:.2e}")
     assert np.abs(Hsc).max() > 0
     ba.close()
 

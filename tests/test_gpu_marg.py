@@ -34,10 +34,11 @@ def test_marginalize_points_parity(capi, orc, synth, cfg, frac, P):
     marginalize_parity(capi, orc, synth, cfg, frac, P)
 
 
-def marginalize_parity(capi, orc, synth, cfg, frac, P, settings=None):
-    """the launch against the oracle on _case(cfg, frac), both at `settings` (dmv_ba_set_params keywords; None: the defaults).  Returns the
-    launch's result."""
-    W, pts = _case(synth, orc, cfg, frac)
+def marginalize_parity(capi, orc, synth, cfg, frac, P, settings=None, W=None, pts=None):
+    """the launch against the oracle on _case(cfg, frac), or on the window W flagging the points pts, both at `settings` (dmv_ba_set_params
+    keywords; None: the defaults).  Returns the launch's result."""
+    if W is None:
+        W, pts = _case(synth, orc, cfg, frac)
     ow = orc.Window(W, settings=settings)
     ba = product_ba_from_oracle(capi, W, ow, chunk_points=P)   # carries the points' priorF (hasDepthPrior)
     if settings:
