@@ -212,7 +212,7 @@ SYMBOLS = [
     "dmv_ct_create", "dmv_ct_destroy", "dmv_ct_set_K", "dmv_ct_set_ref", "dmv_ct_make_coarse_depth", "dmv_ct_set_ref_from_ba", "dmv_ct_get_ref", "dmv_ct_upload_new", "dmv_ct_upload_new_image", "dmv_ct_set_huber",
     "dmv_ci_create", "dmv_ci_destroy", "dmv_ci_set_K", "dmv_ci_upload_first", "dmv_ci_upload_new", "dmv_ci_set_points", "dmv_ci_calc_res_and_gs", "dmv_ci_kernel_launch_count",
     "dmv_ct_calc_res_gs", "dmv_ct_track", "dmv_ct_track_many", "dmv_ct_track_tries", "dmv_ct_track_tries_many", "dmv_ip_default_settings", "dmv_ct_init_points", "dmv_ct_trace_points", "dmv_ct_trace_points_multi", "dmv_ct_trace_many", "dmv_ip_store_create", "dmv_ip_store_destroy", "dmv_ip_store_put", "dmv_ip_store_get", "dmv_ip_store_remove", "dmv_ct_trace_store", "dmv_ct_trace_store_many", "dmv_ct_set_timing", "dmv_ct_last_timing", "dmv_ct_kernel_launch_count", "dmv_ct_last_point_evaluations",
-    "dmv_ct_set_undistort", "dmv_ct_upload_raw_image", "dmv_ct_download_frame", "dmv_ps_default_settings", "dmv_ct_make_new_traces",
+    "dmv_ct_set_undistort", "dmv_ct_upload_raw_image", "dmv_ct_download_frame", "dmv_ps_default_settings", "dmv_ct_make_new_traces", "dmv_ct_make_new_traces_store",
 ]
 
 
@@ -333,6 +333,7 @@ _ARGTYPES = {
     "dmv_ps_default_settings": [C.POINTER(PSSettings)],
     "dmv_ip_default_settings": [C.POINTER(IPSettings)],
     "dmv_ct_make_new_traces": [vp, C.POINTER(NewTracesArgs)],
+    "dmv_ct_make_new_traces_store": [vp, vp, C.c_int, C.POINTER(NewTracesArgs)],
     "dmv_ci_create": [C.POINTER(CTConfig), C.POINTER(vp)],
     "dmv_ci_destroy": [vp],
     "dmv_ci_set_K": [vp, C.c_int, C.c_float, C.c_float, C.c_float, C.c_float],
@@ -790,6 +791,10 @@ def _tables14(tables):
     return tab
 
 
+# the per-point outputs of dmv_new_traces_args: per-point shape and dtype
+_NT_SHAPES = {"u": ((), np.int32), "v": ((), np.int32), "type": ((), np.float32), "color": ((8,), np.float32), "weights": ((8,), np.float32),
+              "gradH": ((4,), np.float32), "energyTH": ((), np.float32)}
+
 IP_OUT_KEYS = ("idepth_min", "idepth_max", "quality", "status", "lastTraceUV", "lastTracePixelInterval")
 
 
@@ -972,6 +977,45 @@ class CT:
         self._check(self.L.dmv_ct_get_ref(self.h, lvl, C.byref(n), *[x.ctypes.data for x in a]))
         return dict(u=a[0], v=a[1], idepth=a[2], color=a[3])
 
+    def _ps_settings(self, settings):
+        if settings is None:
+            return None
+        S = PSSettings()
+        self.L.dmv_ps_default_settings(C.byref(S))
+        for k, val in settings.items():
+            setattr(S, k, val)
+        return S
+
+    def make_new_traces_store(self, store, slot, potential, density=1500.0, recursionsLeft=1, thFactor=1.0, B=None, settings=None, want=("type",),
+                              cap=16384, want_map=False):
+        """FullSystem::makeNewTraces with the new points put straight into slot `slot` of store, an IPStore (dmv_ct_make_new_traces_store);
+        store.counts follows.  want: the per-point outputs to read back from the slot, keys of make_new_traces' points (u, v, type, color,
+        weights, gradH, energyTH); with none, cap does not apply.  Returns dict(points (the wanted ones), n, numPointsTotal, potential (after),
+        map (if want_map)); an overflow raises DmvError and sets last_needed, as make_new_traces does."""
+        W, H = self.size
+        want = tuple(want)
+        bad = [k for k in want if k not in _NT_SHAPES]
+        if bad:
+            raise ValueError(f"unknown outputs {bad}")
+        cap = int(cap) if want else 0
+        pot, n, npt = C.c_int(int(potential)), C.c_int(0), C.c_int(0)
+        P = {k: np.zeros((max(cap, 1),) + _NT_SHAPES[k][0], _NT_SHAPES[k][1]) for k in want}
+        m = np.zeros(W * H, np.float32) if want_map else None
+        Bk = None if B is None else _c(B, np.float32)
+        S = self._ps_settings(settings)
+        ptr = lambda k: P[k].ctypes.data if k in P else None  # noqa: E731
+        a = NewTracesArgs(float(density), int(recursionsLeft), float(thFactor), None if Bk is None else Bk.ctypes.data,
+                          None if S is None else C.addressof(S), C.pointer(pot), cap, C.pointer(n), C.pointer(npt), ptr("u"), ptr("v"), ptr("type"),
+                          ptr("color"), ptr("weights"), ptr("gradH"), ptr("energyTH"), None if m is None else m.ctypes.data)
+        rc = self.L.dmv_ct_make_new_traces_store(self.h, store.h, int(slot), C.byref(a))
+        self.last_needed, self.last_potential = n.value, pot.value
+        self._check(rc)
+        store.counts[slot] = n.value
+        out = dict(points={k: P[k][:n.value] for k in P}, n=n.value, numPointsTotal=npt.value, potential=pot.value)
+        if want_map:
+            out["map"] = m.reshape(H, W)
+        return out
+
     def make_new_traces(self, potential, density=1500.0, recursionsLeft=1, thFactor=1.0, B=None, settings=None, cap=16384, want_map=False):
         """FullSystem::makeNewTraces on the resident frame (dmv_ct_make_new_traces).  potential: the selector's currentPotential before the call.
         cap: point capacity (the default is ten times the default density; an overflow raises DmvError and sets last_needed).
@@ -984,12 +1028,7 @@ class CT:
                  energyTH=np.zeros(max(cap, 1), np.float32))
         m = np.zeros(W * H, np.float32) if want_map else None
         Bk = None if B is None else _c(B, np.float32)
-        S = None
-        if settings is not None:
-            S = PSSettings()
-            self.L.dmv_ps_default_settings(C.byref(S))
-            for k, val in settings.items():
-                setattr(S, k, val)
+        S = self._ps_settings(settings)
         a = NewTracesArgs(float(density), int(recursionsLeft), float(thFactor), None if Bk is None else Bk.ctypes.data,
                           None if S is None else C.addressof(S), C.pointer(pot), cap, C.pointer(n), C.pointer(npt), P["u"].ctypes.data, P["v"].ctypes.data,
                           P["type"].ctypes.data, P["color"].ctypes.data, P["weights"].ctypes.data, P["gradH"].ctypes.data, P["energyTH"].ctypes.data,

@@ -59,27 +59,42 @@ static cudaError_t ip_store_reserve(dmv_ip_store* s, int k, int n) {
 }
 
 // The edit shared by put and remove: the new list is perm (perm.size() rows) over the current buffer and the m rows that the caller wrote
-// into h_edit (ipw layout of capacity m); uploaded, gathered into the other buffer on the store's stream, synchronised, then made current.
-// h_edit already holds room for the rows and perm (ip_store_stage).
-static int ip_store_apply(dmv_ip_store* s, const std::vector<int>& perm, int m, const int* count_after) {
+// into h_edit (ipw layout of capacity m), or, rows_on_device, into d_edit on the store's stream; uploaded (the row map only when the rows
+// are already there), gathered into the other buffer on the store's stream.  Returns the buffer the list lands in; ip_store_commit makes it
+// current.  h_edit / d_edit already hold room for the rows and perm (ip_store_stage).
+static int ip_store_gather(dmv_ip_store* s, const std::vector<int>& perm, int m, bool rows_on_device, int* dst_out) {
   const int n = (int)perm.size();
   const int dst = 1 - s->cur;
   CK(ip_store_reserve(s, dst, n));
-  const size_t words = (size_t)kWords * m + n;
-  std::memcpy(s->h_edit.get() + (size_t)kWords * m, perm.data(), sizeof(int) * (size_t)n);
+  const size_t rows = (size_t)kWords * m, words = rows + n;
+  std::memcpy(s->h_edit.get() + rows, perm.data(), sizeof(int) * (size_t)n);
   if (n > 0) {
-    CK(cudaMemcpyAsync(s->d_edit, s->h_edit, sizeof(float) * words, cudaMemcpyHostToDevice, s->stream));
+    const size_t first = rows_on_device ? rows : 0;
+    CK(cudaMemcpyAsync(s->d_edit + first, s->h_edit + first, sizeof(float) * (words - first), cudaMemcpyHostToDevice, s->stream));
     const dim3 grid((n + 127) / 128, kWords);
     ip_store_gather_kernel<<<grid, 128, 0, s->stream>>>(reinterpret_cast<unsigned*>(s->d_pts[dst].get()), s->cap[dst],
                                                         reinterpret_cast<const unsigned*>(s->d_pts[s->cur].get()), s->cap[s->cur],
                                                         reinterpret_cast<const unsigned*>(s->d_edit.get()), m,
-                                                        reinterpret_cast<const int*>(s->d_edit.get() + (size_t)kWords * m), n);
+                                                        reinterpret_cast<const int*>(s->d_edit.get() + rows), n);
     CK(cudaGetLastError());
   }
+  *dst_out = dst;
+  return DMV_OK;
+}
+
+// synchronises the store's stream, then buffer dst holds the list and count_after its slot counts
+static int ip_store_commit(dmv_ip_store* s, int dst, const int* count_after) {
   CK(cudaStreamSynchronize(s->stream));
   s->cur = dst;
   std::memcpy(s->count, count_after, sizeof(s->count));
   return DMV_OK;
+}
+
+static int ip_store_apply(dmv_ip_store* s, const std::vector<int>& perm, int m, const int* count_after) {
+  int dst = 0;
+  const int rc = ip_store_gather(s, perm, m, false, &dst);
+  if (rc != DMV_OK) return rc;
+  return ip_store_commit(s, dst, count_after);
 }
 
 // h_edit / d_edit hold an edit of m uploaded rows and an n-row map
@@ -196,6 +211,22 @@ static int ip_store_slot_check(const dmv_ip_store* s, int slot) {
   return DMV_OK;
 }
 
+// put's row map: every slot's rows in place, slot `slot` replaced by the m uploaded rows; count = the slot counts after the edit
+static void ip_store_put_map(const dmv_ip_store* s, int slot, int m, std::vector<int>& perm, int* count) {
+  perm.clear();
+  perm.reserve(ip_store_total(s) - s->count[slot] + m);
+  int at = 0;
+  for (int k = 0; k < DMV_IP_STORE_SLOTS; k++) {
+    if (k == slot)
+      for (int q = 0; q < m; q++) perm.push_back(-1 - q);
+    else
+      for (int q = 0; q < s->count[k]; q++) perm.push_back(at + q);
+    at += s->count[k];
+  }
+  std::memcpy(count, s->count, sizeof(s->count));
+  count[slot] = m;
+}
+
 int dmv_ip_store_put(dmv_ip_store* s, int slot, const dmv_ip_points* p) {
   int rc = ip_store_slot_check(s, slot);
   if (rc != DMV_OK) return rc;
@@ -222,20 +253,66 @@ int dmv_ip_store_put(dmv_ip_store* s, int slot, const dmv_ip_points* p) {
     for (size_t q = 0; q < n; q++) setp[q] = slot;
   }
   std::vector<int> perm;
-  perm.reserve(total);
-  int at = 0;
-  for (int k = 0; k < DMV_IP_STORE_SLOTS; k++) {
-    if (k == slot)
-      for (int q = 0; q < m; q++) perm.push_back(-1 - q);
-    else
-      for (int q = 0; q < s->count[k]; q++) perm.push_back(at + q);
-    at += s->count[k];
-  }
   int count[DMV_IP_STORE_SLOTS];
-  std::memcpy(count, s->count, sizeof(count));
-  count[slot] = m;
+  ip_store_put_map(s, slot, m, perm, count);
   return ip_store_apply(s, perm, m, count);
 }
+
+namespace dmv {
+// put with rows the caller writes on the device (ip_store.h).  d_edit: the m rows (ipw layout of capacity m), the row map, then m words for
+// the caller; h_edit: the row map at the same offset, and the downloaded outputs in front of it (24 words per point <= kWords)
+int ip_store_rows_stage(dmv_ip_store* s, int slot, int m, float** d_rows, float** d_extra) {
+  const int total = ip_store_total(s) - s->count[slot] + m;
+  CK(cudaSetDevice(s->device));
+  const int rc = ip_store_stage(s, m, total + m);
+  if (rc != DMV_OK) return rc;
+  *d_rows = s->d_edit;
+  *d_extra = s->d_edit + (size_t)kWords * m + total;
+  return DMV_OK;
+}
+
+int ip_store_rows_put(dmv_ip_store* s, int slot, int m, const dmv_new_traces_args* out) {
+  const int old = s->count[slot];
+  if (m == 0 && old == 0) {   // put leaves the store as it is; the caller's copy kernel has nothing to write
+    CK(cudaStreamSynchronize(s->stream));
+    return DMV_OK;
+  }
+  std::vector<int> perm;
+  int count[DMV_IP_STORE_SLOTS];
+  ip_store_put_map(s, slot, m, perm, count);
+  const float* d_extra = s->d_edit + (size_t)kWords * m + perm.size();
+  int dst = 0;
+  const int rc = ip_store_gather(s, perm, m, true, &dst);
+  if (rc != DMV_OK) return rc;
+  // the requested outputs from the slot's rows in the new buffer; type, which the store does not hold, from the words beside the rows
+  const size_t cap = s->cap[dst], at = ip_store_first(s, slot), n = m;
+  const float* d = s->d_pts[dst];
+  float* hb = s->h_edit;
+  struct Field { const void* want; const float* src; size_t words; };
+  const Field f[7] = {{out->u, d + ipw::u * cap + at, n},
+                      {out->v, d + ipw::v * cap + at, n},
+                      {out->color8, d + ipw::color * cap + 8 * at, 8 * n},
+                      {out->weights8, d + ipw::weights * cap + 8 * at, 8 * n},
+                      {out->gradH4, d + ipw::gradH * cap + 4 * at, 4 * n},
+                      {out->energyTH, d + ipw::energyTH * cap + at, n},
+                      {out->type, d_extra, n}};
+  size_t o = 0;
+  for (const Field& x : f) {
+    if (x.want && n > 0) CK(cudaMemcpyAsync(hb + o, x.src, sizeof(float) * x.words, cudaMemcpyDeviceToHost, s->stream));
+    o += x.words;
+  }
+  const int rc2 = ip_store_commit(s, dst, count);
+  if (rc2 != DMV_OK) return rc2;
+  for (size_t i = 0; out->u && i < n; i++) out->u[i] = (int32_t)hb[i];
+  for (size_t i = 0; out->v && i < n; i++) out->v[i] = (int32_t)hb[n + i];
+  if (out->color8) std::memcpy(out->color8, hb + 2 * n, 32 * n);
+  if (out->weights8) std::memcpy(out->weights8, hb + 10 * n, 32 * n);
+  if (out->gradH4) std::memcpy(out->gradH4, hb + 18 * n, 16 * n);
+  if (out->energyTH) std::memcpy(out->energyTH, hb + 22 * n, 4 * n);
+  if (out->type) std::memcpy(out->type, hb + 23 * n, 4 * n);
+  return DMV_OK;
+}
+}  // namespace dmv
 
 int dmv_ip_store_get(dmv_ip_store* s, int slot, dmv_ip_points* p) {
   const int rc = ip_store_slot_check(s, slot);

@@ -1,5 +1,6 @@
 // The immature-point store's internals (ip_store.cu), shared with the activation fed from a store (dmv_ba_activate_store): the BA side
-// reads the current buffer and the slot counts, and its removals go through the store's one edit path.
+// reads the current buffer and the slot counts, and its removals go through the store's one edit path; pixel selection straight into a
+// store (dmv_ct_make_new_traces_store) writes its rows into the same edit.
 #pragma once
 #include "../../include/dmvio_b200.h"
 #include "common_host.h"
@@ -24,6 +25,14 @@ int ip_store_first(const dmv_ip_store* s, int slot);
 // activatePointsMT's swap-with-back loop (FullSystem.cpp:L761-769, remove_outliers_order), in one gather.  order[k] = slot k's survivors'
 // old indices in their new order (the identity for a slot without alive entries).  No edit, copy or synchronisation when nothing is removed.
 int ip_store_remove_dead(dmv_ip_store* s, const std::vector<char> (&alive)[DMV_IP_STORE_SLOTS], std::vector<int> (&order)[DMV_IP_STORE_SLOTS]);
+
+// dmv_ip_store_put of a slot's m rows that the caller writes on the device instead of uploading them (dmv_ct_make_new_traces_store).
+// ip_store_rows_stage makes room in the edit staging: *d_rows = the rows (ipw layout of capacity m, every word put uploads, set included),
+// *d_extra = m words beside them that the store does not keep.  The caller writes both on the store's stream; ip_store_rows_put then
+// uploads the row map only, gathers as put does, downloads out's non-NULL per-point outputs (u, v, color8, weights8, gradH4, energyTH from
+// the slot's rows after the edit, type from *d_extra) and synchronises once.  Neither checks slot or m.
+int ip_store_rows_stage(dmv_ip_store* s, int slot, int m, float** d_rows, float** d_extra);
+int ip_store_rows_put(dmv_ip_store* s, int slot, int m, const dmv_new_traces_args* out);
 
 // dmv_ba_select_activation's argument checks (ip_select.cu); from_store: the immature points' arrays and action are not the caller's
 int sel_check(const dmv_ba* b, const dmv_ba_select_args* a, bool from_store);

@@ -28,8 +28,10 @@
 // makeMaps' recursion (L203-244) is decided on the device (ps_decide_kernel): recursionsLeft + 1 select passes are queued and the passes after
 // the decision to return are no-ops, so the host waits once.  Sub-selection (L248-265): the k-th nonzero map entry in raster order is cleared
 // when randomPattern[k] > (unsigned char)(255*quotia), a prefix count over the map.  makeNewTraces' loop: a raster compaction of the nonzero
-// entries in [3, w-4) x [3, h-4), the existing ip_init_kernel, and a compaction of the finite energyTH into the caller's pinned output.
+// entries in [3, w-4) x [3, h-4), the existing ip_init_kernel, and a compaction of the finite energyTH into the caller's pinned output, or,
+// for dmv_ct_make_new_traces_store, into an immature-point store's edit staging (ps_store_rows_kernel) in the layout dmv_ip_store_put uploads.
 #include "ct_handle.h"
+#include "ip_store.h"
 #include "ip_trace.h"
 #include <cub/device/device_scan.cuh>
 #include <climits>
@@ -439,6 +441,33 @@ __global__ void ps_scatter_out_kernel(const PSDev D) {
   for (int k = 0; k < 4; k++) o[(19 + k) * O + r] = c[19 * C + 4 * (size_t)i + k];
   o[23 * O + r] = c[23 * C + i];
 }
+// the points into an immature-point store's edit staging (dmv_ct_make_new_traces_store): the rows dmv_ip_store_put uploads, in the ipw
+// layout of capacity m (the point count), u and v as floats, the ImmaturePoint constructor's in/out values (ImmaturePoint.cpp:L39-41) and
+// set = slot; type into its own m words
+__global__ void ps_store_rows_kernel(const PSDev D, float* __restrict__ rows, float* __restrict__ type, int m, int slot) {
+  const int i = blockIdx.x * blockDim.x + threadIdx.x;
+  if (i >= D.w * D.h || !D.flag[i]) return;
+  const int r = D.rank[i];
+  if (r >= m) return;
+  const size_t C = D.cand_cap, M = m;
+  const float* c = D.cand;
+  rows[ipw::u * M + r] = (float)reinterpret_cast<const int*>(c)[i];
+  rows[ipw::v * M + r] = (float)reinterpret_cast<const int*>(c + C)[i];
+  type[r] = c[2 * C + i];
+#pragma unroll
+  for (int k = 0; k < 8; k++) { rows[ipw::color * M + 8 * r + k] = c[3 * C + 8 * (size_t)i + k]; rows[ipw::weights * M + 8 * r + k] = c[11 * C + 8 * (size_t)i + k]; }
+#pragma unroll
+  for (int k = 0; k < 4; k++) rows[ipw::gradH * M + 4 * r + k] = c[19 * C + 4 * (size_t)i + k];
+  rows[ipw::energyTH * M + r] = c[23 * C + i];
+  rows[ipw::idepth_min * M + r] = 0.f;
+  rows[ipw::idepth_max * M + r] = __int_as_float(0x7FC00000);   // NaN, as the host's quiet NaN
+  rows[ipw::quality * M + r] = 10000.f;
+  reinterpret_cast<int*>(rows + ipw::status * M)[r] = 5;        // IPS_UNINITIALIZED
+  rows[ipw::uv * M + 2 * r] = 0.f;
+  rows[ipw::uv * M + 2 * r + 1] = 0.f;
+  rows[ipw::interval * M + r] = 0.f;
+  reinterpret_cast<int*>(rows + ipw::set * M)[r] = slot;
+}
 __global__ void ps_init_state_kernel(PSState* S, int pot, int recLeft) {
   S->pot = pot; S->recLeft = recLeft; S->done = 0; S->n3 = 0; S->n4 = 0; S->numHaveSub = 0; S->ideal = pot; S->quotia = 0.f;
   S->n_cand = 0; S->n_points = 0; S->n_mixed = 0; S->pad = 0;
@@ -502,9 +531,8 @@ static int ps_alloc(PSScratch& S, int w, int h) {
   return DMV_OK;
 }
 
-// every launch of the call: the points and the final PSState land in S.h_out, which the host reads after one stream synchronisation;
-// the selection map stays in S.map.  *kernels = kernels launched (CUB's own launches not counted)
-static cudaError_t ps_launch(const PSArgs& A, PSScratch& S, cudaStream_t s, int* kernels) {
+// what every kernel of the call reads
+static PSDev ps_dev(const PSArgs& A, PSScratch& S) {
   const int w = A.w, h = A.h, n = w * h;
   PSDev D;
   D.w = w; D.h = h; D.w1 = w >> 1; D.h1 = h >> 1; D.w2 = w >> 2; D.h2 = h >> 2; D.nbW = w / 16; D.nbH = h / 16;
@@ -518,6 +546,13 @@ static cudaError_t ps_launch(const PSArgs& A, PSScratch& S, cudaStream_t s, int*
   D.scan_in = S.scan_in; D.scan = S.scan; D.mixed = S.mixed; D.delta = S.delta; D.n2b = S.n2b; D.map = S.map; D.flag = S.flag; D.rank = S.rank;
   D.cand = S.cand; D.cand_cap = n; D.st = S.st;
   D.out = S.h_out; D.out_cap = A.out_cap;
+  return D;
+}
+
+// the selection up to its final compaction: makeMaps, the sub-selection, the raster loop with ip_init_kernel, and the scan of the points with
+// a finite energyTH (flag, rank over the candidates).  *kernels = kernels launched (CUB's own launches not counted)
+static cudaError_t ps_select_launch(const PSArgs& A, const PSDev& D, PSScratch& S, cudaStream_t s, int* kernels) {
+  const int w = A.w, h = A.h, n = w * h;
   int k = 0;
   cudaError_t e;
   const dim3 rows((w + 127) / 128, h);
@@ -556,9 +591,18 @@ static cudaError_t ps_launch(const PSArgs& A, PSScratch& S, cudaStream_t s, int*
   launch_ip_init(I, s); k++;
   ps_flag_ok_kernel<<<pb, 256, 0, s>>>(D); k++;
   if ((e = cub::DeviceScan::ExclusiveSum(S.temp, tb, S.flag.get(), S.rank.get(), n, s)) != cudaSuccess) return e;
-  ps_scatter_out_kernel<<<pb, 256, 0, s>>>(D); k++;
-  if ((e = cudaMemcpyAsync(S.h_out, S.st, sizeof(PSState), cudaMemcpyDeviceToHost, s)) != cudaSuccess) return e;
   *kernels = k;
+  return cudaGetLastError();
+}
+
+// every launch of dmv_ct_make_new_traces: the points and the final PSState land in S.h_out, which the host reads after one stream
+// synchronisation; the selection map stays in S.map.  *kernels = kernels launched (CUB's own launches not counted)
+static cudaError_t ps_launch(const PSArgs& A, PSScratch& S, cudaStream_t s, int* kernels) {
+  const PSDev D = ps_dev(A, S);
+  cudaError_t e;
+  if ((e = ps_select_launch(A, D, S, s, kernels)) != cudaSuccess) return e;
+  ps_scatter_out_kernel<<<(A.w * A.h + 255) / 256, 256, 0, s>>>(D); (*kernels)++;
+  if ((e = cudaMemcpyAsync(S.h_out, S.st, sizeof(PSState), cudaMemcpyDeviceToHost, s)) != cudaSuccess) return e;
   return cudaGetLastError();
 }
 
@@ -572,22 +616,28 @@ void dmv_ps_default_settings(dmv_ps_settings* s) {
   s->selectDirectionDistribution = 1; s->gammaWeightsPixelSelect = 1;
 }
 
-// FullSystem::makeNewTraces on the resident frame
-int dmv_ct_make_new_traces(dmv_ct* c, const dmv_new_traces_args* a) {
-  if (!c || !a) return set_error(DMV_ERR_INVALID, "null argument");
+// the checks of dmv_ct_make_new_traces (outputs_optional: those of dmv_ct_make_new_traces_store, where every per-point output may be NULL);
+// *st = the settings.  No CUDA call.
+static int ps_check(const dmv_ct* c, const dmv_new_traces_args* a, bool outputs_optional, dmv_ps_settings* st) {
   if (c->cfg.levels < 3) return set_error(DMV_ERR_INVALID, "pixel selection reads levels 0-2: the handle has %d", c->cfg.levels);
   const int w = c->w[0], h = c->h[0];
   if (w % 16 || h % 16) return set_error(DMV_ERR_INVALID, "pixel selection needs w and h divisible by 16 (%d x %d)", w, h);
-  if (!a->potential || !a->n || !a->numPointsTotal || a->cap < 0 || (a->cap > 0 && (!a->u || !a->v || !a->type || !a->color8 || !a->weights8 || !a->gradH4 || !a->energyTH)))
+  const bool outputs = a->u && a->v && a->type && a->color8 && a->weights8 && a->gradH4 && a->energyTH;
+  if (!a->potential || !a->n || !a->numPointsTotal || a->cap < 0 || (a->cap > 0 && !outputs_optional && !outputs))
     return set_error(DMV_ERR_INVALID, "null argument");
   if (*a->potential < 1) return set_error(DMV_ERR_INVALID, "potential %d < 1", *a->potential);
   if (!(a->density > 0.f) || !std::isfinite(a->density)) return set_error(DMV_ERR_INVALID, "density must be finite and > 0");
   if (!(a->thFactor > 0.f) || !std::isfinite(a->thFactor)) return set_error(DMV_ERR_INVALID, "thFactor must be finite and > 0");
   if (a->recursionsLeft < 0 || a->recursionsLeft > 8) return set_error(DMV_ERR_INVALID, "recursionsLeft must be in 0..8");
-  dmv_ps_settings st;
-  if (a->settings) st = *a->settings; else dmv_ps_default_settings(&st);
-  if (!(st.minGradHistCut < 0.99f) || !std::isfinite(st.minGradHistCut) || !std::isfinite(st.minGradHistAdd) || !std::isfinite(st.gradDownweightPerLevel))
+  if (a->settings) *st = *a->settings; else dmv_ps_default_settings(st);
+  if (!(st->minGradHistCut < 0.99f) || !std::isfinite(st->minGradHistCut) || !std::isfinite(st->minGradHistAdd) || !std::isfinite(st->gradDownweightPerLevel))
     return set_error(DMV_ERR_INVALID, "bad dmv_ps_settings");
+  return DMV_OK;
+}
+
+// the handle's scratch for its frame size with room for out_cap points in h_out, the staging free, and B on its way; *A = the launch's arguments
+static int ps_prepare(dmv_ct* c, const dmv_new_traces_args* a, const dmv_ps_settings& st, int out_cap, PSArgs* A) {
+  const int w = c->w[0], h = c->h[0];
   CK(cudaSetDevice(c->device));
   if (!c->ps) c->ps.reset(new PSScratch());
   PSScratch& P = *c->ps;
@@ -596,17 +646,30 @@ int dmv_ct_make_new_traces(dmv_ct* c, const dmv_new_traces_args* a) {
     const int rc = ps_alloc(P, w, h);
     if (rc != DMV_OK) { P = PSScratch(); return rc; }
   }
-  const int out_cap = std::min(a->cap, w * h);
   CK(P.h_out.reserve(sizeof(PSState) / sizeof(float) + 24 * (size_t)std::max(out_cap, 1)));
   CK(ct_wait_staging(c));
   float B[256];
   for (int i = 0; i < 256; i++) B[i] = a->B ? a->B[i] : (float)i;   // CalibHessian's constructor: B[i] = i
   CK(cudaMemcpyAsync(P.B, B, sizeof(B), cudaMemcpyHostToDevice, c->stream));
+  A->w = w; A->h = h;
+  for (int l = 0; l < 3; l++) A->img[l] = c->d_img[l];
+  A->s = st; A->density = a->density; A->thFactor = a->thFactor; A->recursionsLeft = a->recursionsLeft; A->potential = *a->potential;
+  A->out_cap = out_cap;
+  return DMV_OK;
+}
+
+// FullSystem::makeNewTraces on the resident frame
+int dmv_ct_make_new_traces(dmv_ct* c, const dmv_new_traces_args* a) {
+  if (!c || !a) return set_error(DMV_ERR_INVALID, "null argument");
+  dmv_ps_settings st;
+  int rc = ps_check(c, a, false, &st);
+  if (rc != DMV_OK) return rc;
+  const int w = c->w[0], h = c->h[0];
+  const int out_cap = std::min(a->cap, w * h);
   PSArgs A;
-  A.w = w; A.h = h;
-  for (int l = 0; l < 3; l++) A.img[l] = c->d_img[l];
-  A.s = st; A.density = a->density; A.thFactor = a->thFactor; A.recursionsLeft = a->recursionsLeft; A.potential = *a->potential;
-  A.out_cap = out_cap;
+  rc = ps_prepare(c, a, st, out_cap, &A);
+  if (rc != DMV_OK) return rc;
+  PSScratch& P = *c->ps;
   int kernels = 0;
   CK(ps_launch(A, P, c->stream, &kernels));
   c->launches += kernels;
@@ -627,5 +690,52 @@ int dmv_ct_make_new_traces(dmv_ct* c, const dmv_new_traces_args* a) {
   for (size_t i = 0; i < n; i++)
     for (int k = 0; k < 4; k++) a->gradH4[4 * i + k] = o[(19 + k) * O + i];
   std::memcpy(a->energyTH, o + 23 * O, 4 * n);
+  return DMV_OK;
+}
+
+// makeNewTraces straight into slot `slot` of an immature-point store: the selection as above, its point count read back (synchronisation 1),
+// ps_store_rows_kernel in place of ps_scatter_out_kernel writing the slot's rows into the store's edit staging, then the store's edit with
+// the requested outputs read from the slot's rows (synchronisation 2)
+int dmv_ct_make_new_traces_store(dmv_ct* c, dmv_ip_store* s, int slot, const dmv_new_traces_args* a) {
+  if (!c || !s || !a) return set_error(DMV_ERR_INVALID, "null argument");
+  dmv_ps_settings st;
+  int rc = ps_check(c, a, true, &st);
+  if (rc != DMV_OK) return rc;
+  if (slot < 0 || slot >= DMV_IP_STORE_SLOTS) return set_error(DMV_ERR_INVALID, "slot %d: expected 0 to %d", slot, DMV_IP_STORE_SLOTS - 1);
+  if (s->device != c->device) return set_error(DMV_ERR_INVALID, "the store is on device %d, the handle on device %d", s->device, c->device);
+  const bool outputs = a->u || a->v || a->type || a->color8 || a->weights8 || a->gradH4 || a->energyTH;
+  const int w = c->w[0], h = c->h[0], npx = w * h;
+  PSArgs A;
+  rc = ps_prepare(c, a, st, 0, &A);
+  if (rc != DMV_OK) return rc;
+  PSScratch& P = *c->ps;
+  const PSDev D = ps_dev(A, P);
+  int kernels = 0;
+  CK(ps_select_launch(A, D, P, c->stream, &kernels));
+  // the point count = rank + flag of the last candidate index, read beside the state
+  int* cnt = reinterpret_cast<int*>(P.h_out + sizeof(PSState) / sizeof(float));
+  CK(cudaMemcpyAsync(P.h_out, P.st, sizeof(PSState), cudaMemcpyDeviceToHost, c->stream));
+  CK(cudaMemcpyAsync(cnt, P.rank + (npx - 1), sizeof(int), cudaMemcpyDeviceToHost, c->stream));
+  CK(cudaMemcpyAsync(cnt + 1, P.flag + (npx - 1), sizeof(int), cudaMemcpyDeviceToHost, c->stream));
+  if (a->map) CK(cudaMemcpyAsync(a->map, P.map, sizeof(float) * (size_t)npx, cudaMemcpyDeviceToHost, c->stream));
+  CK(cudaStreamSynchronize(c->stream));
+  PSState S;
+  std::memcpy(&S, P.h_out, sizeof(S));
+  const int m = cnt[0] + cnt[1];
+  *a->n = m;
+  if (outputs && m > a->cap) {   // as dmv_ct_make_new_traces: the store and the selector's state stay as they were
+    c->launches += kernels;
+    return set_error(DMV_ERR_INVALID, "%d new points exceed cap %d", m, a->cap);
+  }
+  float *rows = nullptr, *type = nullptr;
+  rc = ip_store_rows_stage(s, slot, m, &rows, &type);
+  if (rc != DMV_OK) return rc;
+  ps_store_rows_kernel<<<(npx + 255) / 256, 256, 0, s->stream>>>(D, rows, type, m, slot);
+  CK(cudaGetLastError());
+  c->launches += kernels + 1;
+  rc = ip_store_rows_put(s, slot, m, a);
+  if (rc != DMV_OK) return rc;
+  *a->potential = S.ideal;
+  *a->numPointsTotal = S.numHaveSub;
   return DMV_OK;
 }

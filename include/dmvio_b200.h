@@ -691,6 +691,27 @@ typedef struct dmv_new_traces_args {
  * Errors: DMV_ERR_INVALID for levels < 3, w or h not a multiple of 16, bad arguments (including *potential < 1), or more than cap points
  * (*n = the count needed); DMV_ERR_CUDA. */
 int dmv_ct_make_new_traces(dmv_ct* ct, const dmv_new_traces_args* a);
+/* dmv_ct_make_new_traces with the new points put straight into slot `slot` of an immature-point store, without their round trip through
+ * host memory.  Bit-identical to the pair
+ *   1. dmv_ct_make_new_traces(ct, a),
+ *   2. dmv_ip_store_put(s, slot, pts) with pts = those points, u and v converted to float, and the ImmaturePoint constructor's in/out values:
+ *      idepth_min 0, idepth_max NaN (0x7FC00000), quality 10000, lastTraceStatus 5 (IPS_UNINITIALIZED), lastTraceUV2 (0, 0),
+ *      lastTracePixelInterval 0,
+ * on every observable: the slot's contents and count (the slot is replaced, as by put; no point empties it), the other slots, every later
+ * trace or activation of the store, *potential, *numPointsTotal, *n, map and the requested per-point outputs.
+ * a: as dmv_ct_make_new_traces, but each per-point output (u, v, type, color8, weights8, gradH4, energyTH) may be NULL on its own, and cap is
+ * the capacity of those that are not.  They are read back from the slot's rows after the edit (type, which the store does not hold, from
+ * the staged copy beside them).  A caller that needs only ImmaturePoint::my_type for dmv_ba_activate_store asks for type alone: 4 bytes per
+ * point come down, and the row map of the store's edit (4 bytes per point in the store) goes up.
+ * Overflow: more points than cap with any per-point output requested gives DMV_ERR_INVALID with *n = the count needed, the store,
+ * *potential and *numPointsTotal unchanged (a retry gives the same result); with no per-point output there is no cap.
+ * Launch count: ct's moves as dmv_ct_make_new_traces' does on the same frame (the copy into the store takes the place of the copy into
+ * host memory; the store's gather is not counted, as for put).  On overflow the copy is not launched: one launch fewer.
+ * Two synchronisations: one after the selection (it reads the point count), one after the store's edit.
+ * Errors, all before any allocation, copy or launch (the store, *potential and the launch counts unchanged): those of
+ * dmv_ct_make_new_traces, with the same messages, except for NULL per-point outputs; DMV_ERR_INVALID for a NULL s, slot outside
+ * 0..DMV_IP_STORE_SLOTS-1, or a store on another device than ct. */
+int dmv_ct_make_new_traces_store(dmv_ct* ct, dmv_ip_store* s, int slot, const dmv_new_traces_args* a);
 
 /* enable/disable the CUDA-event timing of dmv_ct_calc_res_gs (off by default); dmv_ct_last_timing()[0] = kernel milliseconds */
 int dmv_ct_set_timing(dmv_ct* ct, int enable);
